@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — GGML_OP_MUL_MAT over block-quantized weights on B200 (contract: the task statement / DESIGN.md §4 and §8).
+"""bench.py — GGML_OP_MUL_MAT over block-quantized weights on H100 (DESIGN.md §4 and §8).
 
 Headline workload (BASELINE.json configs[1]): Q4_K 4096 -> 11008 mat-vec, n_batch = 1 (Llama-7B FFN shape).
-  sweep           NBUF = 13 distinct weight matrices (13 x 25.4 MB = 330 MB > 2 x the 126 MB L2), one mat-vec each: every mat-vec
+  sweep           NBUF = 13 distinct weight matrices (13 x 25.4 MB = 330 MB > 6 x the 50 MB L2), one mat-vec each: every mat-vec
                   streams its weights from HBM
-  step            SWEEPS_PER_STEP = 512 sweeps (6656 mat-vecs, ~30 ms) so that the driver's --steps 20 times >= 0.5 s and the clock
+  step            SWEEPS_PER_STEP = 512 sweeps (6656 mat-vecs, ~60 ms on an H100 at 400 W) so that --steps 20 times >= 0.5 s and the clock
                   sampler sees the load; launched as CUDA-graph replays of 8 sweeps
   value           GB/s of quantized weight bytes processed, whole job (all ranks), inputs resident in HBM, CUDA events, max over ranks
   parity          AFTER the timed region a row sample of every timed output is compared with the CPU oracle (NMSE <= 1e-10 for the
@@ -15,7 +15,7 @@ Headline workload (BASELINE.json configs[1]): Q4_K 4096 -> 11008 mat-vec, n_batc
                   exchange and the host copies inside the timed region
   roofline        algorithmic bytes (weights + x + y) / mean device time per launch vs the measured HBM peak
   extra           every other BASELINE configuration, each with its own parity and roofline: configs[0] Q4_0 4096^2 n=1; the dependent
-                  chain; configs[2] Q8_0 4096^2 x 512 on tcgen05 (TFLOP/s vs the measured sustained bf16 peak); Q4_K / Q8_0
+                  chain; configs[2] Q8_0 4096^2 x 512 on the wgmma GEMM (TFLOP/s vs the measured sustained bf16 peak); Q4_K / Q8_0
                   4096 -> 32000 at n = 1 and 512; configs[3] gpt-2 117M Q4_0 tok/s through the unmodified examples/gpt-2 program;
                   configs[4] Q4_K 8192 x 28672 row-sharded (strong scaling) over the N GPUs with the fused NVLink gather
   cpu_baseline    the unmodified reference's ggml-cpu backend (oracle/_ref) on this box's host cores, same shape
@@ -46,8 +46,8 @@ sys.path.insert(0, str(ROOT))
 WL = {"type": "q4_K", "type_id": 12, "K": 4096, "M": 11008, "N": 1}
 METRIC = "mul_mat_q4_K_4096x11008_n1_weight_throughput"
 UNIT = "GB/s"
-NBUF = 13                # distinct weight matrices per sweep: 13 x 25.4 MB = 330 MB > 2 x the 126 MB L2 (and > the host's last-level cache)
-SWEEPS_PER_STEP = 512    # one step = 512 sweeps = 6656 mat-vecs (~30 ms on one B200)
+NBUF = 13                # distinct weight matrices per sweep: 13 x 25.4 MB = 330 MB > 6 x the 50 MB L2 (and > the host's last-level cache)
+SWEEPS_PER_STEP = 512    # one step = 512 sweeps = 6656 mat-vecs (~62 ms on one H100 at a 400 W power limit)
 SWEEPS_PER_GRAPH = 8
 CONFIG = {"workload": f"q4_K {WL['K']}x{WL['M']} mat-vec n_batch=1 (BASELINE.json configs[1])", "mat_vecs_per_step": NBUF * SWEEPS_PER_STEP,
           "l2_policy": f"inputs larger than L2: {NBUF} distinct weight matrices (330 MB) visited round-robin"}
@@ -385,13 +385,13 @@ def extra_matvec(torch, g, timer, t, M, K, peaks, dependent_too=True, nbuf=None,
 
 
 def extra_gemm(torch, g, timer, t, M, N, K, peaks, seed=11):
-    """batched mat-mul on the tcgen05 path: TFLOP/s over distinct weight matrices, parity against the f64 product on sampled rows"""
+    """batched mat-mul on the tensor-core (wgmma) path: TFLOP/s over distinct weight matrices, parity against the f64 product on sampled rows"""
     wb = weight_bytes(K, M, t)
     nbuf = max(2, math.ceil(260e6 / wb))
     Ws = make_weights(torch, t, nbuf, K, M, seed)
     X = torch.rand(N * K, device="cuda", generator=torch.Generator(device="cuda").manual_seed(5678)) * 2 - 1
     Ys = [torch.empty((1, 1, N, M), dtype=torch.float32, device="cuda") for _ in range(nbuf)]
-    assert g.mul_mat_plan(t, M, N, K) == g.MM_GEMM, "batched shape must run on the tcgen05 kernel"
+    assert g.mul_mat_plan(t, M, N, K) == g.MM_GEMM, "batched shape must run on the tensor-core GEMM kernel"
     F = g.MM_SRC0_STATIC | g.MM_SRC1_STATIC
 
     def sweep():
@@ -424,6 +424,8 @@ def main():
     ap.add_argument("--exchange", default="fused", choices=["fused", "nccl"],
                     help="N > 1: 'fused' = the mat-vec kernel stores its rows into every peer's y over NVLink and signals flags; "
                          "'nccl' = ncclAllGather of the slices after the kernel (the baseline)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last step (y_<i>.npy, float32, one per weight matrix; with --exchange nccl only the last matrix's gathered y) to DIR")
     ap.add_argument("--cpu-baseline-child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--plugin-e2e-child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--gpt2-child", action="store_true", help=argparse.SUPPRESS)
@@ -552,6 +554,19 @@ def main():
     n_mv = nbuf * SWEEPS_PER_STEP * args.steps
     value = world * n_mv * wb / (ms * 1e-3) / 1e9
     us_per_launch = ms * 1e3 / n_mv
+
+    if args.dump_outputs and rank == 0:
+        # what the timed path returned in its last step: one y per weight matrix (inputs are seeded, so two builds compare output for output)
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        torch.cuda.synchronize()
+        if world > 1 and not fused:
+            # the NCCL exchange gathers every mat-vec into the one buffer Yall: only the sweep's last output survives the step
+            np.save(out_dir / f"y_{nbuf - 1:02d}.npy", Yall.view(world * N, M).float().cpu().numpy())
+        else:
+            for i in range(nbuf):
+                y = Ys[i].view(N, M) if world == 1 else ex.y_full(i).view(world * N, M)
+                np.save(out_dir / f"y_{i:02d}.npy", y.float().cpu().numpy())
 
     # ---- parity of the TIMED configuration: the outputs the timed launches wrote, sampled rows against the CPU oracle
     parity = {}

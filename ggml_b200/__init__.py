@@ -1,4 +1,4 @@
-"""ggml_b200 — B200-native (sm_100a) kernels for ggml's block-quantized MUL_MAT / MUL_MAT_ID hot path.
+"""ggml_b200 — H100-native (sm_90a) kernels for ggml's block-quantized MUL_MAT / MUL_MAT_ID hot path.
 
 The product is native code: `libggml-b200-kernels.so` (hand-written CUDA behind the C ABI of
 include/ggml-b200.h) and `libggml-b200.so` (the ggml backend plug-in built on it).  This Python module is only

@@ -24,10 +24,10 @@ void set_error(const char * fmt, ...) {
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -48,8 +48,8 @@ static int validate(const ggml_b200_mul_mat_args * a) {
 }
 
 // the int8 mma.sync consume path (mmvq_mma.cu): default for 2 <= n <= 8, and for n = 1 when the rows are very long (K >= 12288: the dp4a kernel's
-// chunks shrink to a few rows there; measured at K = 14336: Q6_K 21.0 -> 13.5 us, Q4_K 12.2 -> 10.3, Q8_0 18.8 -> 14.6; at K = 8192 the dp4a
-// kernel is still the faster one: Q4_K 8192 x 28672 24.0 vs 31.4 us).
+// chunks shrink to a few rows there; at K = 8192 the dp4a kernel is still the faster one; threshold chosen on a Blackwell part, not re-measured
+// on the H100).
 // GGML_B200_MMA = 0 never, 2 always; per call GGML_B200_MM_GEMV_MMA / GGML_B200_MM_GEMV_DP4A select explicitly
 static bool mma_wanted(const ggml_b200_mul_mat_args & a) {
     static const int env = getenv("GGML_B200_MMA") ? atoi(getenv("GGML_B200_MMA")) : 1;
@@ -83,7 +83,7 @@ using namespace b200;
 extern "C" {
 
 const char * ggml_b200_last_error(void) { return g_err; }
-const char * ggml_b200_version(void) { return "ggml-b200 0.1 (sm_100a)"; }
+const char * ggml_b200_version(void) { return "ggml-b200 0.1 (sm_90a)"; }
 uint64_t ggml_b200_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int ggml_b200_sm_count(void) { return sm_count(); }
 int ggml_b200_prepare(void) { const int rc = prepare_device(); return rc != GGML_B200_OK ? rc : tc_prepare_device(); }

@@ -16,7 +16,7 @@ void set_error(const char * fmt, ...);
 int  sm_count();
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a per-device setting: remember it per (kernel instantiation, device), so that a
-// process that drives several B200s through the backend (one ggml device per GPU) configures every one of them.
+// process that drives several GPUs through the backend (one ggml device per GPU) configures every one of them.
 struct per_device_flag {
     std::atomic<bool> done[64] = {};
     static int dev() { int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) d = 0; return d; }
@@ -58,7 +58,7 @@ bool   mmvq_mma_eligible(const ggml_b200_mul_mat_args & a);
 int    launch_mmvq_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st);
 size_t mmvq_mma_workspace(const ggml_b200_mul_mat_args & a);   // the quantized activation records (written by the pre-kernel)
 
-// mmq_tc.cu (tcgen05 GEMM)
+// mmq_tc.cu (tensor-core GEMM front end: activation conversion, dispatch)
 bool   mmq_tc_eligible(const ggml_b200_mul_mat_args & a);
 size_t mmq_tc_workspace(const ggml_b200_mul_mat_args & a);
 bool   mmq_dense_eligible(const ggml_b200_mul_mat_args & a);   // n >= 9, formats without an operand decoder: dequantize to fp16 + the same GEMM (mmq_tc2.cu)
@@ -68,16 +68,16 @@ size_t mmq_f16w_workspace(int64_t M, int64_t N, int64_t K);         // dense fp1
 int    launch_mmq_f16w(const void * w, size_t nb01, const float * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * ws, size_t ws_size, uint32_t flags, cudaStream_t st);
 bool   mmq_tc_eligible_small(const ggml_b200_mul_mat_args & a);   // 5 <= n <= 8 on the tensor-core path (shapes the mat-vec kernel would have to split)
 int    launch_mmq_tc(const ggml_b200_mul_mat_args & a, cudaStream_t st);
-// mmq_tc2.cu (tcgen05 GEMM on CTA pairs, cta_group::2)
+// mmq_tc2.cu (the wgmma GEMM kernel)
 bool   mmq_tc2_eligible(const ggml_b200_mul_mat_args & a);
 size_t mmq_tc2_workspace(const ggml_b200_mul_mat_args & a);
 int    launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st);
-// expert-grouped MUL_MAT_ID on the pair kernel (mmq_tc2.cu)
+// expert-grouped MUL_MAT_ID on the GEMM kernel (mmq_tc2.cu)
 bool   mmid_grouped_eligible(const ggml_b200_mul_mat_id_args & a);
 size_t mmid_grouped_workspace(const ggml_b200_mul_mat_id_args & a);
 int    launch_mmid_grouped(const ggml_b200_mul_mat_id_args & a, cudaStream_t st);
 unsigned int * tc_flag_slot();   // a zeroed, self-cleaning block of split-K flags from the device's control block (nullptr on error)
 int    tc_prepare_device();
-int tc2_trace_read(unsigned long long * host_dst, int max_ctas);   // developer trace of the CTA-pair GEMM (mmq_tc2.cu)
+int tc2_trace_read(unsigned long long * host_dst, int max_ctas);   // GEMM stamp trace: none is recorded (returns 0)
 
 } // namespace b200

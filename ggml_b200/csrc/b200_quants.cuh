@@ -1,4 +1,4 @@
-// b200_quants.cuh — packed block formats and the 64-element "unit" integer dot product (sm_100a).
+// b200_quants.cuh — packed block formats and the 64-element "unit" integer dot product (sm_90a).
 //
 // Weights stay in the reference's packed block_q* layout in HBM (consumed as-is, never repacked):
 //   Q4_0 18 B / 32   (reference src/ggml-common.h:161-166)   Q8_0 34 B / 32   (:203-208)

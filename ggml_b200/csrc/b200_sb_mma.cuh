@@ -1,7 +1,7 @@
 // b200_sb_mma.cuh — small-batch consume path of the bandwidth mat-vec kernel on the int8 tensor-core instruction
 // `mma.sync.aligned.m16n8k32.s32.s8.s8.s32`: one warp multiplies a tile of 16 weight rows x 32 weights with 8 activation columns.
 //
-// Why (profiles/r02_vs_reference_cuda.md): with 2..8 activation columns the dp4a task dots of b200_sb_tasks.cuh are issue-bound — a
+// Why: with 2..8 activation columns the dp4a task dots of b200_sb_tasks.cuh are issue-bound — a
 // lane decodes its 256 weights once and then pays one dp4a per 4 weights per COLUMN, and every column's int8 record is re-read from
 // shared memory per row.  Here a warp's 32 lanes hold the 16 x 32 weight fragment and the 32 x 8 activation fragment of one
 // sub-block, so eight columns cost the instructions of one, the activations are read once per 16 rows, and the arithmetic stays the

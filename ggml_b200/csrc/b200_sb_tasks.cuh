@@ -569,8 +569,8 @@ template <> __device__ __forceinline__ float task_dot<T_Q3_K>(const uint8_t * w,
 
 // ----------------------------------------------------------------------------- two rows against one activation task
 // Round-2 experiment, host-verified only (not dispatched): the same lane dots task t of TWO weight rows, so every activation chunk
-// is read from shared memory once instead of twice (activation reads are ~47 % of the kernel's shared-memory traffic,
-// profiles/r01_gemv_q4k_final.md).  Per row the operations are those of q45_task, so results are bit-identical to task_dot.
+// is read from shared memory once instead of twice (activation reads are about half of the kernel's shared-memory
+// traffic).  Per row the operations are those of q45_task, so results are bit-identical to task_dot.
 template <int C, bool FIVE>
 __device__ __forceinline__ void q45_chunk2(const uint8_t * qs0, const uint8_t * qs1, const uint32_t (&qh0)[8], const uint32_t (&qh1)[8], const uint8_t * a,
                                             int sa0, int sa1, int sb0, int sb1, int & acc0, int & acc1) {

@@ -1,5 +1,5 @@
-// b200_tc_dequant.cuh — per-thread operand preparation of the tcgen05 GEMM (mmq_tc.cu): raw-unit geometry of the packed W formats and
-// the conversion of 64 weights of one row to fp16 in the UMMA SWIZZLE_128B K-major layout.  Pure per-thread code, split from the
+// b200_tc_dequant.cuh — per-thread operand preparation of the tensor-core GEMM (mmq_tc2.cu): raw-unit geometry of the packed W formats and
+// the conversion of 64 weights of one row to fp16 in the SWIZZLE_128B K-major layout the wgmma descriptors read.  Pure per-thread code, split from the
 // kernel file so that tests/hostemu can compile it for the host and check it against the oracle in the CPU-only suite.
 #pragma once
 #include "b200_quants.cuh"
@@ -19,10 +19,10 @@ template <> struct tcfmt<T_Q4_0> { static constexpr int RAW = 144, STRIDE_WORDS 
 template <> struct tcfmt<T_Q8_0> { static constexpr int RAW = 144, STRIDE_WORDS = 34, UNIT_WORDS = 34, UNIT_KSTEPS = 2, ODD_BACK_WORDS = 2, LOAD_BYTES = 8;  };   // 4 blocks of 34 B
 template <> struct tcfmt<T_Q4_K> { static constexpr int RAW = 144, STRIDE_WORDS = 36, UNIT_WORDS = 36, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };   // one superblock
 template <> struct tcfmt<T_Q5_K> { static constexpr int RAW = 176, STRIDE_WORDS = 44, UNIT_WORDS = 44, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };
-// Q6_K: 210-byte superblocks, 2-byte aligned.  The decoder below is host-verified; the kernel does not dispatch it yet (its TMA box
-// has to start on the 16-byte boundary below the unit and carry up to 14 bytes of lead: RAW = 224, payload offset 210 u mod 16).
+// Q6_K: 210-byte superblocks, 2-byte aligned: the TMA box starts on the 16-byte boundary below the unit and carries up to 14 bytes of
+// lead (RAW = 224, payload offset 210 u mod 16).
 template <> struct tcfmt<T_Q6_K> { static constexpr int RAW = 224, STRIDE_WORDS = 0, UNIT_WORDS = 53, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 2, UNIT_BYTES = 210; };
-// SURVEY §8f-2 formats (decoders host-verified; first B200 run pending).  16-byte-multiple units are loaded like Q4_0; the others
+// SURVEY §8f-2 formats (decoders host-verified, kernels checked by the GPU suite).  16-byte-multiple units are loaded like Q4_0; the others
 // (LOAD_BYTES = 2) use the variable-lead box: RAW = UNIT_BYTES + largest lead, rounded up to 16.
 template <> struct tcfmt<T_Q4_1>   { static constexpr int RAW = 160, STRIDE_WORDS = 40, UNIT_WORDS = 40, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };
 template <> struct tcfmt<T_Q5_0>   { static constexpr int RAW = 176, STRIDE_WORDS = 44, UNIT_WORDS = 44, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };

@@ -1,5 +1,5 @@
-// b200_tc_ptx.cuh — inline-PTX building blocks of the tcgen05 GEMM kernels (mmq_tc.cu: one CTA per tile; mmq_tc2.cu: CTA pairs,
-// cta_group::2): mbarrier, TMA tensor copies, TMEM allocation, UMMA issue / commit, TMEM loads, cluster plumbing.
+// b200_tc_ptx.cuh — inline-PTX building blocks of the tensor-core GEMM (mmq_tc2.cu, sm_90a): mbarrier, TMA tensor copies,
+// warpgroup MMA (wgmma) issue / commit / wait and its shared-memory descriptors, programmatic dependent launch.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -18,135 +18,45 @@ __device__ __forceinline__ void tc_wait(uint64_t * b, uint32_t parity) {
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
         "@p bra TC_DONE;\nbra TC_WAIT;\nTC_DONE:\n}\n" ::"r"(tc_smem(b)), "r"(parity) : "memory");
 }
-// cluster-scope variants: a barrier of this CTA that threads of the peer CTA arrive on (after writing THEIR shared memory)
-__device__ __forceinline__ void tc_wait_cluster(uint64_t * b, uint32_t parity) {
-    asm volatile(
-        "{\n.reg .pred p;\nTC_WAITC:\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra TC_DONEC;\nbra TC_WAITC;\nTC_DONEC:\n}\n" ::"r"(tc_smem(b)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tc_arrive_cluster(uint64_t * b, uint32_t cta_rank) {    // same barrier offset in CTA `cta_rank` of the cluster
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(tc_smem(b)), "r"(cta_rank));
-    // default semantics (release at CTA scope), as cutlass::arch::ClusterBarrier::arrive(cta_id): the data this orders lives in the arriving
-    // CTA's own shared memory and is read by its own SM's tensor core; a cluster-scope release costs a MEMBAR.GPU per stage for nothing
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ void tc_arrive_cluster_release(uint64_t * b, uint32_t cta_rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(tc_smem(b)), "r"(cta_rank));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ uint32_t tc_cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void tc_cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void tc_tma_2d(void * dst, const CUtensorMap * map, int c0, int c1, uint64_t * bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(tc_smem(dst)), "l"(map), "r"(tc_smem(bar)), "r"(c0), "r"(c1) : "memory");
 }
-// shared::cluster address of the object at the same offset in CTA `cta_rank` of the cluster
-__device__ __forceinline__ uint32_t tc_cluster_addr(const void * p, uint32_t cta_rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(tc_smem(p)), "r"(cta_rank));
-    return remote;
-}
-// CTA-pair copy: the data lands in THIS CTA's shared memory, the transaction bytes are counted on the barrier `bar_cluster_addr`
-// (a shared::cluster address: the LEADER CTA's stage barrier, tc_cluster_addr(bar, 0)) -- .cta_group::2 permits a peer barrier
-__device__ __forceinline__ void tc_tma_2d_pair(void * dst, const CUtensorMap * map, int c0, int c1, uint32_t bar_cluster_addr) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(tc_smem(dst)), "l"(map), "r"(bar_cluster_addr), "r"(c0), "r"(c1) : "memory");
-}
-// shared -> global bulk stores (async proxy; the smem source must have been fenced with fence.proxy.async by its writers)
-__device__ __forceinline__ void tc_tma_store_2d(const CUtensorMap * map, const void * src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(tc_smem(src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tc_bulk_store_1d(void * gdst, const void * src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(tc_smem(src)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tc_bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void tc_bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N> __device__ __forceinline__ void tc_bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-// multicast copy: the box lands at the same offset in the shared memory of every CTA of `mask`, each of which gets the bytes counted on the barrier at
-// the same offset in ITS shared memory
-__device__ __forceinline__ void tc_tma_2d_mc(void * dst, const CUtensorMap * map, int c0, int c1, uint64_t * bar, uint16_t mask) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-                 ::"r"(tc_smem(dst)), "l"(map), "r"(tc_smem(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
-}
-// one-CTA MMA, completion signalled on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_mc(uint64_t * bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(tc_smem(bar)), "h"(mask) : "memory");
-}
 __device__ __forceinline__ void tc_prefetch_map(const CUtensorMap * map) { asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory"); }
+// generic-proxy stores to shared memory -> visible to the async proxy (the wgmma operand reads)
 __device__ __forceinline__ void tc_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_tmem_alloc(uint32_t * dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// pair allocation: issued by the same warp of BOTH CTAs of the pair (cute::TMEM::Allocator2Sm), each gets the address in its own slot
-__device__ __forceinline__ void tc_tmem_alloc_pair(uint32_t * dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+// ---- warpgroup MMA (all 128 threads of a warpgroup execute these together)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+__device__ __forceinline__ void wg_fence_operand(float & r) { asm volatile("" : "+f"(r)::"memory"); }
+// D[64 x 64] (f32, registers) += A[64 x 16] . B[64 x 16]^T, A and B fp16 K-major in shared memory
+__device__ __forceinline__ void wg_mma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
     asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// one instruction, two SMs: D[256 x N] (rows 0..127 in this CTA's TMEM, 128..255 in the peer's) += A[256 x 16] . B[N x 16]^T with A's
-// halves and B's halves (N/2 rows each) in the two CTAs' shared memory at the same offsets; issued by the leader CTA only
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tc_smem(bar)) : "memory");
-}
-// arrives (once all previously issued pair MMAs have completed) on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void tc_commit_pair(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(tc_smem(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(1));
 }
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor)
+// wgmma shared-memory descriptor: K-major, SWIZZLE_128B (128-byte rows, 8-row groups 1024 B apart; layout type 1 at bit 62)
 __device__ __forceinline__ uint64_t tc_smem_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 __device__ __forceinline__ void tc_pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void tc_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// host side, shared by the two GEMM translation units (defined in mmq_tc.cu)
+// host side (defined in mmq_tc.cu)
 typedef CUresult (*encode_tiled_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
                                     const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 encode_tiled_fn tc_get_encode();
 // activations f32 -> fp16 rows with an exact power-of-two scale per row (inv_scale[n] undoes it in the epilogue)
 int tc_launch_x_to_f16(const float * x, size_t nb11, __half * xh, float * inv_scale, int64_t K, int64_t N, cudaStream_t st, bool pdl);
-
-__host__ __device__ inline uint32_t tc_tmem_cols(int cols) { return cols <= 32 ? 32u : cols <= 64 ? 64u : cols <= 128 ? 128u : cols <= 256 ? 256u : 512u; }
 
 } // namespace b200

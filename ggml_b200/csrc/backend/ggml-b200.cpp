@@ -1,6 +1,6 @@
 // ggml-b200.cpp — the ggml backend plug-in (include/ggml-b200.h, layer 2).
 //
-// Implements the reference's backend SPI (src/ggml-backend-impl.h:17-207) for NVIDIA B200:
+// Implements the reference's backend SPI (src/ggml-backend-impl.h:17-207) for NVIDIA H100 (sm_90a):
 //   ggml_backend_reg_i          -> "B200" registry entry, one device per visible GPU
 //   ggml_backend_device_i       -> B200<i>: memory, props, supports_op / supports_buft / offload_op, events
 //   ggml_backend_buffer_type_i  -> device memory (cudaMalloc), alignment 128; pinned host buffer type
@@ -264,7 +264,7 @@ bool   host_buft_is_host(ggml_backend_buffer_type_t) { return true; }
 
 int registry_device_count();
 ggml_backend_buffer_type_t host_buffer_type() {
-    if (registry_device_count() == 0) return nullptr;        // no B200 visible: there is no device to hang the buffer type on (reg_get_device would assert)
+    if (registry_device_count() == 0) return nullptr;        // no supported GPU visible: there is no device to hang the buffer type on (reg_get_device would assert)
     static ggml_backend_buffer_type buft = {
         /* .iface   = */ { host_buft_get_name, host_buft_alloc_buffer, host_buft_get_alignment, nullptr, nullptr, host_buft_is_host },
         /* .device  = */ ggml_backend_reg_dev_get(b200_reg(), 0),
@@ -448,7 +448,7 @@ ggml_backend_buffer_type_t split_buffer_type(int main_device, const float * tens
 bool is_b200_weight_type(ggml_type t) {
     switch (t) {
         case GGML_TYPE_Q4_0: case GGML_TYPE_Q8_0: case GGML_TYPE_Q4_K: case GGML_TYPE_Q5_K: case GGML_TYPE_Q6_K:      // north_star formats
-        case GGML_TYPE_Q4_1: case GGML_TYPE_Q5_0: case GGML_TYPE_Q5_1: case GGML_TYPE_Q2_K: case GGML_TYPE_Q3_K:      // SURVEY 8f-2 (validated on a B200 in round 1)
+        case GGML_TYPE_Q4_1: case GGML_TYPE_Q5_0: case GGML_TYPE_Q5_1: case GGML_TYPE_Q2_K: case GGML_TYPE_Q3_K:      // SURVEY 8f-2 (checked on the device by tests/test_gpu_next_formats.py)
         case GGML_TYPE_IQ4_NL: case GGML_TYPE_IQ4_XS:
         case GGML_TYPE_IQ2_XXS: case GGML_TYPE_IQ3_XXS: case GGML_TYPE_IQ1_S:                                         // grid i-quants (generic kernels)
         case GGML_TYPE_IQ2_XS: case GGML_TYPE_IQ2_S: case GGML_TYPE_IQ3_S: case GGML_TYPE_IQ1_M: case GGML_TYPE_TQ1_0: case GGML_TYPE_TQ2_0:
@@ -1271,8 +1271,8 @@ ggml_backend_reg_t b200_reg() {
         for (int i = 0; i < n; ++i) {
             cudaDeviceProp prop;
             if (cudaGetDeviceProperties(&prop, i) != cudaSuccess) { cudaGetLastError(); continue; }
-            if (prop.major != 10) {   // sm_100a binaries only load on Blackwell data-centre parts
-                GGML_LOG_WARN("ggml-b200: skipping device %d (%s, sm_%d%d): kernels are built for sm_100a\n", i, prop.name, prop.major, prop.minor);
+            if (prop.major != 9) {    // sm_90a binaries only load on Hopper (H100 / H200)
+                GGML_LOG_WARN("ggml-b200: skipping device %d (%s, sm_%d%d): kernels are built for sm_90a\n", i, prop.name, prop.major, prop.minor);
                 continue;
             }
             device_ctx * dctx = new device_ctx;

@@ -1,4 +1,4 @@
-// dequant.cu — bit-exact block-format conversion kernels for sm_100a.
+// dequant.cu — bit-exact block-format conversion kernels for sm_90a.
 //
 // Replaces the reference's dequantize_block_* family (src/ggml-cuda/convert.cu:6-278, built there with
 // -use_fast_math) by kernels whose every output is bit-identical to the CPU reference

@@ -1,4 +1,4 @@
-// mmid.cu — GGML_OP_MUL_MAT_ID (mixture-of-experts mat-mul) for sm_100a.
+// mmid.cu — GGML_OP_MUL_MAT_ID (mixture-of-experts mat-mul) for sm_90a.
 //
 // Computes what ggml_compute_forward_mul_mat_id (reference src/ggml-cpu/ggml-cpu.c:7609-7784) computes and
 // replaces ggml_cuda_mul_mat_id (src/ggml-cuda/ggml-cuda.cu:1955-2090), which copies `ids` to the host and

@@ -1,240 +1,29 @@
-// mmq_tc.cu — batched quantized mat-mul (n > 8) on the 5th-generation tensor cores (tcgen05 / TMEM / TMA), sm_100a.
+// mmq_tc.cu — batched quantized mat-mul (n > 8, and 5 <= n <= 8 where the mat-vec kernels cannot take the shape) on the Hopper
+// tensor cores: the front end of the GEMM.  Converts the activations to fp16 (x_to_f16_kernel), owns the tensor-map encoder, and sends
+// the shape to the warpgroup-MMA kernel (mmq_tc2.cu), directly for the formats with an operand decoder, through an fp16 copy of W for
+// the others (launch_mmq_dense).
 //
 // Replaces the reference's mul_mat_q (src/ggml-cuda/mmq.cuh:2499-2655: int8 mma.sync tiles + stream-k fix-up) and its
 // cuBLAS fallback (dequantize_block_* -> cublasGemmEx, src/ggml-cuda/ggml-cuda.cu:1158-1300); computes GGML_OP_MUL_MAT
 // for block-quantized src0 and f32 src1 as ggml_compute_forward_mul_mat does (src/ggml-cpu/ggml-cpu.c:7428).
 //
-// Per-block scales cannot be interposed in a TMEM accumulation that runs over the whole K loop, so the scales are
-// folded into the operand: W tiles are dequantized to fp16 in shared memory (UMMA K-major SWIZZLE_128B layout),
-// X is converted to fp16 once (each activation row pre-scaled by a power of two when its largest magnitude would leave the
-// fp16 range; the epilogue undoes the scale, so nothing overflows and the scaling is exact), D accumulates in f32 in TMEM.
-// tcgen05 kind::f16 requires A and B in the same 16-bit format (a mixed fp16 x bf16 descriptor raises an illegal-instruction
-// fault on sm_100a); fp16 is chosen over bf16 because integer codes convert to fp16 with two packed-half instructions per two
-// weights and carry 11 instead of 8 significant bits.  NMSE against the CPU backend ~1e-7 .. 1e-6
-// against the CPU backend (gate 5e-4, tests/test-backend-ops.cpp:1915-1917).
-//
-// One CTA = one 128 (W rows) x BN (activation rows, <= 256) output tile over a K range (split-K so that the grid
-// fills the 148 SMs).  Warp roles (10 warps):
-//   warp 0      TMA producer: the fp16 X tiles (BN x 64) with a SWIZZLE_128B tensor map into a deep B ring.
-//   warp 1      allocates TMEM, issues tcgen05.mma (one elected lane): 4 x (128 x BN x 16) per 64-wide K step,
-//               tcgen05.commit releases operand stages and finally signals the epilogue.
-//   warps 2-9   dequantize raw W -> fp16 -> swizzled A stage (generic-proxy stores + fence.proxy.async), then run
-//               the epilogue: tcgen05.ld the accumulator (each warp its TMEM lane quarter and column half), and
-//               either write Y, or hand a split-K partial to the CTA that owns the tile (flag in the workspace;
-//               partial producers are scheduled first, so the wait cannot deadlock).
+// Per-block scales cannot be interposed in an accumulation that runs over the whole K loop, so the scales are folded into the
+// operand: W tiles are dequantized to fp16 in shared memory (K-major SWIZZLE_128B layout), X is converted to fp16 once (each
+// activation row pre-scaled by a power of two when its largest magnitude would leave the fp16 range; the epilogue undoes the scale,
+// so nothing overflows and the scaling is exact), D accumulates in f32.  fp16 is chosen over bf16 because integer codes convert to
+// fp16 with two packed-half instructions per two weights and carry 11 instead of 8 significant bits.  NMSE against the CPU backend
+// ~1e-7 .. 1e-6 (the reference's gate is 5e-4, tests/test-backend-ops.cpp:1915-1917).
 #include "b200_internal.h"
 #include "b200_quants.cuh"
-#include "b200_tc_dequant.cuh"   // raw-unit geometry, tc_load_unit, dq64 (also compiled for the host by tests/hostemu)
-#include "b200_tc_ptx.cuh"       // mbarrier / TMA / TMEM / UMMA inline PTX
+#include "b200_tc_dequant.cuh"   // h2u
+#include "b200_tc_ptx.cuh"
 
 #include <cuda.h>
 #include <cuda_fp16.h>
 
-#include <cstdlib>
 #include <mutex>
 
 namespace b200 {
-
-// ----------------------------------------------------------------------------- kernel
-// CTA tile = HALVES x 128 W rows x BN activation rows.  HALVES = 2: two 128-row tcgen05 sub-tiles share every B (activation)
-// stage, so the activation bytes a CTA pulls per flop are half those of a 128-row tile (the operand feed, not the tensor pipe or
-// the dequantizers, bounds this kernel); used when 256-row tiles alone fill the GPU.  HALVES = 1: 128-row tiles (+ split-K) for
-// the smaller problems.  Accumulators: TMEM columns [0, BN) (rows 0..127) and, HALVES = 2, [BN, 2 BN) (rows 128..255).
-constexpr int TC_BM = 128, TC_BK = 64, TC_DQ_WARPS = 8, TC_THREADS = (2 + TC_DQ_WARPS) * 32;
-constexpr int TC_MAX_STAGES = 4;
-
-struct tc_params {
-    float * y; float * partials; unsigned int * flags; const float * inv_scale;
-    int64_t M, N;
-    int32_t BN, m_tiles, n_tiles, splitk, units_total, nstages;
-};
-
-
-template <int T, int KS>
-__device__ __forceinline__ void tc_dequant_step(int nstages, int step, bool valid, const uint32_t (&u)[tcfmt<T>::UNIT_WORDS], uint8_t * a_ring, int stage_bytes, int a_row_off,
-                                                uint32_t sw, int lane, uint64_t * full, uint64_t * empty) {
-    const int s = step % nstages;
-    if (step >= nstages) tc_wait(&empty[s], (uint32_t)((step / nstages) - 1) & 1u);
-    if (valid) dq64<T, KS>(u, a_ring + s * stage_bytes + a_row_off, sw);
-    tc_fence_async_smem();
-    tc_arrive(&full[s]);        // every writer arrives for itself after its own proxy fence (an elected lane after __syncwarp() lost rows in the pair kernel: mmq_tc2.cu)
-}
-
-template <int T, int HALVES>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-mmq_tc_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const tc_params p) {
-    constexpr int RAW = tcfmt<T>::RAW, UK = tcfmt<T>::UNIT_KSTEPS, ROWS = HALVES * TC_BM;
-    extern __shared__ __align__(1024) uint8_t smem[];
-    // [operand ring: nstages x (A: HALVES x 16 KB | B: BN*128)][raw: 2 x ROWS*RAW][barriers]
-    constexpr int a_bytes = ROWS * TC_BK * 2;
-    const int b_bytes = p.BN * TC_BK * 2, stage_bytes = a_bytes + b_bytes;
-    uint8_t * ring = smem;
-    uint8_t * raw  = ring + p.nstages * stage_bytes;
-    uint64_t * bars = (uint64_t *)(raw + 2 * ROWS * RAW);
-    uint64_t * full = bars, * empty = bars + TC_MAX_STAGES, * raw_full = bars + 2 * TC_MAX_STAGES, * raw_empty = raw_full + 2, * acc_full = raw_empty + 2;
-    uint32_t * tmem_slot = (uint32_t *)(acc_full + 1);
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // work item: partial producers (ks > 0) first, tile owners (ks == 0) last
-    const int tiles = p.m_tiles * p.n_tiles;
-    const int ks = p.splitk - 1 - (int)blockIdx.x / tiles;
-    const int tile = (int)blockIdx.x % tiles, tm = tile % p.m_tiles, tn = tile / p.m_tiles;
-    const int ubeg = (int)((int64_t)p.units_total * ks / p.splitk), uend = (int)((int64_t)p.units_total * (ks + 1) / p.splitk);
-    const int nunits = uend - ubeg, nsteps = UK * nunits;
-    const int64_t rows_left = p.M - (int64_t)tm * ROWS;          // > 0
-    const bool two_halves = HALVES == 2 && rows_left > TC_BM;    // the second 128-row sub-tile exists
-
-    if (tid == 0) {
-        // a stage's A part is written by all 8 dequantizer warps (HALVES = 2) or by the 4 that own its K-step (HALVES = 1), every thread arrives; + the B TMA
-        for (int s = 0; s < p.nstages; ++s) { tc_mbar_init(&full[s], (HALVES == 2 ? TC_DQ_WARPS : TC_DQ_WARPS / 2) * 32 + 1); tc_mbar_init(&empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { tc_mbar_init(&raw_full[s], 1); tc_mbar_init(&raw_empty[s], TC_DQ_WARPS); }
-        tc_mbar_init(acc_full, 1);
-        tc_fence_init();
-        tc_prefetch_map(&map_w); tc_prefetch_map(&map_x);
-    }
-    if (warp == 1) tc_tmem_alloc(tmem_slot, tc_tmem_cols(HALVES * p.BN));
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-
-    if (warp == 0) {
-        // ===================== TMA producer
-        if (lane == 0) {
-            for (int u = 0; u < nunits; ++u) {
-                const int rs = u & 1;
-                if (u >= 2) tc_wait(&raw_empty[rs], (uint32_t)((u >> 1) - 1) & 1u);
-                tc_expect_tx(&raw_full[rs], ROWS * RAW);
-                int coord;                                        // first 4-byte word of the box: 16-byte aligned start at or below the unit
-                if constexpr (tcfmt<T>::LOAD_BYTES == 2) coord = (((ubeg + u) * tcfmt<T>::UNIT_BYTES) & ~15) >> 2;   // unaligned units: lead bytes in front of the payload
-                else                       coord = (ubeg + u) * tcfmt<T>::STRIDE_WORDS - ((ubeg + u) & 1) * tcfmt<T>::ODD_BACK_WORDS;
-                tc_tma_2d(raw + rs * ROWS * RAW, &map_w, coord, tm * ROWS, &raw_full[rs]);
-                for (int q = 0; q < UK; ++q) {
-                    const int step = UK * u + q, s = step % p.nstages;
-                    if (step >= p.nstages) tc_wait(&empty[s], (uint32_t)((step / p.nstages) - 1) & 1u);
-                    tc_expect_tx(&full[s], (uint32_t)b_bytes);
-                    tc_tma_2d(ring + s * stage_bytes + a_bytes, &map_x, ((ubeg + u) * UK + q) * TC_BK, tn * p.BN, &full[s]);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer
-        // instruction descriptor: D = f32 (bit 4), A = B = f16 (bits 7-9 and 10-12 = 0), both K-major, N >> 3, M >> 4
-        const uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-        for (int step = 0; step < nsteps; ++step) {
-            const int s = step % p.nstages;
-            tc_wait(&full[s], (uint32_t)(step / p.nstages) & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint64_t bd = tc_smem_desc(tc_smem(ring + s * stage_bytes + a_bytes));
-                for (int h = 0; h < (two_halves ? 2 : 1); ++h) {
-                    const uint64_t ad = tc_smem_desc(tc_smem(ring + s * stage_bytes + h * (TC_BM * TC_BK * 2)));
-#pragma unroll
-                    for (int k = 0; k < TC_BK / 16; ++k)
-                        tc_mma_f16(tmem + (uint32_t)(h * p.BN), ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, (step | k) != 0 ? 1u : 0u);   // +32 bytes per K=16
-                }
-                tc_commit(&empty[s]);
-                if (step == nsteps - 1) tc_commit(acc_full);
-            }
-            __syncwarp();
-        }
-    } else {
-        // ===================== dequantizers.  HALVES = 2: one thread per tile row, all K-steps of a unit.
-        //                       HALVES = 1: two threads per row (warps 2-5 / 6-9), each half of the unit's K-steps.
-        const int dq = tid - 64, dwarp = dq >> 5;
-        const int row = HALVES == 2 ? dq : (dq & 127), ksel = HALVES == 2 ? 0 : (dq >> 7);
-        const bool valid = row < rows_left;                      // rows past M: the TMA box is zero-filled, nothing to convert
-        const uint32_t sw = (uint32_t)(row & 7);
-        const int a_row_off = (row >> 7) * (TC_BM * TC_BK * 2) + ((row & 127) >> 3) * 1024 + (row & 7) * 128;
-        uint32_t ub[tcfmt<T>::UNIT_WORDS];
-        for (int u = 0; u < nunits; ++u) {
-            const int rs = u & 1;
-            tc_wait(&raw_full[rs], (uint32_t)(u >> 1) & 1u);
-            int lead;                                             // bytes between the box start and the unit's first byte
-            if constexpr (tcfmt<T>::LOAD_BYTES == 2) lead = ((ubeg + u) * tcfmt<T>::UNIT_BYTES) & 15;
-            else                       lead = ((ubeg + u) & 1) * (4 * tcfmt<T>::ODD_BACK_WORDS);
-            tc_load_unit<T>(raw + rs * ROWS * RAW + row * RAW + lead, ub);
-            __syncwarp();
-            if (lane == 0) tc_arrive(&raw_empty[rs]);            // the unit is in registers: the buffer can be refilled
-            if constexpr (HALVES == 2) {
-                tc_dequant_step<T, 0>(p.nstages, UK * u + 0, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                tc_dequant_step<T, 1>(p.nstages, UK * u + 1, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                if constexpr (UK == 4) {
-                    tc_dequant_step<T, 2>(p.nstages, UK * u + 2, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                    tc_dequant_step<T, 3>(p.nstages, UK * u + 3, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                }
-            } else if constexpr (UK == 4) {
-                if (ksel == 0) {
-                    tc_dequant_step<T, 0>(p.nstages, UK * u + 0, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                    tc_dequant_step<T, 1>(p.nstages, UK * u + 1, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                } else {
-                    tc_dequant_step<T, 2>(p.nstages, UK * u + 2, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                    tc_dequant_step<T, 3>(p.nstages, UK * u + 3, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                }
-            } else {
-                if (ksel == 0) tc_dequant_step<T, 0>(p.nstages, UK * u + 0, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-                else           tc_dequant_step<T, 1>(p.nstages, UK * u + 1, valid, ub, ring, stage_bytes, a_row_off, sw, lane, full, empty);
-            }
-        }
-        // ===================== epilogue
-        tc_wait(acc_full, 0);
-        tc_fence_after();
-        // each warp owns its TMEM lane quarter (hardware: warp id % 4) and, HALVES = 2, one accumulator half (all BN columns),
-        // HALVES = 1, one half of the columns (BN >= 64) or all of them (warps 2-5 only)
-        const int lg = warp & 3, grp = dwarp >> 2;
-        const int h = HALVES == 2 ? grp : 0;
-        const bool split_cols = HALVES == 1 && p.BN >= 64;
-        const bool active = HALVES == 2 ? (h == 0 || two_halves) : (split_cols || grp == 0);
-        const int ncol = split_cols ? p.BN / 2 : p.BN, col0 = split_cols ? grp * ncol : 0;
-        const int64_t m = (int64_t)tm * ROWS + h * TC_BM + lg * 32 + lane;
-        const int64_t n_base = (int64_t)tn * p.BN + col0;
-        const uint32_t tacc = tmem + ((uint32_t)(lg * 32) << 16) + (uint32_t)(h * p.BN + col0);
-        const int mloc = h * TC_BM + lg * 32 + lane;
-        float * part = p.partials ? p.partials + ((size_t)tile * (p.splitk - 1)) * (size_t)(p.BN * ROWS) : nullptr;
-        if (ks > 0) {
-            // split-K partial: [ks-1][n_local][m_local]
-            float * dst = part + (size_t)(ks - 1) * (p.BN * ROWS);
-            if (active) {
-                for (int c0 = 0; c0 < ncol; c0 += 32) {
-                    float v[32];
-                    tc_ld32(tacc + (uint32_t)c0, v);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) dst[(size_t)(col0 + c0 + i) * ROWS + mloc] = v[i];
-                }
-            }
-            __threadfence();
-            asm volatile("bar.sync 1, %0;" ::"n"(TC_DQ_WARPS * 32) : "memory");
-            if (dq == 0) atomicAdd(&p.flags[tile], 1u);
-        } else {
-            if (p.splitk > 1) {
-                if (dq == 0) { while (atomicAdd(&p.flags[tile], 0u) < (unsigned)(p.splitk - 1)) __nanosleep(64); __threadfence(); }
-                asm volatile("bar.sync 1, %0;" ::"n"(TC_DQ_WARPS * 32) : "memory");
-            }
-            if (active) {
-                for (int c0 = 0; c0 < ncol; c0 += 32) {
-                    float v[32];
-                    tc_ld32(tacc + (uint32_t)c0, v);
-                    for (int j = 1; j < p.splitk; ++j) {
-                        const float * src = part + (size_t)(j - 1) * (p.BN * ROWS);
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) v[i] += __ldcg(&src[(size_t)(col0 + c0 + i) * ROWS + mloc]);
-                    }
-                    if (m < p.M) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) { const int64_t n = n_base + c0 + i; if (n < p.N) p.y[(size_t)n * p.M + m] = v[i] * __ldg(p.inv_scale + n); }
-                    }
-                }
-            }
-            if (p.splitk > 1) {
-                asm volatile("bar.sync 1, %0;" ::"n"(TC_DQ_WARPS * 32) : "memory");
-                if (dq == 0) p.flags[tile] = 0;                 // leave the flag clean for the next launch
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tc_tmem_dealloc(tmem, tc_tmem_cols(HALVES * p.BN)); }
-}
 
 // ----------------------------------------------------------------------------- X -> fp16 prologue
 // one CTA per activation row: largest magnitude -> exact power-of-two scale that puts it into [2^13, 2^14) (neither overflow nor
@@ -299,141 +88,18 @@ encode_tiled_fn tc_get_encode() {
     return fn;
 }
 
-struct tc_plan {
-    int BN, halves, m_tiles, n_tiles, splitk, chunks, nstages, smem, grid;
-    size_t xb_bytes, partial_bytes, flags_bytes, scale_bytes;
-};
-
-static bool make_tc_plan(const ggml_b200_mul_mat_args & a, tc_plan & pl) {
-    // every format of the mat-vec path has an operand decoder (b200_tc_dequant.cuh); Q6_K and the SURVEY 8f-2 formats passed their
-    // first B200 run at the end of round 1 (GGML_B200_TC_Q6K=0 turns the Q6_K path off again, for A/B comparisons)
-    static const bool env_q6k_off = getenv("GGML_B200_TC_Q6K") && atoi(getenv("GGML_B200_TC_Q6K")) == 0;
-    const bool next_fmt = a.type == T_Q4_1 || a.type == T_Q5_0 || a.type == T_Q5_1 || a.type == T_IQ4_NL || a.type == T_IQ4_XS || a.type == T_Q2_K || a.type == T_Q3_K;
-    if (a.type != T_Q4_0 && a.type != T_Q8_0 && a.type != T_Q4_K && a.type != T_Q5_K && !(a.type == T_Q6_K && !env_q6k_off) && !next_fmt) return false;
-    if (a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
-    // n >= 9: every batch the mat-vec kernels do not take (the reference's mul_mat_q threshold, ggml-cuda.cu:1852-1875); also 5 <= n <= 8
-    // when the mat-vec kernel cannot hold that many activation records next to its weight stages (very long rows: api.cu decides);
-    // columns beyond n in the 32-wide minimum tile are zero-filled by the TMA box and never stored
-    if (a.N < 5 || a.K % 256 != 0 || a.K < 256 || a.M < 1) return false;
-    const size_t rb = row_bytes(a.type, a.K);
-    if (a.nb01 != rb || (rb % 16) != 0 || ((uintptr_t)a.src0 & 15) != 0 || ((uintptr_t)a.src1 & 3) != 0 || (a.nb11 & 3) != 0) return false;
-    if (a.M >= (1ll << 31) || a.N >= (1ll << 31) || rb >= (1ull << 31)) return false;
-    if (!tc_get_encode()) return false;
-    int BN = a.N >= 256 ? 256 : (int)((a.N + 15) / 16 * 16);
-    if (BN > 128 && BN < 256) BN = 256;
-    if (BN > 64 && BN < 128) BN = 128;
-    if (BN < 32) BN = 32;                                    // TMEM allocations are powers of two >= 32 columns
-    if (BN > 32 && BN < 64) BN = 64;
-    pl.BN = BN;
-    pl.n_tiles = (int)((a.N + BN - 1) / BN);
-    pl.chunks = (int)(a.K / (a.type == T_Q8_0 ? 128 : 256));          // raw units along K (tcfmt<T>::UNIT_KSTEPS x 64 weights each)
-    // 256-row tiles when they fill most of the GPU on their own (half the activation traffic per flop); else 128-row tiles + split-K
-    static const int env_halves = getenv("GGML_B200_TC_HALVES") ? atoi(getenv("GGML_B200_TC_HALVES")) : 0;
-    const int tiles256 = (int)((a.M + 255) / 256) * pl.n_tiles;
-    pl.halves = env_halves == 1 || env_halves == 2 ? env_halves : (tiles256 >= sm_count() / 2 ? 2 : 1);
-    if (a.type == T_Q6_K) pl.halves = 1;                         // 224-byte raw boxes: two 256-row buffers would not leave room for the operand ring
-    const int rows = pl.halves * TC_BM;
-    pl.m_tiles = (int)((a.M + rows - 1) / rows);
-    const int tiles = pl.m_tiles * pl.n_tiles;
-    int splitk = sm_count() / tiles; if (splitk < 1) splitk = 1; if (splitk > 8) splitk = 8; if (splitk > pl.chunks) splitk = pl.chunks;
-    static const int env_splitk = getenv("GGML_B200_TC_SPLITK") ? atoi(getenv("GGML_B200_TC_SPLITK")) : 0;
-    if (env_splitk > 0 && env_splitk <= pl.chunks) splitk = env_splitk;
-    pl.splitk = splitk;
-    int raw = 144;                                               // tcfmt<T>::RAW
-    switch (a.type) {
-        case T_Q5_K: case T_Q5_0: raw = 176; break;
-        case T_Q6_K: raw = 224; break;
-        case T_Q4_1: raw = 160; break;
-        case T_Q5_1: raw = 192; break;
-        case T_Q2_K: raw = 96;  break;
-        case T_Q3_K: raw = 128; break;
-        default: break;                                          // Q4_0, Q8_0 (half units), Q4_K, IQ4_NL, IQ4_XS: 144
-    }
-    auto smem_of = [&](int ns) { return ns * (rows * TC_BK * 2 + BN * TC_BK * 2) + 2 * rows * raw + 256 + 1024; };
-    int nstages = TC_MAX_STAGES;
-    while (nstages > 2 && smem_of(nstages) > 227 * 1024) nstages--;
-    if (smem_of(nstages) > 227 * 1024) return false;
-    pl.nstages = nstages; pl.smem = smem_of(nstages);
-    pl.grid = tiles * splitk;
-    pl.xb_bytes = ((size_t)a.N * a.K * 2 + 255) & ~(size_t)255;
-    pl.partial_bytes = splitk > 1 ? (size_t)tiles * (splitk - 1) * BN * rows * 4 : 0;
-    pl.flags_bytes = ((size_t)tiles * 4 + 255) & ~(size_t)255;
-    pl.scale_bytes = ((size_t)a.N * 4 + 255) & ~(size_t)255;
-    return true;
-}
-
-bool mmq_tc_eligible(const ggml_b200_mul_mat_args & a) { tc_plan pl; return a.N >= 9 && (make_tc_plan(a, pl) || mmq_dense_eligible(a)); }
-bool mmq_tc_eligible_small(const ggml_b200_mul_mat_args & a) { tc_plan pl; return a.N >= 5 && make_tc_plan(a, pl); }
+bool mmq_tc_eligible(const ggml_b200_mul_mat_args & a) { return a.N >= 9 && (mmq_tc2_eligible(a) || mmq_dense_eligible(a)); }
+bool mmq_tc_eligible_small(const ggml_b200_mul_mat_args & a) { return a.N >= 5 && mmq_tc2_eligible(a); }
 size_t mmq_tc_workspace(const ggml_b200_mul_mat_args & a) {
     if (mmq_dense_eligible(a)) return mmq_dense_workspace(a);
-    if (mmq_tc2_eligible(a)) return mmq_tc2_workspace(a);
-    tc_plan pl;
-    if (!make_tc_plan(a, pl)) return 0;
-    return pl.xb_bytes + pl.partial_bytes + pl.flags_bytes + pl.scale_bytes + 1024;
-}
-
-template <int T, int HALVES> static int launch_tc(const ggml_b200_mul_mat_args & a, const tc_plan & pl, cudaStream_t st) {
-    const size_t need = pl.xb_bytes + pl.partial_bytes + pl.flags_bytes + pl.scale_bytes + 1024;
-    if (!a.workspace || a.workspace_size < need) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, need); return GGML_B200_EWORKSPACE; }
-    uint8_t * ws = (uint8_t *)(((uintptr_t)a.workspace + 255) & ~(uintptr_t)255);
-    __half * xb = (__half *)ws;
-    float * partials = pl.partial_bytes ? (float *)(ws + pl.xb_bytes) : nullptr;
-    unsigned int * flags = (unsigned int *)(ws + pl.xb_bytes + pl.partial_bytes);
-    float * inv_scale = (float *)(ws + pl.xb_bytes + pl.partial_bytes + pl.flags_bytes);
-
-    // flags must start at zero: the tile owners leave them clean, but the workspace may be fresh memory
-    B200_CUDA_TRY(cudaMemsetAsync(flags, 0, pl.flags_bytes, st));
-    { const int rc = tc_launch_x_to_f16(a.src1, a.nb11, xb, inv_scale, a.K, a.N, st, false); if (rc != GGML_B200_OK) return rc; }
-    const size_t rb = row_bytes(a.type, a.K);
-    alignas(64) CUtensorMap map_w, map_x;
-    {
-        const cuuint64_t dims[2] = { (cuuint64_t)(rb / 4), (cuuint64_t)a.M };
-        const cuuint64_t strides[1] = { (cuuint64_t)rb };
-        const cuuint32_t box[2] = { (cuuint32_t)(tcfmt<T>::RAW / 4), (cuuint32_t)(HALVES * TC_BM) };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void *)a.src0, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                  CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(W) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
-    {
-        const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)a.N };
-        const cuuint64_t strides[1] = { (cuuint64_t)a.K * 2 };
-        const cuuint32_t box[2] = { (cuuint32_t)TC_BK, (cuuint32_t)pl.BN };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)xb, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(X) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
-    tc_params p;
-    p.y = a.dst; p.partials = partials; p.flags = flags; p.inv_scale = inv_scale; p.M = a.M; p.N = a.N;
-    p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.n_tiles; p.splitk = pl.splitk; p.units_total = pl.chunks; p.nstages = pl.nstages;
-    static per_device_flag attr_set;
-    if (!attr_set.test()) { B200_CUDA_TRY(cudaFuncSetAttribute(mmq_tc_kernel<T, HALVES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_set.set(); }
-    mmq_tc_kernel<T, HALVES><<<pl.grid, TC_THREADS, pl.smem, st>>>(map_w, map_x, p);
-    B200_LAUNCH_CHECK();
-    return GGML_B200_OK;
+    return mmq_tc2_workspace(a);
 }
 
 int launch_mmq_tc(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
     if (mmq_dense_eligible(a)) return launch_mmq_dense(a, st);             // formats without an operand decoder: fp16 copy + the same GEMM
-    if (mmq_tc2_eligible(a)) return launch_mmq_tc2(a, st);              // CTA pairs (cta_group::2) where the problem is large enough
-    tc_plan pl;
-    if (!make_tc_plan(a, pl)) { set_error("mul_mat: shape not eligible for the tcgen05 kernel"); return GGML_B200_EUNSUPPORTED; }
-    switch (a.type) {
-        case T_Q4_0: return pl.halves == 2 ? launch_tc<T_Q4_0, 2>(a, pl, st) : launch_tc<T_Q4_0, 1>(a, pl, st);
-        case T_Q8_0: return pl.halves == 2 ? launch_tc<T_Q8_0, 2>(a, pl, st) : launch_tc<T_Q8_0, 1>(a, pl, st);
-        case T_Q4_K: return pl.halves == 2 ? launch_tc<T_Q4_K, 2>(a, pl, st) : launch_tc<T_Q4_K, 1>(a, pl, st);
-        case T_Q5_K: return pl.halves == 2 ? launch_tc<T_Q5_K, 2>(a, pl, st) : launch_tc<T_Q5_K, 1>(a, pl, st);
-        case T_Q6_K: return pl.halves == 2 ? launch_tc<T_Q6_K, 2>(a, pl, st) : launch_tc<T_Q6_K, 1>(a, pl, st);
-        case T_Q4_1: return pl.halves == 2 ? launch_tc<T_Q4_1, 2>(a, pl, st) : launch_tc<T_Q4_1, 1>(a, pl, st);
-        case T_Q5_0: return pl.halves == 2 ? launch_tc<T_Q5_0, 2>(a, pl, st) : launch_tc<T_Q5_0, 1>(a, pl, st);
-        case T_Q5_1: return pl.halves == 2 ? launch_tc<T_Q5_1, 2>(a, pl, st) : launch_tc<T_Q5_1, 1>(a, pl, st);
-        case T_IQ4_NL: return pl.halves == 2 ? launch_tc<T_IQ4_NL, 2>(a, pl, st) : launch_tc<T_IQ4_NL, 1>(a, pl, st);
-        case T_IQ4_XS: return pl.halves == 2 ? launch_tc<T_IQ4_XS, 2>(a, pl, st) : launch_tc<T_IQ4_XS, 1>(a, pl, st);
-        case T_Q2_K: return pl.halves == 2 ? launch_tc<T_Q2_K, 2>(a, pl, st) : launch_tc<T_Q2_K, 1>(a, pl, st);
-        case T_Q3_K: return pl.halves == 2 ? launch_tc<T_Q3_K, 2>(a, pl, st) : launch_tc<T_Q3_K, 1>(a, pl, st);
-        default: set_error("mul_mat: unsupported weight type %d for the tcgen05 kernel", a.type); return GGML_B200_EUNSUPPORTED;
-    }
+    if (mmq_tc2_eligible(a)) return launch_mmq_tc2(a, st);
+    set_error("mul_mat: shape not eligible for the tensor-core kernel");
+    return GGML_B200_EUNSUPPORTED;
 }
 
 } // namespace b200

@@ -1,26 +1,24 @@
-// mmq_tc2.cu — batched quantized mat-mul on CTA PAIRS: tcgen05.mma.cta_group::2, one 256 (W rows) x BN (activation rows) tile per
-// pair of SMs, the second generation of mmq_tc.cu's kernel (same operand preparation: W dequantized to fp16 in the UMMA
-// SWIZZLE_128B layout, X converted to fp16 once with an exact power-of-two row scale, f32 accumulation in TMEM).
+// mmq_tc2.cu — the tensor-core GEMM kernel (sm_90a): one 256 (W rows) x BN (activation rows) output tile per CTA over a K range,
+// fp16 operands in shared memory, f32 accumulation in registers by warpgroup MMA (wgmma.mma_async m64n64k16).
 //
-// Why pairs (profiles/r01_gemm_q8_0_tcgen05.md: 410 TFLOP/s = 0.28 of the measured peak at 4096^2 x 512, the tensor pipe 30 % busy):
-// the one-CTA kernel pulls a whole BN x 64 activation stage per 128 W rows, so its operand feed (64 B/clk/SM of L2 traffic at BN = 256)
-// and its 2-4 stage ring, not the tensor pipe, set the pace.  With cta_group::2
-//   * each CTA stages only HALF of the activation tile (BN/2 rows): the MMA reads both halves, the L2 -> SM activation traffic
-//     per flop halves and so does the stage size: 5 stages of 32 KB where the 256-row one-CTA tile had 2 stages of 64 KB;
-//   * each CTA dequantizes only its own 128 W rows (two threads per row), so the dequantizers are never the bottleneck;
-//   * one elected thread of the LEADER CTA issues every MMA for both SMs; tcgen05.commit multicasts "stage free" / "accumulator
-//     ready" to the barriers of both CTAs;
-//   * the activation conversion kernel and this kernel are chained with programmatic dependent launch: TMEM allocation, barrier set-up,
-//     tensor-map prefetch, the raw W stream and the first dequantized stages run while the conversion is still in flight; only the
-//     activation TMA waits for it.  Split-K flags live in a self-cleaning per-device block: no memset per call.
+// Operands: W is dequantized to fp16 in shared memory (K-major SWIZZLE_128B, the layout the wgmma descriptors read), X was converted
+// to fp16 once by mmq_tc.cu with an exact power-of-two row scale (undone in the epilogue).  T_F16: the A operand already is fp16
+// (dense f16 weights, or a format without an operand decoder dequantized into the workspace first) and arrives by TMA like X.
 //
-// Warp roles per CTA (10 warps): warp 0 = TMA producer (raw W units for the own 128 rows into a 2-deep raw ring; the own half of every
-// activation stage, signalled on the LEADER's stage barrier); warp 1 = TMEM allocation (both CTAs) and, in the leader, the MMA issuer;
-// warps 2-9 = dequantizers (two threads per row, each half of a unit's K-steps; the non-leader's warps arrive on the leader's stage
-// barrier through the cluster), then the epilogue (each CTA its 128 accumulator lanes).
+// Warp roles (12 warps, three warpgroups; setmaxnreg moves the producer's registers to the consumers):
+//   warps 0-7   two consumer warpgroups; thread t owns W row t of the tile.  Per K-step (64 weights) each thread dequantizes its
+//               row into the stage (generic-proxy stores + fence.proxy.async, then a warpgroup barrier), the warpgroup waits for the
+//               stage's activation tile and issues 4 x (2 x BN/64) wgmma over its 128 rows.  The MMAs of a step run while the next
+//               step is dequantized (wgmma.wait_group 1); a finished step releases its stage to the producer.
+//   warp 8      TMA producer (warps 9-11 idle): raw W units of the 256 rows (packed bytes of UNIT_KSTEPS x 64 weights per row) into a 2-deep raw ring,
+//               one unit ahead, and the BN x 64 activation tile of every K-step into the operand ring (for T_F16 also the A tile).
+// Split-K when the tiles alone do not fill the GPU: partial producers (ks > 0) are scheduled first and hand their accumulators to
+// the tile owner through the workspace (flag per tile in a self-cleaning per-device block), so the owner's wait cannot deadlock.
+// The activation conversion kernel and this kernel are chained with programmatic dependent launch: barrier set-up, tensor-map
+// prefetch and (static weights) the first raw W unit run while the conversion is still in flight.
 //
-// Replaces the reference's mul_mat_q (src/ggml-cuda/mmq.cuh:2499-2655) for the shapes make_tc2_plan accepts; everything else stays on
-// mmq_tc.cu.  Results are those of mmq_tc.cu (same operand values, f32 accumulation; only the summation grouping of split-K differs).
+// Replaces the reference's mul_mat_q (src/ggml-cuda/mmq.cuh:2499-2655) and its dequantize + cuBLAS route for the shapes make_tc2_plan
+// accepts.
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_tc_dequant.cuh"
@@ -31,36 +29,19 @@
 
 namespace b200 {
 
-constexpr int T2_BM = 128;                    // W rows per CTA (256 per pair)
+constexpr int T2_BM = 256;                    // W rows per CTA (128 per consumer warpgroup)
 constexpr int T2_BK = 64;
-constexpr int T2_DQ_WARPS = 8, T2_THREADS = (3 + T2_DQ_WARPS) * 32;
-constexpr int T2_MAX_STAGES = 8, T2_MAX_RAW = 8;
-constexpr int T2_TRACE_CTAS = 4096;
+constexpr int T2_CONSUMERS = 256, T2_THREADS = T2_CONSUMERS + 128;     // + the producer warpgroup
+constexpr int T2_MAX_STAGES = 6;
 
-// raw-unit geometry of this kernel: mmq_tc.cu's, except Q8_0, whose unit is 8 blocks (272 B = 17 x 16: always 16-byte aligned, no lead) so that,
-// like every other format, a dequantizer group owns two consecutive K-steps per unit (one unit load, one proxy fence per two stages) and the
-// row pitch of the raw box (272 = 16 mod 128) keeps the 128-bit shared-memory loads conflict-free
+// raw-unit geometry (b200_tc_dequant.cuh); T_F16: no raw ring, one K-step per "unit"
 template <int T> struct tc2fmt : tcfmt<T> {};
-template <> struct tc2fmt<T_Q8_0> { static constexpr int RAW = 272, STRIDE_WORDS = 68, UNIT_WORDS = 68, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };
-// T_F16: the A operand already is fp16 (dense f16 weights, or a format without an operand decoder dequantized into the workspace first):
-// the weight producer copies every K-step's 128 x 64 tile straight into the operand ring (SWIZZLE_128B), no raw ring, no dequantizers
-template <> struct tc2fmt<T_F16> { static constexpr int RAW = 16, STRIDE_WORDS = 0, UNIT_WORDS = 1, UNIT_KSTEPS = 4, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };
-template <int T> __device__ __forceinline__ void tc2_load_unit(const uint8_t * g, uint32_t (&u)[tc2fmt<T>::UNIT_WORDS]) {     // g: the unit in shared memory
-    if constexpr (T == T_F16) {
-        u[0] = 0;
-    } else if constexpr (T == T_Q8_0) {
-#pragma unroll
-        for (int i = 0; i < 17; ++i) { const uint4 v = *((const uint4 *)g + i); u[4 * i] = v.x; u[4 * i + 1] = v.y; u[4 * i + 2] = v.z; u[4 * i + 3] = v.w; }
-    } else {
-        tc_load_unit<T>(g, u);
-    }
-}
+template <> struct tc2fmt<T_F16> { static constexpr int RAW = 0, STRIDE_WORDS = 0, UNIT_WORDS = 1, UNIT_KSTEPS = 1, ODD_BACK_WORDS = 0, LOAD_BYTES = 16; };
 
 struct tc2_params {
     float * y; float * partials; unsigned int * flags; const float * inv_scale;
-    unsigned long long * trace;                 // developer aid (GGML_B200_TC2_TRACE=1): 8 globaltimer stamps per CTA, else nullptr
     int64_t M, N;
-    int32_t BN, m_tiles, n_tiles, splitk, units_total, nstages, nraw, w_static, tma_epi, solo, dbg;
+    int32_t BN, m_tiles, n_tiles, splitk, units_total, nstages, w_static;
     // grouped mode (MUL_MAT_ID, expert-grouped): the activation rows are SORTED by expert (position -> (token, slot) pair in `perm`), n-tiles are
     // enumerated per expert (tile_base: prefix of tiles per expert, off: prefix of positions per expert, both n_expert + 1 long, device-resident:
     // no host synchronisation); W is the [n_expert x M] row stack; y rows are scattered back through perm
@@ -68,66 +49,45 @@ struct tc2_params {
     int32_t n_expert;
 };
 
-__device__ __forceinline__ void tc2_stamp(unsigned long long * trace, int ev) {
-    if (trace) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); trace[(size_t)blockIdx.x * 8 + ev] = t; }
+// one K-step of A: the thread's 64 weights of its row, converted into the swizzled stage row (KS: K-step within the unit)
+template <int T>
+__device__ __forceinline__ void tc2_dequant(int ks, const uint32_t (&u)[tc2fmt<T>::UNIT_WORDS], uint8_t * dst, uint32_t sw) {
+    if constexpr (T != T_F16) {
+        if (ks == 0) dq64<T, 0>(u, dst, sw);
+        else if (ks == 1) dq64<T, 1>(u, dst, sw);
+        if constexpr (tc2fmt<T>::UNIT_KSTEPS == 4) {
+            if (ks == 2) dq64<T, 2>(u, dst, sw);
+            else if (ks == 3) dq64<T, 3>(u, dst, sw);
+        }
+    }
 }
-
-// position in a ring of n slots without run-time division: slot index + parity of the round
-struct tc2_ring_pos {
-    int s; uint32_t par; bool first;
-    __device__ __forceinline__ void advance(int d, int n) { s += d; if (s >= n) { s -= n; par ^= 1u; first = false; } }     // d <= n
-};
-
-// one K-step of A: wait for the stage to be free, dequantize the thread's 64 weights into its swizzled row
-template <int T, int KS>
-__device__ __forceinline__ void tc2_dequant_write(const tc2_ring_pos & pos, bool valid, const uint32_t (&u)[tc2fmt<T>::UNIT_WORDS], uint8_t * ring, int stage_bytes, int a_row_off,
-                                                  uint32_t sw, uint64_t * empty, long long * acct) {
-    long long t0 = 0;
-    if (acct) t0 = clock64();
-    if (!pos.first) tc_wait(&empty[pos.s], pos.par ^ 1u);
-    if (acct) { const long long t1 = clock64(); acct[1] += t1 - t0; }
-    if (valid) dq64<T, KS>(u, ring + pos.s * stage_bytes + a_row_off, sw);
-}
-// Hand-over of a dequantized stage to the tensor core, as it has to be for a CTA pair:
-//   * EVERY writer arrives for itself, after its own proxy fence (generic-proxy stores -> visible to the async proxy), on the stage barrier
-//     of ITS OWN CTA (release at CTA scope).  An elected lane arriving for the warp after __syncwarp() lost rows when the MMA was issued the
-//     moment the barrier completed (tests/gpu_tc2_stress.py, profiles/r02_gemm_pair_v2.md);
-//   * in the non-leader CTA the otherwise idle warp 1 waits for that local barrier and RELAYS it to the leader's stage barrier with one
-//     cluster-scope release (cumulative over the 128 writers it has acquired); the leader's MMA issuer acquires at cluster scope.  A CTA-scope
-//     release sent straight to the leader's barrier by every writer of the peer still lost a row once per ~50 launches when the tensor pipe
-//     was waiting for the dequantizers (BN <= 128), and a cluster-scope release per writer costs a GPU-scope memory barrier per thread.
-__device__ __forceinline__ void tc2_stage_arrive(int s, uint64_t * full) { tc_arrive(&full[s]); }
 
 template <int T, bool GROUPED = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(T2_THREADS, 1)
-mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y, const tc2_params p) {
+__global__ void __launch_bounds__(T2_THREADS, 1)
+mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const tc2_params p) {
     constexpr int RAW = tc2fmt<T>::RAW, UK = tc2fmt<T>::UNIT_KSTEPS;
-    constexpr bool DENSE = T == T_F16;                            // fp16 A tiles by TMA: no dequantizers, no generic-proxy hand-over
-    extern __shared__ __align__(1024) uint8_t smem[];
-    // identical layout in both CTAs: [ring: nstages x (A 16 KB | B half BN/2 x 128 B)][raw: nraw x 128 x RAW][barriers][tmem slot][inv_scale tile]
+    constexpr bool DENSE = T == T_F16;                            // fp16 A tiles by TMA: no raw ring, no dequantizers
+    extern __shared__ uint8_t smem_raw[];
+    // [ring: nstages x (A: 256 x 128 B | B: BN x 128 B)][raw: 2 x 256 x RAW][barriers][inv_scale of the tile's columns]
+    uint8_t * smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);      // SWIZZLE_128B tiles: 1024-byte aligned
     constexpr int a_bytes = T2_BM * T2_BK * 2;
-    // pair mode: each CTA holds its HALF of the activation tile; solo mode: each CTA holds the WHOLE tile (its half + the peer's, by TMA multicast)
-    const int b_half = (p.BN / 2) * T2_BK * 2, b_bytes = p.solo ? 2 * b_half : b_half, stage_bytes = a_bytes + b_bytes;
+    const int b_bytes = p.BN * T2_BK * 2, stage_bytes = a_bytes + b_bytes;
     uint8_t * ring = smem;
     uint8_t * raw  = ring + p.nstages * stage_bytes;
-    uint64_t * bars = (uint64_t *)(raw + p.nraw * T2_BM * RAW);
-    uint64_t * full = bars, * empty = bars + T2_MAX_STAGES, * raw_full = bars + 2 * T2_MAX_STAGES, * raw_empty = raw_full + T2_MAX_RAW, * acc_full = raw_empty + T2_MAX_RAW;
-    uint32_t * tmem_slot = (uint32_t *)(acc_full + 1);
-    float * s_inv = (float *)(tmem_slot + 2);                     // inv_scale of the tile's BN columns (epilogue)
+    uint64_t * bars = (uint64_t *)(raw + 2 * T2_BM * RAW);
+    uint64_t * full = bars, * empty = bars + T2_MAX_STAGES, * raw_full = bars + 2 * T2_MAX_STAGES, * raw_empty = raw_full + 2;
+    float * s_inv = (float *)(raw_empty + 2);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t rank = tc_cluster_ctarank();                   // 0 = leader
-    if (tid == 0) tc2_stamp(p.trace, 0);
     tc_pdl_launch_dependents();
-    // work item of the pair: partial producers (ks > 0) first, tile owners (ks == 0) last
-    const int pair = (int)blockIdx.x >> 1;
+    // work item: partial producers (ks > 0) first, tile owners (ks == 0) last
     const int tiles = p.m_tiles * p.n_tiles;
-    const int ks = p.splitk - 1 - pair / tiles;
-    const int tile = pair % tiles, tm = tile % p.m_tiles, tn = tile / p.m_tiles;
+    const int ks = p.splitk - 1 - (int)blockIdx.x / tiles;
+    const int tile = (int)blockIdx.x % tiles, tm = tile % p.m_tiles, tn = tile / p.m_tiles;
     const int ubeg = (int)((int64_t)p.units_total * ks / p.splitk), uend = (int)((int64_t)p.units_total * (ks + 1) / p.splitk);
-    const int nunits = uend - ubeg, nsteps = UK * nunits;
+    const int nunits = uend - ubeg;
     // grouped mode: n-tile tn of the enumeration belongs to expert gx, covers sorted positions [gn0, gn0 + gcols); tiles past the last one
-    // (the grid is sized for the worst case) retire at once -- both CTAs of the pair see the same table, so the exit is pair-uniform
+    // (the grid is sized for the worst case) retire at once
     int gx = 0, gn0 = 0, gcols = 0;
     if constexpr (GROUPED) {
         if (tn >= p.g_tile_base[p.n_expert]) return;
@@ -137,296 +97,183 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         gn0 = p.g_off[gx] + (tn - p.g_tile_base[gx]) * p.BN;
         gcols = min(p.BN, p.g_off[gx + 1] - gn0);
     }
-    const int64_t row_base = (int64_t)tm * (2 * T2_BM) + (int64_t)rank * T2_BM;     // first W row of this CTA (within the expert's matrix)
-    const int64_t rows_left = p.M - row_base;                     // may be <= 0 for the second CTA of the last tile
+    const int64_t row_base = (int64_t)tm * T2_BM;                 // first W row of the tile (within the expert's matrix)
     const int64_t w_row0 = GROUPED ? (int64_t)gx * p.M + row_base : row_base;       // row in the [n_expert x M] stack
-    const int x_row0 = GROUPED ? gn0 + (int)rank * (p.BN / 2) : tn * p.BN + (int)rank * (p.BN / 2);
+    const int x_row0 = GROUPED ? gn0 : tn * p.BN;
 
     if (tid == 0) {
-        // stage barrier: the 128 dequantizer threads of this CTA that own the K-step; in the leader also its activation producer (expect_tx for
-        // both activation halves) and the non-leader's relay warp.  empty / acc_full: one multicast commit each.
-        for (int s = 0; s < p.nstages; ++s) {
-            if (p.solo) { tc_mbar_init(&full[s], DENSE ? 2 : T2_DQ_WARPS / 2 * 32 + 1); tc_mbar_init(&empty[s], p.solo == 2 ? 1 : 2); }      // own producer's expect_tx; (multicast: both CTAs' MMAs release a stage)
-            else        { tc_mbar_init(&full[s], DENSE ? 2 : T2_DQ_WARPS / 2 * 32 + (rank == 0 ? 2 : 0)); tc_mbar_init(&empty[s], 1); }   // (DENSE: the leader's two expect_tx)
-        }
-        for (int s = 0; s < p.nraw; ++s) { tc_mbar_init(&raw_full[s], 1); tc_mbar_init(&raw_empty[s], (p.dbg & 4) ? T2_DQ_WARPS * 32 : T2_DQ_WARPS); }
-        tc_mbar_init(acc_full, 1);
+        for (int s = 0; s < p.nstages; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 2); }     // producer's expect_tx; one release per warpgroup
+        for (int s = 0; s < 2; ++s) { tc_mbar_init(&raw_full[s], 1); tc_mbar_init(&raw_empty[s], T2_CONSUMERS / 32); }
         tc_fence_init();
         tc_prefetch_map(&map_w); tc_prefetch_map(&map_x);
-        if (p.tma_epi) tc_prefetch_map(&map_y);
     }
-    if (warp == 1) { if (p.solo) tc_tmem_alloc(tmem_slot, tc_tmem_cols(p.BN)); else tc_tmem_alloc_pair(tmem_slot, tc_tmem_cols(p.BN)); }
-    tc_fence_before();
     __syncthreads();
-    auto issue_raw = [&](int u, int rs) {
-        tc_expect_tx(&raw_full[rs], T2_BM * RAW);
-        int coord;                                                // first 4-byte word of the box: 16-byte aligned start at or below the unit
-        if constexpr (tc2fmt<T>::LOAD_BYTES == 2) coord = (((ubeg + u) * tc2fmt<T>::UNIT_BYTES) & ~15) >> 2;
-        else                        coord = (ubeg + u) * tc2fmt<T>::STRIDE_WORDS - ((ubeg + u) & 1) * tc2fmt<T>::ODD_BACK_WORDS;
-        tc_tma_2d(raw + rs * T2_BM * RAW, &map_w, coord, (int)w_row0, &raw_full[rs]);
-    };
-    // the weight stream only involves this CTA's own barriers: its first requests leave between the two halves of the cluster-wide sync (the
-    // descriptor fetch and the HBM latency overlap the wait; issuing them before the arrive delayed the whole pair by 1.5 us)
-    const int raw_issued = (DENSE || (p.dbg & 2)) ? 0 : (nunits < p.nraw ? nunits : p.nraw);   // (nraw < number of units of a ring round: advance() wraps at most once)
-    tc_cluster_arrive();
-    if (tid == 0 && !DENSE) {
-        if (!p.w_static) tc_pdl_wait();                           // W produced by the preceding kernel: nothing may be read before it is done
-        for (int u = 0; u < raw_issued; ++u) issue_raw(u, u);
-    }
-    __syncwarp();
-    tc_cluster_wait();                                            // the peer's barriers exist before anything is signalled on them
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    if (tid == 0) tc2_stamp(p.trace, 1);
 
-    if (warp == 0) {
-        // ===================== raw W producer (both CTAs): the packed units of the own 128 rows, nraw units ahead of the dequantizers
-        if (DENSE && lane == 0) {
-            // fp16 weights: the K-step's A tile goes straight into the operand ring
-            if (!p.w_static) tc_pdl_wait();
-            tc2_ring_pos pos{ 0, 0u, true };
-            for (int step = 0; step < nsteps; ++step, pos.advance(1, p.nstages)) {
-                if (!pos.first) tc_wait(&empty[pos.s], pos.par ^ 1u);
-                if (p.solo) {
-                    tc_expect_tx(&full[pos.s], (uint32_t)a_bytes);
-                    tc_tma_2d(ring + pos.s * stage_bytes, &map_w, (ubeg * UK + step) * T2_BK, (int)w_row0, &full[pos.s]);
-                } else {
-                    // pair mode: both CTAs' A tiles are counted on the leader's stage barrier (everything on the async proxy: no relay needed)
-                    if (rank == 0) tc_expect_tx(&full[pos.s], (uint32_t)(2 * a_bytes));
-                    tc_tma_2d_pair(ring + pos.s * stage_bytes, &map_w, (ubeg * UK + step) * T2_BK, (int)w_row0, tc_cluster_addr(&full[pos.s], 0));
+    if (warp >= T2_CONSUMERS / 32) {
+        // ===================== TMA producer
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (warp == T2_CONSUMERS / 32 && lane == 0) {
+            auto issue_raw = [&](int u) {
+                const int rs = u & 1;
+                tc_expect_tx(&raw_full[rs], T2_BM * RAW);
+                int coord;                                        // first 4-byte word of the box: 16-byte aligned start at or below the unit
+                if constexpr (tc2fmt<T>::LOAD_BYTES == 2) coord = (((ubeg + u) * tc2fmt<T>::UNIT_BYTES) & ~15) >> 2;   // unaligned units: lead bytes in front of the payload
+                else                        coord = (ubeg + u) * tc2fmt<T>::STRIDE_WORDS - ((ubeg + u) & 1) * tc2fmt<T>::ODD_BACK_WORDS;
+                tc_tma_2d(raw + rs * T2_BM * RAW, &map_w, coord, (int)w_row0, &raw_full[rs]);
+            };
+            if (!DENSE && p.w_static) issue_raw(0);               // static weights: the first unit streams while the conversion kernel runs
+            tc_pdl_wait();                                        // the fp16 activations (and non-static W) are written by the preceding kernels
+            if (!DENSE && !p.w_static) issue_raw(0);
+            for (int u = 0; u < nunits; ++u) {
+                if (!DENSE && u + 1 < nunits) {
+                    if (u + 1 >= 2) tc_wait(&raw_empty[(u + 1) & 1], (uint32_t)(((u + 1) >> 1) - 1) & 1u);
+                    issue_raw(u + 1);
                 }
-            }
-        } else if (lane == 0) {
-            tc2_ring_pos rpos{ 0, 0u, true };
-            rpos.advance(raw_issued, p.nraw);                     // the first units were requested before the cluster-wide sync
-            for (int u = raw_issued; u < nunits; ++u, rpos.advance(1, p.nraw)) {
-                if (!rpos.first) tc_wait(&raw_empty[rpos.s], rpos.par ^ 1u);
-                issue_raw(u, rpos.s);
-            }
-        }
-    } else if (warp == 2 + T2_DQ_WARPS) {
-        // ===================== activation producer (both CTAs): the own half of every stage's B tile, signalled on the LEADER's stage barrier
-        if (lane == 0) {
-            tc_pdl_wait();                                        // the fp16 activations are written by the conversion kernel just before this one
-            tc2_stamp(p.trace, 2);
-            const uint32_t full0 = tc_cluster_addr(&full[0], 0);
-            long long bwait = 0;
-            tc2_ring_pos pos{ 0, 0u, true };
-            for (int step = 0; step < nsteps; ++step, pos.advance(1, p.nstages)) {
-                const int s = pos.s;
-                const long long t0 = p.trace ? clock64() : 0;
-                if (!pos.first) tc_wait(&empty[s], pos.par ^ 1u);
-                if (p.trace) bwait += clock64() - t0;
-                if (p.solo == 2) {
-                    // independent CTAs: both halves of the activation tile by this CTA's own copies
-                    const int xr = x_row0 - (int)rank * (p.BN / 2);
-                    tc_expect_tx(&full[s], (uint32_t)(2 * b_half));
-                    tc_tma_2d(ring + s * stage_bytes + a_bytes, &map_x, (ubeg * UK + step) * T2_BK, xr, &full[s]);
-                    tc_tma_2d(ring + s * stage_bytes + a_bytes + b_half, &map_x, (ubeg * UK + step) * T2_BK, xr + p.BN / 2, &full[s]);
-                } else if (p.solo) {
-                    // own half of the tile into BOTH CTAs (same offset), counted on each CTA's own stage barrier; this CTA expects both halves
-                    tc_expect_tx(&full[s], (uint32_t)(2 * b_half));
-                    tc_tma_2d_mc(ring + s * stage_bytes + a_bytes + (int)rank * b_half, &map_x, (ubeg * UK + step) * T2_BK, x_row0, &full[s], (uint16_t)3);
-                } else {
-                    if (rank == 0) tc_expect_tx(&full[s], (uint32_t)(2 * b_half));
-                    tc_tma_2d_pair(ring + s * stage_bytes + a_bytes, &map_x, (ubeg * UK + step) * T2_BK, x_row0, full0 + (uint32_t)(s * 8));
-                }
-            }
-            if (p.trace && (int)blockIdx.x < T2_TRACE_CTAS / 2) p.trace[((size_t)(T2_TRACE_CTAS / 2) + blockIdx.x) * 8 + 7] = (unsigned long long)bwait;
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: the leader for the pair (cta_group::2), or every CTA for itself (solo, cta_group::1)
-        if (rank == 0 || p.solo) {
-            // instruction descriptor: D = f32 (bit 4), A = B = f16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24 (M = 256: the pair; 128: solo)
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(((p.solo ? 1 : 2) * T2_BM) >> 4) << 24);
-            long long mma_wait = 0;
-            tc2_ring_pos pos{ 0, 0u, true };
-            for (int step = 0; step < nsteps; ++step, pos.advance(1, p.nstages)) {
-                const int s = pos.s;
-                const long long t0 = p.trace ? clock64() : 0;
-                if (p.solo) tc_wait(&full[s], pos.par); else tc_wait_cluster(&full[s], pos.par);
-                if (p.trace) mma_wait += clock64() - t0;
-                tc_fence_after();
-                if (lane == 0) {
-                    if (step == 0) tc2_stamp(p.trace, 3);
-                    const uint64_t ad = tc_smem_desc(tc_smem(ring + s * stage_bytes));
-                    const uint64_t bd = tc_smem_desc(tc_smem(ring + s * stage_bytes + a_bytes));
-                    if (p.solo) {
-#pragma unroll
-                        for (int k = 0; k < T2_BK / 16; ++k)
-                            tc_mma_f16(tmem, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, (step | k) != 0 ? 1u : 0u);
-                        if (p.solo == 2) tc_commit(&empty[s]); else tc_commit_mc(&empty[s], (uint16_t)3);   // multicast: the stage holds the peer's half too, both CTAs must be done with it
-                        if (step == nsteps - 1) tc_commit(acc_full);
+                for (int q = 0; q < UK; ++q) {
+                    const int step = UK * u + q, s = step % p.nstages;
+                    if (step >= p.nstages) tc_wait(&empty[s], (uint32_t)((step / p.nstages) - 1) & 1u);
+                    const int kc = ((ubeg + u) * UK + q) * T2_BK;
+                    uint8_t * st = ring + s * stage_bytes;
+                    if constexpr (DENSE) {
+                        tc_expect_tx(&full[s], (uint32_t)(a_bytes + b_bytes));
+                        tc_tma_2d(st, &map_w, kc, (int)w_row0, &full[s]);
                     } else {
-#pragma unroll
-                        for (int k = 0; k < T2_BK / 16; ++k)
-                            tc_mma_f16_pair(tmem, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, (step | k) != 0 ? 1u : 0u);   // +32 bytes per K = 16
-                        tc_commit_pair(&empty[s]);
-                        if (step == nsteps - 1) tc_commit_pair(acc_full);
+                        tc_expect_tx(&full[s], (uint32_t)b_bytes);
                     }
+                    tc_tma_2d(st + a_bytes, &map_x, kc, x_row0, &full[s]);
                 }
-                __syncwarp();
-            }
-            if (p.trace && lane == 0 && (int)blockIdx.x < T2_TRACE_CTAS / 2) p.trace[((size_t)(T2_TRACE_CTAS / 2) + blockIdx.x) * 8 + 3] = (unsigned long long)mma_wait;
-        } else if (!DENSE && lane < p.nstages) {
-            // non-leader: relay "this CTA's half of stage s is written" to the leader's barrier.  One lane per stage slot: the cluster-scope
-            // release costs a GPU-scope memory barrier (~1 us), a single relay thread would serialize the ring on it
-            uint32_t par = 0;
-            for (int step = lane; step < nsteps; step += p.nstages, par ^= 1u) {
-                tc_wait(&full[lane], par);
-                tc_arrive_cluster_release(&full[lane], 0);
             }
         }
-    } else {
-        // ===================== dequantizers: two threads per row (warps 2-5 / 6-9), each half of the unit's K-steps
-        const int dq = tid - 64, dwarp = dq >> 5;
-        const int row = dq & 127, ksel = dq >> 7;
-        const bool valid = row < rows_left;                       // rows past M: the TMA box is zero-filled, nothing to convert
-        const uint32_t sw = (uint32_t)(row & 7);
-        const int a_row_off = (row >> 3) * 1024 + (row & 7) * 128;
-        uint32_t ub[tc2fmt<T>::UNIT_WORDS];
-        // developer accounting (trace on): lane 0 of the first warp of each group sums its cycles waiting for raw units [0] / free stages [1]
-        long long acct_store[2] = { 0, 0 };
-        long long * acct = (p.trace && lane == 0 && (dwarp & 3) == 0) ? acct_store : nullptr;
-        const long long loop_t0 = acct ? clock64() : 0;
-        // this group's K-steps: UK = 4: steps 4u + 2 ksel, + 1 (two consecutive stages, one proxy fence); UK = 2: step 2u + ksel
-        constexpr int PER = UK / 2;
-        tc2_ring_pos pos{ ksel * PER, 0u, true };                 // ring position of the group's next K-step (PER <= 2 < nstages)
-        tc2_ring_pos rpos{ 0, 0u, true };                         // raw ring
-        const uint8_t * my_raw = raw + row * RAW;
-        for (int u = 0; u < (DENSE ? 0 : nunits); ++u) {
-            { const long long t0 = acct ? clock64() : 0;
-              tc_wait(&raw_full[rpos.s], rpos.par);
-              if (acct) acct[0] += clock64() - t0; }
+        return;
+    }
+
+    // ===================== consumers: thread tid owns W row tid of the tile; warpgroup wg multiplies rows 128 wg .. 128 wg + 127
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");        // 128 accumulators + a raw unit + addressing per thread
+    const int wg = tid >> 7, row = tid;
+    const uint32_t sw = (uint32_t)(row & 7);
+    const int a_row_off = (row >> 3) * 1024 + (row & 7) * 128;
+    const bool two_n = p.BN == 128;
+    float acc[2][2][32];
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int nj = 0; nj < 2; ++nj)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[mi][nj][i] = 0.0f;
+    uint32_t ub[tc2fmt<T>::UNIT_WORDS];
+    for (int u = 0; u < nunits; ++u) {
+        if constexpr (!DENSE) {
+            const int rs = u & 1;
+            tc_wait(&raw_full[rs], (uint32_t)(u >> 1) & 1u);
             int lead;                                             // bytes between the box start and the unit's first byte
             if constexpr (tc2fmt<T>::LOAD_BYTES == 2) lead = ((ubeg + u) * tc2fmt<T>::UNIT_BYTES) & 15;
-            else                       lead = ((ubeg + u) & 1) * (4 * tc2fmt<T>::ODD_BACK_WORDS);
-            tc2_load_unit<T>(my_raw + rpos.s * (T2_BM * RAW) + lead, ub);
-            if (p.dbg & 4) tc_arrive(&raw_empty[rpos.s]);
-            else { __syncwarp(); if (lane == 0) tc_arrive(&raw_empty[rpos.s]); }       // the unit is in registers: the buffer can be refilled
-            rpos.advance(1, p.nraw);
-            if constexpr (UK == 4) {
-                tc2_ring_pos pos2 = pos; pos2.advance(1, p.nstages);
-                if (ksel == 0) {
-                    tc2_dequant_write<T, 0>(pos,  valid, ub, ring, stage_bytes, a_row_off, sw, empty, acct);
-                    if (p.dbg & 1) { tc_fence_async_smem(); tc2_stage_arrive(pos.s, full); }
-                    tc2_dequant_write<T, 1>(pos2, valid, ub, ring, stage_bytes, a_row_off, sw, empty, acct);
-                } else {
-                    tc2_dequant_write<T, 2>(pos,  valid, ub, ring, stage_bytes, a_row_off, sw, empty, acct);
-                    if (p.dbg & 1) { tc_fence_async_smem(); tc2_stage_arrive(pos.s, full); }
-                    tc2_dequant_write<T, 3>(pos2, valid, ub, ring, stage_bytes, a_row_off, sw, empty, acct);
-                }
+            else                        lead = ((ubeg + u) & 1) * (4 * tc2fmt<T>::ODD_BACK_WORDS);
+            tc_load_unit<T>(raw + rs * T2_BM * RAW + row * RAW + lead, ub);
+            // the unit is in registers: the buffer can be refilled.  The refill is a TMA write (async proxy) after these generic-proxy reads,
+            // so every reader fences before its warp releases the buffer; without the fence, Q8_0 tiles (the fastest raw-ring turnover) read
+            // units that were already being overwritten whenever the release came from the last busy warp.
+            tc_fence_async_smem();
+            __syncwarp();
+            if (lane == 0) tc_arrive(&raw_empty[rs]);
+        }
+#pragma unroll
+        for (int q = 0; q < UK; ++q) {
+            const int step = UK * u + q, s = step % p.nstages;
+            uint8_t * st = ring + s * stage_bytes;
+            if constexpr (!DENSE) {
+                // this warpgroup's rows of the stage were last read by its own MMAs of step - nstages <= step - 2: complete (wait_group 1 below)
+                if (row < p.M - row_base) tc2_dequant<T>(q, ub, st + a_row_off, sw);     // rows past M: zero-filled box, results never stored
                 tc_fence_async_smem();
-                if (!(p.dbg & 1)) tc2_stage_arrive(pos.s, full);
-                tc2_stage_arrive(pos2.s, full);
-                pos = pos2; pos.advance(3, p.nstages);
-            } else {
-                if (ksel == 0) tc2_dequant_write<T, 0>(pos, valid, ub, ring, stage_bytes, a_row_off, sw, empty, acct);
-                else           tc2_dequant_write<T, 1>(pos, valid, ub, ring, stage_bytes, a_row_off, sw, empty, acct);
-                tc_fence_async_smem();
-                tc2_stage_arrive(pos.s, full);
-                pos.advance(2, p.nstages);
+                asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
             }
-        }
-        if (acct && (int)blockIdx.x < T2_TRACE_CTAS / 2) {
-            unsigned long long * w = p.trace + ((size_t)(T2_TRACE_CTAS / 2) + blockIdx.x) * 8 + (ksel ? 4 : 0);
-            w[0] = (unsigned long long)acct[0]; w[1] = (unsigned long long)acct[1]; w[2] = (unsigned long long)(clock64() - loop_t0);
-        }
-        // ===================== epilogue: this CTA's 128 accumulator lanes x BN columns
-        tc_wait(acc_full, 0);
-        tc_fence_after();
-        if (dq == 0) tc2_stamp(p.trace, 4);
-        // each warp owns its TMEM lane quarter (hardware: warp id % 4) and one half of the columns
-        const int lg = warp & 3, grp = dwarp >> 2;
-        const int ncol = p.BN / 2, col0 = grp * ncol;
-        const int64_t m = row_base + lg * 32 + lane;
-        const int64_t n_base = (int64_t)tn * p.BN + col0;
-        const uint32_t tacc = tmem + ((uint32_t)(lg * 32) << 16) + (uint32_t)col0;
-        const int mloc = lg * 32 + lane;
-        const int fidx = tile * 2 + (int)rank;
-        float * part = p.partials ? p.partials + ((size_t)fidx * (p.splitk - 1)) * (size_t)(p.BN * T2_BM) : nullptr;
-        // bulk-store epilogue (dense output): each column-half group (4 warps = the 128 accumulator lanes) stages a [32 columns][128 rows] slab in
-        // the now idle operand ring and one thread hands it to the TMA (2-D store into y, clipped at the M / N edges by the tensor map; 1-D 16 KB
-        // stores for split-K partials); two slabs per group alternate.  Replaces 32 scattered 128-byte warp stores per slab and thread.
-        const bool tma_epi = !GROUPED && p.tma_epi != 0;
-        float * slabs = (float *)ring + grp * (2 * 32 * T2_BM);
-        const int gtid = dq & 127;
-        auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory"); };
-        if (ks > 0) {
-            // split-K partial: [ks-1][n_local][m_local]
-            float * dst = part + (size_t)(ks - 1) * (p.BN * T2_BM);
-            for (int c0 = 0; c0 < ncol; c0 += 32) {
-                float v[32];
-                if (tma_epi) {
-                    float * buf = slabs + ((c0 >> 5) & 1) * (32 * T2_BM);
-                    if (c0 >= 64) { if (gtid == 0) tc_bulk_wait_read<1>(); group_sync(); }
-                    tc_ld32(tacc + (uint32_t)c0, v);
+            tc_wait(&full[s], (uint32_t)(step / p.nstages) & 1u);
+            wg_fence();
+            const uint64_t ad = tc_smem_desc(tc_smem(st + wg * (128 * 128)));
+            const uint64_t bd = tc_smem_desc(tc_smem(st + a_bytes));
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) buf[i * T2_BM + mloc] = v[i];
-                    tc_fence_async_smem();
-                    group_sync();
-                    if (gtid == 0) { tc_bulk_store_1d(dst + (size_t)(col0 + c0) * T2_BM, buf, 32 * T2_BM * 4); tc_bulk_commit(); }
-                } else {
-                    tc_ld32(tacc + (uint32_t)c0, v);
+            for (int k = 0; k < T2_BK / 16; ++k) {               // +32 bytes per K = 16; +8 KB per 64 rows (A) / 64 columns (B)
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) dst[(size_t)(col0 + c0 + i) * T2_BM + mloc] = v[i];
+                for (int mi = 0; mi < 2; ++mi) {
+                    wg_mma_m64n64k16(acc[mi][0], ad + (uint64_t)(2 * k + mi * 512), bd + (uint64_t)(2 * k));
+                    if (two_n) wg_mma_m64n64k16(acc[mi][1], ad + (uint64_t)(2 * k + mi * 512), bd + (uint64_t)(2 * k + 512));
                 }
             }
-            if (tma_epi && gtid == 0) { tc_bulk_wait<0>(); tc_fence_async_all(); }     // the partial is in global memory before the flag goes up
-            __threadfence();
-            asm volatile("bar.sync 1, %0;" ::"n"(T2_DQ_WARPS * 32) : "memory");
-            if (dq == 0) atomicAdd(&p.flags[fidx], 1u);
-        } else {
-            // inv_scale of the tile's columns -> shared memory: one L2 round trip for the tile instead of one in front of every store
-            for (int c = dq; c < p.BN; c += T2_DQ_WARPS * 32) {
-                const int64_t n = GROUPED ? (int64_t)gn0 + c : (int64_t)tn * p.BN + c;
-                s_inv[c] = (GROUPED ? c < gcols : n < p.N) ? __ldcg(p.inv_scale + n) : 0.0f;
-            }
-            if (p.splitk > 1 && dq == 0) { while (atomicAdd(&p.flags[fidx], 0u) < (unsigned)(p.splitk - 1)) __nanosleep(64); __threadfence(); }
-            asm volatile("bar.sync 1, %0;" ::"n"(T2_DQ_WARPS * 32) : "memory");
-            if (dq == 0) tc2_stamp(p.trace, 5);
-            for (int c0 = 0; c0 < ncol; c0 += 32) {
-                float v[32];
-                float * buf = slabs + ((c0 >> 5) & 1) * (32 * T2_BM);
-                if (tma_epi && c0 >= 64) { if (gtid == 0) tc_bulk_wait_read<1>(); group_sync(); }
-                tc_ld32(tacc + (uint32_t)c0, v);
-                for (int j = 1; j < p.splitk; ++j) {
-                    const float * src = part + (size_t)(j - 1) * (p.BN * T2_BM);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] += __ldcg(&src[(size_t)(col0 + c0 + i) * T2_BM + mloc]);
-                }
-                if (tma_epi) {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) buf[i * T2_BM + mloc] = v[i] * s_inv[col0 + c0 + i];
-                    tc_fence_async_smem();
-                    group_sync();
-                    if (gtid == 0 && rows_left > 0 && n_base + c0 < p.N) { tc_tma_store_2d(&map_y, buf, (int)row_base, (int)(n_base + c0)); tc_bulk_commit(); }
-                } else if (m < p.M) {
-                    if constexpr (GROUPED) {
-                        int prm[32];
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) prm[i] = (col0 + c0 + i) < gcols ? __ldg(p.g_perm + gn0 + col0 + c0 + i) : -1;
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) if (prm[i] >= 0) p.y[(size_t)prm[i] * p.M + m] = v[i] * s_inv[col0 + c0 + i];
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) { const int64_t n = n_base + c0 + i; if (n < p.N) p.y[(size_t)n * p.M + m] = v[i] * s_inv[col0 + c0 + i]; }
-                    }
-                }
-            }
-            if (tma_epi && gtid == 0) tc_bulk_wait_read<0>();        // the slabs are read out before the CTA gives its shared memory back
-            if (p.splitk > 1) {
-                asm volatile("bar.sync 1, %0;" ::"n"(T2_DQ_WARPS * 32) : "memory");
-                if (dq == 0) p.flags[fidx] = 0;                  // leave the flag clean for the next launch that gets this slot
-            }
+            wg_commit();
+            wg_wait<1>();                                         // the MMAs of step - 1 are complete: release its stage
+            if (step > 0 && (tid & 127) == 0) tc_arrive(&empty[(step - 1) % p.nstages]);
         }
-        if (dq == 0) tc2_stamp(p.trace, 6);
-        tc_fence_before();
     }
-    __syncthreads();
-    tc_cluster_sync();                                            // neither CTA retires (nor frees TMEM) while the pair still works
-    if (warp == 1) { tc_fence_after(); if (p.solo) tc_tmem_dealloc(tmem, tc_tmem_cols(p.BN)); else tc_tmem_dealloc_pair(tmem, tc_tmem_cols(p.BN)); }
-    if (tid == 0) tc2_stamp(p.trace, 7);
+    wg_wait<0>();
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int nj = 0; nj < 2; ++nj)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) wg_fence_operand(acc[mi][nj][i]);
+
+    // ===================== epilogue.  wgmma m64nN fragment: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8), register 4 j + 2 h + e
+    // is row + 8 h, column 8 j + 2 (lane % 4) + e
+    tc_pdl_wait();                                                // inv_scale comes from the conversion kernel
+    const int r0 = wg * 128 + ((tid & 127) >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    const int nregs = (two_n ? 2 : 1) * 64;                       // accumulator registers per thread (partials layout: [register][thread])
+    auto consumers_sync = [] { asm volatile("bar.sync 3, %0;" ::"n"(T2_CONSUMERS) : "memory"); };
+    float * part = p.partials ? p.partials + (size_t)tile * (p.splitk - 1) * (size_t)(p.BN * T2_BM) : nullptr;
+    if (ks > 0) {
+        float * dst = part + (size_t)(ks - 1) * (p.BN * T2_BM);
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int nj = 0; nj < 2; ++nj)
+                if (nj == 0 || two_n) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) __stcg(&dst[(size_t)(mi * (nregs / 2) + nj * 32 + i) * T2_CONSUMERS + tid], acc[mi][nj][i]);
+                }
+        __threadfence();
+        consumers_sync();
+        if (tid == 0) atomicAdd(&p.flags[tile], 1u);
+        return;
+    }
+    // inv_scale of the tile's columns -> shared memory
+    for (int c = tid; c < p.BN; c += T2_CONSUMERS) {
+        const int64_t n = GROUPED ? (int64_t)gn0 + c : (int64_t)tn * p.BN + c;
+        s_inv[c] = (GROUPED ? c < gcols : n < p.N) ? __ldcg(p.inv_scale + n) : 0.0f;
+    }
+    if (p.splitk > 1 && tid == 0) { while (atomicAdd(&p.flags[tile], 0u) < (unsigned)(p.splitk - 1)) __nanosleep(64); __threadfence(); }
+    consumers_sync();
+    for (int j = 1; j < p.splitk; ++j) {
+        const float * src = part + (size_t)(j - 1) * (p.BN * T2_BM);
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int nj = 0; nj < 2; ++nj)
+                if (nj == 0 || two_n) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) acc[mi][nj][i] += __ldcg(&src[(size_t)(mi * (nregs / 2) + nj * 32 + i) * T2_CONSUMERS + tid]);
+                }
+    }
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int nj = 0; nj < 2; ++nj) {
+            if (nj == 1 && !two_n) continue;
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                const int rl = r0 + mi * 64 + ((i >> 1) & 1) * 8, c = nj * 64 + (i >> 2) * 8 + c0 + (i & 1);
+                const int64_t m = row_base + rl;
+                if (m >= p.M) continue;
+                const float v = acc[mi][nj][i] * s_inv[c];
+                if constexpr (GROUPED) {
+                    if (c < gcols) p.y[(size_t)__ldg(p.g_perm + gn0 + c) * p.M + m] = v;
+                } else {
+                    const int64_t n = (int64_t)tn * p.BN + c;
+                    if (n < p.N) p.y[(size_t)n * p.M + m] = v;
+                }
+            }
+        }
+    if (p.splitk > 1) {
+        consumers_sync();
+        if (tid == 0) p.flags[tile] = 0;                          // leave the flag clean for the next launch that gets this slot
+    }
 }
 
 // ----------------------------------------------------------------------------- split-K flags: persistent, zero-initialised, self-cleaning
@@ -456,118 +303,76 @@ unsigned int * tc_flag_slot() {
     return b + (size_t)(seq.fetch_add(1, std::memory_order_relaxed) % T2_FLAG_SLOTS) * T2_FLAGS_PER_SLOT;
 }
 
-// ----------------------------------------------------------------------------- developer trace (GGML_B200_TC2_TRACE=1): the last launch's per-CTA stamps
-static unsigned long long * tc2_trace_buf() {
-    static const bool on = getenv("GGML_B200_TC2_TRACE") && atoi(getenv("GGML_B200_TC2_TRACE")) != 0;
-    if (!on) return nullptr;
-    static unsigned long long * buf = nullptr;
-    static std::mutex mu;
-    std::lock_guard<std::mutex> lock(mu);
-    if (!buf) { if (cudaMalloc(&buf, (size_t)T2_TRACE_CTAS * 8 * sizeof(unsigned long long)) != cudaSuccess) { cudaGetLastError(); buf = nullptr; } else cudaMemset(buf, 0, (size_t)T2_TRACE_CTAS * 8 * sizeof(unsigned long long)); }
-    return buf;
-}
-int tc2_trace_read(unsigned long long * host_dst, int max_ctas) {
-    unsigned long long * b = tc2_trace_buf();
-    if (!b) return 0;
-    const int n = max_ctas < T2_TRACE_CTAS ? max_ctas : T2_TRACE_CTAS;
-    if (cudaMemcpy(host_dst, b, (size_t)n * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return n;
-}
+// this kernel records no per-CTA stamp trace
+int tc2_trace_read(unsigned long long * host_dst, int max_ctas) { (void)host_dst; (void)max_ctas; return 0; }
 
 // ----------------------------------------------------------------------------- host side
 struct tc2_plan {
-    int BN, m_tiles, n_tiles, splitk, chunks, nstages, nraw, smem, grid, mode;
+    int BN, m_tiles, n_tiles, splitk, chunks, nstages, smem, grid;
     size_t xb_bytes, partial_bytes, scale_bytes;
 };
 
-static int tc2_raw_bytes(int type) {
+static int tc2_raw_bytes(int type) {                                // tcfmt<T>::RAW
     switch (type) {
+        case T_F16: return 0;
         case T_Q5_K: case T_Q5_0: return 176;
         case T_Q6_K: return 224;
         case T_Q4_1: return 160;
         case T_Q5_1: return 192;
         case T_Q2_K: return 96;
         case T_Q3_K: return 128;
-        case T_Q8_0: return 272;
-        default: return 144;                                         // Q4_0, Q4_K, IQ4_NL, IQ4_XS
+        default: return 144;                                         // Q4_0, Q8_0 (half units), Q4_K, IQ4_NL, IQ4_XS
     }
 }
+static int tc2_unit_ksteps(int type) { return type == T_F16 ? 1 : type == T_Q8_0 ? 2 : 4; }     // tc2fmt<T>::UNIT_KSTEPS
 
-// shared-memory split: the operand ring only has to cover the dequantize -> MMA hand-over and the L2 latency of the activation tiles; what is
-// left goes to the raw W ring, which covers the HBM latency of the weight stream (profiles/r02_gemm_pair.md: with 2 raw units in flight the
-// dequantizers spent a quarter of their time waiting for the next unit)
-// MMA mode of a launch (GGML_B200_TC2_SOLO overrides).  0 (default): cta_group::2 pair MMAs; quantized formats hand the non-leader's dequantized
-// half-stage over through the relay warp (cluster-scope release), fp16 A tiles arrive by TMA and need no relay.  It is the only mode that is clean both
-// under tests/gpu_tc2_stress.py (one matrix, repeated launches) and under scripts/gemm_bench_parity.py (the bench's pattern: many distinct matrices,
-// PDL-overlapped launches, every element checked).  1: cta_group::1 per CTA with the activation tile shared by TMA multicast; 2: cta_group::1, fully
-// independent CTAs.  Both are 10 % faster and both compute wrong rows as soon as consecutive launches overlap (mode 2 passes the stress test, then
-// fails every matrix of the bench pattern; with programmatic launch off it still loses single rows): kept for study only, never selected.
-static int tc2_mode_for(bool dense) {
-    static const int env = getenv("GGML_B200_TC2_SOLO") ? atoi(getenv("GGML_B200_TC2_SOLO")) : -1;
-    if (env >= 0 && env <= 2) return env;
-    (void)dense;
-    return 0;
-}
-static bool tc2_smem_plan(int BN, int raw, int mode, int & nstages, int & nraw, int & smem) {
+// shared memory: the raw ring (2 units of 256 rows) first, then as many operand stages (>= 2: a stage is rewritten two steps after
+// its MMAs were issued, and wait_group 1 has completed them by then) as fit the 227 KB an H100 block may use
+static bool tc2_smem_plan(int BN, int raw, int & nstages, int & smem) {
     static const int env_stages = getenv("GGML_B200_TC2_STAGES") ? atoi(getenv("GGML_B200_TC2_STAGES")) : 0;
-    static const int env_raw = getenv("GGML_B200_TC2_RAW") ? atoi(getenv("GGML_B200_TC2_RAW")) : 0;
-    const int stage = T2_BM * T2_BK * 2 + (mode != 0 ? BN : BN / 2) * T2_BK * 2, tail = 2 * (T2_MAX_STAGES + T2_MAX_RAW) * 8 + 64 + 256 * 4 + 1024;
-    const int budget = 227 * 1024 - tail;
-    // at least 3 stages: a dequantizer group revisits the ring every <= 3 K-steps, and the parity wait on a stage's "empty" barrier is only
-    // unambiguous while the barrier is at most one phase behind the waiter (2 stages fault: the wait returns on the previous phase)
-    int ns = env_stages >= 3 && env_stages <= T2_MAX_STAGES ? env_stages : 4;
-    while (ns > 3 && ns * stage + 2 * T2_BM * raw > budget) ns--;
-    if (ns * stage + 2 * T2_BM * raw > budget) return false;
-    int nr = raw > 0 ? (budget - ns * stage) / (T2_BM * raw) : 0;
-    if (nr > T2_MAX_RAW) nr = T2_MAX_RAW;
-    if (env_raw >= 2 && env_raw < nr && raw > 0) nr = env_raw;
-    // leftover after a full raw ring: deepen the operand ring
-    if (!(env_stages >= 3)) while (ns < T2_MAX_STAGES && (ns + 1) * stage + nr * T2_BM * raw <= budget) ns++;
-    nstages = ns; nraw = nr; smem = ns * stage + nr * T2_BM * raw + tail;
+    const int stage = T2_BM * T2_BK * 2 + BN * T2_BK * 2;
+    const int tail = 2 * T2_BM * raw + (2 * T2_MAX_STAGES + 4) * 8 + BN * 4 + 1024;       // + 1024: alignment of the ring
+    int ns = (227 * 1024 - tail) / stage;
+    if (ns > T2_MAX_STAGES) ns = T2_MAX_STAGES;
+    if (env_stages >= 2 && env_stages < ns) ns = env_stages;
+    if (ns < 2) return false;
+    nstages = ns; smem = ns * stage + tail;
     return true;
 }
 
 static bool make_tc2_plan(const ggml_b200_mul_mat_args & a, tc2_plan & pl) {
-    static const int env_mode = getenv("GGML_B200_TC_PAIR") ? atoi(getenv("GGML_B200_TC_PAIR")) : 1;     // 0 = off (one-CTA kernel everywhere)
-    if (env_mode == 0) return false;
-    // Q6_K stays on the one-CTA kernel (mmq_tc.cu): on CTA pairs its variable-lead raw units lose rows 0..15 of a tile now and then even with
-    // one launch at a time (scripts/gemm_bench_parity.py q6_K 4096 512 4096 --serial: 4 of 19 matrices), the one-CTA kernel is clean on the same
-    // pattern and as fast (45 vs 48 us).  GGML_B200_TC2_Q6K=1 puts it back on the pair kernel for study.
-    static const bool env_q6k_off = !(getenv("GGML_B200_TC2_Q6K") && atoi(getenv("GGML_B200_TC2_Q6K")) != 0);
     const bool dense = a.type == T_F16;                            // fp16 A tiles (launch_mmq_dense / launch_mmq_f16w)
     switch (a.type) {
-        case T_Q4_0: case T_Q8_0: case T_Q4_K: case T_Q5_K: case T_Q4_1: case T_Q5_0: case T_Q5_1: case T_IQ4_NL: case T_IQ4_XS: case T_Q2_K: case T_Q3_K: break;
-        case T_Q6_K: if (env_q6k_off) return false; break;
+        case T_Q4_0: case T_Q8_0: case T_Q4_K: case T_Q5_K: case T_Q6_K: case T_Q4_1: case T_Q5_0: case T_Q5_1: case T_IQ4_NL: case T_IQ4_XS: case T_Q2_K: case T_Q3_K: break;
         case T_F16: break;
         default: return false;
     }
     if (a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
-    // pairs pay off once a 256-row tile is mostly full and the batch fills at least a 64-column tile; smaller problems keep the one-CTA kernel
-    // (the dense path has no other tensor-core kernel: it takes every n >= 9)
-    if (a.N < (dense ? 9 : 33) || a.M < (dense ? 1 : 192) || a.K % 256 != 0 || a.K < 256) return false;
+    // n >= 9: every batch the mat-vec kernels do not take (the reference's mul_mat_q threshold, ggml-cuda.cu:1852-1875); also 5 <= n <= 8
+    // when the mat-vec kernel cannot hold that many activation records next to its weight stages (very long rows: api.cu decides);
+    // columns beyond n in the 64-wide minimum tile are zero-filled by the TMA box and never stored
+    if (a.N < (dense ? 9 : 5) || a.M < 1 || a.K % 256 != 0 || a.K < 256) return false;
     const size_t rb = dense ? (size_t)a.K * 2 : row_bytes(a.type, a.K);
     if ((dense ? (a.nb01 < rb || (a.nb01 % 16) != 0) : a.nb01 != rb) || (rb % 16) != 0 || ((uintptr_t)a.src0 & 15) != 0 || ((uintptr_t)a.src1 & 3) != 0 || (a.nb11 & 3) != 0) return false;
     if (a.M >= (1ll << 31) || a.N >= (1ll << 31) || rb >= (1ull << 31)) return false;
     if (!tc_get_encode()) return false;
     static const int env_bn = getenv("GGML_B200_TC2_BN") ? atoi(getenv("GGML_B200_TC2_BN")) : 0;
-    int BN = a.N > 128 ? 256 : a.N > 64 ? 128 : 64;
-    if (env_bn == 64 || env_bn == 128 || env_bn == 256) BN = env_bn;
+    int BN = a.N > 64 ? 128 : 64;                                  // 2 x 128 rows x 128 columns of f32 accumulators: 128 registers per thread
+    if (env_bn == 64 || env_bn == 128) BN = env_bn;
     pl.BN = BN;
     pl.n_tiles = (int)((a.N + BN - 1) / BN);
-    pl.m_tiles = (int)((a.M + 2 * T2_BM - 1) / (2 * T2_BM));
-    pl.chunks = (int)(a.K / 256);                                // raw units along K (4 K-steps of 64 weights each)
+    pl.m_tiles = (int)((a.M + T2_BM - 1) / T2_BM);
+    pl.chunks = (int)(a.K / (T2_BK * tc2_unit_ksteps(a.type)));  // units along K
     const int tiles = pl.m_tiles * pl.n_tiles;
-    const int pairs = sm_count() / 2;
-    int splitk = pairs / tiles; if (splitk < 1) splitk = 1; if (splitk > 8) splitk = 8; if (splitk > pl.chunks) splitk = pl.chunks;
+    int splitk = sm_count() / tiles; if (splitk < 1) splitk = 1; if (splitk > 8) splitk = 8; if (splitk > pl.chunks) splitk = pl.chunks;
     static const int env_splitk = getenv("GGML_B200_TC_SPLITK") ? atoi(getenv("GGML_B200_TC_SPLITK")) : 0;
     if (env_splitk > 0 && env_splitk <= pl.chunks) splitk = env_splitk;
-    if (splitk > 1 && tiles * 2 > T2_FLAGS_PER_SLOT) splitk = 1;
+    if (splitk > 1 && tiles > T2_FLAGS_PER_SLOT) splitk = 1;
     pl.splitk = splitk;
-    pl.mode = tc2_mode_for(dense);
-    if (!tc2_smem_plan(BN, dense ? 0 : tc2_raw_bytes(a.type), pl.mode, pl.nstages, pl.nraw, pl.smem)) return false;
-    pl.grid = 2 * tiles * splitk;
+    if (!tc2_smem_plan(BN, tc2_raw_bytes(a.type), pl.nstages, pl.smem)) return false;
+    pl.grid = tiles * splitk;
     pl.xb_bytes = ((size_t)a.N * a.K * 2 + 255) & ~(size_t)255;
-    pl.partial_bytes = splitk > 1 ? (size_t)tiles * 2 * (splitk - 1) * BN * T2_BM * 4 : 0;
+    pl.partial_bytes = splitk > 1 ? (size_t)tiles * (splitk - 1) * BN * T2_BM * 4 : 0;
     pl.scale_bytes = ((size_t)a.N * 4 + 255) & ~(size_t)255;
     return true;
 }
@@ -594,7 +399,7 @@ template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const t
     const size_t rb = T == T_F16 ? (size_t)a.K * 2 : row_bytes(a.type, a.K);
     alignas(64) CUtensorMap map_w, map_x;
     if constexpr (T == T_F16) {
-        // fp16 weights [M][K]: 128 x 64 tiles straight into the swizzled operand ring
+        // fp16 weights [M][K]: 256 x 64 tiles straight into the swizzled operand ring
         const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)a.M };
         const cuuint64_t strides[1] = { (cuuint64_t)a.nb01 };
         const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)T2_BM };
@@ -614,34 +419,16 @@ template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const t
     {
         const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)a.N };
         const cuuint64_t strides[1] = { (cuuint64_t)a.K * 2 };
-        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)(pl.BN / 2) };
+        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)pl.BN };
         const cuuint32_t es[2] = { 1, 1 };
         CUresult r = tc_get_encode()(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)xb, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(X) failed: %d", (int)r); return GGML_B200_ECUDA; }
     }
-    static const bool env_tma_epi_off = getenv("GGML_B200_TC2_TMA_EPI") && atoi(getenv("GGML_B200_TC2_TMA_EPI")) == 0;
-    const int stage_bytes_h = T2_BM * T2_BK * 2 + (pl.mode != 0 ? pl.BN : pl.BN / 2) * T2_BK * 2;
-    const bool tma_epi = !env_tma_epi_off && (a.M % 4) == 0 && ((uintptr_t)a.dst & 15) == 0 && (size_t)pl.nstages * stage_bytes_h >= 2 * 2 * 32 * T2_BM * 4;
-    alignas(64) CUtensorMap map_y = map_x;                         // placeholder when the bulk-store epilogue is off
-    if (tma_epi) {
-        const cuuint64_t dims[2] = { (cuuint64_t)a.M, (cuuint64_t)a.N };
-        const cuuint64_t strides[1] = { (cuuint64_t)a.M * 4 };
-        const cuuint32_t box[2] = { (cuuint32_t)T2_BM, 32 };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_y, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)a.dst, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(Y) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
-    tc2_params p;
+    tc2_params p{};
     p.y = a.dst; p.partials = partials; p.flags = flags; p.inv_scale = inv_scale; p.M = a.M; p.N = a.N;
-    p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.n_tiles; p.splitk = pl.splitk; p.units_total = pl.chunks; p.nstages = pl.nstages; p.nraw = pl.nraw;
+    p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.n_tiles; p.splitk = pl.splitk; p.units_total = pl.chunks; p.nstages = pl.nstages;
     p.w_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
-    p.tma_epi = tma_epi ? 1 : 0;
-    p.solo = pl.mode;
-    static const int env_dbg = getenv("GGML_B200_TC2_DBG") ? atoi(getenv("GGML_B200_TC2_DBG")) : 0;     // developer switches: 1 fence per stage, 2 no early weight requests, 4 per-thread raw release
-    p.dbg = env_dbg;
-    p.trace = pl.grid < T2_TRACE_CTAS / 2 ? tc2_trace_buf() : nullptr;
     static per_device_flag attr_set;
     if (!attr_set.test()) { B200_CUDA_TRY(cudaFuncSetAttribute(mmq_tc2_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_set.set(); }
     cudaLaunchConfig_t cfg = {};
@@ -649,15 +436,15 @@ template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const t
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;             // the cluster shape is compiled in (__cluster_dims__)
-    B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, mmq_tc2_kernel<T>, map_w, map_x, map_y, p));
+    cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;
+    B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, mmq_tc2_kernel<T>, map_w, map_x, p));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
 int launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
     tc2_plan pl;
-    if (!make_tc2_plan(a, pl)) { set_error("mul_mat: shape not eligible for the CTA-pair tcgen05 kernel"); return GGML_B200_EUNSUPPORTED; }
+    if (!make_tc2_plan(a, pl)) { set_error("mul_mat: shape not eligible for the tensor-core kernel"); return GGML_B200_EUNSUPPORTED; }
     switch (a.type) {
         case T_Q4_0:   return launch_tc2<T_Q4_0>(a, pl, st);
         case T_Q8_0:   return launch_tc2<T_Q8_0>(a, pl, st);
@@ -671,14 +458,14 @@ int launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
         case T_IQ4_XS: return launch_tc2<T_IQ4_XS>(a, pl, st);
         case T_Q2_K:   return launch_tc2<T_Q2_K>(a, pl, st);
         case T_Q3_K:   return launch_tc2<T_Q3_K>(a, pl, st);
-        default: set_error("mul_mat: unsupported weight type %d for the tcgen05 kernel", a.type); return GGML_B200_EUNSUPPORTED;
+        default: set_error("mul_mat: unsupported weight type %d for the tensor-core kernel", a.type); return GGML_B200_EUNSUPPORTED;
     }
 }
 
 // ----------------------------------------------------------------------------- formats without an operand decoder (grid i-quants, ternary): n >= 9
 // W is dequantized to fp16 into the workspace by the bit-exact conversion kernel (dequant.cu) and the same GEMM runs with plain fp16 A tiles.
-// One extra pass over W (2 bytes per weight written, then read N / BN times), against the generic kernel's one warp per output element:
-// 7.2-10.6 ms -> see profiles/r02_results.md at 4096 x 14336 x 512.  Replaces the reference's dequantize + cuBLAS route
+// One extra pass over W (2 bytes per weight written, then read N / BN times), against the generic kernel's one warp per output element.
+// Replaces the reference's dequantize + cuBLAS route
 // (src/ggml-cuda/ggml-cuda.cu:1158-1300) for these formats.
 static bool dense_source_type(int t) {
     switch (t) {
@@ -745,7 +532,7 @@ int launch_mmq_f16w(const void * w, size_t nb01, const float * x, size_t nb11, f
 // The reference groups the rows per expert on the HOST (ids copied back, stream synchronised: src/ggml-cuda/ggml-cuda.cu:1975-2090; the CPU
 // backend builds matrix_rows the same way, src/ggml-cpu/ggml-cpu.c:7679-7694).  Here the grouping stays on the device: one small kernel counts
 // the (token, slot) pairs per expert, scans, and scatters the pair indices into a position list sorted by expert; the activation conversion
-// writes row `position`; the pair GEMM runs over a worst-case tile grid whose tiles look their expert / position range up in the device
+// writes row `position`; the GEMM runs over a worst-case tile grid whose tiles look their expert / position range up in the device
 // tables, streaming every expert's weights once per 256-row tile instead of once per pair.  No host synchronisation anywhere.
 constexpr int MMID_MAX_EXPERTS = 1024;
 __global__ void __launch_bounds__(1024) mmid_group_kernel(const uint8_t * ids, size_t ids_nb1, int n_tok, int n_used, int n_expert, int BN,
@@ -804,10 +591,10 @@ __global__ void __launch_bounds__(256) mmid_x_to_f16_kernel(const uint8_t * __re
     }
 }
 
-struct mmid_g_plan { int BN, m_tiles, max_tiles, chunks, nstages, nraw, smem, mode; size_t xb_bytes, scale_bytes, tab_bytes, perm_bytes; int64_t n_pairs; };
+struct mmid_g_plan { int BN, m_tiles, max_tiles, chunks, nstages, smem; size_t xb_bytes, scale_bytes, tab_bytes, perm_bytes; int64_t n_pairs; };
 
 static bool make_mmid_g_plan(const ggml_b200_mul_mat_id_args & a, mmid_g_plan & pl) {
-    static const int env_on = getenv("GGML_B200_MMID_GROUPED") ? atoi(getenv("GGML_B200_MMID_GROUPED")) : 0;      // passes tests/gpu_mmid_grouped_check.py on a B200; opt-in until the reference's whole MUL_MAT_ID sweep has run with it
+    static const int env_on = getenv("GGML_B200_MMID_GROUPED") ? atoi(getenv("GGML_B200_MMID_GROUPED")) : 0;      // opt-in until the reference's whole MUL_MAT_ID sweep has run with it (tests/gpu_mmid_grouped_check.py checks it)
     if (!env_on) return false;
     switch (a.type) {
         case T_Q4_0: case T_Q8_0: case T_Q4_K: case T_Q5_K: case T_Q6_K: case T_Q4_1: case T_Q5_0: case T_Q5_1: case T_IQ4_NL: case T_IQ4_XS: case T_Q2_K: case T_Q3_K: break;
@@ -821,13 +608,12 @@ static bool make_mmid_g_plan(const ggml_b200_mul_mat_id_args & a, mmid_g_plan & 
     if (a.n_expert * a.M >= (1ll << 31) || n_pairs >= (1ll << 30) || !tc_get_encode()) return false;
     // tile width: the average group size decides (Mixtral-like 8 x 2 at 512 tokens -> 128 per expert)
     const int64_t avg = n_pairs / (a.n_expert > 0 ? a.n_expert : 1);
-    pl.BN = avg > 160 ? 256 : avg > 80 ? 128 : 64;
-    pl.m_tiles = (int)((a.M + 2 * T2_BM - 1) / (2 * T2_BM));
+    pl.BN = avg > 80 ? 128 : 64;
+    pl.m_tiles = (int)((a.M + T2_BM - 1) / T2_BM);
     pl.max_tiles = (int)((n_pairs + pl.BN - 1) / pl.BN + a.n_expert);
-    pl.chunks = (int)(a.K / 256);
-    pl.mode = tc2_mode_for(false);
-    if (!tc2_smem_plan(pl.BN, tc2_raw_bytes(a.type), pl.mode, pl.nstages, pl.nraw, pl.smem)) return false;
-    if ((int64_t)pl.m_tiles * pl.max_tiles * 2 > 0x7fffffffLL) return false;
+    pl.chunks = (int)(a.K / (T2_BK * tc2_unit_ksteps(a.type)));
+    if (!tc2_smem_plan(pl.BN, tc2_raw_bytes(a.type), pl.nstages, pl.smem)) return false;
+    if ((int64_t)pl.m_tiles * pl.max_tiles > 0x7fffffffLL) return false;
     pl.n_pairs = n_pairs;
     pl.xb_bytes = ((size_t)(n_pairs + pl.BN) * a.K * 2 + 255) & ~(size_t)255;        // + one tile of slack rows (read past the last position, never used)
     pl.scale_bytes = ((size_t)(n_pairs + pl.BN) * 4 + 255) & ~(size_t)255;
@@ -869,7 +655,7 @@ template <int T> static int launch_mmid_g(const ggml_b200_mul_mat_id_args & a, c
     {
         const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)(pl.n_pairs + pl.BN) };
         const cuuint64_t strides[1] = { (cuuint64_t)a.K * 2 };
-        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)(pl.BN / 2) };
+        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)pl.BN };
         const cuuint32_t es[2] = { 1, 1 };
         CUresult r = tc_get_encode()(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)xb, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -877,12 +663,12 @@ template <int T> static int launch_mmid_g(const ggml_b200_mul_mat_id_args & a, c
     }
     tc2_params p{};
     p.y = a.dst; p.partials = nullptr; p.flags = nullptr; p.inv_scale = inv_scale; p.M = a.M; p.N = pl.n_pairs;
-    p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.max_tiles; p.splitk = 1; p.units_total = pl.chunks; p.nstages = pl.nstages; p.nraw = pl.nraw; p.w_static = 0; p.tma_epi = 0; p.solo = pl.mode; p.dbg = 0;
+    p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.max_tiles; p.splitk = 1; p.units_total = pl.chunks; p.nstages = pl.nstages; p.w_static = 0;
     p.g_off = off; p.g_tile_base = tile_base; p.g_perm = perm; p.n_expert = (int32_t)a.n_expert;
     static per_device_flag attr_set;
     if (!attr_set.test()) { B200_CUDA_TRY(cudaFuncSetAttribute(mmq_tc2_kernel<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_set.set(); }
     // plain launch (no programmatic dependency): the tile tables are read at kernel entry and must be complete
-    mmq_tc2_kernel<T, true><<<(unsigned)(2 * pl.m_tiles * pl.max_tiles), T2_THREADS, (size_t)pl.smem, st>>>(map_w, map_x, map_x, p);
+    mmq_tc2_kernel<T, true><<<(unsigned)(pl.m_tiles * pl.max_tiles), T2_THREADS, (size_t)pl.smem, st>>>(map_w, map_x, p);
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

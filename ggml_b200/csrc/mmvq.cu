@@ -1,4 +1,4 @@
-// mmvq.cu — quantized mat-vec kernels (n <= 8 activation columns) for sm_100a.
+// mmvq.cu — quantized mat-vec kernels (n <= 8 activation columns) for sm_90a.
 //
 // Replaces the reference's mul_mat_vec_q (src/ggml-cuda/mmvq.cu:50-130) + quantize_q8_1
 // (src/ggml-cuda/quantize.cu:4-38) and computes what ggml_compute_forward_mul_mat

@@ -15,7 +15,7 @@
 // Activations: quantized ONCE per launch by a small pre-kernel (mma_quantize_kernel, chained with programmatic dependent launch) into
 // planar per-column records (int8 codes + block sums + scales, as ggml-cpu quantizes them) in the workspace; every CTA of the main
 // kernel pulls them into shared memory with one bulk copy per column while its first weight stages are in flight.  (First version:
-// every CTA quantized all columns itself -- 3.4 us per column at K = 14336, on the critical path of every CTA.)
+// every CTA quantized all columns itself, on the critical path of every CTA.)
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_sb_ptx.cuh"
@@ -202,14 +202,13 @@ template <int T> static bool make_mma_plan(const ggml_b200_mul_mat_args & a, mma
     p.counters = nullptr; p.rec_global = nullptr;
     p.src0_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
     p.src1_static = (a.flags & GGML_B200_MM_SRC1_STATIC) ? 1 : 0;
-    static const int e_l2_mb = getenv("GGML_B200_SB_L2_MB") ? atoi(getenv("GGML_B200_SB_L2_MB")) : 48;
+    static const int e_l2_mb = getenv("GGML_B200_SB_L2_MB") ? atoi(getenv("GGML_B200_SB_L2_MB")) : 8;      // L2 prefetch cap: see mmvq_sb.cu
     p.l2_prefetch_bytes = (p.src0_static && e_l2_mb > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)e_l2_mb << 20) : 0;
     // slices of KS tasks (a multiple of the warp count): whole rows when at least three such stages fit next to the records
     static const int e_ks = getenv("GGML_B200_MMA_KS") ? atoi(getenv("GGML_B200_MMA_KS")) : 0;
     static const int e_stages = getenv("GGML_B200_MMA_STAGES") ? atoi(getenv("GGML_B200_MMA_STAGES")) : 0;
-    // consumer groups per CTA: 1 by default, GGML_B200_MMA_GROUPS = 2 for two independent groups.  Measured (profiles/r02_mma_small_batch.md):
-    // 16 warps on ONE tile 5-10 % slower than 8; two groups of 8 within +-8 % of one group (faster on long rows, slower on short ones) --
-    // the time per tile does not follow the warp count, i.e. the consume phase is bound by a per-SM rate, not by latency.
+    // consumer groups per CTA: 1 by default, GGML_B200_MMA_GROUPS = 2 for two independent groups (the consume phase is bound by a per-SM
+    // rate, not by latency, so more warps on one tile do not help).
     static const int e_groups = getenv("GGML_B200_MMA_GROUPS") ? atoi(getenv("GGML_B200_MMA_GROUPS")) : 1;
     const size_t budget = 226 * 1024;
     for (int ng = e_groups == 2 ? 2 : 1; ng >= 1; --ng) {            // two groups when each gets a ring of >= 2 stages next to the records

@@ -1,6 +1,6 @@
 // mmvq_sb.cu — the bandwidth-path quantized mat-vec (1 <= n <= 8), second generation: "one lane per 256-weight task".
 //
-// Why (profiles/r01_gemv_q4k_v1.md): the first TMA kernel moved exactly the algorithmic bytes from DRAM but spent
+// Why: the first TMA kernel moved exactly the algorithmic bytes from DRAM but spent
 // 5.0 M warp-instructions on a 45 M-weight matrix (6-bit scale decode repeated per 64 weights with a run-time
 // sub-block index, activation quantization repeated by 444 small CTAs on their critical path, 12 warps per SM),
 // i.e. it was issue/latency-bound at 30 % of the HBM roofline.  Here:
@@ -320,7 +320,7 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     const size_t rb = row_bytes(a.type, a.K);
     if (a.nb01 != rb || ((uintptr_t)a.src0 & 15) != 0 || ((uintptr_t)a.src1 & 3) != 0) return false;
     if ((a.M * rb) % 16 != 0) return false;
-    // Two operating points (profiles/r01_gemv_q4k_final.md): launches flagged independent of their predecessor (SRC1_STATIC) run as
+    // Two operating points: launches flagged independent of their predecessor (SRC1_STATIC) run as
     // small CTAs (4 consumer warps, 18 KB stages) of which four launches share an SM, a deep pipeline ACROSS launches; a dependent
     // launch wants its prologue short and its prefetch deep: 8 consumer warps, 36 KB stages, two launches per SM, W pulled into L2.
     const bool ind = (a.flags & GGML_B200_MM_SRC1_STATIC) != 0 && a.N == 1;
@@ -329,16 +329,18 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     static const int env_ctas   = getenv("GGML_B200_SB_CTAS")     ? atoi(getenv("GGML_B200_SB_CTAS"))     : 1;
     static const int e_warps    = getenv("GGML_B200_SB_WARPS")    ? atoi(getenv("GGML_B200_SB_WARPS"))    : 0;
     static const int e_resident = getenv("GGML_B200_SB_RESIDENT") ? atoi(getenv("GGML_B200_SB_RESIDENT")) : 0;
-    static const int e_l2_mb    = getenv("GGML_B200_SB_L2_MB")    ? atoi(getenv("GGML_B200_SB_L2_MB"))    : 48;
+    // L2 prefetch cap of dependent launches: 8 MB of the H100's 50 MB L2 (GGML_B200_SB_L2_MB=<MB> python scripts/gemv_sweep.py on an H100:
+    // q4_K n = 1 and n = 8 dependent launches 12-17 % faster than with 48 MB, within a few % of no prefetch)
+    static const int e_l2_mb    = getenv("GGML_B200_SB_L2_MB")    ? atoi(getenv("GGML_B200_SB_L2_MB"))    : 8;
     const int env_warps    = e_warps    ? e_warps    : (ind ? 4 : 8);
     const int env_resident = e_resident ? e_resident : (ind ? 4 : 2);
     const int env_stage_kb = e_stage_kb ? e_stage_kb : (ind ? 18 : 36);
     const int SB_CONSUMER_WARPS = (env_warps == 4 && nc == 1) ? 4 : 8;
     pl.nw = SB_CONSUMER_WARPS;
     constexpr int RPW = 32 / F::LPR;
-    // two rows per lane group sharing the activation loads (Q4_K / Q5_K, n = 1): measured on the dependent chain of the headline shape
-    // 8.0 -> 6.6 us (the consume phase is bounded by shared-memory traffic, 60 % of which are activation reads), but 4.43 -> 4.83 us for
-    // independent launches (fewer co-resident CTAs): default for DEPENDENT launches with enough tasks per row.  GGML_B200_SB_TWOROW = 0 off, 1 always
+    // two rows per lane group sharing the activation loads (Q4_K / Q5_K, n = 1): faster on dependent launches (the consume phase is bounded by
+    // shared-memory traffic, most of it activation reads), slower for independent launches (fewer co-resident CTAs): default for DEPENDENT
+    // launches with enough tasks per row.  GGML_B200_SB_TWOROW = 0 off, 1 always
     static const int e_two = getenv("GGML_B200_SB_TWOROW") ? atoi(getenv("GGML_B200_SB_TWOROW")) : 2;
     pl.two = nc == 1 && (T == T_Q4_K || T == T_Q5_K) && (e_two == 1 || (e_two == 2 && !ind && a.K >= 2048 && a.M >= 2048 && (size_t)(SB_CONSUMER_WARPS * RPW * 2) * rb <= 100 * 1024));
     int granule = 1; while ((granule * rb) % 16 != 0) granule *= 2;

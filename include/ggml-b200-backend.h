@@ -27,7 +27,7 @@ GGML_B200_API ggml_backend_t             ggml_backend_b200_init(int device);
 GGML_B200_API bool                       ggml_backend_is_b200(ggml_backend_t backend);
 GGML_B200_API ggml_backend_buffer_type_t ggml_backend_b200_buffer_type(int device);
 GGML_B200_API ggml_backend_buffer_type_t ggml_backend_b200_host_buffer_type(void);
-/* weights split by rows over every visible B200 (tensor_split: relative shares per device, NULL = equal), MUL_MAT only; the same thing is
+/* weights split by rows over every visible GPU (tensor_split: relative shares per device, NULL = equal), MUL_MAT only; the same thing is
  * returned by ggml_backend_reg_get_proc_address(reg, "ggml_backend_split_buffer_type") (reference: ggml_backend_cuda_split_buffer_type,
  * src/ggml-cuda/ggml-cuda.cu:1000) */
 GGML_B200_API ggml_backend_buffer_type_t ggml_backend_b200_split_buffer_type(int main_device, const float * tensor_split);

@@ -2,7 +2,7 @@
  *
  * Two layers, both plain C (pointers, sizes, an opaque stream handle; no torch / ggml C++ types):
  *
- *  (1) KERNEL-LAUNCH SHIM  — libggml-b200-kernels.so.  Hand-written sm_100a kernels for the hot path
+ *  (1) KERNEL-LAUNCH SHIM  — libggml-b200-kernels.so.  Hand-written sm_90a kernels for the hot path
  *      GGML_OP_MUL_MAT / GGML_OP_MUL_MAT_ID over block-quantized weights + their dequantize family.
  *      Replaces, in the reference (paths relative to the ggml tree @ 9a4acb37):
  *        ggml_cuda_op_mul_mat_vec_q   src/ggml-cuda/mmvq.cu:338      (quantized GEMV, n <= 8)
@@ -85,7 +85,7 @@ enum {
     GGML_B200_MM_AUTO        = 0,
     GGML_B200_MM_FORCE_GENERIC = 1,   /* strided one-warp-per-output kernel (any shape) */
     GGML_B200_MM_FORCE_GEMV  = 2,     /* TMA-staged bandwidth kernel (N <= 8) */
-    GGML_B200_MM_FORCE_GEMM  = 4,     /* tcgen05 tensor-core kernel */
+    GGML_B200_MM_FORCE_GEMM  = 4,     /* tensor-core (wgmma) kernel */
     GGML_B200_MM_SRC0_STATIC = 16,    /* src0 is not written by the preceding kernel on this stream (model weights): the mat-vec may
                                          prefetch it before waiting for that kernel (programmatic dependent launch) */
     GGML_B200_MM_SRC1_STATIC = 32,    /* src1 is not written by ANY kernel still in flight on this stream (inputs that were final before the
@@ -248,8 +248,7 @@ GGML_B200_API int          ggml_b200_sm_count(void);
 GGML_B200_API int          ggml_b200_prepare(void);
 /* number of kernels this library has launched since load (for bench.py's gpu_launches) */
 GGML_B200_API uint64_t     ggml_b200_launch_count(void);
-/* developer diagnostic (env GGML_B200_TC2_TRACE=1, else returns 0): copies the per-CTA %globaltimer stamps of the LAST CTA-pair GEMM launch
-   (8 per CTA: entry, prologue done, activations ready, first MMA, accumulator ready, split-K hand-over, epilogue done, exit) */
+/* developer diagnostic kept for ABI stability: the GEMM kernel records no per-CTA stamps, so this copies nothing and returns 0 */
 GGML_B200_API int          ggml_b200_debug_gemm_trace(uint64_t * host_dst, int32_t max_ctas);
 GGML_B200_API const char * ggml_b200_version(void);
 /* developer aid (GGML_B200_SB_DEBUG=1): %globaltimer stamps of CTA 0 for the last 32 mat-vec launches, 8 per launch */

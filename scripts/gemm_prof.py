@@ -1,5 +1,5 @@
 """Developer aid: one batched mul_mat shape on the tensor-core path, timed with CUDA events over CUDA-graph replays (and a plain warm loop for ncu).
-usage: python scripts/gemm_prof.py TYPE M N K [--ncu]   (env GGML_B200_TC_PAIR / TC2_BN / TC_SPLITK / TC2_STAGES select the kernel variant)"""
+usage: python scripts/gemm_prof.py TYPE M N K [--ncu]   (env GGML_B200_TC2_BN / TC_SPLITK / TC2_STAGES select the kernel variant)"""
 import os
 import sys
 from pathlib import Path
@@ -30,38 +30,6 @@ def sweep():
 for _ in range(3):
     sweep()
 torch.cuda.synchronize()
-if "--trace" in sys.argv:
-    # per-CTA timeline of the last pair-kernel launch (needs GGML_B200_TC2_TRACE=1)
-    import ctypes
-    for rep in range(2):
-        g.mul_mat(t, Ws[rep], X, M, N, K, out=Ys[rep], flags=F)
-        torch.cuda.synchronize()
-    buf = (ctypes.c_uint64 * (4096 * 8))()
-    fn = g.lib().ggml_b200_debug_gemm_trace
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int32]
-    n = fn(buf, 4096)
-    tr_all = np.frombuffer(buf, dtype=np.uint64).reshape(-1, 8).astype(np.int64)
-    acct = tr_all[2048:]
-    acct = acct[acct[:, 2] > 0]
-    tr = tr_all[:2048]
-    tr = tr[(tr[:, 0] > 0) & (tr[:, 7] >= tr[:, 0])]
-    tr = tr[tr[:, 0] > tr[:, 0].max() - 10_000_000]                       # the last launch only (stale rows of larger earlier grids dropped)
-    t0 = tr[:, 0].min()
-    names = ["entry", "prologue done", "x ready (pdl)", "first MMA", "acc ready", "splitk handover", "epilogue done", "exit"]
-    print(f"trace: {len(tr)} CTAs, kernel span {(tr[:, 7].max() - t0) / 1e3:.2f} us")
-    for e, nm in enumerate(names):
-        col = tr[:, e][tr[:, e] > 0] - t0
-        if len(col):
-            print(f"  {nm:16s} n={len(col):4d}  min {col.min() / 1e3:7.2f}  median {np.median(col) / 1e3:7.2f}  max {col.max() / 1e3:7.2f} us")
-    if len(acct):
-        an = ["g0 raw wait", "g0 empty wait", "g0 loop total", "MMA full wait (leader)", "g1 raw wait", "g1 empty wait", "g1 loop total", "B producer empty wait"]
-        print(f"cycle accounts ({len(acct)} CTAs, SM clocks):")
-        for e, nm in enumerate(an):
-            col = acct[:, e][acct[:, e] > 0]
-            if len(col):
-                print(f"  {nm:24s} n={len(col):4d}  median {np.median(col):9.0f}  max {col.max():9.0f}")
-    sys.exit(0)
 if "--ncu" in sys.argv:
     sweep()
     torch.cuda.synchronize()

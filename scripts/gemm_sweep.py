@@ -1,4 +1,4 @@
-"""Developer sweep: device time of the tcgen05 GEMM (n = 512 etc.)"""
+"""Developer sweep: device time of the tensor-core (wgmma) GEMM (n = 512 etc.)"""
 import json, sys
 from pathlib import Path
 import numpy as np, torch

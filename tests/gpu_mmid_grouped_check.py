@@ -1,5 +1,5 @@
-"""Run in a SUBPROCESS with GGML_B200_MMID_GROUPED=1: MUL_MAT_ID with the rows grouped per expert on the device and multiplied on the CTA-pair
-tcgen05 kernel (mmq_tc2.cu, GROUPED mode) against the CPU oracle; --time prints the device time of the Mixtral-like case (8 experts, 2 used,
+"""Run in a SUBPROCESS with GGML_B200_MMID_GROUPED=1: MUL_MAT_ID with the rows grouped per expert on the device and multiplied on the
+tensor-core GEMM kernel (mmq_tc2.cu, GROUPED mode) against the CPU oracle; --time prints the device time of the Mixtral-like case (8 experts, 2 used,
 512 tokens, 4096 x 4096 Q4_K) for the grouped path and for the per-pair mat-vec path.  Exit code 0 = all checks passed."""
 import os
 import sys

@@ -35,7 +35,7 @@ def main():
         z = np.load(G / f"mulmat_{name}.npz")
         for ci in range(int(z["ncases"])):
             M, N, K = (int(v) for v in z[f"shape{ci}"])
-            for flags in (g.MM_AUTO, g.MM_GENERIC):           # AUTO = superblock kernel (n <= 8) / tcgen05 GEMM (n >= 16) where eligible
+            for flags in (g.MM_AUTO, g.MM_GENERIC):           # AUTO = superblock kernel (n <= 8) / tensor-core GEMM (n >= 9) where eligible
                 Y = g.mul_mat(t, dev(z[f"W{ci}"]), dev(z[f"X{ci}"]), M, N, K, flags=flags).cpu().numpy()[0, 0]
                 tol = 1e-4 if g.mul_mat_plan(t, M, N, K, flags) == g.MM_GEMM else TOL     # fp16 operands on the tensor-core path
                 assert O.nmse(Y, z[f"Y{ci}"]) < tol, ("golden mul_mat", name, ci, flags)

@@ -1,4 +1,4 @@
-"""Run by tests/test_gpu_next_formats.py in a SUBPROCESS: the tcgen05 path for Q6_K (variable-lead TMA boxes for the 2-byte-aligned
+"""Run by tests/test_gpu_next_formats.py in a SUBPROCESS: the tensor-core GEMM path for Q6_K (variable-lead TMA boxes for the 2-byte-aligned
 210-byte superblocks) against the oracle, incl. batches of 9..15 columns.  Exit code 0 = all checks passed."""
 import os
 import sys
@@ -35,7 +35,7 @@ def main():
         err = O.nmse(Y[:, rows], want)
         assert err < 2e-5, (M, N, K, err)
     torch.cuda.synchronize()
-    print("q6_K tcgen05 GEMM OK")
+    print("q6_K tensor-core GEMM OK")
 
 
 if __name__ == "__main__":

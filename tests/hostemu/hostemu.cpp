@@ -1,7 +1,7 @@
 // hostemu.cpp — TEST INFRASTRUCTURE ONLY: the per-thread decode logic of ggml_b200/csrc (unit dot products, element decoders)
 // compiled for the host through tests/hostemu/shim, exported with a C ABI for tests/test_hostemu_kernel_logic.py.
 // It checks indexing / bit manipulation of the block formats on the CPU; it says nothing about scheduling, memory movement or
-// the PTX-level instructions (dp2a, prmt, tcgen05 ...) of the fast kernels — those are covered by the `-m gpu` parity tests.
+// the PTX-level instructions (dp2a, prmt, wgmma ...) of the fast kernels — those are covered by the `-m gpu` parity tests.
 #define B200_HOST_EMU 1
 #include "cuda_shim.h"
 #include <vector>
@@ -32,7 +32,7 @@ template <int T> static void dequant_all(const uint8_t * src, float * dst, int64
 
 #define FOR_TYPES(X) X(T_Q4_0) X(T_Q8_0) X(T_Q4_K) X(T_Q5_K) X(T_Q6_K) X(T_Q4_1) X(T_Q5_0) X(T_Q5_1) X(T_Q2_K) X(T_Q3_K) X(T_IQ4_NL) X(T_IQ4_XS) X(T_IQ2_XXS) X(T_IQ3_XXS) X(T_IQ1_S) X(T_IQ2_XS) X(T_IQ2_S) X(T_IQ3_S) X(T_IQ1_M) X(T_TQ1_0) X(T_TQ2_0)
 
-// tcgen05 GEMM operand preparation: one W row -> K fp16 values (swizzle key 0: the 8 chunks of a K-step land in order)
+// tensor-core GEMM operand preparation: one W row -> K fp16 values (swizzle key 0: the 8 chunks of a K-step land in order)
 template <int T> static void tc_row(const uint8_t * row, int64_t K, uint16_t * out) {
     constexpr int UK = tcfmt<T>::UNIT_KSTEPS, UW = tcfmt<T>::UNIT_WORDS;
     const int64_t nunits = K / (64 * UK);

@@ -1,4 +1,4 @@
-"""GPU parity: the hand-written sm_100a kernels, called through the C ABI (include/ggml-b200.h), against the CPU
+"""GPU parity: the hand-written sm_90a kernels, called through the C ABI (include/ggml-b200.h), against the CPU
 oracle on identical seeded inputs and against the reference's golden vectors.
 
 Bars: dequantize / quantize / activation quantizer are BIT-EXACT; MUL_MAT(_ID) within NMSE 1e-10 of the oracle
@@ -21,7 +21,7 @@ TOL = 1e-10
 @pytest.fixture(scope="module")
 def g():
     import torch
-    assert torch.cuda.is_available(), "these tests need a B200"
+    assert torch.cuda.is_available(), "these tests need an H100"
     import ggml_b200
     ggml_b200.lib()
     return ggml_b200
@@ -110,7 +110,7 @@ def test_mul_mat_golden(t, g):
         M, N, K = (int(v) for v in z[f"shape{ci}"])
         for flags in (g.MM_AUTO, g.MM_GENERIC):
             Y = g.mul_mat(t, dev(z[f"W{ci}"]), dev(z[f"X{ci}"]), M, N, K, flags=flags).cpu().numpy()[0, 0]
-            # the tcgen05 path (n >= 16) computes with bf16 operands: stated tolerance 1e-4 (reference gate 5e-4); int8 paths 1e-10
+            # the tensor-core path (n >= 9) computes with fp16 operands: stated tolerance 1e-4 (reference gate 5e-4); int8 paths 1e-10
             tol = 1e-4 if g.mul_mat_plan(t, M, N, K, flags) == g.MM_GEMM else TOL
             assert O.nmse(Y, z[f"Y{ci}"]) < tol, (ci, M, N, K, flags)
 
@@ -274,7 +274,7 @@ GEMM_TYPES = [O.Q4_0, O.Q8_0, O.Q4_K, O.Q5_K, O.Q6_K]
 
 @pytest.mark.parametrize("t", GEMM_TYPES, ids=[O.TYPE_NAMES[t] for t in GEMM_TYPES])
 def test_gemm_tcgen05_vs_oracle(t, g, oracle):
-    """tcgen05 path (fp16 operands, f32 TMEM accumulation).  Tolerances, stated: NMSE <= 1e-4 against the oracle (which
+    """Tensor-core GEMM path (fp16 operands, f32 accumulation by wgmma).  Tolerances, stated: NMSE <= 1e-4 against the oracle (which
     itself carries the int8 activation-quantization noise), <= 2e-5 against the exact f64 product of the dequantized
     weights; the reference's own gate is 5e-4 (tests/test-backend-ops.cpp:1915-1917)."""
     # n = 9 .. 15 (the batches between the mat-vec kernels and a full 16-column tile) run on the tensor cores too

@@ -249,7 +249,7 @@ def test_gemm_operand_dequantization_matches_oracle(t, emu, oracle):
         out = np.zeros(K, dtype=np.uint16)
         rc = emu.emu_tc_dequant_row(t, _p(wp), K, _p(out))
         if rc != 0:
-            pytest.skip("format not in the tcgen05 GEMM yet")
+            pytest.skip("format not in the tensor-core GEMM yet")
         got = out.view(np.float16).astype(np.float32)
         want = oracle.dequantize(t, w, K)
         blk = np.abs(want).reshape(-1, 32).max(1).repeat(32) + 1e-12
