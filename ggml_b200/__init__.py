@@ -397,3 +397,61 @@ def op_cpy2(src_a, dst_a, src_b, dst_b):
     L.ggml_b200_op_cpy2.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.c_void_p]
     a, b, c, d = tensor_desc(src_a), tensor_desc(dst_a), tensor_desc(src_b), tensor_desc(dst_b)
     check(L.ggml_b200_op_cpy2(C.byref(a), C.byref(b), C.byref(c), C.byref(d), _stream()), "ggml_b200_op_cpy2")
+
+
+class RopeParams(C.Structure):
+    """ggml_b200_rope_params (include/ggml-b200.h)"""
+    _fields_ = [("n_dims", C.c_int32), ("mode", C.c_int32), ("sections", C.c_int32 * 4), ("freq_scale", C.c_float), ("ext_factor", C.c_float),
+                ("mscale", C.c_float), ("theta_scale", C.c_float), ("corr_dims", C.c_float * 2)]
+
+
+ROPE_NORM, ROPE_NEOX, ROPE_MROPE, ROPE_VISION = 0, 2, 8, 24
+
+
+def _libm():
+    m = C.CDLL("libm.so.6")
+    for fn in ("powf", "logf", "floorf", "ceilf"):
+        getattr(m, fn).restype = C.c_float
+    m.powf.argtypes = [C.c_float, C.c_float]
+    m.logf.argtypes = m.floorf.argtypes = m.ceilf.argtypes = [C.c_float]
+    return m
+
+
+def rope_params(n_dims: int, mode: int = ROPE_NORM, sections=(0, 0, 0, 0), n_ctx_orig: int = 0, freq_base: float = 10000.0, freq_scale: float = 1.0,
+                ext_factor: float = 0.0, attn_factor: float = 1.0, beta_fast: float = 32.0, beta_slow: float = 1.0) -> RopeParams:
+    """the per-op constants of a ROPE node, derived as the CPU backend derives them: f32 arithmetic and the C library's powf / logf
+    (theta_scale = powf(freq_base, -2/n_dims), the YaRN corr dims of ggml_rope_yarn_corr_dims, mscale = attn_factor * (1 + 0.1 logf(1/freq_scale))
+    when ext_factor != 0).  theta_scale must be bit-exact: the kernel raises it to the power of the pair index by repeated multiplication."""
+    import numpy as np
+    f, m = np.float32, _libm()
+    p = RopeParams()
+    p.n_dims, p.mode = n_dims, mode
+    for i in range(4):
+        p.sections[i] = int(sections[i])
+    p.freq_scale, p.ext_factor = freq_scale, ext_factor
+    with np.errstate(divide="ignore", invalid="ignore"):
+        p.theta_scale = m.powf(freq_base, float(f(-2.0) / f(n_dims)))
+
+        def corr_dim(n_rot):
+            return f(f(n_dims) * f(m.logf(float(f(n_ctx_orig) / (f(n_rot) * f(2) * f(np.pi)))))) / (f(2) * f(m.logf(freq_base)))
+        start, end = m.floorf(float(corr_dim(beta_fast))), m.ceilf(float(corr_dim(beta_slow)))
+    p.corr_dims[0] = max(0.0, start)
+    p.corr_dims[1] = min(float(n_dims - 1), end)
+    ms = f(attn_factor)
+    if ext_factor != 0.0:
+        ms = ms * (f(1) + f(0.1) * f(m.logf(float(f(1) / f(freq_scale)))))
+    p.mscale = float(ms)
+    return p
+
+
+def op_rope(x, pos, params: RopeParams, freq_factors=None, inplace: bool = False):
+    """GGML_OP_ROPE on a contiguous f32 / f16 torch tensor [ne3, n_pos, n_head, ne0] (ggml order reversed) with i32 positions `pos`
+    ([n_pos], or [4 * n_pos] for MROPE / VISION) and optional f32 freq_factors; params from rope_params().  inplace: dst is x."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_rope.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.POINTER(RopeParams), C.c_void_p]
+    y = x if inplace else torch.empty_like(x)
+    s, p, d = tensor_desc(x), tensor_desc(pos), tensor_desc(y)
+    f = C.byref(tensor_desc(freq_factors)) if freq_factors is not None else None
+    check(L.ggml_b200_op_rope(C.byref(s), C.byref(p), f, C.byref(d), C.byref(params), _stream()), "ggml_b200_op_rope")
+    return y

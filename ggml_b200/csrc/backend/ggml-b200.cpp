@@ -490,6 +490,29 @@ bool supports_mul_mat_float(const ggml_tensor * op) {
     return (a->type == GGML_TYPE_F32 || a->type == GGML_TYPE_F16) && b->type == GGML_TYPE_F32 && op->type == GGML_TYPE_F32;
 }
 
+// GGML_OP_ROPE: exactly what ggml_b200_op_rope runs (the CPU backend's asserts, ggml-cpu.c:9286-9328, plus the kernel's limits)
+bool supports_rope(const ggml_tensor * op) {
+    const ggml_tensor * a = op->src[0], * pos = op->src[1], * ff = op->src[2];
+    if (!((a->type == GGML_TYPE_F32 || a->type == GGML_TYPE_F16) && op->type == a->type)) return false;
+    if (a->nb[0] != ggml_type_size(a->type) || op->nb[0] != ggml_type_size(op->type) || !ggml_are_same_shape(a, op)) return false;
+    const int n_dims = ggml_get_op_params_i32(op, 1), mode = ggml_get_op_params_i32(op, 2);
+    if (mode != 0 && mode != GGML_ROPE_TYPE_NEOX && mode != GGML_ROPE_TYPE_MROPE && mode != GGML_ROPE_TYPE_VISION) return false;
+    if (n_dims < 0 || n_dims % 2 != 0 || n_dims > a->ne[0] || a->ne[0] % 2 != 0) return false;
+    if (mode == GGML_ROPE_TYPE_VISION && 2 * (int64_t) n_dims != a->ne[0]) return false;
+    const int64_t ncache = mode == GGML_ROPE_TYPE_VISION ? n_dims : n_dims / 2;
+    if (ncache > 512) return false;
+    if (mode & GGML_ROPE_TYPE_MROPE) {
+        int32_t s[4];
+        memcpy(s, (const int32_t *) op->op_params + 11, sizeof(s));
+        if (s[0] < 0 || s[1] < 0 || s[2] < 0 || s[3] < 0 || (s[0] == 0 && s[1] == 0 && s[2] == 0)) return false;
+        if ((int64_t) s[0] + s[1] + s[2] + s[3] > a->ne[0]) return false;
+    }
+    if (pos->type != GGML_TYPE_I32 || !ggml_is_contiguous(pos) || pos->ne[0] < a->ne[2] * ((mode & GGML_ROPE_TYPE_MROPE) ? 4 : 1)) return false;
+    if (ff && (ff->type != GGML_TYPE_F32 || !ggml_is_contiguous(ff) || ff->ne[0] < ncache)) return false;
+    const int64_t heads_per_cta = std::max<int64_t>(1, 256 / std::max<int64_t>(a->ne[0], 2));     // the launcher's grid: (n_pos, head blocks, b)
+    return a->ne[2] <= INT32_MAX && a->ne[3] <= 65535 && (a->ne[1] + heads_per_cta - 1) / heads_per_cta <= 65535;
+}
+
 bool supports_small_op(const ggml_tensor * op) {
     const ggml_tensor * a = op->src[0], * b = op->src[1];
     switch (op->op) {
@@ -518,6 +541,7 @@ bool supports_small_op(const ggml_tensor * op) {
             return a->type == GGML_TYPE_F32 && (d->type == GGML_TYPE_Q8_0 || d->type == GGML_TYPE_Q4_0) && a->nb[0] == sizeof(float) &&
                    a->ne[0] % 32 == 0 && d->ne[0] % 32 == 0 && d->nb[0] == ggml_type_size(d->type) && ggml_is_contiguous(d);
         }
+        case GGML_OP_ROPE: return supports_rope(op);       // GGML_OP_ROPE_BACK (training) stays declined
         default: return false;
     }
 }
@@ -767,6 +791,26 @@ void compute_small_op(backend_ctx * ctx, ggml_tensor * node) {
         } break;
         case GGML_OP_CPY:  { auto s = desc(a), d = desc(b);    SHIM_OK(ggml_b200_op_cpy(&s, &d, st)); } break;
         case GGML_OP_CONT: case GGML_OP_DUP: { auto s = desc(a), d = desc(node); SHIM_OK(ggml_b200_op_cpy(&s, &d, st)); } break;
+        case GGML_OP_ROPE: {
+            // op_params as ggml_rope_impl writes them (read back at ggml-cpu.c:9267-9279); the constants are derived with the CPU's own expressions
+            const int32_t * ip = (const int32_t *) node->op_params;
+            float freq_base, freq_scale, ext_factor, attn_factor, beta_fast, beta_slow;
+            memcpy(&freq_base, ip + 5, sizeof(float));   memcpy(&freq_scale, ip + 6, sizeof(float));
+            memcpy(&ext_factor, ip + 7, sizeof(float));  memcpy(&attn_factor, ip + 8, sizeof(float));
+            memcpy(&beta_fast, ip + 9, sizeof(float));   memcpy(&beta_slow, ip + 10, sizeof(float));
+            ggml_b200_rope_params rp{};
+            rp.n_dims = ip[1]; rp.mode = ip[2];
+            memcpy(rp.sections, ip + 11, sizeof(rp.sections));
+            rp.freq_scale = freq_scale; rp.ext_factor = ext_factor;
+            rp.theta_scale = powf(freq_base, -2.0f / rp.n_dims);
+            ggml_rope_yarn_corr_dims(rp.n_dims, ip[4], freq_base, beta_fast, beta_slow, rp.corr_dims);
+            rp.mscale = attn_factor;
+            if (ext_factor != 0.0f) rp.mscale *= 1.0f + 0.1f * logf(1.0f / freq_scale);
+            auto s = desc(a), p = desc(b), d = desc(node);
+            ggml_b200_tensor f{};
+            if (node->src[2]) f = desc(node->src[2]);
+            SHIM_OK(ggml_b200_op_rope(&s, &p, node->src[2] ? &f : nullptr, &d, &rp, st));
+        } break;
         default:
             GGML_LOG_ERROR("ggml-b200: op %s is not supported (supports_op must have declined it)\n", ggml_op_desc(node));
             GGML_ABORT("unsupported op");

@@ -1,14 +1,17 @@
 // ops.cu — the small device ops either side of the quantized mat-mul in the examples/gpt-2 graph
 // (SURVEY.md §8f-1): GET_ROWS, ADD/MUL/SUB/DIV with broadcast, NORM / RMS_NORM, SCALE, DIAG_MASK_INF, SOFT_MAX,
-// unary GELU/SILU/RELU/…, CPY/CONT/DUP (strided, f32/f16 and f32 -> Q8_0/Q4_0), and the float (f32/f16 x f32)
-// batched strided MUL_MAT used for KQ and KQV.  They exist so that `gpt-2-backend` runs entirely on the device
-// (it has no scheduler to fall back to the CPU).  Semantics follow the CPU backend (src/ggml-cpu/ggml-cpu.c):
+// unary GELU/SILU/RELU/…, CPY/CONT/DUP (strided, f32/f16 and f32 -> Q8_0/Q4_0), the float (f32/f16 x f32)
+// batched strided MUL_MAT used for KQ and KQV, and ROPE (the rotary position embedding of llama-family decoders).  They exist so
+// that `gpt-2-backend` runs entirely on the device (it has no scheduler to fall back to the CPU).  Semantics follow the CPU
+// backend (src/ggml-cpu/ggml-cpu.c):
 //   get_rows :8560-8760   add/mul bcast :4660-5560   norm :8915-8975   rms_norm :8990-9050   scale :8300-8345
 //   diag_mask :9745-9805  soft_max :9810-9925        gelu :6520-6570 (+ fp16 table, ggml-cpu.c:1355)   dup/cpy :3220-4300
+//   rope :9157-9640
 // They replace the reference's getrows.cu, binbcast.cu, norm.cu, scale.cu, diagmask.cu, softmax.cu, unary.cu, cpy.cu, mmv.cu.
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
+#include "b200_rope.cuh"
 
 #include <cfloat>
 #include <cstdlib>
@@ -421,6 +424,51 @@ __global__ void __launch_bounds__(128) flash_attn_ext_kernel(fa_params p) {
     }
 }
 
+// ------------------------------------------------------------------ ROPE (forward; f32 -> f32, f16 -> f16; any row strides; dst may alias src)
+// One CTA per (position i2, block of heads, i3): the cos/sin of every pair at that position is computed once into shared memory (b200_rope.cuh,
+// the CPU's sequential theta product), then applied to each head of the block.  Each thread owns whole pairs (item q of a row: two elements)
+// and reads both before writing either, so the in-place form is safe.  Positions (and freq factors) are read on the device.
+template <typename T> __device__ __forceinline__ float rope_ld(const uint8_t * p) {
+    if constexpr (sizeof(T) == 4) return *(const float *)p; else return __half2float(*(const __half *)p);
+}
+template <typename T> __device__ __forceinline__ void rope_st(uint8_t * p, float v) {
+    if constexpr (sizeof(T) == 4) *(float *)p = v; else *(__half *)p = __float2half_rn(v);
+}
+template <typename T> __global__ void __launch_bounds__(128) rope_kernel(tdesc s, const int32_t * pos, const float * ff, tdesc d, rope_consts c, int heads_per_cta) {
+    pdl_trigger();
+    __shared__ float2 cache[ROPE_MAX_CACHE];
+    const int64_t i2 = blockIdx.x, i3 = blockIdx.z, ne2 = s.ne[2];
+    float p[4];
+    p[0] = (float)pos[i2];
+    if (c.mode & ROPE_MROPE) { p[1] = (float)pos[i2 + ne2]; p[2] = (float)pos[i2 + 2 * ne2]; p[3] = (float)pos[i2 + 3 * ne2]; }
+    else p[1] = p[2] = p[3] = 0.0f;
+    const int ncache = rope_n_cache(c);
+    for (int j = threadIdx.x; j < ncache; j += blockDim.x) {
+        float cs, sn;
+        rope_cos_sin(c, rope_theta(c, p, j), ff ? ff[j] : 1.0f, j, cs, sn);
+        cache[j] = make_float2(cs, sn);
+    }
+    __syncthreads();
+    const int64_t ppr = s.ne[0] / 2, h0 = (int64_t)blockIdx.y * heads_per_cta;
+    const int64_t nh = min((int64_t)heads_per_cta, s.ne[1] - h0);
+    for (int64_t it = threadIdx.x; it < nh * ppr; it += blockDim.x) {
+        const int64_t i1 = h0 + it / ppr, q = it % ppr;
+        const uint8_t * sr = s.data + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3];
+        uint8_t * dr = d.data + i1 * d.nb[1] + i2 * d.nb[2] + i3 * d.nb[3];
+        int64_t e0, e1;
+        const int slot = rope_item(c, q, e0, e1);
+        if (slot < 0) {                                        // tail beyond n_dims: copied bit for bit
+            const T a = *(const T *)(sr + e0 * sizeof(T)), b = *(const T *)(sr + e1 * sizeof(T));
+            *(T *)(dr + e0 * sizeof(T)) = a; *(T *)(dr + e1 * sizeof(T)) = b;
+            continue;
+        }
+        const float x0 = rope_ld<T>(sr + e0 * sizeof(T)), x1 = rope_ld<T>(sr + e1 * sizeof(T));
+        float y0, y1;
+        rope_rotate(x0, x1, cache[slot].x, cache[slot].y, y0, y1);
+        rope_st<T>(dr + e0 * sizeof(T), y0); rope_st<T>(dr + e1 * sizeof(T), y1);
+    }
+}
+
 static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
 } // namespace b200
@@ -592,6 +640,47 @@ int ggml_b200_op_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor
     const int64_t nout = nelem(d);
     if (nout == 0) return GGML_B200_OK;
     B200_CUDA_TRY(launch_pdl(mul_mat_f_kernel, dim3(blocks_for(nout, 4)), dim3(128), (cudaStream_t)stream, a, b, d, nout));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos, const ggml_b200_tensor * freq_factors, const ggml_b200_tensor * dst,
+                      const ggml_b200_rope_params * params, void * stream) {
+    REQUIRE(src && pos && dst && params, "src, pos, dst and params are required");
+    const tdesc s = T(src), p = T(pos), d = T(dst);
+    rope_consts c;
+    c.n_dims = params->n_dims; c.mode = params->mode;
+    for (int i = 0; i < 4; ++i) c.sections[i] = params->sections[i];
+    c.freq_scale = params->freq_scale; c.ext_factor = params->ext_factor; c.mscale = params->mscale; c.theta_scale = params->theta_scale;
+    c.corr_dims[0] = params->corr_dims[0]; c.corr_dims[1] = params->corr_dims[1];
+    REQUIRE((s.type == T_F32 || s.type == T_F16) && d.type == s.type, "src and dst must both be f32 or both f16");
+    const size_t es = s.type == T_F32 ? 4 : 2;
+    REQUIRE(s.nb[0] == es && d.nb[0] == es, "rows must be contiguous along dim 0");
+    REQUIRE(s.ne[0] == d.ne[0] && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "src and dst shapes differ");
+    REQUIRE(c.mode == ROPE_NORM || c.mode == ROPE_NEOX || c.mode == ROPE_MROPE || c.mode == ROPE_VISION, "mode must be 0, 2, 8 or 24");
+    REQUIRE(c.n_dims >= 0 && c.n_dims % 2 == 0 && c.n_dims <= s.ne[0] && s.ne[0] % 2 == 0, "n_dims must be even and <= ne0 (ne0 even)");
+    REQUIRE(c.mode != ROPE_VISION || 2 * (int64_t)c.n_dims == s.ne[0], "VISION mode needs n_dims == ne0/2");
+    if (c.mode & ROPE_MROPE) {
+        REQUIRE(c.sections[0] >= 0 && c.sections[1] >= 0 && c.sections[2] >= 0 && c.sections[3] >= 0, "sections must be >= 0");
+        REQUIRE(c.sections[0] > 0 || c.sections[1] > 0 || c.sections[2] > 0, "MROPE sections must not all be zero");
+        REQUIRE((int64_t)c.sections[0] + c.sections[1] + c.sections[2] + c.sections[3] <= s.ne[0], "MROPE sections exceed ne0");
+    }
+    const int ncache = rope_n_cache(c);
+    REQUIRE(ncache <= ROPE_MAX_CACHE, "n_dims too large (at most 1024 rotated dimensions)");
+    REQUIRE(p.type == 26 /* GGML_TYPE_I32 */ && p.nb[0] == 4 && p.ne[0] >= s.ne[2] * ((c.mode & ROPE_MROPE) ? 4 : 1), "pos must be i32, contiguous, one per position (four in MROPE)");
+    const float * ff = nullptr;
+    if (freq_factors) {
+        const tdesc f = T(freq_factors);
+        REQUIRE(f.type == T_F32 && f.nb[0] == 4 && f.ne[0] >= ncache, "freq_factors must be f32, contiguous, >= n_dims/2 entries (n_dims in VISION mode)");
+        ff = (const float *)f.data;
+    }
+    if (s.ne[0] == 0 || s.ne[1] == 0 || s.ne[2] == 0 || s.ne[3] == 0) return GGML_B200_OK;
+    const int heads_per_cta = (int)std::max<int64_t>(1, 256 / s.ne[0]);
+    const int64_t hb = (s.ne[1] + heads_per_cta - 1) / heads_per_cta;
+    REQUIRE(s.ne[2] <= 0x7fffffff && hb <= 65535 && s.ne[3] <= 65535, "too many positions / heads / batches for one grid");
+    const dim3 grid((unsigned)s.ne[2], (unsigned)hb, (unsigned)s.ne[3]);
+    if (s.type == T_F32) B200_CUDA_TRY(launch_pdl(rope_kernel<float>, grid, dim3(128), (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
+    else                 B200_CUDA_TRY(launch_pdl(rope_kernel<__half>, grid, dim3(128), (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

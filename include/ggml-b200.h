@@ -236,6 +236,23 @@ GGML_B200_API int ggml_b200_op_flash_attn_ext(const ggml_b200_tensor * q, const 
                                               const ggml_b200_tensor * dst, float scale, float max_bias, float logit_softcap, void * stream);
 /* float mat-mul: src0 f32/f16 [K, M, ne02, ne03] (any strides) x src1 f32 [K, N, ne12, ne13] -> dst f32 */
 GGML_B200_API int ggml_b200_op_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_ROPE, forward (ggml_rope_ext / ggml_rope_multi): src f32 or f16 [ne0, n_head, n_pos, b] -> dst of the same type and shape (any row
+ * strides, dim 0 contiguous; dst may be src itself).  pos i32 [n_pos] (MROPE / VISION: [4 * n_pos]) is read on the device.  freq_factors: NULL or
+ * f32 [>= n_dims/2] (VISION: >= n_dims).  The per-op constants are computed by the caller with the CPU backend's expressions:
+ * theta_scale = powf(freq_base, -2.0f/n_dims), corr_dims from ggml_rope_yarn_corr_dims, and mscale = attn_factor, multiplied by
+ * (1 + 0.1 logf(1/freq_scale)) when ext_factor != 0. */
+typedef struct ggml_b200_rope_params {
+    int32_t n_dims;        /* rotated dimensions: even, <= ne0 (VISION: == ne0/2), <= 1024 */
+    int32_t mode;          /* 0 normal (adjacent pairs), 2 NEOX (i, i + n_dims/2), 8 MROPE, 24 VISION (i, i + n_dims) */
+    int32_t sections[4];   /* MROPE / VISION: dimensions per position stream, not all zero */
+    float   freq_scale;
+    float   ext_factor;
+    float   mscale;
+    float   theta_scale;
+    float   corr_dims[2];
+} ggml_b200_rope_params;
+GGML_B200_API int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos, const ggml_b200_tensor * freq_factors, const ggml_b200_tensor * dst,
+                                    const ggml_b200_rope_params * params, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
