@@ -64,9 +64,9 @@ static int plan(const ggml_b200_mul_mat_args & a) {
     if (a.flags & GGML_B200_MM_FORCE_GENERIC) return GGML_B200_MM_FORCE_GENERIC;
     if (a.flags & GGML_B200_MM_FORCE_GEMV) {
         const bool ok = (a.flags & GGML_B200_MM_GEMV_V1) ? mmvq_tma_eligible(a) : (mma_wanted(a) || mmvq_sb_eligible(a) || mmvq_tma_eligible(a));
-        return ok ? GGML_B200_MM_FORCE_GEMV : GGML_B200_EUNSUPPORTED;
+        return ok ? (int)GGML_B200_MM_FORCE_GEMV : (int)GGML_B200_EUNSUPPORTED;
     }
-    if (a.flags & GGML_B200_MM_FORCE_GEMM) return (mmq_tc_eligible(a) || mmq_tc_eligible_small(a)) ? GGML_B200_MM_FORCE_GEMM : GGML_B200_EUNSUPPORTED;
+    if (a.flags & GGML_B200_MM_FORCE_GEMM) return (mmq_tc_eligible(a) || mmq_tc_eligible_small(a)) ? (int)GGML_B200_MM_FORCE_GEMM : (int)GGML_B200_EUNSUPPORTED;
     // 5..8 columns of very long rows: the superblock kernel would need two column-group launches (each re-streaming W, issue-bound); the
     // tensor-core kernel takes them in one pass (fp16-operand tolerance instead of the integer-exact dot: DESIGN.md section 3)
     if (a.N <= 8 && mma_wanted(a)) return GGML_B200_MM_FORCE_GEMV;

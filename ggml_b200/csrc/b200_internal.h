@@ -1,11 +1,14 @@
 // b200_internal.h — host-side plumbing shared by the kernel translation units (not part of the ABI).
 #pragma once
 
+#include <cuda.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <atomic>
 #include <cstdio>
+#include <cstdlib>
 
 #include "../../include/ggml-b200.h"
 
@@ -15,20 +18,41 @@ extern std::atomic<uint64_t> g_launches;
 void set_error(const char * fmt, ...);
 int  sm_count();
 
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a per-device setting: remember it per (kernel instantiation, device), so that a
-// process that drives several GPUs through the backend (one ggml device per GPU) configures every one of them.
-struct per_device_flag {
-    std::atomic<bool> done[64] = {};
-    static int dev() { int d = 0; if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) d = 0; return d; }
-    bool test() const { return done[dev()].load(std::memory_order_acquire); }      // setting the attribute twice is harmless: no lock needed
-    void set() { done[dev()].store(true, std::memory_order_release); }
-};
+// Programmatic dependent launch: kernels launched through launch_pdl may become resident while their predecessor on the stream still
+// runs; each one orders itself against it with griddepcontrol.wait.  The environment knob read below (= 1) launches them plainly.
+inline bool pdl_enabled() {
+    static const bool on = !(getenv("GGML_B200_NO_PDL") && atoi(getenv("GGML_B200_NO_PDL")) != 0);
+    return on;
+}
+template <typename... KArgs, typename... Args>
+cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args &... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
 
-#define B200_CUDA_TRY(expr)                                                                         \
+// Raises Kernel's dynamic shared-memory limit to `bytes`.  The attribute is a per-device setting: it is set once per (kernel, device), so
+// that a process that drives several GPUs through the backend (one ggml device per GPU) configures every one of them.  The flag is keyed
+// on the kernel itself: instantiations that share a signature each need their own.
+template <auto Kernel> cudaError_t set_max_dynamic_smem(int bytes) {
+    static std::atomic<bool> done[64] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+    if (done[dev].load(std::memory_order_acquire)) return cudaSuccess;      // setting the attribute twice is harmless: no lock needed
+    const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) done[dev].store(true, std::memory_order_release);
+    return e;
+}
+
+#define B200_CUDA_TRY(...)   /* variadic: the expression may hold template-argument commas */                \
     do {                                                                                            \
-        cudaError_t e_ = (expr);                                                                    \
+        cudaError_t e_ = (__VA_ARGS__);                                                             \
         if (e_ != cudaSuccess) {                                                                    \
-            ::b200::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(e_)); \
+            ::b200::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #__VA_ARGS__, cudaGetErrorString(e_)); \
             return GGML_B200_ECUDA;                                                                 \
         }                                                                                           \
     } while (0)
@@ -52,6 +76,10 @@ int    launch_mmvq_sb(const ggml_b200_mul_mat_args & a, cudaStream_t st, const g
 int    debug_read_trace(unsigned long long * out);
 int    prepare_device();   // allocate the per-device control block (never inside a stream capture)
 int    launch_gather_wait(const uint32_t * flags, int world, uint32_t epoch, cudaStream_t st);
+// device control block of the bandwidth kernels: [0,64) global control words, [64, 64 + 64*8) 64 per-launch scheduling slots
+unsigned int * sb_control_block();                 // nullptr on error (set_error called)
+unsigned int * sb_next_slot(unsigned int * ctl);   // the next of the 64 self-resetting scheduling slots
+int64_t l2_prefetch_cap();                         // bytes of W a dependent mat-vec launch pulls into L2 ahead of its predecessor's output
 
 // mmvq_mma.cu (bandwidth path, int8 mma.sync consume phase: 2 <= n <= 8, n = 1 on request)
 bool   mmvq_mma_eligible(const ggml_b200_mul_mat_args & a);
@@ -59,6 +87,11 @@ int    launch_mmvq_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st);
 size_t mmvq_mma_workspace(const ggml_b200_mul_mat_args & a);   // the quantized activation records (written by the pre-kernel)
 
 // mmq_tc.cu (tensor-core GEMM front end: activation conversion, dispatch)
+typedef CUresult (*encode_tiled_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
+                                    const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+encode_tiled_fn tc_get_encode();
+// activations f32 -> fp16 rows with an exact power-of-two scale per row (inv_scale[n] undoes it in the epilogue)
+int    tc_launch_x_to_f16(const float * x, size_t nb11, __half * xh, float * inv_scale, int64_t K, int64_t N, cudaStream_t st);
 bool   mmq_tc_eligible(const ggml_b200_mul_mat_args & a);
 size_t mmq_tc_workspace(const ggml_b200_mul_mat_args & a);
 bool   mmq_dense_eligible(const ggml_b200_mul_mat_args & a);   // n >= 9, formats without an operand decoder: dequantize to fp16 + the same GEMM (mmq_tc2.cu)

@@ -1,0 +1,64 @@
+// b200_ptx.cuh — device primitives shared by the kernel files (sm_90a): mbarriers, 1-D bulk copies (TMA) and the L2 bulk prefetch,
+// the async-proxy fence, programmatic dependent launch, %globaltimer, warp reductions.
+#pragma once
+#include <stdint.h>
+
+namespace b200 {
+
+__device__ __forceinline__ uint32_t smem_u32(const void * p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// ---- mbarriers
+__device__ __forceinline__ void mbar_init(uint64_t * bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t * bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t * bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "B200_WAIT:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra B200_DONE;\n"
+        "bra B200_WAIT;\n"
+        "B200_DONE:\n"
+        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+
+// ---- bulk copies
+// global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
+__device__ __forceinline__ void bulk_g2s(void * dst_smem, const void * src_gmem, uint32_t bytes, uint64_t * bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// pull a byte range into L2 without occupying shared memory (16-byte aligned address and size)
+__device__ __forceinline__ void bulk_prefetch_l2(const void * src_gmem, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
+}
+// generic-proxy stores to shared memory -> visible to the async proxy (TMA writes, wgmma operand reads)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---- programmatic dependent launch: let the next kernel's prologue start / wait for the previous kernel's results
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+__device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
+
+// ---- warp reductions (butterfly: every lane gets the result)
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+} // namespace b200

@@ -19,11 +19,28 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace b200 {
 
 // enum ggml_type ids (reference include/ggml.h:351-390)
 enum : int { T_F32 = 0, T_F16 = 1, T_Q4_0 = 2, T_Q4_1 = 3, T_Q5_0 = 6, T_Q5_1 = 7, T_Q8_0 = 8, T_Q2_K = 10, T_Q3_K = 11, T_Q4_K = 12, T_Q5_K = 13, T_Q6_K = 14, T_IQ4_NL = 20, T_IQ4_XS = 23,
               T_IQ2_XXS = 16, T_IQ3_XXS = 18, T_IQ1_S = 19, T_IQ2_XS = 17, T_IQ3_S = 21, T_IQ2_S = 22, T_IQ1_M = 29, T_TQ1_0 = 34, T_TQ2_0 = 35 };
+
+// The formats each kernel family is instantiated for.  A family's planning, workspace and launch code all dispatch through its one list.
+template <int... Ts> struct format_list {};
+// bandwidth mat-vec (mmvq_sb.cu, mmvq_mma.cu), tensor-core GEMM and grouped MUL_MAT_ID (mmq_tc2.cu)
+using TC_FORMATS = format_list<T_Q4_0, T_Q8_0, T_Q4_K, T_Q5_K, T_Q6_K, T_Q4_1, T_Q5_0, T_Q5_1, T_IQ4_NL, T_IQ4_XS, T_Q2_K, T_Q3_K>;
+// first-generation TMA mat-vec (mmvq_tma_kernel)
+using TMA_FORMATS = format_list<T_Q4_0, T_Q8_0, T_Q4_K, T_Q5_K, T_Q6_K>;
+// every block format: generic mat-vec, mmid_kernel, dequantize_kernel
+using ALL_FORMATS = format_list<T_Q4_0, T_Q8_0, T_Q4_K, T_Q5_K, T_Q6_K, T_Q4_1, T_Q5_0, T_Q5_1, T_Q2_K, T_Q3_K, T_IQ4_NL, T_IQ4_XS,
+                                T_IQ2_XXS, T_IQ3_XXS, T_IQ1_S, T_IQ2_XS, T_IQ2_S, T_IQ3_S, T_IQ1_M, T_TQ1_0, T_TQ2_0>;
+
+// Calls f(std::integral_constant<int, T>()) for the format T of the list that equals `type`; false when the list does not hold it.
+template <int... Ts, typename F> inline bool with_format(format_list<Ts...>, int type, F && f) {
+    return ((type == Ts ? (f(std::integral_constant<int, Ts>()), true) : false) || ...);
+}
 
 template <int T> struct fmt;
 template <> struct fmt<T_Q4_0> { static constexpr int QK = 32,  BYTES = 18,  ACT_K = 0; };

@@ -37,29 +37,9 @@ template <typename OUT> static int dequantize_dispatch(int type, const void * sr
     const int64_t n4 = n / 4;
     const unsigned grid = (unsigned)((n4 + 255) / 256);
     const uint8_t * s = (const uint8_t *)src;
-    switch (type) {
-        case T_Q4_0: dequantize_kernel<T_Q4_0, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q8_0: dequantize_kernel<T_Q8_0, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q4_K: dequantize_kernel<T_Q4_K, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q5_K: dequantize_kernel<T_Q5_K, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q6_K: dequantize_kernel<T_Q6_K, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q4_1: dequantize_kernel<T_Q4_1, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q5_0: dequantize_kernel<T_Q5_0, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q5_1: dequantize_kernel<T_Q5_1, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q2_K: dequantize_kernel<T_Q2_K, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_Q3_K: dequantize_kernel<T_Q3_K, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ4_NL: dequantize_kernel<T_IQ4_NL, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ4_XS: dequantize_kernel<T_IQ4_XS, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ2_XXS: dequantize_kernel<T_IQ2_XXS, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ3_XXS: dequantize_kernel<T_IQ3_XXS, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ1_S: dequantize_kernel<T_IQ1_S, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ2_XS: dequantize_kernel<T_IQ2_XS, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ2_S: dequantize_kernel<T_IQ2_S, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ3_S: dequantize_kernel<T_IQ3_S, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_IQ1_M: dequantize_kernel<T_IQ1_M, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_TQ1_0: dequantize_kernel<T_TQ1_0, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        case T_TQ2_0: dequantize_kernel<T_TQ2_0, OUT><<<grid, 256, 0, st>>>(s, dst, n4); break;
-        default: set_error("dequantize: unsupported type %d", type); return GGML_B200_EUNSUPPORTED;
+    if (!with_format(ALL_FORMATS(), type, [&](auto t) { dequantize_kernel<t, OUT><<<grid, 256, 0, st>>>(s, dst, n4); })) {
+        set_error("dequantize: unsupported type %d", type);
+        return GGML_B200_EUNSUPPORTED;
     }
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;

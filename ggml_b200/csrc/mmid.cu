@@ -8,6 +8,7 @@
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_iq.cuh"
+#include "b200_ptx.cuh"
 
 namespace b200 {
 
@@ -18,12 +19,6 @@ struct mmid_params {
     act_layout L;
     int64_t nrg;
 };
-
-__device__ __forceinline__ float warp_sum_id(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 template <int T>
 __global__ void __launch_bounds__(128) mmid_kernel(mmid_params p) {
@@ -47,7 +42,7 @@ __global__ void __launch_bounds__(128) mmid_kernel(mmid_params p) {
             if ((p.K & 63) != 0 && lane == 0) acc += tail_block_dot<T>(row + (size_t)nunits * 2 * fmt<T>::BYTES, rec, p.L, nunits * 2);
         }
     }
-    acc = warp_sum_id(acc);
+    acc = warp_sum(acc);
     if (lane == 0) p.y[(size_t)pair * p.M + m] = acc;
 }
 
@@ -86,30 +81,7 @@ int ggml_b200_mul_mat_id(const ggml_b200_mul_mat_id_args * a, void * stream) {
     p.nrg = (a->M + 3) / 4;
     const int64_t nblk = p.nrg * a->n_used * a->n_tok;
     if (nblk > 0x7fffffffLL) { set_error("mul_mat_id: grid too large"); return GGML_B200_EUNSUPPORTED; }
-    switch (a->type) {
-        case T_Q4_0: mmid_kernel<T_Q4_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q8_0: mmid_kernel<T_Q8_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q4_K: mmid_kernel<T_Q4_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q5_K: mmid_kernel<T_Q5_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q6_K: mmid_kernel<T_Q6_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q4_1: mmid_kernel<T_Q4_1><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q5_0: mmid_kernel<T_Q5_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q5_1: mmid_kernel<T_Q5_1><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q2_K: mmid_kernel<T_Q2_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q3_K: mmid_kernel<T_Q3_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ4_NL: mmid_kernel<T_IQ4_NL><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ4_XS: mmid_kernel<T_IQ4_XS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ2_XXS: mmid_kernel<T_IQ2_XXS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ3_XXS: mmid_kernel<T_IQ3_XXS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ1_S: mmid_kernel<T_IQ1_S><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ2_XS: mmid_kernel<T_IQ2_XS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ2_S: mmid_kernel<T_IQ2_S><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ3_S: mmid_kernel<T_IQ3_S><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ1_M: mmid_kernel<T_IQ1_M><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_TQ1_0: mmid_kernel<T_TQ1_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_TQ2_0: mmid_kernel<T_TQ2_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        default: return GGML_B200_EUNSUPPORTED;
-    }
+    if (!with_format(ALL_FORMATS(), a->type, [&](auto t) { mmid_kernel<t><<<(unsigned)nblk, 128, 0, st>>>(p); })) return GGML_B200_EUNSUPPORTED;
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

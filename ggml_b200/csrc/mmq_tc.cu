@@ -16,10 +16,7 @@
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_tc_dequant.cuh"   // h2u
-#include "b200_tc_ptx.cuh"
-
-#include <cuda.h>
-#include <cuda_fp16.h>
+#include "b200_ptx.cuh"
 
 #include <mutex>
 
@@ -32,8 +29,8 @@ namespace b200 {
 __global__ void __launch_bounds__(256) x_to_f16_kernel(const float * __restrict__ x, size_t nb11, __half * __restrict__ xh, float * __restrict__ inv_scale, int64_t K) {
     // programmatic dependent launch (no-ops for a plain launch): the GEMM that follows may start its prologue and its weight stream
     // now; this kernel itself waits for its predecessor (which may have produced x, and may still be reading the fp16 buffer)
-    tc_pdl_launch_dependents();
-    tc_pdl_wait();
+    pdl_launch_dependents();
+    pdl_wait();
     const int64_t n = blockIdx.x;
     const float * xr = (const float *)((const uint8_t *)x + n * nb11);
     __shared__ float s_max[8];
@@ -42,8 +39,7 @@ __global__ void __launch_bounds__(256) x_to_f16_kernel(const float * __restrict_
         const float4 a = load_f4(xr + k), b = load_f4(xr + k + 4);
         amax = fmaxf(amax, fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))), fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w)))));
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    amax = warp_max(amax);
     if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = amax;
     __syncthreads();
     amax = s_max[0];
@@ -64,14 +60,8 @@ __global__ void __launch_bounds__(256) x_to_f16_kernel(const float * __restrict_
 }
 
 // ----------------------------------------------------------------------------- host side
-int tc_launch_x_to_f16(const float * x, size_t nb11, __half * xh, float * inv_scale, int64_t K, int64_t N, cudaStream_t st, bool pdl) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)N); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, x_to_f16_kernel, x, nb11, xh, inv_scale, K));
+int tc_launch_x_to_f16(const float * x, size_t nb11, __half * xh, float * inv_scale, int64_t K, int64_t N, cudaStream_t st) {
+    B200_CUDA_TRY(launch_pdl(x_to_f16_kernel, dim3((unsigned)N), dim3(256), 0, st, x, nb11, xh, inv_scale, K));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

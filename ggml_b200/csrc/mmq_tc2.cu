@@ -79,7 +79,7 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     float * s_inv = (float *)(raw_empty + 2);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    tc_pdl_launch_dependents();
+    pdl_launch_dependents();
     // work item: partial producers (ks > 0) first, tile owners (ks == 0) last
     const int tiles = p.m_tiles * p.n_tiles;
     const int ks = p.splitk - 1 - (int)blockIdx.x / tiles;
@@ -102,9 +102,9 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     const int x_row0 = GROUPED ? gn0 : tn * p.BN;
 
     if (tid == 0) {
-        for (int s = 0; s < p.nstages; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 2); }     // producer's expect_tx; one release per warpgroup
-        for (int s = 0; s < 2; ++s) { tc_mbar_init(&raw_full[s], 1); tc_mbar_init(&raw_empty[s], T2_CONSUMERS / 32); }
-        tc_fence_init();
+        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }     // producer's expect_tx; one release per warpgroup
+        for (int s = 0; s < 2; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], T2_CONSUMERS / 32); }
+        mbar_fence_init();
         tc_prefetch_map(&map_w); tc_prefetch_map(&map_x);
     }
     __syncthreads();
@@ -115,30 +115,30 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
         if (warp == T2_CONSUMERS / 32 && lane == 0) {
             auto issue_raw = [&](int u) {
                 const int rs = u & 1;
-                tc_expect_tx(&raw_full[rs], T2_BM * RAW);
+                mbar_expect_tx(&raw_full[rs], T2_BM * RAW);
                 int coord;                                        // first 4-byte word of the box: 16-byte aligned start at or below the unit
                 if constexpr (tc2fmt<T>::LOAD_BYTES == 2) coord = (((ubeg + u) * tc2fmt<T>::UNIT_BYTES) & ~15) >> 2;   // unaligned units: lead bytes in front of the payload
                 else                        coord = (ubeg + u) * tc2fmt<T>::STRIDE_WORDS - ((ubeg + u) & 1) * tc2fmt<T>::ODD_BACK_WORDS;
                 tc_tma_2d(raw + rs * T2_BM * RAW, &map_w, coord, (int)w_row0, &raw_full[rs]);
             };
             if (!DENSE && p.w_static) issue_raw(0);               // static weights: the first unit streams while the conversion kernel runs
-            tc_pdl_wait();                                        // the fp16 activations (and non-static W) are written by the preceding kernels
+            pdl_wait();                                           // the fp16 activations (and non-static W) are written by the preceding kernels
             if (!DENSE && !p.w_static) issue_raw(0);
             for (int u = 0; u < nunits; ++u) {
                 if (!DENSE && u + 1 < nunits) {
-                    if (u + 1 >= 2) tc_wait(&raw_empty[(u + 1) & 1], (uint32_t)(((u + 1) >> 1) - 1) & 1u);
+                    if (u + 1 >= 2) mbar_wait(&raw_empty[(u + 1) & 1], (uint32_t)(((u + 1) >> 1) - 1) & 1u);
                     issue_raw(u + 1);
                 }
                 for (int q = 0; q < UK; ++q) {
                     const int step = UK * u + q, s = step % p.nstages;
-                    if (step >= p.nstages) tc_wait(&empty[s], (uint32_t)((step / p.nstages) - 1) & 1u);
+                    if (step >= p.nstages) mbar_wait(&empty[s], (uint32_t)((step / p.nstages) - 1) & 1u);
                     const int kc = ((ubeg + u) * UK + q) * T2_BK;
                     uint8_t * st = ring + s * stage_bytes;
                     if constexpr (DENSE) {
-                        tc_expect_tx(&full[s], (uint32_t)(a_bytes + b_bytes));
+                        mbar_expect_tx(&full[s], (uint32_t)(a_bytes + b_bytes));
                         tc_tma_2d(st, &map_w, kc, (int)w_row0, &full[s]);
                     } else {
-                        tc_expect_tx(&full[s], (uint32_t)b_bytes);
+                        mbar_expect_tx(&full[s], (uint32_t)b_bytes);
                     }
                     tc_tma_2d(st + a_bytes, &map_x, kc, x_row0, &full[s]);
                 }
@@ -164,7 +164,7 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     for (int u = 0; u < nunits; ++u) {
         if constexpr (!DENSE) {
             const int rs = u & 1;
-            tc_wait(&raw_full[rs], (uint32_t)(u >> 1) & 1u);
+            mbar_wait(&raw_full[rs], (uint32_t)(u >> 1) & 1u);
             int lead;                                             // bytes between the box start and the unit's first byte
             if constexpr (tc2fmt<T>::LOAD_BYTES == 2) lead = ((ubeg + u) * tc2fmt<T>::UNIT_BYTES) & 15;
             else                        lead = ((ubeg + u) & 1) * (4 * tc2fmt<T>::ODD_BACK_WORDS);
@@ -172,9 +172,9 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
             // the unit is in registers: the buffer can be refilled.  The refill is a TMA write (async proxy) after these generic-proxy reads,
             // so every reader fences before its warp releases the buffer; without the fence, Q8_0 tiles (the fastest raw-ring turnover) read
             // units that were already being overwritten whenever the release came from the last busy warp.
-            tc_fence_async_smem();
+            fence_proxy_async_smem();
             __syncwarp();
-            if (lane == 0) tc_arrive(&raw_empty[rs]);
+            if (lane == 0) mbar_arrive(&raw_empty[rs]);
         }
 #pragma unroll
         for (int q = 0; q < UK; ++q) {
@@ -183,13 +183,13 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
             if constexpr (!DENSE) {
                 // this warpgroup's rows of the stage were last read by its own MMAs of step - nstages <= step - 2: complete (wait_group 1 below)
                 if (row < p.M - row_base) tc2_dequant<T>(q, ub, st + a_row_off, sw);     // rows past M: zero-filled box, results never stored
-                tc_fence_async_smem();
+                fence_proxy_async_smem();
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
             }
-            tc_wait(&full[s], (uint32_t)(step / p.nstages) & 1u);
+            mbar_wait(&full[s], (uint32_t)(step / p.nstages) & 1u);
             wg_fence();
-            const uint64_t ad = tc_smem_desc(tc_smem(st + wg * (128 * 128)));
-            const uint64_t bd = tc_smem_desc(tc_smem(st + a_bytes));
+            const uint64_t ad = tc_smem_desc(smem_u32(st + wg * (128 * 128)));
+            const uint64_t bd = tc_smem_desc(smem_u32(st + a_bytes));
 #pragma unroll
             for (int k = 0; k < T2_BK / 16; ++k) {               // +32 bytes per K = 16; +8 KB per 64 rows (A) / 64 columns (B)
 #pragma unroll
@@ -200,7 +200,7 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
             }
             wg_commit();
             wg_wait<1>();                                         // the MMAs of step - 1 are complete: release its stage
-            if (step > 0 && (tid & 127) == 0) tc_arrive(&empty[(step - 1) % p.nstages]);
+            if (step > 0 && (tid & 127) == 0) mbar_arrive(&empty[(step - 1) % p.nstages]);
         }
     }
     wg_wait<0>();
@@ -213,7 +213,7 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
 
     // ===================== epilogue.  wgmma m64nN fragment: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8), register 4 j + 2 h + e
     // is row + 8 h, column 8 j + 2 (lane % 4) + e
-    tc_pdl_wait();                                                // inv_scale comes from the conversion kernel
+    pdl_wait();                                                   // inv_scale comes from the conversion kernel
     const int r0 = wg * 128 + ((tid & 127) >> 5) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
     const int nregs = (two_n ? 2 : 1) * 64;                       // accumulator registers per thread (partials layout: [register][thread])
     auto consumers_sync = [] { asm volatile("bar.sync 3, %0;" ::"n"(T2_CONSUMERS) : "memory"); };
@@ -312,19 +312,10 @@ struct tc2_plan {
     size_t xb_bytes, partial_bytes, scale_bytes;
 };
 
-static int tc2_raw_bytes(int type) {                                // tcfmt<T>::RAW
-    switch (type) {
-        case T_F16: return 0;
-        case T_Q5_K: case T_Q5_0: return 176;
-        case T_Q6_K: return 224;
-        case T_Q4_1: return 160;
-        case T_Q5_1: return 192;
-        case T_Q2_K: return 96;
-        case T_Q3_K: return 128;
-        default: return 144;                                         // Q4_0, Q8_0 (half units), Q4_K, IQ4_NL, IQ4_XS
-    }
+// raw-ring bytes per row and K-steps per raw unit of a format with an operand decoder; false for the other formats
+static bool tc2_unit_geometry(int type, int & raw, int & ksteps) {
+    return with_format(TC_FORMATS(), type, [&](auto t) { raw = tc2fmt<t>::RAW; ksteps = tc2fmt<t>::UNIT_KSTEPS; });
 }
-static int tc2_unit_ksteps(int type) { return type == T_F16 ? 1 : type == T_Q8_0 ? 2 : 4; }     // tc2fmt<T>::UNIT_KSTEPS
 
 // shared memory: the raw ring (2 units of 256 rows) first, then as many operand stages (>= 2: a stage is rewritten two steps after
 // its MMAs were issued, and wait_group 1 has completed them by then) as fit the 227 KB an H100 block may use
@@ -342,11 +333,8 @@ static bool tc2_smem_plan(int BN, int raw, int & nstages, int & smem) {
 
 static bool make_tc2_plan(const ggml_b200_mul_mat_args & a, tc2_plan & pl) {
     const bool dense = a.type == T_F16;                            // fp16 A tiles (launch_mmq_dense / launch_mmq_f16w)
-    switch (a.type) {
-        case T_Q4_0: case T_Q8_0: case T_Q4_K: case T_Q5_K: case T_Q6_K: case T_Q4_1: case T_Q5_0: case T_Q5_1: case T_IQ4_NL: case T_IQ4_XS: case T_Q2_K: case T_Q3_K: break;
-        case T_F16: break;
-        default: return false;
-    }
+    int raw = 0, ksteps = 1;                                       // T_F16: no raw ring, one K-step per unit
+    if (!dense && !tc2_unit_geometry(a.type, raw, ksteps)) return false;
     if (a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
     // n >= 9: every batch the mat-vec kernels do not take (the reference's mul_mat_q threshold, ggml-cuda.cu:1852-1875); also 5 <= n <= 8
     // when the mat-vec kernel cannot hold that many activation records next to its weight stages (very long rows: api.cu decides);
@@ -362,14 +350,14 @@ static bool make_tc2_plan(const ggml_b200_mul_mat_args & a, tc2_plan & pl) {
     pl.BN = BN;
     pl.n_tiles = (int)((a.N + BN - 1) / BN);
     pl.m_tiles = (int)((a.M + T2_BM - 1) / T2_BM);
-    pl.chunks = (int)(a.K / (T2_BK * tc2_unit_ksteps(a.type)));  // units along K
+    pl.chunks = (int)(a.K / (T2_BK * ksteps));                     // units along K
     const int tiles = pl.m_tiles * pl.n_tiles;
     int splitk = sm_count() / tiles; if (splitk < 1) splitk = 1; if (splitk > 8) splitk = 8; if (splitk > pl.chunks) splitk = pl.chunks;
     static const int env_splitk = getenv("GGML_B200_TC_SPLITK") ? atoi(getenv("GGML_B200_TC_SPLITK")) : 0;
     if (env_splitk > 0 && env_splitk <= pl.chunks) splitk = env_splitk;
     if (splitk > 1 && tiles > T2_FLAGS_PER_SLOT) splitk = 1;
     pl.splitk = splitk;
-    if (!tc2_smem_plan(BN, tc2_raw_bytes(a.type), pl.nstages, pl.smem)) return false;
+    if (!tc2_smem_plan(BN, raw, pl.nstages, pl.smem)) return false;
     pl.grid = tiles * splitk;
     pl.xb_bytes = ((size_t)a.N * a.K * 2 + 255) & ~(size_t)255;
     pl.partial_bytes = splitk > 1 ? (size_t)tiles * (splitk - 1) * BN * T2_BM * 4 : 0;
@@ -384,6 +372,19 @@ size_t mmq_tc2_workspace(const ggml_b200_mul_mat_args & a) {
     return pl.xb_bytes + pl.partial_bytes + pl.scale_bytes + 1024;
 }
 
+// 2-D tensor map over a row-major matrix (dims and box innermost first, row stride in bytes); false with the error set on failure
+static bool encode_2d(CUtensorMap * map, CUtensorMapDataType dtype, const void * base, uint64_t cols, uint64_t rows, uint64_t row_stride,
+                      uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle, const char * what) {
+    const cuuint64_t dims[2] = { cols, rows };
+    const cuuint64_t strides[1] = { row_stride };
+    const cuuint32_t box[2] = { box_cols, box_rows };
+    const cuuint32_t es[2] = { 1, 1 };
+    const CUresult r = tc_get_encode()(map, dtype, 2, (void *)base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); return false; }
+    return true;
+}
+
 template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const tc2_plan & pl, cudaStream_t st) {
     const size_t need = pl.xb_bytes + pl.partial_bytes + pl.scale_bytes + 1024;
     if (!a.workspace || a.workspace_size < need) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, need); return GGML_B200_EWORKSPACE; }
@@ -393,51 +394,22 @@ template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const t
     float * inv_scale = (float *)(ws + pl.xb_bytes + pl.partial_bytes);
     unsigned int * flags = tc_flag_slot();
     if (!flags) return GGML_B200_ECUDA;
-    static const bool use_pdl = !(getenv("GGML_B200_NO_PDL") && atoi(getenv("GGML_B200_NO_PDL")) != 0);
 
-    { const int rc = tc_launch_x_to_f16(a.src1, a.nb11, xb, inv_scale, a.K, a.N, st, use_pdl); if (rc != GGML_B200_OK) return rc; }
+    { const int rc = tc_launch_x_to_f16(a.src1, a.nb11, xb, inv_scale, a.K, a.N, st); if (rc != GGML_B200_OK) return rc; }
     const size_t rb = T == T_F16 ? (size_t)a.K * 2 : row_bytes(a.type, a.K);
     alignas(64) CUtensorMap map_w, map_x;
-    if constexpr (T == T_F16) {
-        // fp16 weights [M][K]: 256 x 64 tiles straight into the swizzled operand ring
-        const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)a.M };
-        const cuuint64_t strides[1] = { (cuuint64_t)a.nb01 };
-        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)T2_BM };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)a.src0, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(W fp16) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    } else {
-        const cuuint64_t dims[2] = { (cuuint64_t)(rb / 4), (cuuint64_t)a.M };
-        const cuuint64_t strides[1] = { (cuuint64_t)rb };
-        const cuuint32_t box[2] = { (cuuint32_t)(tc2fmt<T>::RAW / 4), (cuuint32_t)T2_BM };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void *)a.src0, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(W) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
-    {
-        const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)a.N };
-        const cuuint64_t strides[1] = { (cuuint64_t)a.K * 2 };
-        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)pl.BN };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)xb, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(X) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
+    bool ok;
+    if constexpr (T == T_F16)       // fp16 weights [M][K]: 256 x 64 tiles straight into the swizzled operand ring
+        ok = encode_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a.src0, a.K, a.M, a.nb01, T2_BK, T2_BM, CU_TENSOR_MAP_SWIZZLE_128B, "W fp16");
+    else
+        ok = encode_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT32, a.src0, rb / 4, a.M, rb, tc2fmt<T>::RAW / 4, T2_BM, CU_TENSOR_MAP_SWIZZLE_NONE, "W");
+    if (!ok || !encode_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, xb, a.K, a.N, a.K * 2, T2_BK, pl.BN, CU_TENSOR_MAP_SWIZZLE_128B, "X")) return GGML_B200_ECUDA;
     tc2_params p{};
     p.y = a.dst; p.partials = partials; p.flags = flags; p.inv_scale = inv_scale; p.M = a.M; p.N = a.N;
     p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.n_tiles; p.splitk = pl.splitk; p.units_total = pl.chunks; p.nstages = pl.nstages;
     p.w_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
-    static per_device_flag attr_set;
-    if (!attr_set.test()) { B200_CUDA_TRY(cudaFuncSetAttribute(mmq_tc2_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_set.set(); }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)pl.grid); cfg.blockDim = dim3(T2_THREADS); cfg.dynamicSmemBytes = (size_t)pl.smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;
-    B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, mmq_tc2_kernel<T>, map_w, map_x, p));
+    B200_CUDA_TRY(set_max_dynamic_smem<mmq_tc2_kernel<T>>(227 * 1024));
+    B200_CUDA_TRY(launch_pdl(mmq_tc2_kernel<T>, dim3((unsigned)pl.grid), dim3(T2_THREADS), (size_t)pl.smem, st, map_w, map_x, p));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -445,21 +417,12 @@ template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const t
 int launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
     tc2_plan pl;
     if (!make_tc2_plan(a, pl)) { set_error("mul_mat: shape not eligible for the tensor-core kernel"); return GGML_B200_EUNSUPPORTED; }
-    switch (a.type) {
-        case T_Q4_0:   return launch_tc2<T_Q4_0>(a, pl, st);
-        case T_Q8_0:   return launch_tc2<T_Q8_0>(a, pl, st);
-        case T_Q4_K:   return launch_tc2<T_Q4_K>(a, pl, st);
-        case T_Q5_K:   return launch_tc2<T_Q5_K>(a, pl, st);
-        case T_Q6_K:   return launch_tc2<T_Q6_K>(a, pl, st);
-        case T_Q4_1:   return launch_tc2<T_Q4_1>(a, pl, st);
-        case T_Q5_0:   return launch_tc2<T_Q5_0>(a, pl, st);
-        case T_Q5_1:   return launch_tc2<T_Q5_1>(a, pl, st);
-        case T_IQ4_NL: return launch_tc2<T_IQ4_NL>(a, pl, st);
-        case T_IQ4_XS: return launch_tc2<T_IQ4_XS>(a, pl, st);
-        case T_Q2_K:   return launch_tc2<T_Q2_K>(a, pl, st);
-        case T_Q3_K:   return launch_tc2<T_Q3_K>(a, pl, st);
-        default: set_error("mul_mat: unsupported weight type %d for the tensor-core kernel", a.type); return GGML_B200_EUNSUPPORTED;
+    int rc = GGML_B200_OK;
+    if (!with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_tc2<t>(a, pl, st); })) {
+        set_error("mul_mat: unsupported weight type %d", a.type);
+        return GGML_B200_EUNSUPPORTED;
     }
+    return rc;
 }
 
 // ----------------------------------------------------------------------------- formats without an operand decoder (grid i-quants, ternary): n >= 9
@@ -571,8 +534,7 @@ __global__ void __launch_bounds__(256) mmid_x_to_f16_kernel(const uint8_t * __re
         const float4 a = load_f4(xr + k), c = load_f4(xr + k + 4);
         amax = fmaxf(amax, fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))), fmaxf(fmaxf(fabsf(c.x), fabsf(c.y)), fmaxf(fabsf(c.z), fabsf(c.w)))));
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    amax = warp_max(amax);
     if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = amax;
     __syncthreads();
     amax = s_max[0];
@@ -596,10 +558,8 @@ struct mmid_g_plan { int BN, m_tiles, max_tiles, chunks, nstages, smem; size_t x
 static bool make_mmid_g_plan(const ggml_b200_mul_mat_id_args & a, mmid_g_plan & pl) {
     static const int env_on = getenv("GGML_B200_MMID_GROUPED") ? atoi(getenv("GGML_B200_MMID_GROUPED")) : 0;      // opt-in until the reference's whole MUL_MAT_ID sweep has run with it (tests/gpu_mmid_grouped_check.py checks it)
     if (!env_on) return false;
-    switch (a.type) {
-        case T_Q4_0: case T_Q8_0: case T_Q4_K: case T_Q5_K: case T_Q6_K: case T_Q4_1: case T_Q5_0: case T_Q5_1: case T_IQ4_NL: case T_IQ4_XS: case T_Q2_K: case T_Q3_K: break;
-        default: return false;
-    }
+    int raw, ksteps;
+    if (!tc2_unit_geometry(a.type, raw, ksteps)) return false;
     const int64_t n_pairs = a.n_used * a.n_tok;
     if (n_pairs < 32 || a.n_expert > MMID_MAX_EXPERTS || a.M < 128 || a.K % 256 != 0 || a.K < 256) return false;
     const size_t rb = row_bytes(a.type, a.K);
@@ -611,8 +571,8 @@ static bool make_mmid_g_plan(const ggml_b200_mul_mat_id_args & a, mmid_g_plan & 
     pl.BN = avg > 80 ? 128 : 64;
     pl.m_tiles = (int)((a.M + T2_BM - 1) / T2_BM);
     pl.max_tiles = (int)((n_pairs + pl.BN - 1) / pl.BN + a.n_expert);
-    pl.chunks = (int)(a.K / (T2_BK * tc2_unit_ksteps(a.type)));
-    if (!tc2_smem_plan(pl.BN, tc2_raw_bytes(a.type), pl.nstages, pl.smem)) return false;
+    pl.chunks = (int)(a.K / (T2_BK * ksteps));
+    if (!tc2_smem_plan(pl.BN, raw, pl.nstages, pl.smem)) return false;
     if ((int64_t)pl.m_tiles * pl.max_tiles > 0x7fffffffLL) return false;
     pl.n_pairs = n_pairs;
     pl.xb_bytes = ((size_t)(n_pairs + pl.BN) * a.K * 2 + 255) & ~(size_t)255;        // + one tile of slack rows (read past the last position, never used)
@@ -643,30 +603,14 @@ template <int T> static int launch_mmid_g(const ggml_b200_mul_mat_id_args & a, c
     B200_LAUNCH_CHECK();
     const size_t rb = row_bytes(a.type, a.K);
     alignas(64) CUtensorMap map_w, map_x;
-    {
-        const cuuint64_t dims[2] = { (cuuint64_t)(rb / 4), (cuuint64_t)(a.n_expert * a.M) };
-        const cuuint64_t strides[1] = { (cuuint64_t)rb };
-        const cuuint32_t box[2] = { (cuuint32_t)(tc2fmt<T>::RAW / 4), (cuuint32_t)T2_BM };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void *)a.src0, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(W experts) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
-    {
-        const cuuint64_t dims[2] = { (cuuint64_t)a.K, (cuuint64_t)(pl.n_pairs + pl.BN) };
-        const cuuint64_t strides[1] = { (cuuint64_t)a.K * 2 };
-        const cuuint32_t box[2] = { (cuuint32_t)T2_BK, (cuuint32_t)pl.BN };
-        const cuuint32_t es[2] = { 1, 1 };
-        CUresult r = tc_get_encode()(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)xb, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(X sorted) failed: %d", (int)r); return GGML_B200_ECUDA; }
-    }
+    if (!encode_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT32, a.src0, rb / 4, a.n_expert * a.M, rb, tc2fmt<T>::RAW / 4, T2_BM, CU_TENSOR_MAP_SWIZZLE_NONE, "W experts") ||
+        !encode_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, xb, a.K, pl.n_pairs + pl.BN, a.K * 2, T2_BK, pl.BN, CU_TENSOR_MAP_SWIZZLE_128B, "X sorted"))
+        return GGML_B200_ECUDA;
     tc2_params p{};
     p.y = a.dst; p.partials = nullptr; p.flags = nullptr; p.inv_scale = inv_scale; p.M = a.M; p.N = pl.n_pairs;
     p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.max_tiles; p.splitk = 1; p.units_total = pl.chunks; p.nstages = pl.nstages; p.w_static = 0;
     p.g_off = off; p.g_tile_base = tile_base; p.g_perm = perm; p.n_expert = (int32_t)a.n_expert;
-    static per_device_flag attr_set;
-    if (!attr_set.test()) { B200_CUDA_TRY(cudaFuncSetAttribute(mmq_tc2_kernel<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_set.set(); }
+    B200_CUDA_TRY(set_max_dynamic_smem<mmq_tc2_kernel<T, true>>(227 * 1024));
     // plain launch (no programmatic dependency): the tile tables are read at kernel entry and must be complete
     mmq_tc2_kernel<T, true><<<(unsigned)(pl.m_tiles * pl.max_tiles), T2_THREADS, (size_t)pl.smem, st>>>(map_w, map_x, p);
     B200_LAUNCH_CHECK();
@@ -676,21 +620,9 @@ template <int T> static int launch_mmid_g(const ggml_b200_mul_mat_id_args & a, c
 int launch_mmid_grouped(const ggml_b200_mul_mat_id_args & a, cudaStream_t st) {
     mmid_g_plan pl;
     if (!make_mmid_g_plan(a, pl)) { set_error("mul_mat_id: shape not eligible for the grouped tensor-core path"); return GGML_B200_EUNSUPPORTED; }
-    switch (a.type) {
-        case T_Q4_0:   return launch_mmid_g<T_Q4_0>(a, pl, st);
-        case T_Q8_0:   return launch_mmid_g<T_Q8_0>(a, pl, st);
-        case T_Q4_K:   return launch_mmid_g<T_Q4_K>(a, pl, st);
-        case T_Q5_K:   return launch_mmid_g<T_Q5_K>(a, pl, st);
-        case T_Q6_K:   return launch_mmid_g<T_Q6_K>(a, pl, st);
-        case T_Q4_1:   return launch_mmid_g<T_Q4_1>(a, pl, st);
-        case T_Q5_0:   return launch_mmid_g<T_Q5_0>(a, pl, st);
-        case T_Q5_1:   return launch_mmid_g<T_Q5_1>(a, pl, st);
-        case T_IQ4_NL: return launch_mmid_g<T_IQ4_NL>(a, pl, st);
-        case T_IQ4_XS: return launch_mmid_g<T_IQ4_XS>(a, pl, st);
-        case T_Q2_K:   return launch_mmid_g<T_Q2_K>(a, pl, st);
-        case T_Q3_K:   return launch_mmid_g<T_Q3_K>(a, pl, st);
-        default: return GGML_B200_EUNSUPPORTED;
-    }
+    int rc = GGML_B200_EUNSUPPORTED;                                 // make_mmid_g_plan accepts TC_FORMATS only
+    with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_mmid_g<t>(a, pl, st); });
+    return rc;
 }
 
 } // namespace b200

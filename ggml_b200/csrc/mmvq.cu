@@ -17,43 +17,11 @@
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_iq.cuh"
+#include "b200_ptx.cuh"
 
 #include <cstdlib>
 
 namespace b200 {
-
-// =============================================================================== PTX helpers
-__device__ __forceinline__ uint32_t smem_u32(const void * p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t * bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t * bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "B200_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra B200_DONE;\n"
-        "bra B200_WAIT;\n"
-        "B200_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// TMA bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void tma_bulk_g2s(void * dst_smem, const void * src_gmem, uint32_t bytes, uint64_t * bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // =============================================================================== activation quantizer
 template <bool KQ>
@@ -131,29 +99,9 @@ int launch_mmvq_generic(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
     const int64_t nblk = p.nrg * cols;
     if (nblk <= 0) return GGML_B200_OK;
     if (nblk > 0x7fffffffLL) { set_error("mul_mat: grid too large"); return GGML_B200_EUNSUPPORTED; }
-    switch (a.type) {
-        case T_Q4_0: mmvq_generic_kernel<T_Q4_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q8_0: mmvq_generic_kernel<T_Q8_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q4_K: mmvq_generic_kernel<T_Q4_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q5_K: mmvq_generic_kernel<T_Q5_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q6_K: mmvq_generic_kernel<T_Q6_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q4_1: mmvq_generic_kernel<T_Q4_1><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q5_0: mmvq_generic_kernel<T_Q5_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q5_1: mmvq_generic_kernel<T_Q5_1><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q2_K: mmvq_generic_kernel<T_Q2_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_Q3_K: mmvq_generic_kernel<T_Q3_K><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ4_NL: mmvq_generic_kernel<T_IQ4_NL><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ4_XS: mmvq_generic_kernel<T_IQ4_XS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ2_XXS: mmvq_generic_kernel<T_IQ2_XXS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ3_XXS: mmvq_generic_kernel<T_IQ3_XXS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ1_S: mmvq_generic_kernel<T_IQ1_S><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ2_XS: mmvq_generic_kernel<T_IQ2_XS><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ2_S: mmvq_generic_kernel<T_IQ2_S><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ3_S: mmvq_generic_kernel<T_IQ3_S><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_IQ1_M: mmvq_generic_kernel<T_IQ1_M><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_TQ1_0: mmvq_generic_kernel<T_TQ1_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        case T_TQ2_0: mmvq_generic_kernel<T_TQ2_0><<<(unsigned)nblk, 128, 0, st>>>(p); break;
-        default: set_error("mul_mat: unsupported weight type %d", a.type); return GGML_B200_EUNSUPPORTED;
+    if (!with_format(ALL_FORMATS(), a.type, [&](auto t) { mmvq_generic_kernel<t><<<(unsigned)nblk, 128, 0, st>>>(p); })) {
+        set_error("mul_mat: unsupported weight type %d", a.type);
+        return GGML_B200_EUNSUPPORTED;
     }
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
@@ -217,13 +165,13 @@ __global__ void __launch_bounds__(256) mmvq_tma_kernel(const tma_params p) {
         const int64_t row0 = (int64_t)(first + it) * p.RB;
         const int rows = (int)min((int64_t)p.RB, p.M - row0);
         const uint32_t bytes = (uint32_t)rows * (uint32_t)p.row_bytes;      // multiple of 16 by construction
-        mbar_arrive_expect_tx(&full[s], bytes);
-        tma_bulk_g2s(stages + (size_t)s * p.stage_bytes, p.w + (size_t)row0 * p.row_bytes, bytes, &full[s]);
+        mbar_expect_tx(&full[s], bytes);
+        bulk_g2s(stages + (size_t)s * p.stage_bytes, p.w + (size_t)row0 * p.row_bytes, bytes, &full[s]);
     };
 
     if (tid == 0) {
         for (int s = 0; s < p.nstages; ++s) mbar_init(&full[s], 1);
-        fence_mbar_init();
+        mbar_fence_init();
         for (int it = 0; it < p.nstages && it < mine; ++it) issue(it);
     }
     // quantize the activation column(s) while the first stages are in flight
@@ -292,7 +240,7 @@ struct tma_plan {
 };
 
 static bool make_tma_plan(const ggml_b200_mul_mat_args & a, tma_plan & pl) {
-    if (a.type != T_Q4_0 && a.type != T_Q8_0 && a.type != T_Q4_K && a.type != T_Q5_K && a.type != T_Q6_K) return false;   // the other formats: generic kernel
+    if (!with_format(TMA_FORMATS(), a.type, [](auto) {})) return false;   // the other formats: generic kernel
     if (a.N < 1 || a.N > 8 || a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
     if (a.K % 64 != 0 || a.K < 64 || a.M < 1) return false;                 // whole units; Q4_0/Q8_0 pairs 4-byte aligned
     const size_t rb = row_bytes(a.type, a.K);
@@ -351,11 +299,7 @@ bool mmvq_tma_eligible(const ggml_b200_mul_mat_args & a) {
 }
 
 template <int T, int NC, int R> static int launch_tma_inst(const tma_plan & pl, cudaStream_t st) {
-    static per_device_flag attr_set;   // per instantiation and device
-    if (!attr_set.test()) {
-        B200_CUDA_TRY(cudaFuncSetAttribute(mmvq_tma_kernel<T, NC, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr_set.set();
-    }
+    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_tma_kernel<T, NC, R>>(200 * 1024));
     mmvq_tma_kernel<T, NC, R><<<pl.grid, pl.block, pl.smem, st>>>(pl.p);
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
@@ -373,14 +317,9 @@ template <int T> static int launch_tma_type(const tma_plan & pl, cudaStream_t st
 int launch_mmvq_tma(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
     tma_plan pl;
     if (!make_tma_plan(a, pl)) { set_error("mul_mat: shape not eligible for the TMA mat-vec kernel"); return GGML_B200_EUNSUPPORTED; }
-    switch (a.type) {
-        case T_Q4_0: return launch_tma_type<T_Q4_0>(pl, st);
-        case T_Q8_0: return launch_tma_type<T_Q8_0>(pl, st);
-        case T_Q4_K: return launch_tma_type<T_Q4_K>(pl, st);
-        case T_Q5_K: return launch_tma_type<T_Q5_K>(pl, st);
-        case T_Q6_K: return launch_tma_type<T_Q6_K>(pl, st);
-        default: set_error("mul_mat: unsupported weight type %d", a.type); return GGML_B200_EUNSUPPORTED;
-    }
+    int rc = GGML_B200_EUNSUPPORTED;                                 // make_tma_plan accepts TMA_FORMATS only
+    with_format(TMA_FORMATS(), a.type, [&](auto t) { rc = launch_tma_type<t>(pl, st); });
+    return rc;
 }
 
 } // namespace b200

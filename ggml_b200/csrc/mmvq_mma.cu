@@ -18,7 +18,7 @@
 // every CTA quantized all columns itself, on the critical path of every CTA.)
 #include "b200_internal.h"
 #include "b200_quants.cuh"
-#include "b200_sb_ptx.cuh"
+#include "b200_ptx.cuh"
 #include "b200_sb_mma.cuh"
 
 #include <algorithm>
@@ -75,9 +75,9 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
 
     pdl_launch_dependents();
     if (wg == 0 && lane == 0) {
-        for (int s = 0; s < p.nstages; ++s) { sb_mbar_init(&full[s], 1); sb_mbar_init(&empty[s], GW); }
-        if (grp == 0) sb_mbar_init(rec_full, 1);
-        sb_fence_mbar_init();
+        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], GW); }
+        if (grp == 0) mbar_init(rec_full, 1);
+        mbar_fence_init();
     }
     __syncthreads();
     const int vcta = (int)blockIdx.x * NG + grp, vgrid = (int)gridDim.x * NG;
@@ -96,20 +96,20 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
             if (p.counters && valid && lane == 0) next = (int)atomicAdd(&p.counters[0], 1u) + vgrid;
             const int nsl = valid ? p.nslices : 1;
             for (int sl = 0; sl < nsl; ++sl) {
-                if (wrapped) sb_mbar_wait(&empty[s], par ^ 1u);
+                if (wrapped) mbar_wait(&empty[s], par ^ 1u);
                 if (valid) {
                     const int64_t row0 = (int64_t)tile * MMA_TILE;
                     const int rows = (int)min((int64_t)MMA_TILE, p.M - row0);
                     const int nt = min(p.ks, p.ntask_row - sl * p.ks);
                     const uint32_t seg = (uint32_t)nt * (uint32_t)F::TASK_B;
-                    if (lane == 0) { unit_of[s] = make_int2(tile, sl); sb_mbar_expect_tx(&full[s], (uint32_t)rows * seg); }
+                    if (lane == 0) { unit_of[s] = make_int2(tile, sl); mbar_expect_tx(&full[s], (uint32_t)rows * seg); }
                     __syncwarp();
                     if (lane < rows)
-                        sb_tma_g2s(stages + (size_t)s * p.stage_bytes + (size_t)lane * p.pitch,
+                        bulk_g2s(stages + (size_t)s * p.stage_bytes + (size_t)lane * p.pitch,
                                    p.w + (size_t)(row0 + lane) * p.row_bytes + (size_t)sl * p.ks * F::TASK_B, seg, &full[s]);
                 } else if (lane == 0) {
                     unit_of[s] = make_int2(-1, 0);
-                    sb_mbar_arrive(&full[s]);                       // publish the end marker
+                    mbar_arrive(&full[s]);                       // publish the end marker
                 }
                 if (++s == p.nstages) { s = 0; par ^= 1u; wrapped = true; }
             }
@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
                 const int64_t per = ((p.l2_prefetch_bytes + vgrid - 1) / vgrid + 15) & ~(int64_t)15;
                 const int64_t lo = (int64_t)vcta * per;
                 const int64_t hi = min(lo + per, p.l2_prefetch_bytes & ~(int64_t)15);
-                for (int64_t o = lo; o < hi; o += 32768) sb_prefetch_l2(p.w + o, (uint32_t)min((int64_t)32768, hi - o));
+                for (int64_t o = lo; o < hi; o += 32768) bulk_prefetch_l2(p.w + o, (uint32_t)min((int64_t)32768, hi - o));
             }
             first = false;
             if (!valid) break;
@@ -136,11 +136,11 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
     // ===== consumers: the quantized activation columns (written by the pre-kernel just before this one) -> shared memory
     if (tid == 0) {
         pdl_wait();
-        sb_mbar_expect_tx(rec_full, (uint32_t)p.ncols * (uint32_t)p.A.col_bytes);
+        mbar_expect_tx(rec_full, (uint32_t)p.ncols * (uint32_t)p.A.col_bytes);
         for (int c = 0; c < p.ncols; ++c)
-            sb_tma_g2s(rec + (size_t)c * p.A.col_bytes, p.rec_global + (size_t)c * p.A.col_bytes, (uint32_t)p.A.col_bytes, rec_full);
+            bulk_g2s(rec + (size_t)c * p.A.col_bytes, p.rec_global + (size_t)c * p.A.col_bytes, (uint32_t)p.A.col_bytes, rec_full);
     }
-    sb_mbar_wait(rec_full, 0u);
+    mbar_wait(rec_full, 0u);
 
     const int g = lane >> 2, t = lane & 3;
     const int gtid = wg * 32 + lane;                                                // thread index within the group's consumers
@@ -152,7 +152,7 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
     int buf = 0;
     int s = 0; uint32_t par = 0;                                                    // ring position: stage, parity of the round
     for (;;) {
-        sb_mbar_wait(&full[s], par);
+        mbar_wait(&full[s], par);
         const int2 unit = unit_of[s];
         if (unit.x < 0) break;
         const int nt = min(p.ks, p.ntask_row - unit.y * p.ks);
@@ -160,7 +160,7 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
         for (int i = wg; i < nt; i += GW)
             mma_task<T>(st + (size_t)i * F::TASK_B, st + (size_t)i * F::TASK_B + (size_t)8 * p.pitch, C, p.A, unit.y * p.ks + i, t, facc);
         __syncwarp();
-        if (lane == 0) sb_mbar_arrive(&empty[s]);
+        if (lane == 0) mbar_arrive(&empty[s]);
         if (++s == p.nstages) { s = 0; par ^= 1u; }
         if (unit.y == p.nslices - 1) {
             // tile finished: the group's eight partial fragments meet in shared memory and are summed in warp order
@@ -202,8 +202,8 @@ template <int T> static bool make_mma_plan(const ggml_b200_mul_mat_args & a, mma
     p.counters = nullptr; p.rec_global = nullptr;
     p.src0_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
     p.src1_static = (a.flags & GGML_B200_MM_SRC1_STATIC) ? 1 : 0;
-    static const int e_l2_mb = getenv("GGML_B200_SB_L2_MB") ? atoi(getenv("GGML_B200_SB_L2_MB")) : 8;      // L2 prefetch cap: see mmvq_sb.cu
-    p.l2_prefetch_bytes = (p.src0_static && e_l2_mb > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)e_l2_mb << 20) : 0;
+    const int64_t l2_cap = l2_prefetch_cap();
+    p.l2_prefetch_bytes = (p.src0_static && l2_cap > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)l2_cap) : 0;
     // slices of KS tasks (a multiple of the warp count): whole rows when at least three such stages fit next to the records
     static const int e_ks = getenv("GGML_B200_MMA_KS") ? atoi(getenv("GGML_B200_MMA_KS")) : 0;
     static const int e_stages = getenv("GGML_B200_MMA_STAGES") ? atoi(getenv("GGML_B200_MMA_STAGES")) : 0;
@@ -242,16 +242,9 @@ template <int T> static bool make_mma_plan(const ggml_b200_mul_mat_args & a, mma
 
 static size_t mma_rec_bytes(const mma_plan & pl) { return (size_t)pl.p.ncols * pl.p.A.col_bytes; }
 
-template <int T, int NG> static int launch_mma_ng(const mma_plan & pl, cudaStream_t st, const cudaLaunchAttribute * attr, int nattr) {
-    static per_device_flag attr_set;
-    if (!attr_set.test()) {
-        B200_CUDA_TRY(cudaFuncSetAttribute(mmvq_mma_kernel<T, NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set.set();
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(pl.grid); cfg.blockDim = dim3(NG * (MMA_GROUP_WARPS + 1) * 32); cfg.dynamicSmemBytes = pl.smem; cfg.stream = st;
-    cfg.attrs = const_cast<cudaLaunchAttribute *>(attr); cfg.numAttrs = nattr;
-    B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, mmvq_mma_kernel<T, NG>, pl.p));
+template <int T, int NG> static int launch_mma_ng(const mma_plan & pl, cudaStream_t st) {
+    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_mma_kernel<T, NG>>(227 * 1024));
+    B200_CUDA_TRY(launch_pdl(mmvq_mma_kernel<T, NG>, dim3(pl.grid), dim3(NG * (MMA_GROUP_WARPS + 1) * 32), pl.smem, st, pl.p));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -268,76 +261,35 @@ template <int T> static int launch_mma(const ggml_b200_mul_mat_args & a, cudaStr
     if (!ctl) return GGML_B200_ECUDA;
     static const bool e_dynamic = getenv("GGML_B200_MMA_DYNAMIC") && atoi(getenv("GGML_B200_MMA_DYNAMIC")) != 0;
     pl.p.counters = e_dynamic ? sb_next_slot(ctl) : nullptr;
-    static const bool use_pdl = !(getenv("GGML_B200_NO_PDL") && atoi(getenv("GGML_B200_NO_PDL")) != 0);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((unsigned)((pl.p.ncols * pl.p.A.ntask + 15) / 16)); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-        cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;
-        B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, mma_quantize_kernel<F::KQ, F::S16, mma_s81<T>::value>, a.src1, pl.p.x_stride, (int)pl.p.ncols, pl.p.A, rec));
-        B200_LAUNCH_CHECK();
-    }
-    return pl.ng == 1 ? launch_mma_ng<T, 1>(pl, st, attr, use_pdl ? 1 : 0) : launch_mma_ng<T, 2>(pl, st, attr, use_pdl ? 1 : 0);
+    B200_CUDA_TRY(launch_pdl(mma_quantize_kernel<F::KQ, F::S16, mma_s81<T>::value>, dim3((unsigned)((pl.p.ncols * pl.p.A.ntask + 15) / 16)), dim3(256), 0, st,
+                             a.src1, pl.p.x_stride, (int)pl.p.ncols, pl.p.A, rec));
+    B200_LAUNCH_CHECK();
+    return pl.ng == 1 ? launch_mma_ng<T, 1>(pl, st) : launch_mma_ng<T, 2>(pl, st);
+}
+
+static bool mma_plan_of(const ggml_b200_mul_mat_args & a, mma_plan & pl) {
+    bool ok = false;
+    with_format(TC_FORMATS(), a.type, [&](auto t) { ok = make_mma_plan<t>(a, pl); });
+    return ok;
 }
 
 size_t mmvq_mma_workspace(const ggml_b200_mul_mat_args & a) {
     mma_plan pl;
-    bool ok = false;
-    switch (a.type) {
-        case T_Q4_0: ok = make_mma_plan<T_Q4_0>(a, pl); break;
-        case T_Q8_0: ok = make_mma_plan<T_Q8_0>(a, pl); break;
-        case T_Q4_K: ok = make_mma_plan<T_Q4_K>(a, pl); break;
-        case T_Q5_K: ok = make_mma_plan<T_Q5_K>(a, pl); break;
-        case T_Q6_K: ok = make_mma_plan<T_Q6_K>(a, pl); break;
-        case T_Q5_0: ok = make_mma_plan<T_Q5_0>(a, pl); break;
-        case T_Q4_1: ok = make_mma_plan<T_Q4_1>(a, pl); break;
-        case T_Q5_1: ok = make_mma_plan<T_Q5_1>(a, pl); break;
-        case T_IQ4_NL: ok = make_mma_plan<T_IQ4_NL>(a, pl); break;
-        case T_IQ4_XS: ok = make_mma_plan<T_IQ4_XS>(a, pl); break;
-        case T_Q2_K: ok = make_mma_plan<T_Q2_K>(a, pl); break;
-        case T_Q3_K: ok = make_mma_plan<T_Q3_K>(a, pl); break;
-        default: break;
-    }
-    return ok ? mma_rec_bytes(pl) + 256 : 0;
+    return mma_plan_of(a, pl) ? mma_rec_bytes(pl) + 256 : 0;
 }
 
 bool mmvq_mma_eligible(const ggml_b200_mul_mat_args & a) {
     mma_plan pl;
-    switch (a.type) {
-        case T_Q4_0: return make_mma_plan<T_Q4_0>(a, pl);
-        case T_Q8_0: return make_mma_plan<T_Q8_0>(a, pl);
-        case T_Q4_K: return make_mma_plan<T_Q4_K>(a, pl);
-        case T_Q5_K: return make_mma_plan<T_Q5_K>(a, pl);
-        case T_Q6_K: return make_mma_plan<T_Q6_K>(a, pl);
-        case T_Q5_0: return make_mma_plan<T_Q5_0>(a, pl);
-        case T_Q4_1: return make_mma_plan<T_Q4_1>(a, pl);
-        case T_Q5_1: return make_mma_plan<T_Q5_1>(a, pl);
-        case T_IQ4_NL: return make_mma_plan<T_IQ4_NL>(a, pl);
-        case T_IQ4_XS: return make_mma_plan<T_IQ4_XS>(a, pl);
-        case T_Q2_K: return make_mma_plan<T_Q2_K>(a, pl);
-        case T_Q3_K: return make_mma_plan<T_Q3_K>(a, pl);
-        default: return false;
-    }
+    return mma_plan_of(a, pl);
 }
 
 int launch_mmvq_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
-    switch (a.type) {
-        case T_Q4_0: return launch_mma<T_Q4_0>(a, st);
-        case T_Q8_0: return launch_mma<T_Q8_0>(a, st);
-        case T_Q4_K: return launch_mma<T_Q4_K>(a, st);
-        case T_Q5_K: return launch_mma<T_Q5_K>(a, st);
-        case T_Q6_K: return launch_mma<T_Q6_K>(a, st);
-        case T_Q5_0: return launch_mma<T_Q5_0>(a, st);
-        case T_Q4_1: return launch_mma<T_Q4_1>(a, st);
-        case T_Q5_1: return launch_mma<T_Q5_1>(a, st);
-        case T_IQ4_NL: return launch_mma<T_IQ4_NL>(a, st);
-        case T_IQ4_XS: return launch_mma<T_IQ4_XS>(a, st);
-        case T_Q2_K: return launch_mma<T_Q2_K>(a, st);
-        case T_Q3_K: return launch_mma<T_Q3_K>(a, st);
-        default: set_error("mul_mat: unsupported weight type %d for the mma kernel", a.type); return GGML_B200_EUNSUPPORTED;
+    int rc = GGML_B200_OK;
+    if (!with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_mma<t>(a, st); })) {
+        set_error("mul_mat: unsupported weight type %d", a.type);
+        return GGML_B200_EUNSUPPORTED;
     }
+    return rc;
 }
 
 } // namespace b200

@@ -24,7 +24,7 @@
 // (int8 activations quantized as ggml-cpu does, integer dots, f32 scaling); only the f32 summation order differs.
 #include "b200_internal.h"
 #include "b200_quants.cuh"
-#include "b200_sb_ptx.cuh"
+#include "b200_ptx.cuh"
 #include "b200_sb_tasks.cuh"   // dp4a_us, task geometry, activation-record layout, task dot products (also compiled for the host by tests/hostemu)
 
 #include <atomic>
@@ -82,8 +82,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
     }
 
     if (tid == 0) {
-        for (int s = 0; s < p.nstages; ++s) { sb_mbar_init(&full[s], 1); sb_mbar_init(&empty[s], SB_CONSUMER_WARPS); }
-        sb_fence_mbar_init();
+        for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], SB_CONSUMER_WARPS); }
+        mbar_fence_init();
     }
     __syncthreads();
 
@@ -93,10 +93,10 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
             const int64_t row0 = (int64_t)chunk * p.rows_per_chunk;
             const int rows = (int)min((int64_t)p.rows_per_chunk, p.M - row0);
             const uint32_t bytes = (uint32_t)rows * (uint32_t)p.row_bytes;
-            sb_mbar_expect_tx(&full[s], bytes);
-            sb_tma_g2s(stages + (size_t)s * p.stage_bytes, p.w + (size_t)row0 * p.row_bytes, bytes, &full[s]);
+            mbar_expect_tx(&full[s], bytes);
+            bulk_g2s(stages + (size_t)s * p.stage_bytes, p.w + (size_t)row0 * p.row_bytes, bytes, &full[s]);
         } else {
-            sb_mbar_arrive(&full[s]);                             // publish the end marker
+            mbar_arrive(&full[s]);                             // publish the end marker
         }
     };
 
@@ -111,7 +111,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
                 const int64_t per = ((p.l2_prefetch_bytes + gridDim.x - 1) / gridDim.x + 15) & ~(int64_t)15;
                 const int64_t lo = (int64_t)blockIdx.x * per;
                 const int64_t hi = min(lo + per, p.l2_prefetch_bytes & ~(int64_t)15);
-                for (int64_t o = lo; o < hi; o += 32768) sb_prefetch_l2(p.w + o, (uint32_t)min((int64_t)32768, hi - o));
+                for (int64_t o = lo; o < hi; o += 32768) bulk_prefetch_l2(p.w + o, (uint32_t)min((int64_t)32768, hi - o));
             }
             if (dbg) dbg[1] = gtime();                            // first TMA issued
             // (the scheduling counters are per launch slot, so the producer never has to wait for the previous grid on their account)
@@ -125,7 +125,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
                 while (!done) {
                     const int s = it % p.nstages;
                     const int chunk = (int)blockIdx.x + it * (int)gridDim.x;
-                    if (it >= p.nstages) sb_mbar_wait(&empty[s], (uint32_t)((it / p.nstages) - 1) & 1u);
+                    if (it >= p.nstages) mbar_wait(&empty[s], (uint32_t)((it / p.nstages) - 1) & 1u);
                     issue(s, chunk);
                     done = chunk >= p.nchunks;
                     ++it;
@@ -135,7 +135,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
             while (!done) {
                 const int s = it % p.nstages;
                 const int chunk = (int)atomicAdd(&p.counters[0], 1u) + (int)gridDim.x;
-                if (it >= p.nstages) sb_mbar_wait(&empty[s], (uint32_t)((it / p.nstages) - 1) & 1u);
+                if (it >= p.nstages) mbar_wait(&empty[s], (uint32_t)((it / p.nstages) - 1) & 1u);
                 issue(s, chunk);
                 done = chunk >= p.nchunks;
                 ++it;
@@ -164,7 +164,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
     const int sub = lane / LPR, l = lane % LPR;
     for (int it = 0;; ++it) {
         const int s = it % p.nstages;
-        sb_mbar_wait(&full[s], (uint32_t)(it / p.nstages) & 1u);
+        mbar_wait(&full[s], (uint32_t)(it / p.nstages) & 1u);
         if (dbg && tid == 0 && it == 0) dbg[4] = gtime();        // first stage landed
         const int chunk = chunk_of[s];
         if (chunk < 0) { if (dbg && tid == 0) dbg[5] = gtime(); if (dbg_all && tid == 0) atomicMax(dbg_all + 6, gtime()); break; }   // last stage done
@@ -204,43 +204,41 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
                 for (int o = LPR / 2; o > 0; o >>= 1) { a0 += __shfl_xor_sync(0xffffffffu, a0, o); a1 += __shfl_xor_sync(0xffffffffu, a1, o); }
                 if (l == 0 && r < rows) { store_row(row0 + r, a0); if (r + 1 < rows) store_row(row0 + r + 1, a1); }
             }
-            __syncwarp();
-            if (lane == 0) sb_mbar_arrive(&empty[s]);
-            continue;
-        }
-        // the row loop is warp-uniform (both half-warps iterate together): the shuffles below use the full mask
-        for (int r0 = warp * RPW; r0 < rows; r0 += SB_CONSUMER_WARPS * RPW) {
-            const int r = r0 + sub;
-            if constexpr (NC > 1) {
-                float accn[NC];
+        } else {
+            // the row loop is warp-uniform (both half-warps iterate together): the shuffles below use the full mask
+            for (int r0 = warp * RPW; r0 < rows; r0 += SB_CONSUMER_WARPS * RPW) {
+                const int r = r0 + sub;
+                if constexpr (NC > 1) {
+                    float accn[NC];
 #pragma unroll
-                for (int c = 0; c < NC; ++c) accn[c] = 0.0f;
+                    for (int c = 0; c < NC; ++c) accn[c] = 0.0f;
+                    if (r < rows) {
+                        const uint8_t * row = st + (size_t)r * p.row_bytes;
+                        for (int t = l; t < p.ntasks_row; t += LPR) task_dot_nc<T, NC>(row + (size_t)t * F::TASK_B, rec, p.A.bytes, t, p.ncols, accn);
+                    }
+#pragma unroll
+                    for (int c = 0; c < NC; ++c) {
+#pragma unroll
+                        for (int o = LPR / 2; o > 0; o >>= 1) accn[c] += __shfl_xor_sync(0xffffffffu, accn[c], o);
+                    }
+                    if (l == 0 && r < rows) {
+#pragma unroll
+                        for (int c = 0; c < NC; ++c) if (c < p.ncols) p.y[(size_t)c * p.M + row0 + r] = accn[c];
+                    }
+                    continue;
+                }
+                float acc = 0.0f;
                 if (r < rows) {
                     const uint8_t * row = st + (size_t)r * p.row_bytes;
-                    for (int t = l; t < p.ntasks_row; t += LPR) task_dot_nc<T, NC>(row + (size_t)t * F::TASK_B, rec, p.A.bytes, t, p.ncols, accn);
+                    for (int t = l; t < p.ntasks_row; t += LPR) acc += task_dot<T>(row + (size_t)t * F::TASK_B, rec, t);
                 }
 #pragma unroll
-                for (int c = 0; c < NC; ++c) {
-#pragma unroll
-                    for (int o = LPR / 2; o > 0; o >>= 1) accn[c] += __shfl_xor_sync(0xffffffffu, accn[c], o);
-                }
-                if (l == 0 && r < rows) {
-#pragma unroll
-                    for (int c = 0; c < NC; ++c) if (c < p.ncols) p.y[(size_t)c * p.M + row0 + r] = accn[c];
-                }
-                continue;
+                for (int o = LPR / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+                if (l == 0 && r < rows) store_row(row0 + r, acc);
             }
-            float acc = 0.0f;
-            if (r < rows) {
-                const uint8_t * row = st + (size_t)r * p.row_bytes;
-                for (int t = l; t < p.ntasks_row; t += LPR) acc += task_dot<T>(row + (size_t)t * F::TASK_B, rec, t);
-            }
-#pragma unroll
-            for (int o = LPR / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-            if (l == 0 && r < rows) store_row(row0 + r, acc);
         }
         __syncwarp();
-        if (lane == 0) sb_mbar_arrive(&empty[s]);
+        if (lane == 0) mbar_arrive(&empty[s]);
     }
     // Completion must stay transitive along the stream (a later kernel's griddepcontrol.wait covers only ITS predecessor): a launch
     // whose consumers did not wait for the preceding grid (SRC1_STATIC) does so before it retires, holding no work back.
@@ -310,6 +308,13 @@ unsigned int * sb_control_block() { return sb_counters(); }
 static std::atomic<unsigned> g_sb_slot_seq{0};
 unsigned int * sb_next_slot(unsigned int * ctl) { return ctl + 64 + (g_sb_slot_seq.fetch_add(1, std::memory_order_relaxed) % 64u) * 8; }
 
+// L2 prefetch cap of dependent launches (mmvq_sb and mmvq_mma), in MB below: 8 MB of the H100's 50 MB L2 (scripts/gemv_sweep.py on an H100,
+// sweeping this knob: q4_K n = 1 and n = 8 dependent launches 12-17 % faster than with 48 MB, within a few % of no prefetch)
+int64_t l2_prefetch_cap() {
+    static const int mb = getenv("GGML_B200_SB_L2_MB") ? atoi(getenv("GGML_B200_SB_L2_MB")) : 8;
+    return mb > 0 ? (int64_t)mb << 20 : 0;
+}
+
 template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_plan & pl) {
     using F = sbfmt<T>;
     if (a.N < 1 || a.N > 8 || a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
@@ -329,9 +334,6 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     static const int env_ctas   = getenv("GGML_B200_SB_CTAS")     ? atoi(getenv("GGML_B200_SB_CTAS"))     : 1;
     static const int e_warps    = getenv("GGML_B200_SB_WARPS")    ? atoi(getenv("GGML_B200_SB_WARPS"))    : 0;
     static const int e_resident = getenv("GGML_B200_SB_RESIDENT") ? atoi(getenv("GGML_B200_SB_RESIDENT")) : 0;
-    // L2 prefetch cap of dependent launches: 8 MB of the H100's 50 MB L2 (GGML_B200_SB_L2_MB=<MB> python scripts/gemv_sweep.py on an H100:
-    // q4_K n = 1 and n = 8 dependent launches 12-17 % faster than with 48 MB, within a few % of no prefetch)
-    static const int e_l2_mb    = getenv("GGML_B200_SB_L2_MB")    ? atoi(getenv("GGML_B200_SB_L2_MB"))    : 8;
     const int env_warps    = e_warps    ? e_warps    : (ind ? 4 : 8);
     const int env_resident = e_resident ? e_resident : (ind ? 4 : 2);
     const int env_stage_kb = e_stage_kb ? e_stage_kb : (ind ? 18 : 36);
@@ -359,7 +361,8 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     p.A = make_sb_act(a.K);
     p.ctl = nullptr; p.counters = nullptr; p.dbg = nullptr;      // assigned at launch (assign_sb_slot): planning has no side effects
     p.src0_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
-    p.l2_prefetch_bytes = (!ind && p.src0_static && e_l2_mb > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)e_l2_mb << 20) : 0;
+    const int64_t l2_cap = l2_prefetch_cap();
+    p.l2_prefetch_bytes = (!ind && p.src0_static && l2_cap > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)l2_cap) : 0;
     p.world = 0; p.rank = 0; p.row_offset = 0; p.epoch = 0;
     p.ep_bias = nullptr; p.ep_y2 = nullptr; p.ep_y3 = nullptr; p.ep_res = nullptr;
     p.src1_static = (a.flags & GGML_B200_MM_SRC1_STATIC) ? 1 : 0;
@@ -402,19 +405,8 @@ static int assign_sb_slot(sb_params & p) {
 }
 
 template <int T, int NW, int NC, bool TWO = false> static int launch_sb_nw(sb_plan & pl, cudaStream_t st) {
-    static per_device_flag attr_set;
-    if (!attr_set.test()) {
-        B200_CUDA_TRY(cudaFuncSetAttribute(mmvq_sb_kernel<T, NW, NC, TWO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 222 * 1024));
-        attr_set.set();
-    }
-    static const bool use_pdl = !(getenv("GGML_B200_NO_PDL") && atoi(getenv("GGML_B200_NO_PDL")) != 0);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(pl.grid); cfg.blockDim = dim3((NW + 1) * 32); cfg.dynamicSmemBytes = pl.smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;
-    B200_CUDA_TRY(cudaLaunchKernelEx(&cfg, mmvq_sb_kernel<T, NW, NC, TWO>, pl.p));
+    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_sb_kernel<T, NW, NC, TWO>>(222 * 1024));
+    B200_CUDA_TRY(launch_pdl(mmvq_sb_kernel<T, NW, NC, TWO>, dim3(pl.grid), dim3((NW + 1) * 32), pl.smem, st, pl.p));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -444,40 +436,18 @@ template <int T> static int launch_sb(const ggml_b200_mul_mat_args & a, const gg
 
 bool mmvq_sb_eligible(const ggml_b200_mul_mat_args & a) {
     sb_plan pl;
-    switch (a.type) {
-        case T_Q4_0: return make_sb_plan<T_Q4_0>(a, pl);
-        case T_Q8_0: return make_sb_plan<T_Q8_0>(a, pl);
-        case T_Q4_K: return make_sb_plan<T_Q4_K>(a, pl);
-        case T_Q5_K: return make_sb_plan<T_Q5_K>(a, pl);
-        case T_Q6_K: return make_sb_plan<T_Q6_K>(a, pl);
-        // next formats (host-verified task dots and quantizer; GPU check: tests/test_gpu_next_formats.py)
-        case T_Q4_1: return make_sb_plan<T_Q4_1>(a, pl);
-        case T_Q5_1: return make_sb_plan<T_Q5_1>(a, pl);
-        case T_Q5_0: return make_sb_plan<T_Q5_0>(a, pl);
-        case T_IQ4_NL: return make_sb_plan<T_IQ4_NL>(a, pl);
-        case T_IQ4_XS: return make_sb_plan<T_IQ4_XS>(a, pl);
-        case T_Q2_K: return make_sb_plan<T_Q2_K>(a, pl);
-        case T_Q3_K: return make_sb_plan<T_Q3_K>(a, pl);
-        default: return false;
-    }
+    bool ok = false;
+    with_format(TC_FORMATS(), a.type, [&](auto t) { ok = make_sb_plan<t>(a, pl); });
+    return ok;
 }
 
 int launch_mmvq_sb(const ggml_b200_mul_mat_args & a, cudaStream_t st, const ggml_b200_gather * ga, const ggml_b200_epilogue * ep) {
-    switch (a.type) {
-        case T_Q4_0: return launch_sb<T_Q4_0>(a, ga, st, ep);
-        case T_Q8_0: return launch_sb<T_Q8_0>(a, ga, st, ep);
-        case T_Q4_K: return launch_sb<T_Q4_K>(a, ga, st, ep);
-        case T_Q5_K: return launch_sb<T_Q5_K>(a, ga, st, ep);
-        case T_Q6_K: return launch_sb<T_Q6_K>(a, ga, st, ep);
-        case T_Q4_1: return launch_sb<T_Q4_1>(a, ga, st, ep);
-        case T_Q5_1: return launch_sb<T_Q5_1>(a, ga, st, ep);
-        case T_Q5_0: return launch_sb<T_Q5_0>(a, ga, st, ep);
-        case T_IQ4_NL: return launch_sb<T_IQ4_NL>(a, ga, st, ep);
-        case T_IQ4_XS: return launch_sb<T_IQ4_XS>(a, ga, st, ep);
-        case T_Q2_K: return launch_sb<T_Q2_K>(a, ga, st, ep);
-        case T_Q3_K: return launch_sb<T_Q3_K>(a, ga, st, ep);
-        default: set_error("mul_mat: unsupported weight type %d", a.type); return GGML_B200_EUNSUPPORTED;
+    int rc = GGML_B200_OK;
+    if (!with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_sb<t>(a, ga, st, ep); })) {
+        set_error("mul_mat: unsupported weight type %d", a.type);
+        return GGML_B200_EUNSUPPORTED;
     }
+    return rc;
 }
 
 int debug_read_trace(unsigned long long * out) {

@@ -11,10 +11,10 @@
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
+#include "b200_ptx.cuh"
 #include "b200_rope.cuh"
 
 #include <cfloat>
-#include <cstdlib>
 
 namespace b200 {
 
@@ -24,20 +24,8 @@ namespace b200 {
 // and only then lets ITS successor launch -- a one-kernel lookahead.  A quantized mat-vec launched after one of these small ops starts
 // its weight prefetch while the small op runs and waits for this kernel's results before reading them.
 __device__ __forceinline__ void pdl_trigger() {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args... args) {
-    static const bool use_pdl = !(getenv("GGML_B200_NO_PDL") && atoi(getenv("GGML_B200_NO_PDL")) != 0);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = use_pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+    pdl_wait();
+    pdl_launch_dependents();
 }
 
 struct tdesc {      // device-side copy of ggml_b200_tensor
@@ -51,26 +39,16 @@ static inline tdesc T(const ggml_b200_tensor * t) {
 static inline int64_t nelem(const tdesc & t) { return t.ne[0] * t.ne[1] * t.ne[2] * t.ne[3]; }
 static inline int64_t nrows(const tdesc & t) { return t.ne[1] * t.ne[2] * t.ne[3]; }
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ float warp_max_f(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
 // block-wide reduce (blockDim multiple of 32, <= 1024); result broadcast to all threads
 template <bool MAX> __device__ __forceinline__ float block_reduce(float v, float * sh) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    v = MAX ? warp_max_f(v) : warp_sum_f(v);
+    v = MAX ? warp_max(v) : warp_sum(v);
     if (nw == 1) return v;
     __syncthreads();
     if (lane == 0) sh[warp] = v;
     __syncthreads();
     float r = lane < nw ? sh[lane] : (MAX ? -INFINITY : 0.0f);
-    r = MAX ? warp_max_f(r) : warp_sum_f(r);
+    r = MAX ? warp_max(r) : warp_sum(r);
     return r;
 }
 
@@ -347,7 +325,7 @@ __global__ void __launch_bounds__(128) mul_mat_f_kernel(tdesc a, tdesc b, tdesc 
         for (int64_t k = lane; k < a.ne[0]; k += 32)
             acc += __half2float(*(const __half *)(ar + k * a.nb[0])) * __half2float(__float2half_rn(*(const float *)(br + k * b.nb[0])));
     }
-    acc = warp_sum_f(acc);
+    acc = warp_sum(acc);
     if (lane == 0) *(float *)(d.data + m * d.nb[0] + n * d.nb[1] + i12 * d.nb[2] + i13 * d.nb[3]) = acc;
 }
 
@@ -390,7 +368,7 @@ __global__ void __launch_bounds__(128) flash_attn_ext_kernel(fa_params p) {
         float part = 0.0f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) { const int d = lane + 32 * i; if (d < D) part += qv[i] * load_elem(krow, p.k.type, d); }
-        float sc = warp_sum_f(part) * p.scale;
+        float sc = warp_sum(part) * p.scale;
         if (p.softcap != 0.0f) sc = p.softcap * tanhf(sc);
         sc += mv;
         float vs = 1.0f;
@@ -486,7 +464,7 @@ int ggml_b200_op_get_rows(const ggml_b200_tensor * src0, const ggml_b200_tensor 
     REQUIRE(d.nb[0] == 4, "dst rows must be contiguous");
     const int64_t rows = i.ne[0] * i.ne[1] * i.ne[2];
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(get_rows_kernel, dim3((unsigned)rows), dim3(256), (cudaStream_t)stream, s, i, d));
+    B200_CUDA_TRY(launch_pdl(get_rows_kernel, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream, s, i, d));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -499,10 +477,10 @@ int ggml_b200_op_bin_bcast(int32_t op, const ggml_b200_tensor * src0, const ggml
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned g = blocks_for(n, 256);
     switch (op) {
-        case 0: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<0>, dim3(g), dim3(256), st, a, b, d, n)); break;
-        case 1: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<1>, dim3(g), dim3(256), st, a, b, d, n)); break;
-        case 2: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<2>, dim3(g), dim3(256), st, a, b, d, n)); break;
-        case 3: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<3>, dim3(g), dim3(256), st, a, b, d, n)); break;
+        case 0: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<0>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
+        case 1: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<1>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
+        case 2: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<2>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
+        case 3: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<3>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
         default: set_error("bin_bcast: bad op %d", op); return GGML_B200_EINVAL;
     }
     B200_LAUNCH_CHECK();
@@ -515,8 +493,8 @@ int ggml_b200_op_norm(int32_t rms, const ggml_b200_tensor * src, const ggml_b200
     const int64_t rows = nrows(s);
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
     const int threads = s.ne[0] >= 1024 ? 256 : s.ne[0] >= 256 ? 128 : 32;
-    if (rms) B200_CUDA_TRY(launch_pdl(norm_kernel<true>, dim3((unsigned)rows), dim3(threads), (cudaStream_t)stream, s, d, eps));
-    else     B200_CUDA_TRY(launch_pdl(norm_kernel<false>, dim3((unsigned)rows), dim3(threads), (cudaStream_t)stream, s, d, eps));
+    if (rms) B200_CUDA_TRY(launch_pdl(norm_kernel<true>, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, s, d, eps));
+    else     B200_CUDA_TRY(launch_pdl(norm_kernel<false>, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, s, d, eps));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -529,22 +507,22 @@ int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const gg
     const int64_t rows = nrows(s);
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
     const int threads = s.ne[0] >= 1024 ? 256 : s.ne[0] >= 256 ? 128 : 32;
-    if (rms) B200_CUDA_TRY(launch_pdl(norm_affine_kernel<true>, dim3((unsigned)rows), dim3(threads), (cudaStream_t)stream, s, d1, gain, d2, bias, d3, eps));
-    else     B200_CUDA_TRY(launch_pdl(norm_affine_kernel<false>, dim3((unsigned)rows), dim3(threads), (cudaStream_t)stream, s, d1, gain, d2, bias, d3, eps));
+    if (rms) B200_CUDA_TRY(launch_pdl(norm_affine_kernel<true>, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, s, d1, gain, d2, bias, d3, eps));
+    else     B200_CUDA_TRY(launch_pdl(norm_affine_kernel<false>, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, s, d1, gain, d2, bias, d3, eps));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
 int ggml_b200_op_scale(const float * src, float * dst, float s, int64_t n, void * stream) {
     if (n <= 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(scale_kernel, dim3(blocks_for(n, 256)), dim3(256), (cudaStream_t)stream, src, dst, s, n));
+    B200_CUDA_TRY(launch_pdl(scale_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, src, dst, s, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
 int ggml_b200_op_diag_mask_inf(const float * src, float * dst, int64_t ne0, int64_t ne1, int64_t n, int32_t n_past, void * stream) {
     if (n <= 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(diag_mask_inf_kernel, dim3(blocks_for(n, 256)), dim3(256), (cudaStream_t)stream, src, dst, ne0, ne1, n_past, n));
+    B200_CUDA_TRY(launch_pdl(diag_mask_inf_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, src, dst, ne0, ne1, n_past, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -552,7 +530,7 @@ int ggml_b200_op_diag_mask_inf(const float * src, float * dst, int64_t ne0, int6
 int ggml_b200_op_unary(int32_t uop, const float * src, float * dst, int64_t n, void * stream) {
     if (n <= 0) return GGML_B200_OK;
     if (uop < 0 || uop > U_SQRT) { set_error("unary: bad op %d", uop); return GGML_B200_EINVAL; }
-    B200_CUDA_TRY(launch_pdl(unary_kernel, dim3(blocks_for(n, 256)), dim3(256), (cudaStream_t)stream, uop, src, dst, n));
+    B200_CUDA_TRY(launch_pdl(unary_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, uop, src, dst, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -570,7 +548,7 @@ int ggml_b200_op_soft_max_diag(const float * src, const void * mask, int32_t mas
     uint32_t n_head_log2 = 1; while (n_head_log2 * 2 <= n_head) n_head_log2 *= 2;
     const float m0 = powf(2.0f, -(max_bias) / n_head_log2), m1 = powf(2.0f, -(max_bias / 2.0f) / n_head_log2);
     const int threads = ne0 >= 1024 ? 256 : ne0 >= 128 ? 128 : 32;
-    B200_CUDA_TRY(launch_pdl(soft_max_kernel, dim3((unsigned)rows), dim3(threads), (cudaStream_t)stream, src, (const uint8_t *)mask, mask_type, dst, ne0, ne1, ne2, scale, max_bias, m0, m1, n_head_log2, (int)diag_n_past));
+    B200_CUDA_TRY(launch_pdl(soft_max_kernel, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, src, (const uint8_t *)mask, mask_type, dst, ne0, ne1, ne2, scale, max_bias, m0, m1, n_head_log2, (int)diag_n_past));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -582,12 +560,12 @@ int ggml_b200_op_cpy(const ggml_b200_tensor * src, const ggml_b200_tensor * dst,
     if (n == 0) return GGML_B200_OK;
     cudaStream_t st = (cudaStream_t)stream;
     if ((s.type == T_F32 || s.type == T_F16) && (d.type == T_F32 || d.type == T_F16)) {
-        B200_CUDA_TRY(launch_pdl(cpy_kernel, dim3(blocks_for(n, 256)), dim3(256), st, s, d, s, d, n));
+        B200_CUDA_TRY(launch_pdl(cpy_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, s, d, s, d, n));
     } else if (s.type == T_F32 && (d.type == T_Q8_0 || d.type == T_Q4_0)) {
         REQUIRE(s.nb[0] == 4 && s.ne[0] % 32 == 0 && d.ne[0] % 32 == 0, "f32 -> q needs dim-0 contiguous rows of whole blocks");
         const int64_t nb = n / 32;
-        if (d.type == T_Q8_0) B200_CUDA_TRY(launch_pdl(cpy_f32_q_kernel<T_Q8_0>, dim3(blocks_for(nb, 128)), dim3(128), st, s, d, nb));
-        else                  B200_CUDA_TRY(launch_pdl(cpy_f32_q_kernel<T_Q4_0>, dim3(blocks_for(nb, 128)), dim3(128), st, s, d, nb));
+        if (d.type == T_Q8_0) B200_CUDA_TRY(launch_pdl(cpy_f32_q_kernel<T_Q8_0>, dim3(blocks_for(nb, 128)), dim3(128), 0, st, s, d, nb));
+        else                  B200_CUDA_TRY(launch_pdl(cpy_f32_q_kernel<T_Q4_0>, dim3(blocks_for(nb, 128)), dim3(128), 0, st, s, d, nb));
     } else {
         set_error("cpy: unsupported type pair %d -> %d", s.type, d.type);
         return GGML_B200_EUNSUPPORTED;
@@ -603,7 +581,7 @@ int ggml_b200_op_cpy2(const ggml_b200_tensor * src_a, const ggml_b200_tensor * d
     auto fl = [](const tdesc & t) { return t.type == T_F32 || t.type == T_F16; };
     if (!(fl(s) && fl(d) && fl(s2) && fl(d2))) { set_error("cpy2: float tensors only"); return GGML_B200_EUNSUPPORTED; }
     if (n == 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(cpy_kernel, dim3(blocks_for(n, 256), 2), dim3(256), (cudaStream_t)stream, s, d, s2, d2, n));
+    B200_CUDA_TRY(launch_pdl(cpy_kernel, dim3(blocks_for(n, 256), 2), dim3(256), 0, (cudaStream_t)stream, s, d, s2, d2, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -627,7 +605,7 @@ int ggml_b200_op_flash_attn_ext(const ggml_b200_tensor * q, const ggml_b200_tens
     uint32_t n_head_log2 = 1; while (n_head_log2 * 2 <= n_head) n_head_log2 *= 2;
     p.n_head_log2 = n_head_log2;
     p.m0 = powf(2.0f, -(max_bias) / n_head_log2); p.m1 = powf(2.0f, -(max_bias / 2.0f) / n_head_log2);
-    B200_CUDA_TRY(launch_pdl(flash_attn_ext_kernel, dim3((unsigned)p.q.ne[1], (unsigned)p.q.ne[2], (unsigned)p.q.ne[3]), dim3(128), (cudaStream_t)stream, p));
+    B200_CUDA_TRY(launch_pdl(flash_attn_ext_kernel, dim3((unsigned)p.q.ne[1], (unsigned)p.q.ne[2], (unsigned)p.q.ne[3]), dim3(128), 0, (cudaStream_t)stream, p));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -639,7 +617,7 @@ int ggml_b200_op_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor
     REQUIRE(b.ne[2] % a.ne[2] == 0 && b.ne[3] % a.ne[3] == 0, "batch dims do not broadcast");
     const int64_t nout = nelem(d);
     if (nout == 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(mul_mat_f_kernel, dim3(blocks_for(nout, 4)), dim3(128), (cudaStream_t)stream, a, b, d, nout));
+    B200_CUDA_TRY(launch_pdl(mul_mat_f_kernel, dim3(blocks_for(nout, 4)), dim3(128), 0, (cudaStream_t)stream, a, b, d, nout));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -679,8 +657,8 @@ int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos
     const int64_t hb = (s.ne[1] + heads_per_cta - 1) / heads_per_cta;
     REQUIRE(s.ne[2] <= 0x7fffffff && hb <= 65535 && s.ne[3] <= 65535, "too many positions / heads / batches for one grid");
     const dim3 grid((unsigned)s.ne[2], (unsigned)hb, (unsigned)s.ne[3]);
-    if (s.type == T_F32) B200_CUDA_TRY(launch_pdl(rope_kernel<float>, grid, dim3(128), (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
-    else                 B200_CUDA_TRY(launch_pdl(rope_kernel<__half>, grid, dim3(128), (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
+    if (s.type == T_F32) B200_CUDA_TRY(launch_pdl(rope_kernel<float>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
+    else                 B200_CUDA_TRY(launch_pdl(rope_kernel<__half>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
