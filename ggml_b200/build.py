@@ -21,7 +21,7 @@ CSRC = PKG / "csrc"
 ROOT = PKG.parent
 REF = Path(os.environ.get("GGML_REFERENCE_DIR", "/root/reference"))
 
-KERNEL_SRCS = ["api.cu", "mmvq.cu", "mmvq_sb.cu", "mmvq_mma.cu", "dequant.cu", "mmid.cu", "mmq_tc.cu", "mmq_tc2.cu", "ops.cu"]
+KERNEL_SRCS = ["api.cu", "mmvq.cu", "mmvq_sb.cu", "mmvq_mma.cu", "dequant.cu", "mmid.cu", "mmq_tc2.cu", "ops.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "--threads", "8"]
 

@@ -33,6 +33,31 @@ int sm_count() {
     return cached[dev];
 }
 
+// One per device, allocated on first use under a mutex (or ahead of time by ggml_b200_prepare, which the backend calls at device
+// initialisation so that no allocation can fall inside a stream capture) and kept for the life of the process.
+unsigned int * control_block() {
+    static unsigned int * ptr[64] = { nullptr };
+    static std::mutex mu;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { set_error("control block: cudaGetDevice failed"); return nullptr; }
+    std::lock_guard<std::mutex> lock(mu);
+    if (!ptr[dev]) {
+        unsigned int * p = nullptr;
+        const size_t bytes = (CTL_SPLITK_FLAGS + (size_t)TC_FLAG_SLOTS * TC_FLAGS_PER_SLOT) * sizeof(unsigned int);
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaSuccess) e = cudaMemset(p, 0, bytes);
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+        if (e != cudaSuccess) {
+            set_error("control block: %s", cudaGetErrorString(e));
+            cudaGetLastError();
+            if (p) cudaFree(p);
+            return nullptr;
+        }
+        ptr[dev] = p;
+    }
+    return ptr[dev];
+}
+
 static int validate(const ggml_b200_mul_mat_args * a) {
     if (!a) { set_error("mul_mat: NULL args"); return GGML_B200_EINVAL; }
     if (type_bytes(a->type) == 0) { set_error("mul_mat: unsupported weight type %d", a->type); return GGML_B200_EUNSUPPORTED; }
@@ -58,22 +83,64 @@ static bool mma_wanted(const ggml_b200_mul_mat_args & a) {
     return mmvq_mma_eligible(a);
 }
 
-static int plan(const ggml_b200_mul_mat_args & a) {
+// The kernel one mul_mat call runs.  The workspace query, the launch and the fused entry point all read it from route(), so they cannot
+// disagree.
+enum route_kind {
+    R_GENERIC,     // one warp per output (mmvq.cu): any shape
+    R_TMA,         // first-generation 64-weight-unit mat-vec (mmvq.cu)
+    R_SB,          // superblock mat-vec (mmvq_sb.cu), all columns in one launch
+    R_SB_GROUPS,   // superblock mat-vec in column groups of `group`
+    R_MMA,         // int8 mma.sync mat-vec (mmvq_mma.cu)
+    R_WGMMA,       // warpgroup-MMA GEMM (mmq_tc2.cu)
+    R_DENSE,       // W dequantized to fp16, then the same GEMM (mmq_tc2.cu)
+};
+struct mm_route { route_kind kind = R_GENERIC; int64_t group = 0; };
+
+// GGML_B200_EUNSUPPORTED when a forced family cannot run the shape; sets no error message
+static int route(const ggml_b200_mul_mat_args & a, mm_route & r) {
     static const bool env_generic = getenv("GGML_B200_FORCE_GENERIC") && atoi(getenv("GGML_B200_FORCE_GENERIC")) != 0;   // debugging aid
-    if (env_generic) return GGML_B200_MM_FORCE_GENERIC;
-    if (a.flags & GGML_B200_MM_FORCE_GENERIC) return GGML_B200_MM_FORCE_GENERIC;
-    if (a.flags & GGML_B200_MM_FORCE_GEMV) {
-        const bool ok = (a.flags & GGML_B200_MM_GEMV_V1) ? mmvq_tma_eligible(a) : (mma_wanted(a) || mmvq_sb_eligible(a) || mmvq_tma_eligible(a));
-        return ok ? (int)GGML_B200_MM_FORCE_GEMV : (int)GGML_B200_EUNSUPPORTED;
+    r = mm_route{};
+    if (env_generic || (a.flags & GGML_B200_MM_FORCE_GENERIC)) return GGML_B200_OK;
+    const bool force_gemv = (a.flags & GGML_B200_MM_FORCE_GEMV) != 0;
+    if (!force_gemv && ((a.flags & GGML_B200_MM_FORCE_GEMM) || a.N > 8)) {
+        if (mmq_dense_eligible(a)) r.kind = R_DENSE;             // formats without an operand decoder (n >= 9 only)
+        else if (mmq_tc2_eligible(a)) r.kind = R_WGMMA;          // n >= 5 only
+        else if (a.flags & GGML_B200_MM_FORCE_GEMM) return GGML_B200_EUNSUPPORTED;
+        return GGML_B200_OK;
     }
-    if (a.flags & GGML_B200_MM_FORCE_GEMM) return (mmq_tc_eligible(a) || mmq_tc_eligible_small(a)) ? (int)GGML_B200_MM_FORCE_GEMM : (int)GGML_B200_EUNSUPPORTED;
+    // the mat-vec family: forced, or n <= 8
+    if (mma_wanted(a)) { r.kind = R_MMA; return GGML_B200_OK; }   // never under GEMV_V1
+    const bool sb = mmvq_sb_eligible(a);
     // 5..8 columns of very long rows: the superblock kernel would need two column-group launches (each re-streaming W, issue-bound); the
     // tensor-core kernel takes them in one pass (fp16-operand tolerance instead of the integer-exact dot: DESIGN.md section 3)
-    if (a.N <= 8 && mma_wanted(a)) return GGML_B200_MM_FORCE_GEMV;
-    if (a.N >= 5 && a.N <= 8 && !mmvq_sb_eligible(a) && mmq_tc_eligible_small(a)) return GGML_B200_MM_FORCE_GEMM;
-    if (a.N <= 8 && (mmvq_sb_eligible(a) || mmvq_tma_eligible(a))) return GGML_B200_MM_FORCE_GEMV;
-    if (a.N > 8 && mmq_tc_eligible(a)) return GGML_B200_MM_FORCE_GEMM;
-    return GGML_B200_MM_FORCE_GENERIC;
+    if (!force_gemv && a.N >= 5 && !sb && mmq_tc2_eligible(a)) { r.kind = R_WGMMA; return GGML_B200_OK; }
+    const bool v1 = (a.flags & GGML_B200_MM_GEMV_V1) != 0;      // the first-generation kernel whenever the family is the mat-vec one
+    if (sb && !v1) { r.kind = R_SB; return GGML_B200_OK; }
+    if (!mmvq_tma_eligible(a) && (force_gemv || !sb)) return force_gemv ? GGML_B200_EUNSUPPORTED : GGML_B200_OK;
+    r.kind = R_TMA;
+    if (v1) return GGML_B200_OK;
+    // long rows x many columns: the activation records of all columns do not fit next to the weight stages.  Column groups of 4 / 2 / 1
+    // on the same kernel re-stream W per group, which is far cheaper than leaving the bandwidth kernel (columns are independent: results
+    // are bit-identical to the one-launch form).  This form is only reached when the first-generation kernel is eligible for the whole
+    // shape (checked above), so a format it does not take (Q4_1, for one) goes to the generic kernel instead, even where the superblock
+    // kernel would take its column groups.
+    if (a.N > 1 && a.ne02 == 1 && a.ne03 == 1 && a.ne12 == 1 && a.ne13 == 1) {
+        for (int64_t g = 4; g >= 1; g >>= 1) {
+            ggml_b200_mul_mat_args sub = a;
+            sub.N = g;
+            if (g < a.N && mmvq_sb_eligible(sub)) { r.kind = R_SB_GROUPS; r.group = g; return GGML_B200_OK; }
+        }
+    }
+    return GGML_B200_OK;
+}
+
+static int family(int rc, const mm_route & r) {
+    if (rc != GGML_B200_OK) return rc;
+    switch (r.kind) {
+        case R_GENERIC: return GGML_B200_MM_FORCE_GENERIC;
+        case R_WGMMA: case R_DENSE: return GGML_B200_MM_FORCE_GEMM;
+        default: return GGML_B200_MM_FORCE_GEMV;
+    }
 }
 
 } // namespace b200
@@ -86,8 +153,9 @@ const char * ggml_b200_last_error(void) { return g_err; }
 const char * ggml_b200_version(void) { return "ggml-b200 0.1 (sm_90a)"; }
 uint64_t ggml_b200_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int ggml_b200_sm_count(void) { return sm_count(); }
-int ggml_b200_prepare(void) { const int rc = prepare_device(); return rc != GGML_B200_OK ? rc : tc_prepare_device(); }
-int ggml_b200_debug_gemm_trace(uint64_t * host_dst, int32_t max_ctas) { return tc2_trace_read((unsigned long long *)host_dst, max_ctas); }
+int ggml_b200_prepare(void) { return control_block() ? GGML_B200_OK : GGML_B200_ECUDA; }
+// the GEMM records no per-CTA stamp trace
+int ggml_b200_debug_gemm_trace(uint64_t * host_dst, int32_t max_ctas) { (void)host_dst; (void)max_ctas; return 0; }
 int ggml_b200_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -113,15 +181,20 @@ int ggml_b200_quantize_activations(int32_t weight_type, const float * src, size_
 int ggml_b200_mul_mat_plan(const ggml_b200_mul_mat_args * args) {
     const int rc = validate(args);
     if (rc != GGML_B200_OK) return rc;
-    return plan(*args);
+    mm_route r;
+    return family(route(*args, r), r);
 }
 
 size_t ggml_b200_mul_mat_workspace_size(const ggml_b200_mul_mat_args * args) {
     if (validate(args) != GGML_B200_OK) return 0;
-    switch (plan(*args)) {
-        case GGML_B200_MM_FORCE_GEMV: return mma_wanted(*args) ? mmvq_mma_workspace(*args) : 0;
-        case GGML_B200_MM_FORCE_GEMM: return mmq_tc_workspace(*args);
-        default: return mmvq_generic_workspace(*args);
+    mm_route r;
+    if (route(*args, r) != GGML_B200_OK) return mmvq_generic_workspace(*args);
+    switch (r.kind) {
+        case R_TMA: case R_SB: case R_SB_GROUPS: return 0;
+        case R_MMA:   return mmvq_mma_workspace(*args);
+        case R_WGMMA: return mmq_tc2_workspace(*args);
+        case R_DENSE: return mmq_dense_workspace(*args);
+        default:      return mmvq_generic_workspace(*args);
     }
 }
 
@@ -130,37 +203,26 @@ int ggml_b200_mul_mat(const ggml_b200_mul_mat_args * args, void * stream) {
     if (rc != GGML_B200_OK) return rc;
     if (args->M == 0 || args->N == 0) return GGML_B200_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    switch (plan(*args)) {
-        case GGML_B200_MM_FORCE_GEMV:
-            // the superblock kernel (mmvq_sb.cu) for 1 <= n <= 8; the first-generation unit kernel (mmvq.cu) on request or as the last resort
-            if (!(args->flags & GGML_B200_MM_GEMV_V1)) {
-                if (mma_wanted(*args)) return launch_mmvq_mma(*args, st);
-                if (mmvq_sb_eligible(*args)) return launch_mmvq_sb(*args, st);
-                // long rows x many columns: the activation records of all columns do not fit next to the weight stages.  Column groups of
-                // 4 / 2 / 1 on the same kernel re-stream W per group, which is far cheaper than leaving the bandwidth kernel
-                // (columns are independent: results are bit-identical to the one-launch form)
-                if (args->N > 1 && args->ne02 == 1 && args->ne03 == 1 && args->ne12 == 1 && args->ne13 == 1) {
-                    for (int64_t g = 4; g >= 1; g >>= 1) {
-                        if (g >= args->N) continue;
-                        ggml_b200_mul_mat_args sub = *args;
-                        sub.N = g;
-                        if (!mmvq_sb_eligible(sub)) continue;
-                        for (int64_t c0 = 0; c0 < args->N; c0 += g) {
-                            sub.N = std::min<int64_t>(g, args->N - c0);
-                            sub.src1 = (const float *)((const char *)args->src1 + (size_t)c0 * args->nb11);
-                            sub.dst = args->dst + (size_t)c0 * args->M;
-                            if (!mmvq_sb_eligible(sub)) { set_error("mul_mat: column group not eligible"); return GGML_B200_EUNSUPPORTED; }
-                            rc = launch_mmvq_sb(sub, st);
-                            if (rc != GGML_B200_OK) return rc;
-                        }
-                        return GGML_B200_OK;
-                    }
-                }
+    mm_route r;
+    if (route(*args, r) != GGML_B200_OK) { set_error("mul_mat: the forced kernel family cannot run this shape"); return GGML_B200_EUNSUPPORTED; }
+    switch (r.kind) {
+        case R_TMA:   return launch_mmvq_tma(*args, st);
+        case R_SB:    return launch_mmvq_sb(*args, st);
+        case R_MMA:   return launch_mmvq_mma(*args, st);
+        case R_WGMMA: return launch_mmq_tc2(*args, st);
+        case R_DENSE: return launch_mmq_dense(*args, st);
+        case R_SB_GROUPS:
+            for (int64_t c0 = 0; c0 < args->N; c0 += r.group) {
+                ggml_b200_mul_mat_args sub = *args;
+                sub.N = std::min<int64_t>(r.group, args->N - c0);
+                sub.src1 = (const float *)((const char *)args->src1 + (size_t)c0 * args->nb11);
+                sub.dst = args->dst + (size_t)c0 * args->M;
+                if (!mmvq_sb_eligible(sub)) { set_error("mul_mat: column group not eligible"); return GGML_B200_EUNSUPPORTED; }
+                rc = launch_mmvq_sb(sub, st);
+                if (rc != GGML_B200_OK) return rc;
             }
-            return launch_mmvq_tma(*args, st);
-        case GGML_B200_MM_FORCE_GEMM:    return launch_mmq_tc(*args, st);
-        case GGML_B200_MM_FORCE_GENERIC: return launch_mmvq_generic(*args, st);
-        default: set_error("mul_mat: the forced kernel family cannot run this shape"); return GGML_B200_EUNSUPPORTED;
+            return GGML_B200_OK;
+        default:      return launch_mmvq_generic(*args, st);
     }
 }
 
@@ -175,7 +237,9 @@ int ggml_b200_mul_mat_fused(const ggml_b200_mul_mat_args * args, const ggml_b200
     int rc = validate(args);
     if (rc != GGML_B200_OK) return rc;
     if (!ep || !ep->bias || !ep->dst_bias || (ep->unary < 0 || ep->unary > 2) || (ep->unary != 0 && !ep->dst_unary) || (ep->unary == 2 && !ep->residual)) { set_error("mul_mat_fused: bad epilogue"); return GGML_B200_EINVAL; }
-    if (args->N != 1 || plan(*args) != GGML_B200_MM_FORCE_GEMV || !mmvq_sb_eligible(*args)) { set_error("mul_mat_fused: only the n = 1 mat-vec kernel has the fused epilogue"); return GGML_B200_EUNSUPPORTED; }
+    // also where the unfused route is the mma kernel (n = 1, very long rows): the epilogue exists on the superblock kernel only
+    mm_route r;
+    if (args->N != 1 || family(route(*args, r), r) != GGML_B200_MM_FORCE_GEMV || !mmvq_sb_eligible(*args)) { set_error("mul_mat_fused: only the n = 1 mat-vec kernel has the fused epilogue"); return GGML_B200_EUNSUPPORTED; }
     if (args->M == 0) return GGML_B200_OK;
     return launch_mmvq_sb(*args, (cudaStream_t)stream, nullptr, ep);
 }

@@ -18,6 +18,14 @@ extern std::atomic<uint64_t> g_launches;
 void set_error(const char * fmt, ...);
 int  sm_count();
 
+// Per-device control block, zeroed once, in 4-byte words:
+//   [0, 64)                    global control words of the mat-vec kernels
+//   [64, 64 + 64 * 8)          64 per-launch scheduling slots of the mat-vec kernels (sb_next_slot)
+//   [1024, 1536)               mat-vec stamp trace (GGML_B200_SB_DEBUG): 32 records of 8 x u64
+//   [2048, 2048 + 64 * 256)    64 slots of 256 self-cleaning split-K flags of the GEMM (tc_flag_slot)
+constexpr int CTL_SPLITK_FLAGS = 2048, TC_FLAG_SLOTS = 64, TC_FLAGS_PER_SLOT = 256;
+unsigned int * control_block();   // nullptr on error (set_error called)
+
 // Programmatic dependent launch: kernels launched through launch_pdl may become resident while their predecessor on the stream still
 // runs; each one orders itself against it with griddepcontrol.wait.  The environment knob read below (= 1) launches them plainly.
 inline bool pdl_enabled() {
@@ -74,10 +82,7 @@ size_t mmvq_generic_workspace(const ggml_b200_mul_mat_args & a);
 bool   mmvq_sb_eligible(const ggml_b200_mul_mat_args & a);
 int    launch_mmvq_sb(const ggml_b200_mul_mat_args & a, cudaStream_t st, const ggml_b200_gather * ga = nullptr, const ggml_b200_epilogue * ep = nullptr);
 int    debug_read_trace(unsigned long long * out);
-int    prepare_device();   // allocate the per-device control block (never inside a stream capture)
 int    launch_gather_wait(const uint32_t * flags, int world, uint32_t epoch, cudaStream_t st);
-// device control block of the bandwidth kernels: [0,64) global control words, [64, 64 + 64*8) 64 per-launch scheduling slots
-unsigned int * sb_control_block();                 // nullptr on error (set_error called)
 unsigned int * sb_next_slot(unsigned int * ctl);   // the next of the 64 self-resetting scheduling slots
 int64_t l2_prefetch_cap();                         // bytes of W a dependent mat-vec launch pulls into L2 ahead of its predecessor's output
 
@@ -86,31 +91,18 @@ bool   mmvq_mma_eligible(const ggml_b200_mul_mat_args & a);
 int    launch_mmvq_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st);
 size_t mmvq_mma_workspace(const ggml_b200_mul_mat_args & a);   // the quantized activation records (written by the pre-kernel)
 
-// mmq_tc.cu (tensor-core GEMM front end: activation conversion, dispatch)
-typedef CUresult (*encode_tiled_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
-                                    const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-encode_tiled_fn tc_get_encode();
-// activations f32 -> fp16 rows with an exact power-of-two scale per row (inv_scale[n] undoes it in the epilogue)
-int    tc_launch_x_to_f16(const float * x, size_t nb11, __half * xh, float * inv_scale, int64_t K, int64_t N, cudaStream_t st);
-bool   mmq_tc_eligible(const ggml_b200_mul_mat_args & a);
-size_t mmq_tc_workspace(const ggml_b200_mul_mat_args & a);
-bool   mmq_dense_eligible(const ggml_b200_mul_mat_args & a);   // n >= 9, formats without an operand decoder: dequantize to fp16 + the same GEMM (mmq_tc2.cu)
+// mmq_tc2.cu (the wgmma GEMM kernel: quantized W with an operand decoder, n >= 5)
+bool   mmq_tc2_eligible(const ggml_b200_mul_mat_args & a);
+size_t mmq_tc2_workspace(const ggml_b200_mul_mat_args & a);
+int    launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st);
+bool   mmq_dense_eligible(const ggml_b200_mul_mat_args & a);   // n >= 9, formats without an operand decoder: dequantize to fp16 + the same GEMM
 size_t mmq_dense_workspace(const ggml_b200_mul_mat_args & a);
 int    launch_mmq_dense(const ggml_b200_mul_mat_args & a, cudaStream_t st);
 size_t mmq_f16w_workspace(int64_t M, int64_t N, int64_t K);         // dense fp16 weights, n >= 9 (0 = not eligible)
 int    launch_mmq_f16w(const void * w, size_t nb01, const float * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * ws, size_t ws_size, uint32_t flags, cudaStream_t st);
-bool   mmq_tc_eligible_small(const ggml_b200_mul_mat_args & a);   // 5 <= n <= 8 on the tensor-core path (shapes the mat-vec kernel would have to split)
-int    launch_mmq_tc(const ggml_b200_mul_mat_args & a, cudaStream_t st);
-// mmq_tc2.cu (the wgmma GEMM kernel)
-bool   mmq_tc2_eligible(const ggml_b200_mul_mat_args & a);
-size_t mmq_tc2_workspace(const ggml_b200_mul_mat_args & a);
-int    launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st);
 // expert-grouped MUL_MAT_ID on the GEMM kernel (mmq_tc2.cu)
 bool   mmid_grouped_eligible(const ggml_b200_mul_mat_id_args & a);
 size_t mmid_grouped_workspace(const ggml_b200_mul_mat_id_args & a);
 int    launch_mmid_grouped(const ggml_b200_mul_mat_id_args & a, cudaStream_t st);
-unsigned int * tc_flag_slot();   // a zeroed, self-cleaning block of split-K flags from the device's control block (nullptr on error)
-int    tc_prepare_device();
-int tc2_trace_read(unsigned long long * host_dst, int max_ctas);   // GEMM stamp trace: none is recorded (returns 0)
 
 } // namespace b200

@@ -603,24 +603,23 @@ int src0_flags(const backend_ctx * ctx, const ggml_tensor * a) {
     return GGML_B200_MM_SRC0_STATIC;
 }
 
-void compute_mul_mat(backend_ctx * ctx, const ggml_tensor * dst) {
-    const ggml_tensor * a = dst->src[0], * b = dst->src[1];
+// the kernel arguments of a MUL_MAT node (no workspace yet); the workspace query before a capture and the launch see the same shape
+ggml_b200_mul_mat_args mul_mat_args(const ggml_tensor * node, int32_t flags) {
+    const ggml_tensor * a = node->src[0], * b = node->src[1];
     ggml_b200_mul_mat_args args{};
     args.type = (int32_t) a->type;
-    args.flags = src0_flags(ctx, a);
+    args.flags = flags;
     args.K = a->ne[0]; args.M = a->ne[1]; args.N = b->ne[1];
     args.ne02 = a->ne[2]; args.ne03 = a->ne[3]; args.ne12 = b->ne[2]; args.ne13 = b->ne[3];
     args.nb01 = a->nb[1]; args.nb02 = a->nb[2]; args.nb03 = a->nb[3];
     args.nb11 = b->nb[1]; args.nb12 = b->nb[2]; args.nb13 = b->nb[3];
-    args.src0 = a->data; args.src1 = (const float *) b->data; args.dst = (float *) dst->data;
-    const size_t need = ggml_b200_mul_mat_workspace_size(&args);
-    args.workspace = ctx->scratch(need);
-    args.workspace_size = ctx->workspace_size;
-    SHIM_OK(ggml_b200_mul_mat(&args, ctx->stream));
+    args.src0 = a->data; args.src1 = (const float *) b->data; args.dst = (float *) node->data;
+    return args;
 }
 
-void compute_mul_mat_id(backend_ctx * ctx, const ggml_tensor * dst) {
-    const ggml_tensor * as = dst->src[0], * b = dst->src[1], * ids = dst->src[2];
+// the kernel arguments of a MUL_MAT_ID node (no workspace yet)
+ggml_b200_mul_mat_id_args mul_mat_id_args(const ggml_tensor * node) {
+    const ggml_tensor * as = node->src[0], * b = node->src[1], * ids = node->src[2];
     ggml_b200_mul_mat_id_args args{};
     args.type = (int32_t) as->type;
     args.K = as->ne[0]; args.M = as->ne[1]; args.n_expert = as->ne[2];
@@ -628,7 +627,20 @@ void compute_mul_mat_id(backend_ctx * ctx, const ggml_tensor * dst) {
     args.nb01 = as->nb[1]; args.nb02 = as->nb[2];
     args.nb11 = b->nb[1]; args.nb12 = b->nb[2];
     args.ids_nb1 = ids->nb[1];
-    args.src0 = as->data; args.src1 = (const float *) b->data; args.ids = (const int32_t *) ids->data; args.dst = (float *) dst->data;
+    args.src0 = as->data; args.src1 = (const float *) b->data; args.ids = (const int32_t *) ids->data; args.dst = (float *) node->data;
+    return args;
+}
+
+void compute_mul_mat(backend_ctx * ctx, const ggml_tensor * dst) {
+    ggml_b200_mul_mat_args args = mul_mat_args(dst, src0_flags(ctx, dst->src[0]));
+    const size_t need = ggml_b200_mul_mat_workspace_size(&args);
+    args.workspace = ctx->scratch(need);
+    args.workspace_size = ctx->workspace_size;
+    SHIM_OK(ggml_b200_mul_mat(&args, ctx->stream));
+}
+
+void compute_mul_mat_id(backend_ctx * ctx, const ggml_tensor * dst) {
+    ggml_b200_mul_mat_id_args args = mul_mat_id_args(dst);
     const size_t need = ggml_b200_mul_mat_id_workspace_size(&args);
     args.workspace = ctx->scratch(need);
     args.workspace_size = ctx->workspace_size;
@@ -913,22 +925,13 @@ bool f16_weights_on_tensor_cores(const ggml_tensor * node) {
 
 size_t node_scratch_need(const ggml_tensor * node) {
     if (node->op == GGML_OP_MUL_MAT && is_b200_weight_type(node->src[0]->type)) {
-        const ggml_tensor * a = node->src[0], * b = node->src[1];
-        ggml_b200_mul_mat_args args{};
-        args.type = (int32_t) a->type;
-        args.K = a->ne[0]; args.M = a->ne[1]; args.N = b->ne[1];
-        args.ne02 = a->ne[2]; args.ne03 = a->ne[3]; args.ne12 = b->ne[2]; args.ne13 = b->ne[3];
-        args.nb01 = a->nb[1]; args.nb02 = a->nb[2]; args.nb03 = a->nb[3];
-        args.nb11 = b->nb[1]; args.nb12 = b->nb[2]; args.nb13 = b->nb[3];
-        args.src0 = a->data; args.src1 = (const float *) b->data; args.dst = (float *) node->data;
+        // the flags the launch will pass (SRC0_STATIC) select neither the kernel nor the workspace size
+        const ggml_b200_mul_mat_args args = mul_mat_args(node, GGML_B200_MM_AUTO);
         return ggml_b200_mul_mat_workspace_size(&args);
     }
     if (node->op == GGML_OP_MUL_MAT && f16_weights_on_tensor_cores(node)) return ggml_b200_mul_mat_f16_workspace_size(node->src[0]->ne[1], node->src[1]->ne[1], node->src[0]->ne[0]);
     if (node->op == GGML_OP_MUL_MAT_ID) {
-        const ggml_tensor * as = node->src[0], * b = node->src[1];
-        ggml_b200_mul_mat_id_args args{};
-        args.type = (int32_t) as->type; args.K = as->ne[0]; args.M = as->ne[1]; args.n_expert = as->ne[2];
-        args.n_used = node->src[2]->ne[0]; args.nb1cols = b->ne[1]; args.n_tok = b->ne[2];
+        const ggml_b200_mul_mat_id_args args = mul_mat_id_args(node);
         return ggml_b200_mul_mat_id_workspace_size(&args);
     }
     return 0;
@@ -967,14 +970,7 @@ int try_fuse_mul_mat(backend_ctx * ctx, ggml_cgraph * cgraph, int i) {
         auto overlaps = [&](const void * p) { const char * y0 = (const char *) p, * y1 = y0 + mm->ne[0] * sizeof(float); return p && y0 < x1 && x0 < y1; };
         if (overlaps(ep.dst_bias) || overlaps(ep.dst_unary) || overlaps(mm->data)) return 0;
     }
-    ggml_b200_mul_mat_args args{};
-    args.type = (int32_t) a->type;
-    args.flags = src0_flags(ctx, a);
-    args.K = a->ne[0]; args.M = a->ne[1]; args.N = 1;
-    args.ne02 = a->ne[2]; args.ne03 = a->ne[3]; args.ne12 = b->ne[2]; args.ne13 = b->ne[3];
-    args.nb01 = a->nb[1]; args.nb02 = a->nb[2]; args.nb03 = a->nb[3];
-    args.nb11 = b->nb[1]; args.nb12 = b->nb[2]; args.nb13 = b->nb[3];
-    args.src0 = a->data; args.src1 = (const float *) b->data; args.dst = (float *) mm->data;
+    const ggml_b200_mul_mat_args args = mul_mat_args(mm, src0_flags(ctx, a));
     const int rc = ggml_b200_mul_mat_fused(&args, &ep, ctx->stream);
     if (rc == GGML_B200_EUNSUPPORTED) return 0;              // shape not on the mat-vec kernel: run the nodes one by one
     SHIM_OK(rc);

@@ -1,9 +1,16 @@
-// mmq_tc2.cu — the tensor-core GEMM kernel (sm_90a): one 256 (W rows) x BN (activation rows) output tile per CTA over a K range,
-// fp16 operands in shared memory, f32 accumulation in registers by warpgroup MMA (wgmma.mma_async m64n64k16).
+// mmq_tc2.cu — batched quantized mat-mul (n > 8, and 5 <= n <= 8 where the mat-vec kernels cannot take the shape) on the Hopper
+// tensor cores (sm_90a): one 256 (W rows) x BN (activation rows) output tile per CTA over a K range, fp16 operands in shared memory,
+// f32 accumulation in registers by warpgroup MMA (wgmma.mma_async m64n64k16).  Computes GGML_OP_MUL_MAT for block-quantized src0 and
+// f32 src1 as ggml_compute_forward_mul_mat does (src/ggml-cpu/ggml-cpu.c:7428).
 //
-// Operands: W is dequantized to fp16 in shared memory (K-major SWIZZLE_128B, the layout the wgmma descriptors read), X was converted
-// to fp16 once by mmq_tc.cu with an exact power-of-two row scale (undone in the epilogue).  T_F16: the A operand already is fp16
-// (dense f16 weights, or a format without an operand decoder dequantized into the workspace first) and arrives by TMA like X.
+// Per-block scales cannot be interposed in an accumulation that runs over the whole K loop, so the scales are folded into the
+// operand: W is dequantized to fp16 in shared memory (K-major SWIZZLE_128B, the layout the wgmma descriptors read), X is converted
+// to fp16 once (x_to_f16_kernel: each activation row pre-scaled by a power of two when its largest magnitude would leave the fp16
+// range; the epilogue undoes the scale, so nothing overflows and the scaling is exact).  fp16 is chosen over bf16 because integer
+// codes convert to fp16 with two packed-half instructions per two weights and carry 11 instead of 8 significant bits.  NMSE against
+// the CPU backend ~1e-7 .. 1e-6 (the reference's gate is 5e-4, tests/test-backend-ops.cpp:1915-1917).  T_F16: the A operand already
+// is fp16 (dense f16 weights, or a format without an operand decoder dequantized into the workspace first, launch_mmq_dense) and
+// arrives by TMA like X.
 //
 // Warp roles (12 warps, three warpgroups; setmaxnreg moves the producer's registers to the consumers):
 //   warps 0-7   two consumer warpgroups; thread t owns W row t of the tile.  Per K-step (64 weights) each thread dequantizes its
@@ -17,8 +24,8 @@
 // The activation conversion kernel and this kernel are chained with programmatic dependent launch: barrier set-up, tensor-map
 // prefetch and (static weights) the first raw W unit run while the conversion is still in flight.
 //
-// Replaces the reference's mul_mat_q (src/ggml-cuda/mmq.cuh:2499-2655) and its dequantize + cuBLAS route for the shapes make_tc2_plan
-// accepts.
+// Replaces the reference's mul_mat_q (src/ggml-cuda/mmq.cuh:2499-2655: int8 mma.sync tiles + stream-k fix-up) and its dequantize +
+// cuBLAS route (dequantize_block_* -> cublasGemmEx, src/ggml-cuda/ggml-cuda.cu:1158-1300) for the shapes make_tc2_plan accepts.
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_tc_dequant.cuh"
@@ -60,6 +67,46 @@ __device__ __forceinline__ void tc2_dequant(int ks, const uint32_t (&u)[tc2fmt<T
             else if (ks == 3) dq64<T, 3>(u, dst, sw);
         }
     }
+}
+
+// ----------------------------------------------------------------------------- X -> fp16 prologue
+// one CTA of 256 threads per activation row: largest magnitude -> exact power-of-two scale that puts it into [2^13, 2^14) (neither
+// overflow nor a row of fp16 subnormals, whatever the row's magnitude), then the conversion.  *inv_scale is applied to the row's column
+// of the result in the GEMM epilogue.
+__device__ __forceinline__ void row_to_f16(const float * __restrict__ xr, __half * __restrict__ xh, float * __restrict__ inv_scale, int64_t K) {
+    __shared__ float s_max[8];
+    float amax = 0.0f;
+    for (int64_t k = (int64_t)threadIdx.x * 8; k < K; k += 256 * 8) {
+        const float4 a = load_f4(xr + k), b = load_f4(xr + k + 4);
+        amax = fmaxf(amax, fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))), fmaxf(fmaxf(fabsf(b.x), fabsf(b.y)), fmaxf(fabsf(b.z), fabsf(b.w)))));
+    }
+    amax = warp_max(amax);
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = amax;
+    __syncthreads();
+    amax = s_max[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) amax = fmaxf(amax, s_max[i]);
+    // e = exponent(amax) - 13 (finite non-zero amax only; zero / inf / nan rows keep scale 1 and propagate), |e| <= 100
+    int e = 0;
+    if (amax > 0.0f && amax <= 3.0e38f) e = max(-100, min(100, (int)((__float_as_uint(amax) >> 23) & 0xFF) - 127 - 13));
+    const float sc = __uint_as_float((uint32_t)(127 - e) << 23);            // 2^-e, exact
+    if (threadIdx.x == 0) *inv_scale = __uint_as_float((uint32_t)(127 + e) << 23);
+    for (int64_t k = (int64_t)threadIdx.x * 8; k < K; k += 256 * 8) {
+        const float4 a = load_f4(xr + k), b = load_f4(xr + k + 4);
+        __half2 h0 = __floats2half2_rn(a.x * sc, a.y * sc), h1 = __floats2half2_rn(a.z * sc, a.w * sc);
+        __half2 h2 = __floats2half2_rn(b.x * sc, b.y * sc), h3 = __floats2half2_rn(b.z * sc, b.w * sc);
+        uint4 o; o.x = h2u(h0); o.y = h2u(h1); o.z = h2u(h2); o.w = h2u(h3);
+        *(uint4 *)(xh + k) = o;
+    }
+}
+
+__global__ void __launch_bounds__(256) x_to_f16_kernel(const float * __restrict__ x, size_t nb11, __half * __restrict__ xh, float * __restrict__ inv_scale, int64_t K) {
+    // programmatic dependent launch (no-ops for a plain launch): the GEMM that follows may start its prologue and its weight stream
+    // now; this kernel itself waits for its predecessor (which may have produced x, and may still be reading the fp16 buffer)
+    pdl_launch_dependents();
+    pdl_wait();
+    const int64_t n = blockIdx.x;
+    row_to_f16((const float *)((const uint8_t *)x + n * nb11), xh + n * K, inv_scale + n, K);
 }
 
 template <int T, bool GROUPED = false>
@@ -276,37 +323,37 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     }
 }
 
-// ----------------------------------------------------------------------------- split-K flags: persistent, zero-initialised, self-cleaning
-constexpr int T2_FLAG_SLOTS = 64, T2_FLAGS_PER_SLOT = 256;
-static unsigned int * tc_flag_block() {
-    static unsigned int * ptr[64] = { nullptr };
-    static std::mutex mu;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { set_error("tc flags: cudaGetDevice failed"); return nullptr; }
-    std::lock_guard<std::mutex> lock(mu);
-    if (!ptr[dev]) {
-        unsigned int * p = nullptr;
-        const size_t bytes = (size_t)T2_FLAG_SLOTS * T2_FLAGS_PER_SLOT * sizeof(unsigned int);
-        cudaError_t e = cudaMalloc(&p, bytes);
-        if (e == cudaSuccess) e = cudaMemset(p, 0, bytes);
-        if (e == cudaSuccess) e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) { set_error("tc flags: %s", cudaGetErrorString(e)); cudaGetLastError(); if (p) cudaFree(p); return nullptr; }
-        ptr[dev] = p;
-    }
-    return ptr[dev];
-}
-int tc_prepare_device() { return tc_flag_block() ? GGML_B200_OK : GGML_B200_ECUDA; }
-unsigned int * tc_flag_slot() {
-    unsigned int * b = tc_flag_block();
+// ----------------------------------------------------------------------------- host side
+// the next slot of split-K flags in the device's control block: zeroed once, left clean by every launch that used it
+static unsigned int * tc_flag_slot() {
+    unsigned int * b = control_block();
     if (!b) return nullptr;
     static std::atomic<unsigned> seq{0};
-    return b + (size_t)(seq.fetch_add(1, std::memory_order_relaxed) % T2_FLAG_SLOTS) * T2_FLAGS_PER_SLOT;
+    return b + CTL_SPLITK_FLAGS + (size_t)(seq.fetch_add(1, std::memory_order_relaxed) % TC_FLAG_SLOTS) * TC_FLAGS_PER_SLOT;
 }
 
-// this kernel records no per-CTA stamp trace
-int tc2_trace_read(unsigned long long * host_dst, int max_ctas) { (void)host_dst; (void)max_ctas; return 0; }
+// activations f32 -> fp16 rows with an exact power-of-two scale per row (inv_scale[n] undoes it in the epilogue)
+static int tc_launch_x_to_f16(const float * x, size_t nb11, __half * xh, float * inv_scale, int64_t K, int64_t N, cudaStream_t st) {
+    B200_CUDA_TRY(launch_pdl(x_to_f16_kernel, dim3((unsigned)N), dim3(256), 0, st, x, nb11, xh, inv_scale, K));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
 
-// ----------------------------------------------------------------------------- host side
+// cuTensorMapEncodeTiled from the driver (nullptr without one: no GEMM shape is eligible then)
+typedef CUresult (*encode_tiled_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
+                                    const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static encode_tiled_fn tc_get_encode() {
+    static encode_tiled_fn fn = nullptr;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        void * p = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess) fn = (encode_tiled_fn)p;
+        else cudaGetLastError();
+    });
+    return fn;
+}
+
 struct tc2_plan {
     int BN, m_tiles, n_tiles, splitk, chunks, nstages, smem, grid;
     size_t xb_bytes, partial_bytes, scale_bytes;
@@ -355,7 +402,7 @@ static bool make_tc2_plan(const ggml_b200_mul_mat_args & a, tc2_plan & pl) {
     int splitk = sm_count() / tiles; if (splitk < 1) splitk = 1; if (splitk > 8) splitk = 8; if (splitk > pl.chunks) splitk = pl.chunks;
     static const int env_splitk = getenv("GGML_B200_TC_SPLITK") ? atoi(getenv("GGML_B200_TC_SPLITK")) : 0;
     if (env_splitk > 0 && env_splitk <= pl.chunks) splitk = env_splitk;
-    if (splitk > 1 && tiles > T2_FLAGS_PER_SLOT) splitk = 1;
+    if (splitk > 1 && tiles > TC_FLAGS_PER_SLOT) splitk = 1;
     pl.splitk = splitk;
     if (!tc2_smem_plan(BN, raw, pl.nstages, pl.smem)) return false;
     pl.grid = tiles * splitk;
@@ -527,30 +574,7 @@ __global__ void __launch_bounds__(256) mmid_x_to_f16_kernel(const uint8_t * __re
     const int pos = blockIdx.x;
     if (pos >= off[n_expert]) return;                            // positions past the valid pairs (invalid expert ids) stay unused
     const int pr = perm[pos], t = pr / n_used, e = pr % n_used;
-    const float * xr = (const float *)(b + (size_t)t * nb12 + (size_t)(e % nb1cols) * nb11);
-    __shared__ float s_max[8];
-    float amax = 0.0f;
-    for (int64_t k = (int64_t)threadIdx.x * 8; k < K; k += 256 * 8) {
-        const float4 a = load_f4(xr + k), c = load_f4(xr + k + 4);
-        amax = fmaxf(amax, fmaxf(fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))), fmaxf(fmaxf(fabsf(c.x), fabsf(c.y)), fmaxf(fabsf(c.z), fabsf(c.w)))));
-    }
-    amax = warp_max(amax);
-    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = amax;
-    __syncthreads();
-    amax = s_max[0];
-#pragma unroll
-    for (int i = 1; i < 8; ++i) amax = fmaxf(amax, s_max[i]);
-    int ex = 0;
-    if (amax > 0.0f && amax <= 3.0e38f) ex = max(-100, min(100, (int)((__float_as_uint(amax) >> 23) & 0xFF) - 127 - 13));
-    const float sc = __uint_as_float((uint32_t)(127 - ex) << 23);
-    if (threadIdx.x == 0) inv_scale[pos] = __uint_as_float((uint32_t)(127 + ex) << 23);
-    for (int64_t k = (int64_t)threadIdx.x * 8; k < K; k += 256 * 8) {
-        const float4 a = load_f4(xr + k), c = load_f4(xr + k + 4);
-        __half2 h0 = __floats2half2_rn(a.x * sc, a.y * sc), h1 = __floats2half2_rn(a.z * sc, a.w * sc);
-        __half2 h2 = __floats2half2_rn(c.x * sc, c.y * sc), h3 = __floats2half2_rn(c.z * sc, c.w * sc);
-        uint4 o; o.x = h2u(h0); o.y = h2u(h1); o.z = h2u(h2); o.w = h2u(h3);
-        *(uint4 *)(xh + (size_t)pos * K + k) = o;
-    }
+    row_to_f16((const float *)(b + (size_t)t * nb12 + (size_t)(e % nb1cols) * nb11), xh + (size_t)pos * K, inv_scale + pos, K);
 }
 
 struct mmid_g_plan { int BN, m_tiles, max_tiles, chunks, nstages, smem; size_t xb_bytes, scale_bytes, tab_bytes, perm_bytes; int64_t n_pairs; };

@@ -257,7 +257,7 @@ template <int T> static int launch_mma(const ggml_b200_mul_mat_args & a, cudaStr
     if (!a.workspace || a.workspace_size < need) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, need); return GGML_B200_EWORKSPACE; }
     uint8_t * rec = (uint8_t *)(((uintptr_t)a.workspace + 255) & ~(uintptr_t)255);
     pl.p.rec_global = rec;
-    unsigned int * ctl = sb_control_block();
+    unsigned int * ctl = control_block();
     if (!ctl) return GGML_B200_ECUDA;
     static const bool e_dynamic = getenv("GGML_B200_MMA_DYNAMIC") && atoi(getenv("GGML_B200_MMA_DYNAMIC")) != 0;
     pl.p.counters = e_dynamic ? sb_next_slot(ctl) : nullptr;

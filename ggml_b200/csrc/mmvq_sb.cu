@@ -29,7 +29,6 @@
 
 #include <atomic>
 #include <cstdlib>
-#include <mutex>
 
 namespace b200 {
 
@@ -278,33 +277,6 @@ __global__ void gather_wait_kernel(const uint32_t * flags, int world, uint32_t e
 
 struct sb_plan { sb_params p; int grid, smem, nw, nc; bool two; };
 
-// device control block: [0,64) global control words, [64, 64 + 64*8) 64 per-launch scheduling slots, byte 4096.. trace.
-// One per device, allocated on first use under a mutex (or ahead of time by ggml_b200_prepare, which the backend calls at
-// device initialisation so that no allocation can fall inside a stream capture) and kept for the life of the process.
-static unsigned int * sb_counters() {
-    static unsigned int * ptr[64] = { nullptr };
-    static std::mutex mu;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { set_error("control block: cudaGetDevice failed"); return nullptr; }
-    std::lock_guard<std::mutex> lock(mu);
-    if (!ptr[dev]) {
-        unsigned int * p = nullptr;
-        cudaError_t e = cudaMalloc(&p, 8192);
-        if (e == cudaSuccess) e = cudaMemset(p, 0, 8192);
-        if (e == cudaSuccess) e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) {
-            set_error("control block: %s", cudaGetErrorString(e));
-            cudaGetLastError();
-            if (p) cudaFree(p);
-            return nullptr;
-        }
-        ptr[dev] = p;
-    }
-    return ptr[dev];
-}
-
-int prepare_device() { return sb_counters() ? GGML_B200_OK : GGML_B200_ECUDA; }
-unsigned int * sb_control_block() { return sb_counters(); }
 static std::atomic<unsigned> g_sb_slot_seq{0};
 unsigned int * sb_next_slot(unsigned int * ctl) { return ctl + 64 + (g_sb_slot_seq.fetch_add(1, std::memory_order_relaxed) % 64u) * 8; }
 
@@ -395,7 +367,7 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
 // a launch takes the next of the 64 scheduling slots of this device's control block (self-resetting counters: a slot is free again
 // when its launch has finished scheduling, and 64 launches never overlap on one device) and, in trace mode, the next trace record
 static int assign_sb_slot(sb_params & p) {
-    p.ctl = sb_counters();
+    p.ctl = control_block();
     if (!p.ctl) return GGML_B200_ECUDA;
     p.counters = sb_next_slot(p.ctl);
     static const bool env_dbg = getenv("GGML_B200_SB_DEBUG") && atoi(getenv("GGML_B200_SB_DEBUG")) != 0;
@@ -451,7 +423,7 @@ int launch_mmvq_sb(const ggml_b200_mul_mat_args & a, cudaStream_t st, const ggml
 }
 
 int debug_read_trace(unsigned long long * out) {
-    unsigned int * c = sb_counters();
+    unsigned int * c = control_block();
     if (!c) return GGML_B200_ECUDA;
     B200_CUDA_TRY(cudaDeviceSynchronize());
     B200_CUDA_TRY(cudaMemcpy(out, c + 1024, 32 * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
@@ -459,7 +431,7 @@ int debug_read_trace(unsigned long long * out) {
 }
 
 int launch_gather_wait(const uint32_t * flags, int world, uint32_t epoch, cudaStream_t st) {
-    gather_wait_kernel<<<1, 32, 0, st>>>(flags, world, epoch, sb_counters());
+    gather_wait_kernel<<<1, 32, 0, st>>>(flags, world, epoch, control_block());
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

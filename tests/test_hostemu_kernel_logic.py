@@ -236,7 +236,7 @@ TC_TYPES = [O.Q4_0, O.Q8_0, O.Q4_K, O.Q5_K, O.Q6_K, O.Q4_1, O.Q5_0, O.Q5_1, O.IQ
 
 @pytest.mark.parametrize("t", TC_TYPES, ids=[O.TYPE_NAMES[t] for t in TC_TYPES])
 def test_gemm_operand_dequantization_matches_oracle(t, emu, oracle):
-    """mmq_tc.cu's packed-half dequantization (integer code -> 1024 + code by PRMT, HSUB2, HMUL2 / HFMA2): every fp16 weight within
+    """the GEMM's packed-half dequantization (b200_tc_dequant.cuh, mmq_tc2.cu; integer code -> 1024 + code by PRMT, HSUB2, HMUL2 / HFMA2): every fp16 weight within
     fp16 rounding of the oracle's exact dequantization (the scale product and the result are each rounded once to fp16)"""
     rng = np.random.default_rng(800 + t)
     K = 1024
