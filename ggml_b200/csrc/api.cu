@@ -1,6 +1,8 @@
-// api.cu — extern "C" kernel-launch shim (include/ggml-b200.h, layer 1): argument validation, kernel-family
-// selection, workspace accounting.  No CPU fallback anywhere: unsupported combinations return an error code.
+// api.cu — extern "C" kernel-launch shim (include/ggml-b200.h, layer 1): argument validation, kernel selection, workspace
+// accounting.  route() picks the kernel of a mul_mat call and keeps the plan it made for it (b200_mm_plan.h): the workspace query
+// reports that plan's workspace and the launch runs that plan.  No CPU fallback anywhere: unsupported combinations return an error code.
 #include "b200_internal.h"
+#include "b200_mm_plan.h"
 #include "b200_quants.cuh"
 
 #include <algorithm>
@@ -76,49 +78,54 @@ static int validate(const ggml_b200_mul_mat_args * a) {
 // chunks shrink to a few rows there; at K = 8192 the dp4a kernel is still the faster one; threshold chosen on a Blackwell part, not re-measured
 // on the H100).
 // GGML_B200_MMA = 0 never, 2 always; per call GGML_B200_MM_GEMV_MMA / GGML_B200_MM_GEMV_DP4A select explicitly
-static bool mma_wanted(const ggml_b200_mul_mat_args & a) {
+static bool mma_wanted(const ggml_b200_mul_mat_args & a, mma_plan & pl) {
     static const int env = getenv("GGML_B200_MMA") ? atoi(getenv("GGML_B200_MMA")) : 1;
     if (a.flags & (GGML_B200_MM_GEMV_V1 | GGML_B200_MM_GEMV_DP4A)) return false;
     if (!(a.flags & GGML_B200_MM_GEMV_MMA) && (env == 0 || (a.N < 2 && env != 2 && a.K < 12288))) return false;
-    return mmvq_mma_eligible(a);
+    return plan_mma(a, pl);
 }
 
-// The kernel one mul_mat call runs.  The workspace query, the launch and the fused entry point all read it from route(), so they cannot
-// disagree.
-enum route_kind {
-    R_GENERIC,     // one warp per output (mmvq.cu): any shape
-    R_TMA,         // first-generation 64-weight-unit mat-vec (mmvq.cu)
-    R_SB,          // superblock mat-vec (mmvq_sb.cu), all columns in one launch
-    R_SB_GROUPS,   // superblock mat-vec in column groups of `group`
-    R_MMA,         // int8 mma.sync mat-vec (mmvq_mma.cu)
-    R_WGMMA,       // warpgroup-MMA GEMM (mmq_tc2.cu)
-    R_DENSE,       // W dequantized to fp16, then the same GEMM (mmq_tc2.cu)
-};
-struct mm_route { route_kind kind = R_GENERIC; int64_t group = 0; };
+// columns [c0, c0 + g) of a, or to the last column
+static ggml_b200_mul_mat_args column_group(const ggml_b200_mul_mat_args & a, int64_t c0, int64_t g) {
+    ggml_b200_mul_mat_args sub = a;
+    sub.N = std::min<int64_t>(g, a.N - c0);
+    sub.src1 = (const float *)((const char *)a.src1 + (size_t)c0 * a.nb11);
+    sub.dst = a.dst + (size_t)c0 * a.M;
+    return sub;
+}
 
-// GGML_B200_EUNSUPPORTED when a forced family cannot run the shape; sets no error message
-static int route(const ggml_b200_mul_mat_args & a, mm_route & r) {
+static int chosen(mm_plan & pl, route_kind kind, size_t workspace) {
+    pl.kind = kind;
+    pl.workspace = workspace;
+    return GGML_B200_OK;
+}
+
+// The kernel one mul_mat call runs, with its plan.  The workspace query, the launch and the fused entry point all read it from route(),
+// so they cannot disagree.  GGML_B200_EUNSUPPORTED when a forced family cannot run the shape, or when the last of the column groups
+// cannot be planned; sets no error message.
+static int route(const ggml_b200_mul_mat_args & a, mm_plan & pl) {
     static const bool env_generic = getenv("GGML_B200_FORCE_GENERIC") && atoi(getenv("GGML_B200_FORCE_GENERIC")) != 0;   // debugging aid
-    r = mm_route{};
-    if (env_generic || (a.flags & GGML_B200_MM_FORCE_GENERIC)) return GGML_B200_OK;
+    pl.group = 0;
+    if (env_generic || (a.flags & GGML_B200_MM_FORCE_GENERIC)) return chosen(pl, R_GENERIC, mmvq_generic_workspace(a));
     const bool force_gemv = (a.flags & GGML_B200_MM_FORCE_GEMV) != 0;
     if (!force_gemv && ((a.flags & GGML_B200_MM_FORCE_GEMM) || a.N > 8)) {
-        if (mmq_dense_eligible(a)) r.kind = R_DENSE;             // formats without an operand decoder (n >= 9 only)
-        else if (mmq_tc2_eligible(a)) r.kind = R_WGMMA;          // n >= 5 only
-        else if (a.flags & GGML_B200_MM_FORCE_GEMM) return GGML_B200_EUNSUPPORTED;
-        return GGML_B200_OK;
+        if (plan_dense(a, pl.dense)) return chosen(pl, R_DENSE, pl.dense.workspace);     // formats without an operand decoder (n >= 9 only)
+        if (plan_wgmma(a, pl.wgmma)) return chosen(pl, R_WGMMA, pl.wgmma.workspace);     // n >= 5 only
+        if (a.flags & GGML_B200_MM_FORCE_GEMM) return GGML_B200_EUNSUPPORTED;
+        return chosen(pl, R_GENERIC, mmvq_generic_workspace(a));
     }
     // the mat-vec family: forced, or n <= 8
-    if (mma_wanted(a)) { r.kind = R_MMA; return GGML_B200_OK; }   // never under GEMV_V1
-    const bool sb = mmvq_sb_eligible(a);
+    if (mma_wanted(a, pl.mma)) return chosen(pl, R_MMA, pl.mma.workspace);   // never under GEMV_V1
+    const bool sb = plan_sb(a, pl.sb);
     // 5..8 columns of very long rows: the superblock kernel would need two column-group launches (each re-streaming W, issue-bound); the
     // tensor-core kernel takes them in one pass (fp16-operand tolerance instead of the integer-exact dot: DESIGN.md section 3)
-    if (!force_gemv && a.N >= 5 && !sb && mmq_tc2_eligible(a)) { r.kind = R_WGMMA; return GGML_B200_OK; }
+    if (!force_gemv && a.N >= 5 && !sb && plan_wgmma(a, pl.wgmma)) return chosen(pl, R_WGMMA, pl.wgmma.workspace);
     const bool v1 = (a.flags & GGML_B200_MM_GEMV_V1) != 0;      // the first-generation kernel whenever the family is the mat-vec one
-    if (sb && !v1) { r.kind = R_SB; return GGML_B200_OK; }
-    if (!mmvq_tma_eligible(a) && (force_gemv || !sb)) return force_gemv ? GGML_B200_EUNSUPPORTED : GGML_B200_OK;
-    r.kind = R_TMA;
-    if (v1) return GGML_B200_OK;
+    if (sb && !v1) return chosen(pl, R_SB, 0);
+    const bool tma = plan_tma(a, pl.tma);
+    if (!tma && (force_gemv || !sb)) return force_gemv ? GGML_B200_EUNSUPPORTED : chosen(pl, R_GENERIC, mmvq_generic_workspace(a));
+    if (!tma) return chosen(pl, R_TMA_UNFIT, 0);                // v1 and sb here
+    if (v1) return chosen(pl, R_TMA, 0);
     // long rows x many columns: the activation records of all columns do not fit next to the weight stages.  Column groups of 4 / 2 / 1
     // on the same kernel re-stream W per group, which is far cheaper than leaving the bandwidth kernel (columns are independent: results
     // are bit-identical to the one-launch form).  This form is only reached when the first-generation kernel is eligible for the whole
@@ -126,15 +133,18 @@ static int route(const ggml_b200_mul_mat_args & a, mm_route & r) {
     // kernel would take its column groups.
     if (a.N > 1 && a.ne02 == 1 && a.ne03 == 1 && a.ne12 == 1 && a.ne13 == 1) {
         for (int64_t g = 4; g >= 1; g >>= 1) {
-            ggml_b200_mul_mat_args sub = a;
-            sub.N = g;
-            if (g < a.N && mmvq_sb_eligible(sub)) { r.kind = R_SB_GROUPS; r.group = g; return GGML_B200_OK; }
+            if (g < a.N && plan_sb(column_group(a, 0, g), pl.sb)) {
+                // every group is planned before the first one launches
+                if (a.N % g != 0 && !plan_sb(column_group(a, a.N - a.N % g, g), pl.sb_tail)) return GGML_B200_EUNSUPPORTED;
+                pl.group = g;
+                return chosen(pl, R_SB_GROUPS, 0);
+            }
         }
     }
-    return GGML_B200_OK;
+    return chosen(pl, R_TMA, 0);
 }
 
-static int family(int rc, const mm_route & r) {
+static int family(int rc, const mm_plan & r) {
     if (rc != GGML_B200_OK) return rc;
     switch (r.kind) {
         case R_GENERIC: return GGML_B200_MM_FORCE_GENERIC;
@@ -181,21 +191,14 @@ int ggml_b200_quantize_activations(int32_t weight_type, const float * src, size_
 int ggml_b200_mul_mat_plan(const ggml_b200_mul_mat_args * args) {
     const int rc = validate(args);
     if (rc != GGML_B200_OK) return rc;
-    mm_route r;
-    return family(route(*args, r), r);
+    mm_plan pl;
+    return family(route(*args, pl), pl);
 }
 
 size_t ggml_b200_mul_mat_workspace_size(const ggml_b200_mul_mat_args * args) {
     if (validate(args) != GGML_B200_OK) return 0;
-    mm_route r;
-    if (route(*args, r) != GGML_B200_OK) return mmvq_generic_workspace(*args);
-    switch (r.kind) {
-        case R_TMA: case R_SB: case R_SB_GROUPS: return 0;
-        case R_MMA:   return mmvq_mma_workspace(*args);
-        case R_WGMMA: return mmq_tc2_workspace(*args);
-        case R_DENSE: return mmq_dense_workspace(*args);
-        default:      return mmvq_generic_workspace(*args);
-    }
+    mm_plan pl;
+    return route(*args, pl) == GGML_B200_OK ? pl.workspace : mmvq_generic_workspace(*args);
 }
 
 int ggml_b200_mul_mat(const ggml_b200_mul_mat_args * args, void * stream) {
@@ -203,22 +206,19 @@ int ggml_b200_mul_mat(const ggml_b200_mul_mat_args * args, void * stream) {
     if (rc != GGML_B200_OK) return rc;
     if (args->M == 0 || args->N == 0) return GGML_B200_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    mm_route r;
-    if (route(*args, r) != GGML_B200_OK) { set_error("mul_mat: the forced kernel family cannot run this shape"); return GGML_B200_EUNSUPPORTED; }
-    switch (r.kind) {
-        case R_TMA:   return launch_mmvq_tma(*args, st);
-        case R_SB:    return launch_mmvq_sb(*args, st);
-        case R_MMA:   return launch_mmvq_mma(*args, st);
-        case R_WGMMA: return launch_mmq_tc2(*args, st);
-        case R_DENSE: return launch_mmq_dense(*args, st);
+    mm_plan pl;
+    if (route(*args, pl) != GGML_B200_OK) { set_error("mul_mat: the forced kernel family cannot run this shape"); return GGML_B200_EUNSUPPORTED; }
+    switch (pl.kind) {
+        case R_TMA:   return launch_tma(*args, pl.tma, st);
+        case R_TMA_UNFIT: set_error("mul_mat: shape not eligible for the TMA mat-vec kernel"); return GGML_B200_EUNSUPPORTED;
+        case R_SB:    return launch_sb(*args, pl.sb, st);
+        case R_MMA:   return launch_mma(*args, pl.mma, st);
+        case R_WGMMA: return launch_wgmma(*args, pl.wgmma, st);
+        case R_DENSE: return launch_dense(*args, pl.dense, st);
         case R_SB_GROUPS:
-            for (int64_t c0 = 0; c0 < args->N; c0 += r.group) {
-                ggml_b200_mul_mat_args sub = *args;
-                sub.N = std::min<int64_t>(r.group, args->N - c0);
-                sub.src1 = (const float *)((const char *)args->src1 + (size_t)c0 * args->nb11);
-                sub.dst = args->dst + (size_t)c0 * args->M;
-                if (!mmvq_sb_eligible(sub)) { set_error("mul_mat: column group not eligible"); return GGML_B200_EUNSUPPORTED; }
-                rc = launch_mmvq_sb(sub, st);
+            for (int64_t c0 = 0; c0 < args->N; c0 += pl.group) {
+                const ggml_b200_mul_mat_args sub = column_group(*args, c0, pl.group);
+                rc = launch_sb(sub, sub.N == pl.group ? pl.sb : pl.sb_tail, st);
                 if (rc != GGML_B200_OK) return rc;
             }
             return GGML_B200_OK;
@@ -238,10 +238,11 @@ int ggml_b200_mul_mat_fused(const ggml_b200_mul_mat_args * args, const ggml_b200
     if (rc != GGML_B200_OK) return rc;
     if (!ep || !ep->bias || !ep->dst_bias || (ep->unary < 0 || ep->unary > 2) || (ep->unary != 0 && !ep->dst_unary) || (ep->unary == 2 && !ep->residual)) { set_error("mul_mat_fused: bad epilogue"); return GGML_B200_EINVAL; }
     // also where the unfused route is the mma kernel (n = 1, very long rows): the epilogue exists on the superblock kernel only
-    mm_route r;
-    if (args->N != 1 || family(route(*args, r), r) != GGML_B200_MM_FORCE_GEMV || !mmvq_sb_eligible(*args)) { set_error("mul_mat_fused: only the n = 1 mat-vec kernel has the fused epilogue"); return GGML_B200_EUNSUPPORTED; }
+    mm_plan r;
+    sb_plan pl;
+    if (args->N != 1 || family(route(*args, r), r) != GGML_B200_MM_FORCE_GEMV || !plan_sb(*args, pl)) { set_error("mul_mat_fused: only the n = 1 mat-vec kernel has the fused epilogue"); return GGML_B200_EUNSUPPORTED; }
     if (args->M == 0) return GGML_B200_OK;
-    return launch_mmvq_sb(*args, (cudaStream_t)stream, nullptr, ep);
+    return launch_sb(*args, pl, (cudaStream_t)stream, nullptr, ep);
 }
 
 int ggml_b200_mul_mat_gather(const ggml_b200_mul_mat_args * args, const ggml_b200_gather * ga, void * stream) {
@@ -249,12 +250,14 @@ int ggml_b200_mul_mat_gather(const ggml_b200_mul_mat_args * args, const ggml_b20
     if (rc != GGML_B200_OK) return rc;
     if (!ga || ga->world < 1 || ga->world > 8 || ga->rank < 0 || ga->rank >= ga->world) { set_error("mul_mat_gather: bad gather descriptor"); return GGML_B200_EINVAL; }
     for (int q = 0; q < ga->world; ++q) if (!ga->y_peers[q] || !ga->flag_peers[q]) { set_error("mul_mat_gather: NULL peer pointer"); return GGML_B200_EINVAL; }
-    if (args->N != 1 || !mmvq_sb_eligible(*args)) { set_error("mul_mat_gather: only the n = 1 mat-vec path supports the fused gather"); return GGML_B200_EUNSUPPORTED; }
-    return launch_mmvq_sb(*args, (cudaStream_t)stream, ga);
+    sb_plan pl;
+    if (args->N != 1 || !plan_sb(*args, pl)) { set_error("mul_mat_gather: only the n = 1 mat-vec path supports the fused gather"); return GGML_B200_EUNSUPPORTED; }
+    return launch_sb(*args, pl, (cudaStream_t)stream, ga);
 }
 
 int ggml_b200_mul_mat_gather_supported(const ggml_b200_mul_mat_args * args) {
-    return validate(args) == GGML_B200_OK && args->N == 1 && mmvq_sb_eligible(*args) ? 1 : 0;
+    sb_plan pl;
+    return validate(args) == GGML_B200_OK && args->N == 1 && plan_sb(*args, pl) ? 1 : 0;
 }
 
 int ggml_b200_debug_trace(unsigned long long * out256) { return debug_read_trace(out256); }

@@ -71,38 +71,38 @@ template <auto Kernel> cudaError_t set_max_dynamic_smem(int bytes) {
         B200_CUDA_TRY(cudaGetLastError());                                                          \
     } while (0)
 
+// Kernel families: plan_X is true when family X can run the shape and fills the plan (types in b200_mm_plan.h); launch_X runs a plan
+// plan_X made from the same arguments without planning again, and of the arguments checks only the workspace size.
+struct tma_plan; struct sb_plan; struct mma_plan; struct tc2_plan; struct dense_plan; struct mmid_g_plan;
+
 // mmvq.cu
 int    launch_quantize_activations(int type, const float * x, int64_t K, int64_t n11, int64_t n12, int64_t n13,
                                    size_t nb11, size_t nb12, size_t nb13, void * recs, cudaStream_t st);
 int    launch_mmvq_generic(const ggml_b200_mul_mat_args & a, cudaStream_t st);
-bool   mmvq_tma_eligible(const ggml_b200_mul_mat_args & a);
-int    launch_mmvq_tma(const ggml_b200_mul_mat_args & a, cudaStream_t st);
 size_t mmvq_generic_workspace(const ggml_b200_mul_mat_args & a);
+bool   plan_tma(const ggml_b200_mul_mat_args & a, tma_plan & pl);
+int    launch_tma(const ggml_b200_mul_mat_args & a, const tma_plan & pl, cudaStream_t st);
 // mmvq_sb.cu (n = 1 bandwidth path)
-bool   mmvq_sb_eligible(const ggml_b200_mul_mat_args & a);
-int    launch_mmvq_sb(const ggml_b200_mul_mat_args & a, cudaStream_t st, const ggml_b200_gather * ga = nullptr, const ggml_b200_epilogue * ep = nullptr);
+bool   plan_sb(const ggml_b200_mul_mat_args & a, sb_plan & pl);
+int    launch_sb(const ggml_b200_mul_mat_args & a, const sb_plan & pl, cudaStream_t st, const ggml_b200_gather * ga = nullptr, const ggml_b200_epilogue * ep = nullptr);
 int    debug_read_trace(unsigned long long * out);
 int    launch_gather_wait(const uint32_t * flags, int world, uint32_t epoch, cudaStream_t st);
 unsigned int * sb_next_slot(unsigned int * ctl);   // the next of the 64 self-resetting scheduling slots
 int64_t l2_prefetch_cap();                         // bytes of W a dependent mat-vec launch pulls into L2 ahead of its predecessor's output
 
-// mmvq_mma.cu (bandwidth path, int8 mma.sync consume phase: 2 <= n <= 8, n = 1 on request)
-bool   mmvq_mma_eligible(const ggml_b200_mul_mat_args & a);
-int    launch_mmvq_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st);
-size_t mmvq_mma_workspace(const ggml_b200_mul_mat_args & a);   // the quantized activation records (written by the pre-kernel)
+// mmvq_mma.cu (bandwidth path, int8 mma.sync consume phase: 2 <= n <= 8, n = 1 on request); workspace: the quantized activation records
+bool   plan_mma(const ggml_b200_mul_mat_args & a, mma_plan & pl);
+int    launch_mma(const ggml_b200_mul_mat_args & a, const mma_plan & pl, cudaStream_t st);
 
 // mmq_tc2.cu (the wgmma GEMM kernel: quantized W with an operand decoder, n >= 5)
-bool   mmq_tc2_eligible(const ggml_b200_mul_mat_args & a);
-size_t mmq_tc2_workspace(const ggml_b200_mul_mat_args & a);
-int    launch_mmq_tc2(const ggml_b200_mul_mat_args & a, cudaStream_t st);
-bool   mmq_dense_eligible(const ggml_b200_mul_mat_args & a);   // n >= 9, formats without an operand decoder: dequantize to fp16 + the same GEMM
-size_t mmq_dense_workspace(const ggml_b200_mul_mat_args & a);
-int    launch_mmq_dense(const ggml_b200_mul_mat_args & a, cudaStream_t st);
+bool   plan_wgmma(const ggml_b200_mul_mat_args & a, tc2_plan & pl);
+int    launch_wgmma(const ggml_b200_mul_mat_args & a, const tc2_plan & pl, cudaStream_t st);
+bool   plan_dense(const ggml_b200_mul_mat_args & a, dense_plan & pl);   // n >= 9, formats without an operand decoder: dequantize to fp16 + the same GEMM
+int    launch_dense(const ggml_b200_mul_mat_args & a, const dense_plan & pl, cudaStream_t st);
 size_t mmq_f16w_workspace(int64_t M, int64_t N, int64_t K);         // dense fp16 weights, n >= 9 (0 = not eligible)
 int    launch_mmq_f16w(const void * w, size_t nb01, const float * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * ws, size_t ws_size, uint32_t flags, cudaStream_t st);
-// expert-grouped MUL_MAT_ID on the GEMM kernel (mmq_tc2.cu)
-bool   mmid_grouped_eligible(const ggml_b200_mul_mat_id_args & a);
-size_t mmid_grouped_workspace(const ggml_b200_mul_mat_id_args & a);
-int    launch_mmid_grouped(const ggml_b200_mul_mat_id_args & a, cudaStream_t st);
+// expert-grouped MUL_MAT_ID on the GEMM kernel (mmq_tc2.cu); the caller checks the workspace
+bool   plan_mmid_grouped(const ggml_b200_mul_mat_id_args & a, mmid_g_plan & pl);
+int    launch_mmid_grouped(const ggml_b200_mul_mat_id_args & a, const mmid_g_plan & pl, cudaStream_t st);
 
 } // namespace b200

@@ -6,6 +6,7 @@
 // vector dst[t][e][:] = as[ids[t][e]] . b[t][e % nb1cols] is an independent quantized mat-vec whose expert
 // index is read by the kernel itself, so the op is one quantize launch + one mat-vec launch, no host sync.
 #include "b200_internal.h"
+#include "b200_mm_plan.h"
 #include "b200_quants.cuh"
 #include "b200_iq.cuh"
 #include "b200_ptx.cuh"
@@ -46,6 +47,17 @@ __global__ void __launch_bounds__(128) mmid_kernel(mmid_params p) {
     if (lane == 0) p.y[(size_t)pair * p.M + m] = acc;
 }
 
+// The form a MUL_MAT_ID call runs and the workspace it requires: expert-grouped on the GEMM kernel (batched tokens), else one
+// quantized mat-vec per (token, slot) pair over activation records b[K, nb1cols, n_tok] -> record t * nb1cols + c.
+struct mmid_plan { bool grouped; mmid_g_plan g; size_t workspace; };
+
+static mmid_plan plan_mmid(const ggml_b200_mul_mat_id_args & a) {
+    mmid_plan pl;
+    pl.grouped = plan_mmid_grouped(a, pl.g);
+    pl.workspace = pl.grouped ? pl.g.workspace : (size_t)make_act_layout(a.K, type_is_kquant(a.type)).bytes * (size_t)(a.nb1cols * a.n_tok) + 64;
+    return pl;
+}
+
 } // namespace b200
 
 using namespace b200;
@@ -54,8 +66,7 @@ extern "C" {
 
 size_t ggml_b200_mul_mat_id_workspace_size(const ggml_b200_mul_mat_id_args * a) {
     if (!a || type_bytes(a->type) == 0 || a->K <= 0) return 0;
-    if (mmid_grouped_eligible(*a)) return mmid_grouped_workspace(*a);
-    return (size_t)make_act_layout(a->K, type_is_kquant(a->type)).bytes * (size_t)(a->nb1cols * a->n_tok) + 64;
+    return plan_mmid(*a).workspace;
 }
 
 int ggml_b200_mul_mat_id(const ggml_b200_mul_mat_id_args * a, void * stream) {
@@ -66,11 +77,10 @@ int ggml_b200_mul_mat_id(const ggml_b200_mul_mat_id_args * a, void * stream) {
     if (!a->src0 || !a->src1 || !a->ids || !a->dst) { set_error("mul_mat_id: NULL tensor pointer"); return GGML_B200_EINVAL; }
     if ((a->nb11 & 3) || (a->nb12 & 3) || (a->ids_nb1 & 3) || (a->nb01 & 1) || (a->nb02 & 1)) { set_error("mul_mat_id: bad strides"); return GGML_B200_EINVAL; }
     if ((a->type == T_Q4_K || a->type == T_Q5_K) && (((uintptr_t)a->src0 | a->nb01 | a->nb02) & 15)) { set_error("mul_mat_id: Q4_K/Q5_K rows must be 16-byte aligned"); return GGML_B200_EINVAL; }
-    const size_t need = ggml_b200_mul_mat_id_workspace_size(a);
-    if (!a->workspace || a->workspace_size < need) { set_error("mul_mat_id: workspace %zu < %zu", a->workspace_size, need); return GGML_B200_EWORKSPACE; }
+    const mmid_plan pl = plan_mmid(*a);
+    if (!a->workspace || a->workspace_size < pl.workspace) { set_error("mul_mat_id: workspace %zu < %zu", a->workspace_size, pl.workspace); return GGML_B200_EWORKSPACE; }
     cudaStream_t st = (cudaStream_t)stream;
-    if (mmid_grouped_eligible(*a)) return launch_mmid_grouped(*a, st);      // batched tokens: rows grouped per expert on the device, tensor cores
-    // b[K, nb1cols, n_tok] -> records indexed t * nb1cols + c
+    if (pl.grouped) return launch_mmid_grouped(*a, pl.g, st);
     int rc = launch_quantize_activations(a->type, a->src1, a->K, a->nb1cols, a->n_tok, 1, a->nb11, a->nb12, 0, a->workspace, st);
     if (rc != GGML_B200_OK) return rc;
     mmid_params p;

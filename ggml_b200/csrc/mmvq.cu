@@ -15,6 +15,7 @@
 //   mmvq_generic_kernel any K / strides / batch / broadcast: one warp per output element straight from
 //                       global memory, activations pre-quantized by quantize_act_kernel.
 #include "b200_internal.h"
+#include "b200_mm_plan.h"
 #include "b200_quants.cuh"
 #include "b200_iq.cuh"
 #include "b200_ptx.cuh"
@@ -109,22 +110,6 @@ int launch_mmvq_generic(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
 
 // =============================================================================== TMA-staged bandwidth kernel
 constexpr int TMA_MAX_STAGES = 8;
-
-struct tma_params {
-    const uint8_t * w;        // row 0, 16-byte aligned, rows contiguous (nb01 == row_bytes)
-    const float *   x;        // activation columns
-    float *         y;        // [N][M]
-    size_t          nb11;     // activation column stride (bytes)
-    int64_t         M, K;
-    int32_t         N;        // valid columns (<= NC)
-    int32_t         row_bytes;
-    int32_t         RB;       // rows per stage
-    int32_t         P, G;     // warps = G row-groups x P k-parts
-    int32_t         nchunks;  // ceil(M / RB)
-    int32_t         stage_bytes;   // RB * row_bytes rounded up to 128
-    int32_t         nstages;
-    act_layout      L;
-};
 
 // transposing shuffle reduction of 4 per-lane values: returns, in every lane, the full sum of value
 // number ((lane >> 3) & 3); 6 shuffles instead of 20
@@ -234,12 +219,7 @@ __global__ void __launch_bounds__(256) mmvq_tma_kernel(const tma_params p) {
     }
 }
 
-struct tma_plan {
-    tma_params p;
-    int grid, block, smem, nc, r;
-};
-
-static bool make_tma_plan(const ggml_b200_mul_mat_args & a, tma_plan & pl) {
+bool plan_tma(const ggml_b200_mul_mat_args & a, tma_plan & pl) {
     if (!with_format(TMA_FORMATS(), a.type, [](auto) {})) return false;   // the other formats: generic kernel
     if (a.N < 1 || a.N > 8 || a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
     if (a.K % 64 != 0 || a.K < 64 || a.M < 1) return false;                 // whole units; Q4_0/Q8_0 pairs 4-byte aligned
@@ -293,11 +273,6 @@ static bool make_tma_plan(const ggml_b200_mul_mat_args & a, tma_plan & pl) {
     return true;
 }
 
-bool mmvq_tma_eligible(const ggml_b200_mul_mat_args & a) {
-    tma_plan pl;
-    return make_tma_plan(a, pl);
-}
-
 template <int T, int NC, int R> static int launch_tma_inst(const tma_plan & pl, cudaStream_t st) {
     B200_CUDA_TRY(set_max_dynamic_smem<mmvq_tma_kernel<T, NC, R>>(200 * 1024));
     mmvq_tma_kernel<T, NC, R><<<pl.grid, pl.block, pl.smem, st>>>(pl.p);
@@ -314,10 +289,8 @@ template <int T> static int launch_tma_type(const tma_plan & pl, cudaStream_t st
     }
 }
 
-int launch_mmvq_tma(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
-    tma_plan pl;
-    if (!make_tma_plan(a, pl)) { set_error("mul_mat: shape not eligible for the TMA mat-vec kernel"); return GGML_B200_EUNSUPPORTED; }
-    int rc = GGML_B200_EUNSUPPORTED;                                 // make_tma_plan accepts TMA_FORMATS only
+int launch_tma(const ggml_b200_mul_mat_args & a, const tma_plan & pl, cudaStream_t st) {
+    int rc = GGML_B200_EUNSUPPORTED;                                 // plan_tma accepts TMA_FORMATS only
     with_format(TMA_FORMATS(), a.type, [&](auto t) { rc = launch_tma_type<t>(pl, st); });
     return rc;
 }

@@ -17,6 +17,7 @@
 // kernel pulls them into shared memory with one bulk copy per column while its first weight stages are in flight.  (First version:
 // every CTA quantized all columns itself, on the critical path of every CTA.)
 #include "b200_internal.h"
+#include "b200_mm_plan.h"
 #include "b200_quants.cuh"
 #include "b200_ptx.cuh"
 #include "b200_sb_mma.cuh"
@@ -29,18 +30,6 @@ namespace b200 {
 constexpr int MMA_MAX_STAGES = 8;
 constexpr int MMA_TILE = 16;             // rows per tile (the m of m16n8k32)
 constexpr int MMA_GROUP_WARPS = 8;       // consumer warps per group
-
-struct mma_params {
-    const uint8_t * w; const float * x; float * y;
-    int64_t M, K;
-    int32_t row_bytes, ntiles, nslices, ks, ntask_row, pitch, stage_bytes, nstages;
-    unsigned int * counters;      // null: tiles dealt round-robin; else this launch's scheduling slot: [0] next tile, [1] finished producers
-    int32_t ncols; int64_t x_stride;
-    int32_t src1_static, src0_static;
-    int64_t l2_prefetch_bytes;
-    const uint8_t * rec_global;   // ncols planar records written by mma_quantize_kernel (workspace)
-    mma_act A;
-};
 
 // one act-task (256 activations of one column) per half-warp.  Always waits for the preceding kernel: it may have produced x, and the
 // records live in the launch-shared workspace that the previous mat-mul's CTAs may still be reading.
@@ -183,8 +172,6 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
     }
 }
 
-struct mma_plan { mma_params p; int grid, smem, ng; };
-
 template <int T> static bool make_mma_plan(const ggml_b200_mul_mat_args & a, mma_plan & pl) {
     using F = mmafmt<T>;
     if (a.N < 1 || a.N > 8 || a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
@@ -235,12 +222,11 @@ template <int T> static bool make_mma_plan(const ggml_b200_mul_mat_args & a, mma
         p.nstages = nst;
         pl.smem = (int)(fixed + (size_t)ng * p.nstages * p.stage_bytes);
         pl.grid = std::min(sm_count(), (p.ntiles + ng - 1) / ng);
+        pl.workspace = (size_t)p.ncols * p.A.col_bytes + 256;       // the activation records, 256-byte aligned
         return true;
     }
     return false;
 }
-
-static size_t mma_rec_bytes(const mma_plan & pl) { return (size_t)pl.p.ncols * pl.p.A.col_bytes; }
 
 template <int T, int NG> static int launch_mma_ng(const mma_plan & pl, cudaStream_t st) {
     B200_CUDA_TRY(set_max_dynamic_smem<mmvq_mma_kernel<T, NG>>(227 * 1024));
@@ -249,12 +235,9 @@ template <int T, int NG> static int launch_mma_ng(const mma_plan & pl, cudaStrea
     return GGML_B200_OK;
 }
 
-template <int T> static int launch_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
+template <int T> static int launch_mma_t(const ggml_b200_mul_mat_args & a, mma_plan pl, cudaStream_t st) {
     using F = mmafmt<T>;
-    mma_plan pl;
-    if (!make_mma_plan<T>(a, pl)) { set_error("mul_mat: shape not eligible for the mma small-batch kernel"); return GGML_B200_EUNSUPPORTED; }
-    const size_t need = mma_rec_bytes(pl) + 256;
-    if (!a.workspace || a.workspace_size < need) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, need); return GGML_B200_EWORKSPACE; }
+    if (!a.workspace || a.workspace_size < pl.workspace) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, pl.workspace); return GGML_B200_EWORKSPACE; }
     uint8_t * rec = (uint8_t *)(((uintptr_t)a.workspace + 255) & ~(uintptr_t)255);
     pl.p.rec_global = rec;
     unsigned int * ctl = control_block();
@@ -267,28 +250,15 @@ template <int T> static int launch_mma(const ggml_b200_mul_mat_args & a, cudaStr
     return pl.ng == 1 ? launch_mma_ng<T, 1>(pl, st) : launch_mma_ng<T, 2>(pl, st);
 }
 
-static bool mma_plan_of(const ggml_b200_mul_mat_args & a, mma_plan & pl) {
+bool plan_mma(const ggml_b200_mul_mat_args & a, mma_plan & pl) {
     bool ok = false;
     with_format(TC_FORMATS(), a.type, [&](auto t) { ok = make_mma_plan<t>(a, pl); });
     return ok;
 }
 
-size_t mmvq_mma_workspace(const ggml_b200_mul_mat_args & a) {
-    mma_plan pl;
-    return mma_plan_of(a, pl) ? mma_rec_bytes(pl) + 256 : 0;
-}
-
-bool mmvq_mma_eligible(const ggml_b200_mul_mat_args & a) {
-    mma_plan pl;
-    return mma_plan_of(a, pl);
-}
-
-int launch_mmvq_mma(const ggml_b200_mul_mat_args & a, cudaStream_t st) {
-    int rc = GGML_B200_OK;
-    if (!with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_mma<t>(a, st); })) {
-        set_error("mul_mat: unsupported weight type %d", a.type);
-        return GGML_B200_EUNSUPPORTED;
-    }
+int launch_mma(const ggml_b200_mul_mat_args & a, const mma_plan & pl, cudaStream_t st) {
+    int rc = GGML_B200_EUNSUPPORTED;                                 // plan_mma accepts TC_FORMATS only
+    with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_mma_t<t>(a, pl, st); });
     return rc;
 }
 

@@ -23,6 +23,7 @@
 // Weights are read once from HBM in the reference's packed layout.  Numerics are those of b200_quants.cuh
 // (int8 activations quantized as ggml-cpu does, integer dots, f32 scaling); only the f32 summation order differs.
 #include "b200_internal.h"
+#include "b200_mm_plan.h"
 #include "b200_quants.cuh"
 #include "b200_ptx.cuh"
 #include "b200_sb_tasks.cuh"   // dp4a_us, task geometry, activation-record layout, task dot products (also compiled for the host by tests/hostemu)
@@ -34,29 +35,6 @@ namespace b200 {
 
 // ----------------------------------------------------------------------------- kernel
 constexpr int SB_MAX_STAGES = 6;
-
-struct sb_params {
-    const uint8_t * w; const float * x; float * y;
-    int64_t M, K;
-    int32_t row_bytes, rows_per_chunk, nchunks, stage_bytes, nstages, ntasks_row;
-    unsigned int * counters;      // this launch's scheduling slot: [0] next chunk, [1] finished producers, [2] finished CTAs (all return to 0)
-    unsigned int * ctl;           // device-global control words: [0] exchange epoch, [1] trace launch index
-    int32_t ncols; int64_t x_stride;   // activation columns (1..8) and the distance between them in floats; y is [ncols][M]
-    int32_t src1_static;          // activations are not produced by the preceding kernel either: never wait for it (independent ops overlap)
-    int32_t src0_static;          // weights are not produced by the preceding kernel: prefetch them before griddepcontrol.wait
-    int32_t static_chunks;        // chunks dealt round-robin instead of by the atomic counter
-    int64_t l2_prefetch_bytes;    // dependent launches: bytes of W every CTA's share of which is pulled into L2 while the previous kernel still runs (0 = off)
-    // row-sharded multi-GPU: every result is stored straight into each peer's full-length y over NVLink (world == 0: off)
-    // fused epilogue (bias add and GELU of the following ggml nodes): y2 = y + bias, y3 = gelu(y2); null = off
-    const float * ep_bias; float * ep_y2; float * ep_y3; const float * ep_res;    // ep_res: y3 = y2 + residual instead of gelu(y2)
-    unsigned long long * dbg;     // optional %globaltimer trace (GGML_B200_SB_DEBUG=1): 32 launches x 8 stamps
-    int32_t world, rank;
-    int64_t row_offset;
-    uint32_t epoch;
-    float *    y_peers[8];
-    uint32_t * flag_peers[8];
-    sb_act A;
-};
 
 template <int T, int NW, int NC, bool TWO = false>
 __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) mmvq_sb_kernel(const sb_params p) {
@@ -275,8 +253,6 @@ __global__ void gather_wait_kernel(const uint32_t * flags, int world, uint32_t e
     __threadfence_system();
 }
 
-struct sb_plan { sb_params p; int grid, smem, nw, nc; bool two; };
-
 static std::atomic<unsigned> g_sb_slot_seq{0};
 unsigned int * sb_next_slot(unsigned int * ctl) { return ctl + 64 + (g_sb_slot_seq.fetch_add(1, std::memory_order_relaxed) % 64u) * 8; }
 
@@ -325,12 +301,13 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
         if ((size_t)rpc * rb > 100 * 1024) return false;
     }
     sb_params & p = pl.p;
-    p.w = (const uint8_t *)a.src0; p.x = a.src1; p.y = a.dst; p.M = a.M; p.K = a.K;
+    p.M = a.M; p.K = a.K;
     p.row_bytes = (int)rb; p.rows_per_chunk = rpc; p.nchunks = (int)((a.M + rpc - 1) / rpc);
     p.stage_bytes = (int)(((size_t)rpc * rb + 127) & ~(size_t)127);
     p.nstages = env_stages;       // 0 = automatic (below)
     p.ntasks_row = (int)(a.K / F::TASK_W);
     p.A = make_sb_act(a.K);
+    p.w = nullptr; p.x = nullptr; p.y = nullptr;                 // bound at launch (launch_sb_t)
     p.ctl = nullptr; p.counters = nullptr; p.dbg = nullptr;      // assigned at launch (assign_sb_slot): planning has no side effects
     p.src0_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
     const int64_t l2_cap = l2_prefetch_cap();
@@ -383,9 +360,8 @@ template <int T, int NW, int NC, bool TWO = false> static int launch_sb_nw(sb_pl
     return GGML_B200_OK;
 }
 
-template <int T> static int launch_sb(const ggml_b200_mul_mat_args & a, const ggml_b200_gather * ga, cudaStream_t st, const ggml_b200_epilogue * ep = nullptr) {
-    sb_plan pl;
-    if (!make_sb_plan<T>(a, pl)) { set_error("mul_mat: shape not eligible for the superblock mat-vec kernel"); return GGML_B200_EUNSUPPORTED; }
+template <int T> static int launch_sb_t(const ggml_b200_mul_mat_args & a, sb_plan pl, const ggml_b200_gather * ga, cudaStream_t st, const ggml_b200_epilogue * ep) {
+    pl.p.w = (const uint8_t *)a.src0; pl.p.x = a.src1; pl.p.y = a.dst;
     { const int rc = assign_sb_slot(pl.p); if (rc != GGML_B200_OK) return rc; }
     if (ep && ep->bias) {
         pl.p.ep_bias = ep->bias; pl.p.ep_y2 = ep->dst_bias; pl.p.ep_y3 = ep->unary != 0 ? ep->dst_unary : nullptr;
@@ -406,19 +382,15 @@ template <int T> static int launch_sb(const ggml_b200_mul_mat_args & a, const gg
     }
 }
 
-bool mmvq_sb_eligible(const ggml_b200_mul_mat_args & a) {
-    sb_plan pl;
+bool plan_sb(const ggml_b200_mul_mat_args & a, sb_plan & pl) {
     bool ok = false;
     with_format(TC_FORMATS(), a.type, [&](auto t) { ok = make_sb_plan<t>(a, pl); });
     return ok;
 }
 
-int launch_mmvq_sb(const ggml_b200_mul_mat_args & a, cudaStream_t st, const ggml_b200_gather * ga, const ggml_b200_epilogue * ep) {
-    int rc = GGML_B200_OK;
-    if (!with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_sb<t>(a, ga, st, ep); })) {
-        set_error("mul_mat: unsupported weight type %d", a.type);
-        return GGML_B200_EUNSUPPORTED;
-    }
+int launch_sb(const ggml_b200_mul_mat_args & a, const sb_plan & pl, cudaStream_t st, const ggml_b200_gather * ga, const ggml_b200_epilogue * ep) {
+    int rc = GGML_B200_EUNSUPPORTED;                                 // plan_sb accepts TC_FORMATS only
+    with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_sb_t<t>(a, pl, ga, st, ep); });
     return rc;
 }
 
