@@ -59,7 +59,7 @@ struct sb_params {
 };
 
 // w, x and y are bound at launch: the plan of one column group serves every group of its width
-struct sb_plan { sb_params p; int grid, smem, nw, nc; bool two; };
+struct sb_plan { sb_params p; int grid, smem, nw, nc; bool two, act_regs; };
 
 // ----------------------------------------------------------------------------- int8 mma.sync mat-vec (mmvq_mma.cu)
 struct mma_params {

@@ -645,6 +645,119 @@ template <bool FIVE> __device__ __forceinline__ void q45_task2(const uint8_t * w
     }
 }
 
+// ----------------------------------------------------------------------------- activation-stationary form (Q4_K / Q5_K, n = 1, K <= 4096)
+// With at most 16 tasks per row one warp covers a whole row, so a lane's task is the same in every row of the launch.  Lanes 2t and
+// 2t+1 own task t (superblock t of every row); lane 2t + h takes its 64-weight chunks 2h and 2h+1, with the sub-block scales and mins
+// of sc_lo / mn_lo (h = 0) or sc_hi / mn_hi (h = 1).  Each lane loads its half of act-task t from the shared record into registers
+// once (32 code words, two h32 words, the scale) and from then on reads only weights from shared memory.
+// The halves' integer sums are added with an xor-1 shuffle before the f32 scaling, so each task's float is the one q45_task returns,
+// and the row is reduced over lanes xor 16, 8, 4, 2: the tree of the task-per-lane kernel (xor 8, 4, 2, 1 over task indices).
+// The result is bit-identical to the task-per-lane kernel's, and so to column c of the n-column kernel.
+struct q45_acts {
+    int y[32];       // codes 128 h .. 128 h + 127 of act-task t
+    int h32[2];      // the 32-sums of sub-blocks 4h .. 4h + 3, int16 pairs
+    float d;         // the act-task's scale
+};
+__device__ __forceinline__ void q45_load_acts(const uint8_t * rec, int t, int h, q45_acts & A) {
+    const uint8_t * a = rec + (size_t)t * SB_REC;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { const int4 v = lds128(a + 128 * h + 16 * i); A.y[4 * i] = v.x; A.y[4 * i + 1] = v.y; A.y[4 * i + 2] = v.z; A.y[4 * i + 3] = v.w; }
+    const uint2 hv = *(const uint2 *)(a + SB_OFF_H32 + 8 * h);
+    A.h32[0] = (int)hv.x; A.h32[1] = (int)hv.y;
+    A.d = *(const float *)(a + SB_OFF_D);
+}
+
+// chunk C (0, 1) of this lane's half: q45_chunk with the activations taken from registers (qh already shifted by 4h)
+template <int C, bool FIVE>
+__device__ __forceinline__ void q45_chunk_regs(const uint8_t * qs, const uint32_t (&qh)[8], const int (&y)[32], int sc0, int sc1, int & acc_s) {
+    const int4 qa = lds128(qs + 32 * C), qb = lds128(qs + 32 * C + 16);
+    const uint32_t q[8] = { (uint32_t)qa.x, (uint32_t)qa.y, (uint32_t)qa.z, (uint32_t)qa.w, (uint32_t)qb.x, (uint32_t)qb.y, (uint32_t)qb.z, (uint32_t)qb.w };
+    int p0 = 0, p1 = 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t qq = q[4 * h + i];
+            const int yl = y[16 * C + 4 * h + i], yh = y[16 * C + 8 + 4 * h + i];
+            if constexpr (FIVE) {
+                const uint32_t hb = qh[4 * h + i] >> (2 * C);
+                p0 = __dp4a((int)((qq & 0x0F0F0F0F) | ((hb & 0x01010101) << 4)), yl, p0);
+                p1 = __dp4a((int)(((qq >> 4) & 0x0F0F0F0F) | ((hb & 0x02020202) << 3)), yh, p1);
+            } else {
+                p0 = __dp4a((int)(qq & 0x0F0F0F0F), yl, p0);
+                p1 = dp4a_us(qq & 0xF0F0F0F0u, yh, p1);
+            }
+        }
+    }
+    if constexpr (!FIVE) p1 >>= 4;
+    acc_s += sc0 * p0 + sc1 * p1;
+}
+
+// this lane's half of task t of one row (w = the task's first byte): integer sums and the task's d | dmin word
+template <bool FIVE> __device__ __forceinline__ void q45_half_regs(const uint8_t * w, const q45_acts & A, int h, int & acc_s, int & acc_m, uint32_t & dm) {
+    const int4 hdr = lds128(w);                                         // d | dmin | scales[12]
+    uint32_t qh[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
+    if constexpr (FIVE) {
+        const int4 ha = lds128(w + 16), hb = lds128(w + 32);
+        const uint32_t raw[8] = { (uint32_t)ha.x, (uint32_t)ha.y, (uint32_t)ha.z, (uint32_t)ha.w, (uint32_t)hb.x, (uint32_t)hb.y, (uint32_t)hb.z, (uint32_t)hb.w };
+#pragma unroll
+        for (int i = 0; i < 8; ++i) qh[i] = raw[i] >> (4 * h);
+    }
+    const uint8_t * qs = w + (FIVE ? 48 : 16) + 64 * h;
+    const uint32_t s0 = hdr.y, s1 = hdr.z, s2 = hdr.w;
+    const uint32_t sc = h ? ((s2 & 0x0F0F0F0Fu) | ((s0 >> 2) & 0x30303030u)) : (s0 & 0x3F3F3F3Fu);
+    const uint32_t mn = h ? (((s2 >> 4) & 0x0F0F0F0Fu) | ((s1 >> 2) & 0x30303030u)) : (s1 & 0x3F3F3F3Fu);
+    acc_m = dp2a_lo_su(A.h32[0], mn, 0);
+    acc_m = dp2a_hi_su(A.h32[1], mn, acc_m);
+    acc_s = 0;
+    q45_chunk_regs<0, FIVE>(qs, qh, A.y, ubyte<0>(sc), ubyte<1>(sc), acc_s);
+    q45_chunk_regs<1, FIVE>(qs, qh, A.y, ubyte<2>(sc), ubyte<3>(sc), acc_s);
+    dm = (uint32_t)hdr.x;
+}
+
+// R rows (a power of two, mmvq_sb.cu takes 2; row j's first byte at row[j]) against the activations.  All 32 lanes call this together; lanes whose task is
+// beyond the row (t >= ntasks) contribute 0, as idle lanes of the task-per-lane kernel do.  Row j's dot product is returned in lanes
+// 32 j / R .. 32 (j + 1) / R - 1.  While rows remain to be split, a reduction step exchanges rows (a lane keeps the rows of its side of
+// the xor distance and sends the others), so R rows cost one shuffle per row and step at most, and each row is still summed by the
+// tree xor 16, 8, 4, 2.
+template <bool FIVE, int R> __device__ __forceinline__ float q45_rows_regs(const uint8_t * const (&row)[R], const q45_acts & A, int lane, int ntasks) {
+    const int t = lane >> 1, h = lane & 1;
+    int s[R], m[R];
+    uint32_t dm[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) { s[j] = 0; m[j] = 0; dm[j] = 0; }
+    if (t < ntasks) {
+#pragma unroll
+        for (int j = 0; j < R; ++j) q45_half_regs<FIVE>(row[j] + (size_t)t * (FIVE ? 176 : 144), A, h, s[j], m[j], dm[j]);
+    }
+    float x[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) {
+        s[j] += __shfl_xor_sync(0xffffffffu, s[j], 1);                 // integer sums of the whole task: exact
+        m[j] += __shfl_xor_sync(0xffffffffu, m[j], 1);
+        x[j] = 0.0f;
+        if (t < ntasks) {
+            const float d = h2f(dm[j] & 0xFFFF) * A.d, dmin = h2f(dm[j] >> 16) * A.d;
+            x[j] += d * (float)s[j] - dmin * (float)m[j];
+        }
+    }
+#pragma unroll
+    for (int n = R, o = 16; o > 1; o >>= 1) {
+        if (n > 1) {
+            const bool up = (lane & o) != 0;
+#pragma unroll
+            for (int j = 0; j < n / 2; ++j) {
+                const float keep = up ? x[n / 2 + j] : x[j], send = up ? x[j] : x[n / 2 + j];
+                x[j] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+            }
+            n /= 2;
+        } else {
+            x[0] += __shfl_xor_sync(0xffffffffu, x[0], o);
+        }
+    }
+    return x[0];
+}
+
 // ----------------------------------------------------------------------------- several activation columns (2 <= n <= 8)
 // The weights of a task are decoded once and dotted with every column's record (records of column c at rec + c * rec_stride).
 // Per column the floating-point operations are exactly those of the n = 1 path, so column c of an n-column product is

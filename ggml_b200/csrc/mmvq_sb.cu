@@ -14,12 +14,17 @@
 //     stages are in flight, into per-task records whose 368-byte pitch makes every LDS.128 bank-conflict-free;
 //   * a dedicated producer warp keeps a ring of TMA bulk copies (cp.async.bulk + mbarrier complete_tx) in flight;
 //     consumers release stages through per-stage "empty" mbarriers; chunks after the first are handed out by an
-//     atomic counter (self-resetting, one slot per launch), so SMs stay balanced to one chunk;
+//     atomic counter (self-resetting, one slot per launch), so SMs stay balanced to one chunk, or round-robin for
+//     independent launches with at most 16 chunks per CTA (no atomic round trip before a refill);
 //   * programmatic dependent launch: an independent launch (SRC0|SRC1_STATIC) runs as 4-warp CTAs of which four
 //     launches share an SM -- a pipeline across launches; a dependent launch runs 8-warp CTAs, prefetches its first
 //     stages and pulls W into L2 while its predecessor still runs, and only then waits for the predecessor's output;
 //   * 2 <= n <= 8: one activation record per column, the weights of a task are decoded once and dotted with every
-//     column (bit-identical, column by column, to the n = 1 result).
+//     column (bit-identical, column by column, to the n = 1 result);
+//   * Q4_K / Q5_K at n = 1 with K <= 4096 (at most 16 tasks per row), 4-warp CTAs: a warp covers a whole row, so each lane's task is
+//     fixed for the launch; lane pairs split a task in halves whose activations stay in registers (q45_rows_regs, 2 rows per warp
+//     and pass), and the consumers read each stage byte from shared memory once instead of re-reading the activation record for
+//     every row (bit-identical results).
 // Weights are read once from HBM in the reference's packed layout.  Numerics are those of b200_quants.cuh
 // (int8 activations quantized as ggml-cpu does, integer dots, f32 scaling); only the f32 summation order differs.
 #include "b200_internal.h"
@@ -36,7 +41,11 @@ namespace b200 {
 // ----------------------------------------------------------------------------- kernel
 constexpr int SB_MAX_STAGES = 6;
 
-template <int T, int NW, int NC, bool TWO = false>
+// how the consumer lanes split a stage: a task per lane (every format), or, for Q4_K / Q5_K at n = 1, two rows per lane group
+// sharing each activation load, or activations held in registers (a lane's task fixed for the launch, K <= 4096)
+enum sb_consume { SB_TASKS = 0, SB_TWO_ROWS = 1, SB_ACT_REGS = 2 };
+
+template <int T, int NW, int NC, int CM = SB_TASKS>
 __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) mmvq_sb_kernel(const sb_params p) {
     using F = sbfmt<T>;
     constexpr int SB_CONSUMER_WARPS = NW;
@@ -138,6 +147,11 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
     }
     asm volatile("bar.sync 1, %0;" ::"n"(SB_CONSUMER_WARPS * 32) : "memory");        // consumers only
 
+    // rows per warp and pass of the activation-stationary form (0: not used)
+    constexpr int AR = NC == 1 && (T == T_Q4_K || T == T_Q5_K) && CM == SB_ACT_REGS ? 2 : 0;
+    q45_acts acts;                                                // this lane's half of its act-task, loaded once
+    if constexpr (AR > 0) { if ((lane >> 1) < p.ntasks_row) q45_load_acts(rec, lane >> 1, lane & 1, acts); }
+
     const int sub = lane / LPR, l = lane % LPR;
     for (int it = 0;; ++it) {
         const int s = it % p.nstages;
@@ -163,7 +177,17 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
                 for (int q = 0; q < 8; ++q) if (q < p.world) p.y_peers[q][gi] = acc;
             }
         };
-        if constexpr (TWO && NC == 1 && (T == T_Q4_K || T == T_Q5_K)) {
+        if constexpr (AR > 0) {
+            // AR rows per warp and pass, the activations already in registers: only weights are read from shared memory
+            for (int r0 = warp * AR; r0 < rows; r0 += SB_CONSUMER_WARPS * AR) {
+                const uint8_t * rp[AR];
+#pragma unroll
+                for (int j = 0; j < AR; ++j) rp[j] = st + (size_t)min(r0 + j, rows - 1) * p.row_bytes;    // past the end: repeat the last row (not stored)
+                const float acc = q45_rows_regs<T == T_Q5_K, AR>(rp, acts, lane, p.ntasks_row);
+                const int r = r0 + lane / (32 / AR);
+                if (lane % (32 / AR) == 0 && r < rows) store_row(row0 + r, acc);
+            }
+        } else if constexpr (CM == SB_TWO_ROWS && NC == 1 && (T == T_Q4_K || T == T_Q5_K)) {
             // two rows per lane group and pass, sharing every activation load (each row's operations and their order are those of the
             // one-row path: bit-identical results); halves the activation traffic out of shared memory
             for (int r0 = warp * RPW * 2; r0 < rows; r0 += SB_CONSUMER_WARPS * RPW * 2) {
@@ -293,6 +317,12 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     // launches with enough tasks per row.  GGML_B200_SB_TWOROW = 0 off, 1 always
     static const int e_two = getenv("GGML_B200_SB_TWOROW") ? atoi(getenv("GGML_B200_SB_TWOROW")) : 2;
     pl.two = nc == 1 && (T == T_Q4_K || T == T_Q5_K) && (e_two == 1 || (e_two == 2 && !ind && a.K >= 2048 && a.M >= 2048 && (size_t)(SB_CONSUMER_WARPS * RPW * 2) * rb <= 100 * 1024));
+    // activations held in registers (Q4_K / Q5_K, n = 1, at most 16 tasks per row) in the 4-warp kernel of independent launches: each stage
+    // byte is read from shared memory once instead of with a re-read activation record (faster on an H100 at 400 W; the 8-warp kernel of
+    // dependent launches, where it measured slower than the two-row form, keeps the shared-memory paths).  The chunk geometry is unchanged.
+    // GGML_B200_SB_ACT_REGS = 0 keeps the shared-memory consume paths everywhere
+    static const int e_areg = getenv("GGML_B200_SB_ACT_REGS") ? atoi(getenv("GGML_B200_SB_ACT_REGS")) : 1;
+    pl.act_regs = e_areg != 0 && nc == 1 && (T == T_Q4_K || T == T_Q5_K) && a.K <= 16 * 256 && SB_CONSUMER_WARPS == 4;
     int granule = 1; while ((granule * rb) % 16 != 0) granule *= 2;
     int step = SB_CONSUMER_WARPS * RPW * (pl.two ? 2 : 1); while (step % granule != 0) step *= 2;
     int rpc = (int)(((size_t)env_stage_kb * 1024) / rb) / step * step; if (rpc < step) rpc = step;
@@ -315,9 +345,9 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     p.world = 0; p.rank = 0; p.row_offset = 0; p.epoch = 0;
     p.ep_bias = nullptr; p.ep_y2 = nullptr; p.ep_y3 = nullptr; p.ep_res = nullptr;
     p.src1_static = (a.flags & GGML_B200_MM_SRC1_STATIC) ? 1 : 0;
-    // GGML_B200_SB_STATIC: 0 = dynamic hand-out everywhere, 1 = round-robin everywhere, 2 = round-robin for dependent launches only
-    static const int e_static = getenv("GGML_B200_SB_STATIC") ? atoi(getenv("GGML_B200_SB_STATIC")) : 0;
-    p.static_chunks = (e_static == 1 || (e_static == 2 && !ind)) ? 1 : 0;
+    // GGML_B200_SB_STATIC: 0 = dynamic hand-out everywhere, 1 = round-robin everywhere, 2 = round-robin for dependent launches only;
+    // unset: round-robin for independent launches with few chunks per CTA (below)
+    static const int e_static = getenv("GGML_B200_SB_STATIC") ? atoi(getenv("GGML_B200_SB_STATIC")) : -1;
     p.ncols = (int32_t)a.N; p.x_stride = a.N > 1 ? (int64_t)(a.nb11 / 4) : 0;
     for (int q = 0; q < 8; ++q) { p.y_peers[q] = nullptr; p.flag_peers[q] = nullptr; }
     auto smem_of = [&]() { return p.nstages * p.stage_bytes + nc * p.A.bytes + 2 * SB_MAX_STAGES * 8 + SB_MAX_STAGES * 4 + 64; };
@@ -338,6 +368,12 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     pl.smem = smem_of();
     pl.grid = sm_count() * ctas;
     if (pl.grid > p.nchunks) pl.grid = p.nchunks;
+    // Independent launches with at most 16 chunks per CTA take them round-robin: the producer's atomic round trip before each refill is
+    // not hidden by two stages, and the co-resident launches absorb the imbalance of a few chunks.  With more chunks per CTA the SMs'
+    // speed differences add up and the atomic counter balances better.  Measured on an H100 at 700 W: Q4_K 4096 -> 11008 (10 chunks per
+    // CTA) 3164 instead of 3144 GB/s, Q4_0 4096 x 4096 (4) 2937 instead of 2792; Q4_K / Q8_0 4096 -> 32000 (30 / 61) 2.5 / 3.8 % slower
+    // round-robin.  Dependent launches keep the atomic counter.
+    p.static_chunks = (e_static == 1 || (e_static == 2 && !ind) || (e_static < 0 && ind && p.nchunks <= 16 * pl.grid)) ? 1 : 0;
     return true;
 }
 
@@ -353,9 +389,9 @@ static int assign_sb_slot(sb_params & p) {
     return GGML_B200_OK;
 }
 
-template <int T, int NW, int NC, bool TWO = false> static int launch_sb_nw(sb_plan & pl, cudaStream_t st) {
-    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_sb_kernel<T, NW, NC, TWO>>(222 * 1024));
-    B200_CUDA_TRY(launch_pdl(mmvq_sb_kernel<T, NW, NC, TWO>, dim3(pl.grid), dim3((NW + 1) * 32), pl.smem, st, pl.p));
+template <int T, int NW, int NC, int CM = SB_TASKS> static int launch_sb_nw(sb_plan & pl, cudaStream_t st) {
+    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_sb_kernel<T, NW, NC, CM>>(222 * 1024));
+    B200_CUDA_TRY(launch_pdl(mmvq_sb_kernel<T, NW, NC, CM>, dim3(pl.grid), dim3((NW + 1) * 32), pl.smem, st, pl.p));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
@@ -374,7 +410,10 @@ template <int T> static int launch_sb_t(const ggml_b200_mul_mat_args & a, sb_pla
     if (pl.nc > 1 && (ga || (ep && ep->bias))) { set_error("mul_mat: the fused epilogue / gather exist for n = 1 only"); return GGML_B200_EUNSUPPORTED; }
     switch (pl.nc) {
         case 1:
-            if constexpr (T == T_Q4_K || T == T_Q5_K) { if (pl.two) return pl.nw == 4 ? launch_sb_nw<T, 4, 1, true>(pl, st) : launch_sb_nw<T, 8, 1, true>(pl, st); }
+            if constexpr (T == T_Q4_K || T == T_Q5_K) {
+                if (pl.act_regs) return launch_sb_nw<T, 4, 1, SB_ACT_REGS>(pl, st);
+                if (pl.two) return pl.nw == 4 ? launch_sb_nw<T, 4, 1, SB_TWO_ROWS>(pl, st) : launch_sb_nw<T, 8, 1, SB_TWO_ROWS>(pl, st);
+            }
             return pl.nw == 4 ? launch_sb_nw<T, 4, 1>(pl, st) : launch_sb_nw<T, 8, 1>(pl, st);
         case 2:  return launch_sb_nw<T, 8, 2>(pl, st);
         case 4:  return launch_sb_nw<T, 8, 4>(pl, st);
