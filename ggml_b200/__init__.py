@@ -455,3 +455,26 @@ def op_rope(x, pos, params: RopeParams, freq_factors=None, inplace: bool = False
     f = C.byref(tensor_desc(freq_factors)) if freq_factors is not None else None
     check(L.ggml_b200_op_rope(C.byref(s), C.byref(p), f, C.byref(d), C.byref(params), _stream()), "ggml_b200_op_rope")
     return y
+
+
+def op_argsort(x, descending: bool = False):
+    """GGML_OP_ARGSORT of a contiguous f32 torch tensor along its last dim (ggml's ne0, <= 1024): int32 indices of the same shape.
+    Ties come out in ascending index and NaNs last, so every row is a permutation."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_argsort.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_int32, C.c_void_p]
+    y = torch.empty(x.shape, dtype=torch.int32, device=x.device)
+    s, d = tensor_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_argsort(C.byref(s), C.byref(d), int(descending), _stream()), "ggml_b200_op_argsort")
+    return y
+
+
+def op_sum_rows(x):
+    """GGML_OP_SUM_ROWS of a contiguous f32 torch tensor: the sums over its last dim (accumulated in double), shape [..., 1]"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_sum_rows.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p]
+    y = torch.empty(tuple(x.shape[:-1]) + (1,), dtype=torch.float32, device=x.device)
+    s, d = tensor_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_sum_rows(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_sum_rows")
+    return y

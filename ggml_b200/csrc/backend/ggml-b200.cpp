@@ -542,6 +542,15 @@ bool supports_small_op(const ggml_tensor * op) {
                    a->ne[0] % 32 == 0 && d->ne[0] % 32 == 0 && d->nb[0] == ggml_type_size(d->type) && ggml_is_contiguous(d);
         }
         case GGML_OP_ROPE: return supports_rope(op);       // GGML_OP_ROPE_BACK (training) stays declined
+        case GGML_OP_ARGSORT: {
+            // ggml-cpu reads row i at i*nb01 (ggml-cpu.c:10765): only evenly spaced rows mean the same data on both backends
+            const int32_t order = ggml_get_op_params_i32(op, 0);
+            return a->type == GGML_TYPE_F32 && a->nb[0] == sizeof(float) && op->type == GGML_TYPE_I32 && ggml_is_contiguous(op) &&
+                   a->ne[0] <= 1024 && a->nb[2] == a->ne[1] * a->nb[1] && a->nb[3] == a->ne[2] * a->nb[2] &&
+                   (order == GGML_SORT_ORDER_ASC || order == GGML_SORT_ORDER_DESC) && ggml_nrows(a) <= INT32_MAX;
+        }
+        case GGML_OP_SUM_ROWS:
+            return a->type == GGML_TYPE_F32 && op->type == GGML_TYPE_F32 && a->nb[0] == sizeof(float) && op->nb[0] == sizeof(float);
         default: return false;
     }
 }
@@ -823,6 +832,8 @@ void compute_small_op(backend_ctx * ctx, ggml_tensor * node) {
             if (node->src[2]) f = desc(node->src[2]);
             SHIM_OK(ggml_b200_op_rope(&s, &p, node->src[2] ? &f : nullptr, &d, &rp, st));
         } break;
+        case GGML_OP_ARGSORT:  { auto s = desc(a), d = desc(node); SHIM_OK(ggml_b200_op_argsort(&s, &d, ggml_get_op_params_i32(node, 0), st)); } break;
+        case GGML_OP_SUM_ROWS: { auto s = desc(a), d = desc(node); SHIM_OK(ggml_b200_op_sum_rows(&s, &d, st)); } break;
         default:
             GGML_LOG_ERROR("ggml-b200: op %s is not supported (supports_op must have declined it)\n", ggml_op_desc(node));
             GGML_ABORT("unsupported op");

@@ -6,13 +6,16 @@
 // backend (src/ggml-cpu/ggml-cpu.c):
 //   get_rows :8560-8760   add/mul bcast :4660-5560   norm :8915-8975   rms_norm :8990-9050   scale :8300-8345
 //   diag_mask :9745-9805  soft_max :9810-9925        gelu :6520-6570 (+ fp16 table, ggml-cpu.c:1355)   dup/cpy :3220-4300
-//   rope :9157-9640
-// They replace the reference's getrows.cu, binbcast.cu, norm.cu, scale.cu, diagmask.cu, softmax.cu, unary.cu, cpy.cu, mmv.cu.
+//   rope :9157-9640       argsort :10746-10783       sum_rows :5663-5694 (+ ggml_vec_sum_f32 :2118)
+// ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation.
+// They replace the reference's getrows.cu, binbcast.cu, norm.cu, scale.cu, diagmask.cu, softmax.cu, unary.cu, cpy.cu, mmv.cu, argsort.cu,
+// sumrows.cu.
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
 #include "b200_rope.cuh"
+#include "b200_sort.cuh"
 
 #include <cfloat>
 
@@ -447,6 +450,45 @@ template <typename T> __global__ void __launch_bounds__(128) rope_kernel(tdesc s
     }
 }
 
+// ------------------------------------------------------------------ ARGSORT (f32 rows of ne0 <= 1024 -> i32 indices, dst contiguous)
+// One CTA per row: the row's (key, index) items (b200_sort.cuh), padded to P = the next power of two, are sorted by the bitonic network in
+// shared memory, one compare-exchange per thread and step.  The order is a strict total order (ties by index, NaNs last), so each output
+// row is a permutation of 0 .. ne0-1: MUL_MAT_ID and GET_ROWS can index with it whatever the router produced.
+__global__ void __launch_bounds__(512) argsort_kernel(tdesc s, int32_t * dst, int P, int order) {
+    pdl_trigger();
+    __shared__ uint64_t items[SORT_MAX_COLS];
+    const int64_t r = blockIdx.x, ne0 = s.ne[0];
+    const int64_t i1 = r % s.ne[1], i2 = (r / s.ne[1]) % s.ne[2], i3 = r / (s.ne[1] * s.ne[2]);
+    const float * x = (const float *)(s.data + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
+    for (int i = threadIdx.x; i < P; i += blockDim.x) items[i] = i < ne0 ? sort_item(x[i], i, order) : sort_pad(i);
+    __syncthreads();
+    for (int k = 2; k <= P; k <<= 1)
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int t = threadIdx.x; t < P / 2; t += blockDim.x) sort_step(items, k, j, t);
+            __syncthreads();
+        }
+    int32_t * d = dst + r * ne0;
+    for (int i = threadIdx.x; i < ne0; i += blockDim.x) d[i] = (int32_t)(uint32_t)items[i];
+}
+
+// ------------------------------------------------------------------ SUM_ROWS (f32 rows, any strides -> f32 [1, ne1, ne2, ne3])
+// One warp per row.  Like ggml_vec_sum_f32 each row is accumulated in double and rounded once to f32; only the order of the f64 additions
+// differs (lane-strided partial sums, then a butterfly), so the result equals the CPU's whenever the f64 sum is exact and is otherwise
+// at most one f32 ulp apart.
+__global__ void __launch_bounds__(128) sum_rows_kernel(tdesc s, tdesc d, int64_t rows) {
+    pdl_trigger();
+    const int lane = threadIdx.x & 31;
+    const int64_t r = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (r >= rows) return;
+    const int64_t i1 = r % s.ne[1], i2 = (r / s.ne[1]) % s.ne[2], i3 = r / (s.ne[1] * s.ne[2]);
+    const float * x = (const float *)(s.data + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
+    double acc = 0.0;
+    for (int64_t i = lane; i < s.ne[0]; i += 32) acc += (double)x[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) *(float *)(d.data + i1 * d.nb[1] + i2 * d.nb[2] + i3 * d.nb[3]) = (float)acc;
+}
+
 static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
 } // namespace b200
@@ -659,6 +701,40 @@ int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos
     const dim3 grid((unsigned)s.ne[2], (unsigned)hb, (unsigned)s.ne[3]);
     if (s.type == T_F32) B200_CUDA_TRY(launch_pdl(rope_kernel<float>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
     else                 B200_CUDA_TRY(launch_pdl(rope_kernel<__half>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_argsort(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t order, void * stream) {
+    REQUIRE(src && dst, "src and dst are required");
+    if (order != SORT_ASC && order != SORT_DESC) { set_error("argsort: bad order %d (0 ascending, 1 descending)", order); return GGML_B200_EINVAL; }
+    const tdesc s = T(src), d = T(dst);
+    REQUIRE(s.type == T_F32 && d.type == 26 /* GGML_TYPE_I32 */, "src must be f32, dst i32");
+    REQUIRE(s.nb[0] == 4, "src rows must be contiguous along dim 0");
+    REQUIRE(s.ne[0] == d.ne[0] && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "src and dst shapes differ");
+    size_t nb = 4;
+    for (int i = 0; i < 4; ++i) { REQUIRE(d.ne[i] == 1 || d.nb[i] == nb, "dst must be contiguous"); nb *= (size_t)d.ne[i]; }
+    REQUIRE(s.ne[0] <= SORT_MAX_COLS, "rows longer than 1024 are not supported");
+    const int64_t rows = nrows(s);
+    if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
+    REQUIRE(rows <= 0x7fffffff, "too many rows for one grid");
+    const int P = sort_width((int)s.ne[0]);
+    const int threads = std::max(32, std::min(512, P / 2));
+    B200_CUDA_TRY(launch_pdl(argsort_kernel, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, s, (int32_t *)d.data, P, (int)order));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_sum_rows(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    REQUIRE(src && dst, "src and dst are required");
+    const tdesc s = T(src), d = T(dst);
+    REQUIRE(s.type == T_F32 && d.type == T_F32, "src and dst must be f32");
+    REQUIRE(s.nb[0] == 4 && d.nb[0] == 4, "rows must be contiguous along dim 0");
+    REQUIRE(d.ne[0] == 1 && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "dst must be [1, ne1, ne2, ne3] of src");
+    const int64_t rows = nrows(s);
+    if (rows == 0) return GGML_B200_OK;
+    REQUIRE((rows + 3) / 4 <= 0x7fffffff, "too many rows for one grid");
+    B200_CUDA_TRY(launch_pdl(sum_rows_kernel, dim3(blocks_for(rows, 4)), dim3(128), 0, (cudaStream_t)stream, s, d, rows));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

@@ -253,6 +253,13 @@ typedef struct ggml_b200_rope_params {
 } ggml_b200_rope_params;
 GGML_B200_API int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos, const ggml_b200_tensor * freq_factors, const ggml_b200_tensor * dst,
                                     const ggml_b200_rope_params * params, void * stream);
+/* GGML_OP_ARGSORT: src f32 [ne0, ne1, ne2, ne3] (any row strides, dim 0 contiguous), 1 <= ne0 <= 1024 -> dst i32 of the same shape, contiguous:
+ * per row the indices that order it ascending (order 0) or descending (order 1).  Ties come out in ascending index, -0.0 equals +0.0 and
+ * NaNs sort after every number in both orders, so each row of dst is a permutation of 0 .. ne0-1.  No allocation, no host sync. */
+GGML_B200_API int ggml_b200_op_argsort(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t order, void * stream);
+/* GGML_OP_SUM_ROWS: src f32 [ne0, ne1, ne2, ne3] (any row strides, dim 0 contiguous) -> dst f32 [1, ne1, ne2, ne3] (any strides); each row
+ * is accumulated in double and rounded once, as the CPU backend does. */
+GGML_B200_API int ggml_b200_op_sum_rows(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
