@@ -478,3 +478,59 @@ def op_sum_rows(x):
     s, d = tensor_desc(x), tensor_desc(y)
     check(L.ggml_b200_op_sum_rows(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_sum_rows")
     return y
+
+
+def strided_desc(t) -> TensorDesc:
+    """descriptor of a torch tensor with any strides (a view) in ggml order: ne[i] / nb[i] from the torch dim ndim - 1 - i"""
+    import torch
+    d = TensorDesc()
+    d.data = t.data_ptr()
+    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26}[t.dtype]
+    es = t.element_size()
+    shape, strides = list(t.shape)[::-1], list(t.stride())[::-1]
+    for i in range(4):
+        d.ne[i] = shape[i] if i < len(shape) else 1
+        d.nb[i] = strides[i] * es if i < len(shape) else (d.nb[i - 1] * d.ne[i - 1] if i else es)
+    return d
+
+
+def op_concat(a, b, dim: int):
+    """GGML_OP_CONCAT of two f32 (or two i32) torch tensors of equal rank <= 4 along ggml's dim (0 = the last torch dim): a, then b.
+    a must be contiguous along its last dim; b may be any view (a transposed one, as in the Mamba layer).  A new contiguous tensor."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_concat.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_int32, C.c_void_p]
+    shape = list(a.shape)
+    if 0 <= dim < a.dim():
+        shape[a.dim() - 1 - dim] += b.shape[a.dim() - 1 - dim]
+    y = torch.empty(shape, dtype=a.dtype, device=a.device)
+    s0, s1, d = strided_desc(a), strided_desc(b), tensor_desc(y)
+    check(L.ggml_b200_op_concat(C.byref(s0), C.byref(s1), C.byref(d), int(dim), _stream()), "ggml_b200_op_concat")
+    return y
+
+
+def op_ssm_conv(sx, c):
+    """GGML_OP_SSM_CONV: sx f32 [n_s, d_inner, d_conv - 1 + n_t] (rows packed), c f32 [d_inner, d_conv] -> f32 [n_s, n_t, d_inner],
+    out[s, t, i] = sum_k sx[s, i, t + k] * c[i, k], bit-identical to ggml-cpu"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_ssm_conv.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_void_p]
+    n_s, d_inner, ncs = sx.shape
+    y = torch.empty((n_s, ncs - c.shape[-1] + 1, d_inner), dtype=torch.float32, device=sx.device)
+    x, w, d = strided_desc(sx), strided_desc(c), tensor_desc(y)
+    check(L.ggml_b200_op_ssm_conv(C.byref(x), C.byref(w), C.byref(d), _stream()), "ggml_b200_op_ssm_conv")
+    return y
+
+
+def op_ssm_scan(s, x, dt, A, B, C_):
+    """GGML_OP_SSM_SCAN (Mamba-1): s f32 [n_s, d_inner, d_state], x and dt f32 [n_s, n_t, d_inner], A f32 [d_inner, d_state] (all four
+    contiguous), B and C f32 [n_s, n_t, d_state] (last dim contiguous, any other strides).  Returns (y [n_s, n_t, d_inner], s_new
+    [n_s, d_inner, d_state]): views of the one flat result in ggml's layout (y, then the final states)."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_ssm_scan.argtypes = [C.POINTER(TensorDesc)] * 7 + [C.c_void_p]
+    out = torch.empty(x.numel() + s.numel(), dtype=torch.float32, device=x.device)
+    t = [strided_desc(v) for v in (s, x, dt, A, B, C_)]
+    d = tensor_desc(out)
+    check(L.ggml_b200_op_ssm_scan(*[C.byref(v) for v in t], C.byref(d), _stream()), "ggml_b200_op_ssm_scan")
+    return out[: x.numel()].view(x.shape), out[x.numel():].view(s.shape)

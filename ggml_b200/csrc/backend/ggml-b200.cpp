@@ -513,6 +513,44 @@ bool supports_rope(const ggml_tensor * op) {
     return a->ne[2] <= INT32_MAX && a->ne[3] <= 65535 && (a->ne[1] + heads_per_cta - 1) / heads_per_cta <= 65535;
 }
 
+// GGML_OP_CONCAT, GGML_OP_SSM_CONV, GGML_OP_SSM_SCAN: exactly what ggml_b200_op_concat / _ssm_conv / _ssm_scan run (the CPU backend's
+// asserts, ggml-cpu.c:6104-6113, 11394-11397, 11467-11479, the constructors' in ggml.c:4443-4500, and the launch grids)
+bool supports_concat(const ggml_tensor * op) {
+    const ggml_tensor * a = op->src[0], * b = op->src[1];
+    const int32_t dim = ggml_get_op_params_i32(op, 0);
+    if (!((a->type == GGML_TYPE_F32 || a->type == GGML_TYPE_I32) && b->type == a->type && op->type == a->type)) return false;
+    if (a->nb[0] != sizeof(float) || dim < 0 || dim > 3) return false;
+    for (int k = 0; k < 4; ++k)
+        if (k == dim ? op->ne[k] != a->ne[k] + b->ne[k] : (a->ne[k] != b->ne[k] || op->ne[k] != a->ne[k])) return false;
+    return (ggml_nelements(op) + 255) / 256 <= INT32_MAX;
+}
+
+bool supports_ssm_conv(const ggml_tensor * op) {
+    const ggml_tensor * sx = op->src[0], * c = op->src[1];
+    if (sx->type != GGML_TYPE_F32 || c->type != GGML_TYPE_F32 || op->type != GGML_TYPE_F32) return false;
+    // ggml-cpu reads row i1 of c at i1 * d_conv whatever c's nb1 (ggml-cpu.c:11424): only packed rows mean the same data on both backends
+    if (sx->nb[0] != sizeof(float) || c->nb[0] != sizeof(float) || op->nb[0] != sizeof(float)) return false;
+    if (sx->nb[1] != sx->ne[0] * sizeof(float) || c->nb[1] != c->ne[0] * sizeof(float)) return false;
+    if (sx->ne[3] != 1 || c->ne[2] != 1 || c->ne[3] != 1 || c->ne[1] != sx->ne[1] || sx->ne[0] - c->ne[0] + 1 < 0) return false;
+    if (op->ne[0] != sx->ne[1] || op->ne[1] != sx->ne[0] - c->ne[0] + 1 || op->ne[2] != sx->ne[2] || op->ne[3] != 1) return false;
+    return (ggml_nelements(op) + 255) / 256 <= INT32_MAX;
+}
+
+bool supports_ssm_scan(const ggml_tensor * op) {
+    const ggml_tensor * s = op->src[0], * x = op->src[1], * dt = op->src[2], * A = op->src[3], * B = op->src[4], * C = op->src[5];
+    for (const ggml_tensor * t : { s, x, dt, A, B, C, op }) if (t->type != GGML_TYPE_F32) return false;
+    if (!ggml_is_contiguous(s) || !ggml_is_contiguous(x) || !ggml_is_contiguous(dt) || !ggml_is_contiguous(A) || !ggml_is_contiguous(op)) return false;
+    if (B->nb[0] != sizeof(float) || C->nb[0] != sizeof(float)) return false;
+    const int64_t d_state = s->ne[0], d_inner = s->ne[1], n_t = x->ne[1], n_s = s->ne[2];
+    if (s->ne[3] != 1 || x->ne[3] != 1 || B->ne[3] != 1 || A->ne[2] != 1 || A->ne[3] != 1) return false;
+    if (s->nb[0] != sizeof(float) || x->nb[0] != sizeof(float) || dt->nb[0] != sizeof(float) || A->nb[0] != sizeof(float) ||
+        s->nb[1] != d_state * sizeof(float) || s->nb[2] != d_state * d_inner * sizeof(float) || x->nb[3] != ggml_nelements(x) * sizeof(float)) return false;
+    if (x->ne[0] != d_inner || x->ne[2] != n_s || !ggml_are_same_shape(x, dt) || !ggml_are_same_shape(B, C)) return false;
+    if (A->ne[0] != d_state || A->ne[1] != d_inner || B->ne[0] != d_state || B->ne[1] != n_t || B->ne[2] != n_s) return false;
+    if (ggml_nelements(op) != ggml_nelements(x) + ggml_nelements(s)) return false;
+    return n_s <= 65535 && (d_inner + 127) / 128 <= INT32_MAX;
+}
+
 bool supports_small_op(const ggml_tensor * op) {
     const ggml_tensor * a = op->src[0], * b = op->src[1];
     switch (op->op) {
@@ -551,6 +589,9 @@ bool supports_small_op(const ggml_tensor * op) {
         }
         case GGML_OP_SUM_ROWS:
             return a->type == GGML_TYPE_F32 && op->type == GGML_TYPE_F32 && a->nb[0] == sizeof(float) && op->nb[0] == sizeof(float);
+        case GGML_OP_CONCAT:   return supports_concat(op);
+        case GGML_OP_SSM_CONV: return supports_ssm_conv(op);
+        case GGML_OP_SSM_SCAN: return supports_ssm_scan(op);
         default: return false;
     }
 }
@@ -834,6 +875,18 @@ void compute_small_op(backend_ctx * ctx, ggml_tensor * node) {
         } break;
         case GGML_OP_ARGSORT:  { auto s = desc(a), d = desc(node); SHIM_OK(ggml_b200_op_argsort(&s, &d, ggml_get_op_params_i32(node, 0), st)); } break;
         case GGML_OP_SUM_ROWS: { auto s = desc(a), d = desc(node); SHIM_OK(ggml_b200_op_sum_rows(&s, &d, st)); } break;
+        case GGML_OP_CONCAT: {
+            auto x = desc(a), y = desc(b), d = desc(node);
+            SHIM_OK(ggml_b200_op_concat(&x, &y, &d, ggml_get_op_params_i32(node, 0), st));
+        } break;
+        case GGML_OP_SSM_CONV: { auto x = desc(a), c = desc(b), d = desc(node); SHIM_OK(ggml_b200_op_ssm_conv(&x, &c, &d, st)); } break;
+        case GGML_OP_SSM_SCAN: {
+            // sources: s, x, dt, A, B, C (ggml_ssm_scan); dst = y, then the final states
+            ggml_b200_tensor t[6];
+            for (int k = 0; k < 6; ++k) t[k] = desc(node->src[k]);
+            auto d = desc(node);
+            SHIM_OK(ggml_b200_op_ssm_scan(&t[0], &t[1], &t[2], &t[3], &t[4], &t[5], &d, st));
+        } break;
         default:
             GGML_LOG_ERROR("ggml-b200: op %s is not supported (supports_op must have declined it)\n", ggml_op_desc(node));
             GGML_ABORT("unsupported op");

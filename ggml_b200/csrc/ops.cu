@@ -7,15 +7,18 @@
 //   get_rows :8560-8760   add/mul bcast :4660-5560   norm :8915-8975   rms_norm :8990-9050   scale :8300-8345
 //   diag_mask :9745-9805  soft_max :9810-9925        gelu :6520-6570 (+ fp16 table, ggml-cpu.c:1355)   dup/cpy :3220-4300
 //   rope :9157-9640       argsort :10746-10783       sum_rows :5663-5694 (+ ggml_vec_sum_f32 :2118)
-// ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation.
+//   concat :6097-6157     ssm_conv :11379-11445      ssm_scan :11449-11537
+// ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation; CONCAT, SSM_CONV and SSM_SCAN are the
+// rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer.
 // They replace the reference's getrows.cu, binbcast.cu, norm.cu, scale.cu, diagmask.cu, softmax.cu, unary.cu, cpy.cu, mmv.cu, argsort.cu,
-// sumrows.cu.
+// sumrows.cu, concat.cu (the reference has no SSM kernels).
 #include "b200_internal.h"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
 #include "b200_rope.cuh"
 #include "b200_sort.cuh"
+#include "b200_ssm.cuh"
 
 #include <cfloat>
 
@@ -489,6 +492,60 @@ __global__ void __launch_bounds__(128) sum_rows_kernel(tdesc s, tdesc d, int64_t
     if (lane == 0) *(float *)(d.data + i1 * d.nb[1] + i2 * d.nb[2] + i3 * d.nb[3]) = (float)acc;
 }
 
+// ------------------------------------------------------------------ CONCAT (f32 / i32, any dim; src0 dim 0 contiguous, src1 and dst any strides)
+// One thread per dst element, in dst's logical order; each copies one 4-byte word, so the result is bit-identical whatever the values.
+// In the Mamba layer src1 is TRANSPOSE(x): its nb0 is a row stride.
+__global__ void concat_kernel(tdesc a, tdesc b, tdesc d, int dim, int64_t n) {
+    pdl_trigger();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t i0 = i % d.ne[0], i1 = (i / d.ne[0]) % d.ne[1], i2 = (i / (d.ne[0] * d.ne[1])) % d.ne[2], i3 = i / (d.ne[0] * d.ne[1] * d.ne[2]);
+    const uint8_t * sp;
+    if (i0 < a.ne[0] && i1 < a.ne[1] && i2 < a.ne[2] && i3 < a.ne[3]) {
+        sp = a.data + i0 * a.nb[0] + i1 * a.nb[1] + i2 * a.nb[2] + i3 * a.nb[3];
+    } else {                                                    // src1, shifted back by src0's extent along dim
+        sp = b.data + (i0 - (dim == 0 ? a.ne[0] : 0)) * b.nb[0] + (i1 - (dim == 1 ? a.ne[1] : 0)) * b.nb[1] +
+                      (i2 - (dim == 2 ? a.ne[2] : 0)) * b.nb[2] + (i3 - (dim == 3 ? a.ne[3] : 0)) * b.nb[3];
+    }
+    *(uint32_t *)(d.data + i0 * d.nb[0] + i1 * d.nb[1] + i2 * d.nb[2] + i3 * d.nb[3]) = *(const uint32_t *)sp;
+}
+
+// ------------------------------------------------------------------ SSM_CONV (conv_x f32 [d_conv - 1 + n_t, d_inner, n_s], rows contiguous)
+// One thread per output dst[i1, t, s] (i1 fastest, so the stores coalesce): the d_conv-wide window of conv_x row (i1, s) starting at column
+// t, dotted with row i1 of the conv1d weight c [d_conv, d_inner] (b200_ssm.cuh: separately rounded, ascending i0, as ggml-cpu).
+__global__ void ssm_conv_kernel(tdesc sx, tdesc c, tdesc d, int64_t n) {
+    pdl_trigger();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t i1 = i % d.ne[0], t = (i / d.ne[0]) % d.ne[1], s = i / (d.ne[0] * d.ne[1]);
+    const float * win = (const float *)(sx.data + i1 * sx.nb[1] + s * sx.nb[2]) + t;
+    const float * w = (const float *)(c.data + i1 * c.nb[1]);
+    *(float *)(d.data + i1 * d.nb[0] + t * d.nb[1] + s * d.nb[2]) = ssm_conv_dot(win, w, c.ne[0]);
+}
+
+// ------------------------------------------------------------------ SSM_SCAN (the selective scan of Mamba-1)
+// One thread per (row i1, sequence s) walks the n_t tokens in order; for each it runs the d_state recurrence of b200_ssm.cuh and writes
+// y[i1, t, s] and the row's state, which is read back for the next token (as on the CPU: dst's state part is the running state).  The
+// sum over d_state stays a sequential loop in ascending i0 -- spreading it over lanes would change the summation order.  dst holds
+// y [d_inner, n_t, n_s] (x's layout) and then, from byte offset x.nb[3], the final states [d_state, d_inner, n_s] (s0's layout).
+__global__ void __launch_bounds__(128) ssm_scan_kernel(tdesc s0, tdesc x, tdesc dt, tdesc A, tdesc B, tdesc C, uint8_t * dst) {
+    pdl_trigger();
+    const int64_t i1 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, s = blockIdx.y;
+    if (i1 >= x.ne[0]) return;
+    const int64_t nc = s0.ne[0];
+    const float * a = (const float *)(A.data + i1 * A.nb[1]);
+    const float * prev = (const float *)(s0.data + i1 * s0.nb[1] + s * s0.nb[2]);
+    float * st = (float *)(dst + x.nb[3] + i1 * s0.nb[1] + s * s0.nb[2]);
+    for (int64_t t = 0; t < x.ne[1]; ++t) {
+        const float xv = *(const float *)(x.data + i1 * x.nb[0] + t * x.nb[1] + s * x.nb[2]);
+        const float dv = *(const float *)(dt.data + i1 * dt.nb[0] + t * dt.nb[1] + s * dt.nb[2]);
+        const float * b = (const float *)(B.data + t * B.nb[1] + s * B.nb[2]);
+        const float * cc = (const float *)(C.data + t * C.nb[1] + s * C.nb[2]);
+        *(float *)(dst + i1 * x.nb[0] + t * x.nb[1] + s * x.nb[2]) = ssm_scan_token(prev, st, a, b, cc, xv, dv, nc);
+        prev = st;
+    }
+}
+
 static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
 } // namespace b200
@@ -735,6 +792,75 @@ int ggml_b200_op_sum_rows(const ggml_b200_tensor * src, const ggml_b200_tensor *
     if (rows == 0) return GGML_B200_OK;
     REQUIRE((rows + 3) / 4 <= 0x7fffffff, "too many rows for one grid");
     B200_CUDA_TRY(launch_pdl(sum_rows_kernel, dim3(blocks_for(rows, 4)), dim3(128), 0, (cudaStream_t)stream, s, d, rows));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+static bool is_contiguous(const tdesc & t) {
+    size_t nb = 4;
+    for (int i = 0; i < 4; ++i) { if (t.ne[i] != 1 && t.nb[i] != nb) return false; nb *= (size_t)t.ne[i]; }
+    return true;
+}
+
+int ggml_b200_op_concat(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, int32_t dim, void * stream) {
+    REQUIRE(src0 && src1 && dst, "src0, src1 and dst are required");
+    if (dim < 0 || dim > 3) { set_error("concat: bad dim %d (0 .. 3)", dim); return GGML_B200_EINVAL; }
+    const tdesc a = T(src0), b = T(src1), d = T(dst);
+    REQUIRE((a.type == T_F32 || a.type == 26 /* GGML_TYPE_I32 */) && b.type == a.type && d.type == a.type, "src0, src1 and dst must all be f32 or all i32");
+    REQUIRE(a.nb[0] == 4, "src0 must be contiguous along dim 0");
+    for (int k = 0; k < 4; ++k) {
+        if (k == dim) REQUIRE(d.ne[k] == a.ne[k] + b.ne[k], "dst's extent along dim must be src0's plus src1's");
+        else REQUIRE(a.ne[k] == b.ne[k] && d.ne[k] == a.ne[k], "src0, src1 and dst must agree outside dim");
+    }
+    const int64_t n = nelem(d);
+    if (n == 0) return GGML_B200_OK;
+    REQUIRE((n + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    B200_CUDA_TRY(launch_pdl(concat_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, a, b, d, (int)dim, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_ssm_conv(const ggml_b200_tensor * sx, const ggml_b200_tensor * c, const ggml_b200_tensor * dst, void * stream) {
+    REQUIRE(sx && c && dst, "sx, c and dst are required");
+    const tdesc x = T(sx), w = T(c), d = T(dst);
+    REQUIRE(x.type == T_F32 && w.type == T_F32 && d.type == T_F32, "sx, c and dst must be f32");
+    REQUIRE(x.nb[0] == 4 && w.nb[0] == 4 && d.nb[0] == 4, "sx, c and dst must be contiguous along dim 0");
+    // ggml-cpu reads row i1 of sx at i1 * ne0 (it asserts so) and row i1 of c at i1 * d_conv (whatever c's nb1: only packed rows mean the
+    // same data on both backends)
+    REQUIRE(x.nb[1] == (size_t)x.ne[0] * 4 && w.nb[1] == (size_t)w.ne[0] * 4, "the rows of sx and of c must be packed (nb1 == ne0 * 4)");
+    REQUIRE(x.ne[3] == 1 && w.ne[2] == 1 && w.ne[3] == 1, "sx must be 3-D and c a matrix");
+    REQUIRE(w.ne[1] == x.ne[1] && x.ne[0] - w.ne[0] + 1 >= 0, "c must be [d_conv, d_inner] with d_conv <= ne0 of sx + 1");
+    REQUIRE(d.ne[0] == x.ne[1] && d.ne[1] == x.ne[0] - w.ne[0] + 1 && d.ne[2] == x.ne[2] && d.ne[3] == 1, "dst must be [d_inner, n_t, n_s]");
+    const int64_t n = nelem(d);
+    if (n == 0) return GGML_B200_OK;
+    REQUIRE((n + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    B200_CUDA_TRY(launch_pdl(ssm_conv_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, x, w, d, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tensor * x, const ggml_b200_tensor * dt, const ggml_b200_tensor * A,
+                          const ggml_b200_tensor * B, const ggml_b200_tensor * C, const ggml_b200_tensor * dst, void * stream) {
+    REQUIRE(s && x && dt && A && B && C && dst, "s, x, dt, A, B, C and dst are required");
+    const tdesc ts = T(s), tx = T(x), tdt = T(dt), ta = T(A), tb = T(B), tc = T(C), d = T(dst);
+    REQUIRE(ts.type == T_F32 && tx.type == T_F32 && tdt.type == T_F32 && ta.type == T_F32 && tb.type == T_F32 && tc.type == T_F32 && d.type == T_F32,
+            "all tensors must be f32");
+    REQUIRE(is_contiguous(ts) && is_contiguous(tx) && is_contiguous(tdt) && is_contiguous(ta) && is_contiguous(d), "s, x, dt, A and dst must be contiguous");
+    REQUIRE(tb.nb[0] == 4 && tc.nb[0] == 4, "B and C must be contiguous along dim 0");
+    const int64_t d_state = ts.ne[0], d_inner = ts.ne[1], n_t = tx.ne[1], n_s = ts.ne[2];
+    REQUIRE(ts.ne[3] == 1 && tx.ne[3] == 1 && tb.ne[3] == 1 && ta.ne[2] == 1 && ta.ne[3] == 1, "s, x and B must be 3-D, A a matrix");
+    // what the CPU backend asserts beyond contiguity (it also holds where a dimension is 1): the strides dst's layout is built from
+    REQUIRE(ts.nb[0] == 4 && tx.nb[0] == 4 && tdt.nb[0] == 4 && ta.nb[0] == 4 && ts.nb[1] == (size_t)d_state * 4 &&
+            ts.nb[2] == (size_t)(d_state * d_inner) * 4 && tx.nb[3] == (size_t)nelem(tx) * 4, "s and x must have packed strides");
+    REQUIRE(tx.ne[0] == d_inner && tx.ne[2] == n_s, "x must be [d_inner, n_t, n_s]");
+    for (int k = 0; k < 4; ++k) REQUIRE(tdt.ne[k] == tx.ne[k] && tc.ne[k] == tb.ne[k], "dt must have x's shape and C B's");
+    REQUIRE(ta.ne[0] == d_state && ta.ne[1] == d_inner, "A must be [d_state, d_inner]");
+    REQUIRE(tb.ne[0] == d_state && tb.ne[1] == n_t && tb.ne[2] == n_s, "B and C must be [d_state, n_t, n_s]");
+    REQUIRE(nelem(d) == nelem(tx) + nelem(ts), "dst must hold y and the final states");
+    if (d_inner == 0 || n_s == 0) return GGML_B200_OK;
+    REQUIRE(n_s <= 65535 && (d_inner + 127) / 128 <= 0x7fffffff, "too many rows / sequences for one grid");
+    B200_CUDA_TRY(launch_pdl(ssm_scan_kernel, dim3(blocks_for(d_inner, 128), (unsigned)n_s), dim3(128), 0, (cudaStream_t)stream, ts, tx, tdt, ta, tb, tc,
+                             (uint8_t *)d.data));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

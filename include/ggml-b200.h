@@ -260,6 +260,22 @@ GGML_B200_API int ggml_b200_op_argsort(const ggml_b200_tensor * src, const ggml_
 /* GGML_OP_SUM_ROWS: src f32 [ne0, ne1, ne2, ne3] (any row strides, dim 0 contiguous) -> dst f32 [1, ne1, ne2, ne3] (any strides); each row
  * is accumulated in double and rounded once, as the CPU backend does. */
 GGML_B200_API int ggml_b200_op_sum_rows(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_CONCAT: src0 and src1 both f32 or both i32 (src0 contiguous along dim 0, src1 any strides) -> dst of the same type (any strides),
+ * src1 appended after src0 along dim (0 .. 3; any other value: GGML_B200_EINVAL).  Outside dim the three shapes agree.  Copies 4-byte
+ * words, so the result is bit-identical. */
+GGML_B200_API int ggml_b200_op_concat(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, int32_t dim, void * stream);
+/* GGML_OP_SSM_CONV: sx f32 [d_conv - 1 + n_t, d_inner, n_s] (packed rows: nb1 == ne0 * 4; any nb2), c f32 [d_conv, d_inner] (packed rows too:
+ * the CPU backend reads row i1 of c at i1 * d_conv whatever its nb1)
+ * -> dst f32 [d_inner, n_t, n_s] (dim 0 contiguous): dst[i1, t, s] = sum_{i0 < d_conv} sx[t + i0, i1, s] * c[i0, i1], each product and sum
+ * rounded separately in ascending i0, bit-identical to the CPU backend. */
+GGML_B200_API int ggml_b200_op_ssm_conv(const ggml_b200_tensor * sx, const ggml_b200_tensor * c, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_SSM_SCAN (Mamba-1): s f32 [d_state, d_inner, n_s], x and dt f32 [d_inner, n_t, n_s], A f32 [d_state, d_inner] (all four contiguous),
+ * B and C f32 [d_state, n_t, n_s] (dim 0 contiguous, any nb1 / nb2: views of x_db) -> dst f32, contiguous, ne(x) + ne(s) elements: y in x's
+ * layout, then from byte offset x.nb[3] the final states in s's layout.  Per row and sequence, token by token:
+ * dt' = softplus(dt) (dt above 20 kept), state = state * exp(dt' A) + B (x dt'), y = sum over d_state of state * C, in the CPU backend's
+ * order and rounding; any d_state (the states are kept in dst, not in registers), n_s <= 65535. */
+GGML_B200_API int ggml_b200_op_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tensor * x, const ggml_b200_tensor * dt, const ggml_b200_tensor * A,
+                                        const ggml_b200_tensor * B, const ggml_b200_tensor * C, const ggml_b200_tensor * dst, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
