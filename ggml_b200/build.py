@@ -98,12 +98,12 @@ def build_backend(force: bool = False, staged: Path | None = None) -> Path | Non
     ggml = next((d for d in cands if (d / "src" / "ggml-backend-impl.h").exists()), None)
     if ggml is None:
         raise RuntimeError(f"the ggml headers are not available to build {BACKEND_SO} (looked in {', '.join(map(str, cands))})")
-    deps = [src, ROOT / "include" / "ggml-b200.h", ROOT / "include" / "ggml-b200-backend.h", KERNELS_SO]
+    deps = [src, ROOT / "include" / "ggml-b200.h", ROOT / "include" / "ggml-b200-backend.h", CSRC / "b200_op_checks.h", KERNELS_SO]
     if not force and _newer(BACKEND_SO, deps):
         return BACKEND_SO
     cmd = [_nvcc(), "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared",
            "-DGGML_BACKEND_DL", "-DGGML_BACKEND_SHARED", "-DGGML_BACKEND_BUILD", "-DGGML_SHARED",
-           f"-I{ggml}/include", f"-I{ggml}/src", f"-I{ROOT}/include",
+           f"-I{ggml}/include", f"-I{ggml}/src", f"-I{ROOT}/include", f"-I{CSRC}",
            "-o", str(BACKEND_SO), str(src),
            f"-L{PKG}", "-lggml-b200-kernels", "-Xlinker", "-rpath,$ORIGIN"]
     subprocess.run(cmd, check=True)

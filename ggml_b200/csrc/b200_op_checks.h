@@ -1,0 +1,247 @@
+// b200_op_checks.h — what each descriptor-taking op launcher of ops.cu accepts, decided in one place.  Every ggml_b200_op_* below returns
+// the verdict of its check before it launches anything, and the backend's supports_op asks the same check for each such node, so that a
+// node the plug-in accepts is one its launcher runs.  The checks read only the descriptors and the op's scalars: what the launcher cannot
+// see (graph structure, ggml-cpu's own layout assumptions) stays with the caller.  Conditions that matter only for a launch (the grid
+// limits) come after the empty-tensor early return, in the order the launchers have always applied them.
+//
+// Host-only C++: the ABI header and the standard library, no CUDA and no ggml headers, so the plug-in, the launchers and the CPU tests
+// compile the same rules.
+#pragma once
+
+#include "../../include/ggml-b200.h"
+
+#include <algorithm>
+#include <cstdint>
+
+namespace b200 {
+
+enum { ROPE_NORM = 0, ROPE_NEOX = 2, ROPE_MROPE = 8, ROPE_VISION = 24 };
+enum { ROPE_MAX_CACHE = 512 };              // cos/sin pairs per position held in shared memory: n_dims <= 1024
+enum { SORT_MAX_COLS = 1024 };              // row length limit (ne0) of the one-CTA ARGSORT network: 1024 items, 8 KB of shared memory
+enum { SORT_ASC = 0, SORT_DESC = 1 };       // enum ggml_sort_order
+
+// number of cos/sin entries a position needs: pairs j < n_dims/2, or j < n_dims (= ne0/2) in VISION mode
+#ifdef __CUDACC__
+__host__ __device__ __forceinline__
+#else
+inline
+#endif
+int rope_n_cache(const ggml_b200_rope_params & c) { return c.mode == ROPE_VISION ? c.n_dims : c.n_dims / 2; }
+
+// the ROPE grid is (positions, blocks of heads, batches): a CTA takes as many whole heads as fit in 256 elements, at least one (ne0 > 0)
+inline int rope_heads_per_cta(int64_t ne0) { return (int)std::max<int64_t>(1, 256 / ne0); }
+
+struct op_check {
+    int          code;     // GGML_B200_OK, or what the launcher returns: GGML_B200_EUNSUPPORTED or GGML_B200_EINVAL
+    const char * reason;   // nullptr when accepted
+    bool ok() const { return code == GGML_B200_OK; }
+};
+constexpr op_check accepted{ GGML_B200_OK, nullptr };
+
+inline int64_t nelem(const ggml_b200_tensor & t) { return t.ne[0] * t.ne[1] * t.ne[2] * t.ne[3]; }
+inline int64_t nrows(const ggml_b200_tensor & t) { return t.ne[1] * t.ne[2] * t.ne[3]; }
+inline bool same_shape(const ggml_b200_tensor & a, const ggml_b200_tensor & b) {
+    return a.ne[0] == b.ne[0] && a.ne[1] == b.ne[1] && a.ne[2] == b.ne[2] && a.ne[3] == b.ne[3];
+}
+inline bool is_float(int32_t t) { return t == GGML_B200_TYPE_F32 || t == GGML_B200_TYPE_F16; }
+// a tensor of 4-byte elements (f32, i32) stored without gaps, in ggml's order
+inline bool is_packed4(const ggml_b200_tensor & t) {
+    size_t nb = 4;
+    for (int i = 0; i < 4; ++i) { if (t.ne[i] != 1 && t.nb[i] != nb) return false; nb *= (size_t)t.ne[i]; }
+    return true;
+}
+
+// the block formats this library decodes (every one of them also runs the quantized MUL_MAT / MUL_MAT_ID)
+inline bool is_block_type(int32_t t) {
+    switch (t) {
+        case GGML_B200_TYPE_Q4_0: case GGML_B200_TYPE_Q8_0: case GGML_B200_TYPE_Q4_K: case GGML_B200_TYPE_Q5_K: case GGML_B200_TYPE_Q6_K:
+        case GGML_B200_TYPE_Q4_1: case GGML_B200_TYPE_Q5_0: case GGML_B200_TYPE_Q5_1: case GGML_B200_TYPE_Q2_K: case GGML_B200_TYPE_Q3_K:
+        case GGML_B200_TYPE_IQ4_NL: case GGML_B200_TYPE_IQ4_XS:
+        case GGML_B200_TYPE_IQ2_XXS: case GGML_B200_TYPE_IQ3_XXS: case GGML_B200_TYPE_IQ1_S:
+        case GGML_B200_TYPE_IQ2_XS: case GGML_B200_TYPE_IQ2_S: case GGML_B200_TYPE_IQ3_S: case GGML_B200_TYPE_IQ1_M:
+        case GGML_B200_TYPE_TQ1_0: case GGML_B200_TYPE_TQ2_0:
+            return true;
+        default: return false;
+    }
+}
+
+#define B200_REQUIRE(cond, why) do { if (!(cond)) return op_check{ GGML_B200_EUNSUPPORTED, why }; } while (0)
+#define B200_VALID(cond, why)   do { if (!(cond)) return op_check{ GGML_B200_EINVAL, why }; } while (0)
+
+constexpr int32_t F32 = GGML_B200_TYPE_F32, F16 = GGML_B200_TYPE_F16, I32 = GGML_B200_TYPE_I32;
+
+inline op_check check_get_rows(const ggml_b200_tensor * src0, const ggml_b200_tensor * ids, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(dst->type == F32 && ids->type == I32, "dst must be f32, ids i32");
+    B200_REQUIRE(is_float(src0->type) || is_block_type(src0->type), "unsupported row type");
+    B200_REQUIRE(dst->nb[0] == 4, "dst rows must be contiguous");
+    return accepted;
+}
+
+inline op_check check_bin_bcast(int32_t op, const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src0->type == F32 && src1->type == F32 && dst->type == F32, "f32 only");
+    if (nelem(*dst) == 0) return accepted;
+    B200_VALID(op >= 0 && op <= 3, "bad op (0 add, 1 mul, 2 sub, 3 div)");
+    return accepted;
+}
+
+inline op_check check_norm(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src->type == F32 && dst->type == F32 && src->nb[0] == 4 && dst->nb[0] == 4, "f32 rows contiguous along dim 0");
+    return accepted;
+}
+
+inline op_check check_norm_affine(const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const float * gain, const ggml_b200_tensor * dst_mul,
+                                  const float * bias, const ggml_b200_tensor * dst_add) {
+    B200_REQUIRE(src->type == F32 && dst_norm->type == F32 && dst_mul->type == F32 && dst_add->type == F32, "f32 only");
+    B200_REQUIRE(src->nb[0] == 4 && dst_norm->nb[0] == 4 && dst_mul->nb[0] == 4 && dst_add->nb[0] == 4 && gain && bias, "rows contiguous along dim 0");
+    return accepted;
+}
+
+inline op_check check_cpy(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(nelem(*src) == nelem(*dst), "element counts differ");
+    if (nelem(*src) == 0) return accepted;
+    if (is_float(src->type) && is_float(dst->type)) return accepted;
+    B200_REQUIRE(src->type == F32 && (dst->type == GGML_B200_TYPE_Q8_0 || dst->type == GGML_B200_TYPE_Q4_0), "unsupported type pair");
+    B200_REQUIRE(src->nb[0] == 4 && src->ne[0] % 32 == 0 && dst->ne[0] % 32 == 0, "f32 -> q needs dim-0 contiguous rows of whole blocks");
+    return accepted;
+}
+
+inline op_check check_cpy2(const ggml_b200_tensor * src_a, const ggml_b200_tensor * dst_a, const ggml_b200_tensor * src_b, const ggml_b200_tensor * dst_b) {
+    const int64_t n = nelem(*src_a);
+    B200_REQUIRE(n == nelem(*dst_a) && n == nelem(*src_b) && n == nelem(*dst_b), "element counts differ");
+    B200_REQUIRE(is_float(src_a->type) && is_float(dst_a->type) && is_float(src_b->type) && is_float(dst_b->type), "float tensors only");
+    return accepted;
+}
+
+inline op_check check_flash_attn_ext(const ggml_b200_tensor * q, const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * mask,
+                                     const ggml_b200_tensor * dst) {
+    auto decodable = [](int32_t t) { return is_float(t) || is_block_type(t); };
+    B200_REQUIRE(q->type == F32 && dst->type == F32 && q->nb[0] == 4 && dst->nb[0] == 4, "q and dst must be f32 rows");
+    B200_REQUIRE(decodable(k->type) && decodable(v->type), "unsupported K / V type");
+    B200_REQUIRE(q->ne[0] >= 1 && q->ne[0] <= 256 && k->ne[0] == q->ne[0] && v->ne[0] == q->ne[0] && v->ne[1] == k->ne[1], "head size must be <= 256 and agree");
+    B200_REQUIRE(k->ne[2] > 0 && k->ne[3] > 0 && v->ne[2] > 0 && v->ne[3] > 0 && q->ne[2] % k->ne[2] == 0 && q->ne[3] % k->ne[3] == 0 &&
+                 q->ne[2] % v->ne[2] == 0 && q->ne[3] % v->ne[3] == 0, "heads do not broadcast");
+    B200_REQUIRE(!mask || (mask->type == F16 && mask->nb[0] == 2 && mask->ne[0] >= k->ne[1] && mask->ne[1] >= q->ne[1]), "mask must be f16 [n_kv, >= n_q]");
+    if (q->ne[1] == 0 || q->ne[2] == 0 || q->ne[3] == 0) return accepted;
+    B200_REQUIRE(q->ne[2] <= 65535 && q->ne[3] <= 65535, "too many heads / batches for one grid");
+    return accepted;
+}
+
+inline op_check check_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst) {
+    const ggml_b200_tensor & a = *src0, & b = *src1, & d = *dst;
+    B200_REQUIRE(is_float(a.type) && b.type == F32 && d.type == F32, "f32/f16 x f32 -> f32");
+    B200_REQUIRE(a.ne[0] == b.ne[0] && d.ne[0] == a.ne[1] && d.ne[1] == b.ne[1] && d.ne[2] == b.ne[2] && d.ne[3] == b.ne[3], "shape mismatch");
+    B200_REQUIRE(b.ne[2] % a.ne[2] == 0 && b.ne[3] % a.ne[3] == 0, "batch dims do not broadcast");
+    return accepted;
+}
+
+inline op_check check_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos, const ggml_b200_tensor * freq_factors, const ggml_b200_tensor * dst,
+                           const ggml_b200_rope_params * params) {
+    B200_REQUIRE(src && pos && dst && params, "src, pos, dst and params are required");
+    const ggml_b200_tensor & s = *src, & p = *pos, & d = *dst;
+    const ggml_b200_rope_params & c = *params;
+    B200_REQUIRE(is_float(s.type) && d.type == s.type, "src and dst must both be f32 or both f16");
+    const size_t es = s.type == F32 ? 4 : 2;
+    B200_REQUIRE(s.nb[0] == es && d.nb[0] == es, "rows must be contiguous along dim 0");
+    B200_REQUIRE(same_shape(s, d), "src and dst shapes differ");
+    B200_REQUIRE(c.mode == ROPE_NORM || c.mode == ROPE_NEOX || c.mode == ROPE_MROPE || c.mode == ROPE_VISION, "mode must be 0, 2, 8 or 24");
+    B200_REQUIRE(c.n_dims >= 0 && c.n_dims % 2 == 0 && c.n_dims <= s.ne[0] && s.ne[0] % 2 == 0, "n_dims must be even and <= ne0 (ne0 even)");
+    B200_REQUIRE(c.mode != ROPE_VISION || 2 * (int64_t)c.n_dims == s.ne[0], "VISION mode needs n_dims == ne0/2");
+    if (c.mode & ROPE_MROPE) {
+        B200_REQUIRE(c.sections[0] >= 0 && c.sections[1] >= 0 && c.sections[2] >= 0 && c.sections[3] >= 0, "sections must be >= 0");
+        B200_REQUIRE(c.sections[0] > 0 || c.sections[1] > 0 || c.sections[2] > 0, "MROPE sections must not all be zero");
+        B200_REQUIRE((int64_t)c.sections[0] + c.sections[1] + c.sections[2] + c.sections[3] <= s.ne[0], "MROPE sections exceed ne0");
+    }
+    const int ncache = rope_n_cache(c);
+    B200_REQUIRE(ncache <= ROPE_MAX_CACHE, "n_dims too large (at most 1024 rotated dimensions)");
+    B200_REQUIRE(p.type == I32 && p.nb[0] == 4 && p.ne[0] >= s.ne[2] * ((c.mode & ROPE_MROPE) ? 4 : 1), "pos must be i32, contiguous, one per position (four in MROPE)");
+    if (freq_factors)
+        B200_REQUIRE(freq_factors->type == F32 && freq_factors->nb[0] == 4 && freq_factors->ne[0] >= ncache,
+                     "freq_factors must be f32, contiguous, >= n_dims/2 entries (n_dims in VISION mode)");
+    if (s.ne[0] == 0 || s.ne[1] == 0 || s.ne[2] == 0 || s.ne[3] == 0) return accepted;
+    const int hpc = rope_heads_per_cta(s.ne[0]);
+    B200_REQUIRE(s.ne[2] <= 0x7fffffff && (s.ne[1] + hpc - 1) / hpc <= 65535 && s.ne[3] <= 65535, "too many positions / heads / batches for one grid");
+    return accepted;
+}
+
+inline op_check check_argsort(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t order) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    B200_VALID(order == SORT_ASC || order == SORT_DESC, "bad order (0 ascending, 1 descending)");
+    B200_REQUIRE(src->type == F32 && dst->type == I32, "src must be f32, dst i32");
+    B200_REQUIRE(src->nb[0] == 4, "src rows must be contiguous along dim 0");
+    B200_REQUIRE(same_shape(*src, *dst), "src and dst shapes differ");
+    B200_REQUIRE(is_packed4(*dst), "dst must be contiguous");
+    B200_REQUIRE(src->ne[0] <= SORT_MAX_COLS, "rows longer than 1024 are not supported");
+    if (nrows(*src) == 0 || src->ne[0] == 0) return accepted;
+    B200_REQUIRE(nrows(*src) <= 0x7fffffff, "too many rows for one grid");
+    return accepted;
+}
+
+inline op_check check_sum_rows(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == F32 && d.type == F32, "src and dst must be f32");
+    B200_REQUIRE(s.nb[0] == 4 && d.nb[0] == 4, "rows must be contiguous along dim 0");
+    B200_REQUIRE(d.ne[0] == 1 && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "dst must be [1, ne1, ne2, ne3] of src");
+    if (nrows(s) == 0) return accepted;
+    B200_REQUIRE((nrows(s) + 3) / 4 <= 0x7fffffff, "too many rows for one grid");
+    return accepted;
+}
+
+inline op_check check_concat(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, int32_t dim) {
+    B200_REQUIRE(src0 && src1 && dst, "src0, src1 and dst are required");
+    B200_VALID(dim >= 0 && dim <= 3, "bad dim (0 .. 3)");
+    const ggml_b200_tensor & a = *src0, & b = *src1, & d = *dst;
+    B200_REQUIRE((a.type == F32 || a.type == I32) && b.type == a.type && d.type == a.type, "src0, src1 and dst must all be f32 or all i32");
+    B200_REQUIRE(a.nb[0] == 4, "src0 must be contiguous along dim 0");
+    for (int k = 0; k < 4; ++k) {
+        if (k == dim) B200_REQUIRE(d.ne[k] == a.ne[k] + b.ne[k], "dst's extent along dim must be src0's plus src1's");
+        else B200_REQUIRE(a.ne[k] == b.ne[k] && d.ne[k] == a.ne[k], "src0, src1 and dst must agree outside dim");
+    }
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
+inline op_check check_ssm_conv(const ggml_b200_tensor * sx, const ggml_b200_tensor * c, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(sx && c && dst, "sx, c and dst are required");
+    const ggml_b200_tensor & x = *sx, & w = *c, & d = *dst;
+    B200_REQUIRE(x.type == F32 && w.type == F32 && d.type == F32, "sx, c and dst must be f32");
+    B200_REQUIRE(x.nb[0] == 4 && w.nb[0] == 4 && d.nb[0] == 4, "sx, c and dst must be contiguous along dim 0");
+    // ggml-cpu reads row i1 of sx at i1 * ne0 (it asserts so) and row i1 of c at i1 * d_conv (whatever c's nb1: only packed rows mean the
+    // same data on both backends)
+    B200_REQUIRE(x.nb[1] == (size_t)x.ne[0] * 4 && w.nb[1] == (size_t)w.ne[0] * 4, "the rows of sx and of c must be packed (nb1 == ne0 * 4)");
+    B200_REQUIRE(x.ne[3] == 1 && w.ne[2] == 1 && w.ne[3] == 1, "sx must be 3-D and c a matrix");
+    B200_REQUIRE(w.ne[1] == x.ne[1] && x.ne[0] - w.ne[0] + 1 >= 0, "c must be [d_conv, d_inner] with d_conv <= ne0 of sx + 1");
+    B200_REQUIRE(d.ne[0] == x.ne[1] && d.ne[1] == x.ne[0] - w.ne[0] + 1 && d.ne[2] == x.ne[2] && d.ne[3] == 1, "dst must be [d_inner, n_t, n_s]");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
+inline op_check check_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tensor * x, const ggml_b200_tensor * dt, const ggml_b200_tensor * A,
+                               const ggml_b200_tensor * B, const ggml_b200_tensor * C, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(s && x && dt && A && B && C && dst, "s, x, dt, A, B, C and dst are required");
+    const ggml_b200_tensor & ts = *s, & tx = *x, & tdt = *dt, & ta = *A, & tb = *B, & tc = *C, & d = *dst;
+    B200_REQUIRE(ts.type == F32 && tx.type == F32 && tdt.type == F32 && ta.type == F32 && tb.type == F32 && tc.type == F32 && d.type == F32,
+                 "all tensors must be f32");
+    B200_REQUIRE(is_packed4(ts) && is_packed4(tx) && is_packed4(tdt) && is_packed4(ta) && is_packed4(d), "s, x, dt, A and dst must be contiguous");
+    B200_REQUIRE(tb.nb[0] == 4 && tc.nb[0] == 4, "B and C must be contiguous along dim 0");
+    const int64_t d_state = ts.ne[0], d_inner = ts.ne[1], n_t = tx.ne[1], n_s = ts.ne[2];
+    B200_REQUIRE(ts.ne[3] == 1 && tx.ne[3] == 1 && tb.ne[3] == 1 && ta.ne[2] == 1 && ta.ne[3] == 1, "s, x and B must be 3-D, A a matrix");
+    // what the CPU backend asserts beyond contiguity (it also holds where a dimension is 1): the strides dst's layout is built from
+    B200_REQUIRE(ts.nb[0] == 4 && tx.nb[0] == 4 && tdt.nb[0] == 4 && ta.nb[0] == 4 && ts.nb[1] == (size_t)d_state * 4 &&
+                 ts.nb[2] == (size_t)(d_state * d_inner) * 4 && tx.nb[3] == (size_t)nelem(tx) * 4, "s and x must have packed strides");
+    B200_REQUIRE(tx.ne[0] == d_inner && tx.ne[2] == n_s, "x must be [d_inner, n_t, n_s]");
+    B200_REQUIRE(same_shape(tdt, tx) && same_shape(tc, tb), "dt must have x's shape and C B's");
+    B200_REQUIRE(ta.ne[0] == d_state && ta.ne[1] == d_inner, "A must be [d_state, d_inner]");
+    B200_REQUIRE(tb.ne[0] == d_state && tb.ne[1] == n_t && tb.ne[2] == n_s, "B and C must be [d_state, n_t, n_s]");
+    B200_REQUIRE(nelem(d) == nelem(tx) + nelem(ts), "dst must hold y and the final states");
+    if (d_inner == 0 || n_s == 0) return accepted;
+    B200_REQUIRE(n_s <= 65535 && (d_inner + 127) / 128 <= 0x7fffffff, "too many rows / sequences for one grid");
+    return accepted;
+}
+
+#undef B200_REQUIRE
+#undef B200_VALID
+
+} // namespace b200

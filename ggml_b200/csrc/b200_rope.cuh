@@ -9,15 +9,12 @@
 
 #include <cstdint>
 
+#include "b200_op_checks.h"     // the modes, ROPE_MAX_CACHE and rope_n_cache
+
 namespace b200 {
 
-enum { ROPE_NORM = 0, ROPE_NEOX = 2, ROPE_MROPE = 8, ROPE_VISION = 24 };
-enum { ROPE_MAX_CACHE = 512 };              // cos/sin pairs per position held in shared memory: n_dims <= 1024
-
-struct rope_consts {
-    int32_t n_dims, mode, sections[4];
-    float freq_scale, ext_factor, mscale, theta_scale, corr_dims[2];
-};
+// the per-op constants are the ABI struct itself: the launcher hands the caller's ggml_b200_rope_params to the kernel as it is
+using rope_consts = ggml_b200_rope_params;
 
 // separately rounded multiply / add / subtract (no FMA contraction on the device)
 __host__ __device__ __forceinline__ float rp_mul(float a, float b) {
@@ -41,9 +38,6 @@ __host__ __device__ __forceinline__ float rp_sub(float a, float b) {
     return a - b;
 #endif
 }
-
-// number of cos/sin entries a position needs: pairs j < n_dims/2, or j < n_dims (= ne0/2) in VISION mode
-__host__ __device__ __forceinline__ int rope_n_cache(const rope_consts & c) { return c.mode == ROPE_VISION ? c.n_dims : c.n_dims / 2; }
 
 // theta of pair j (cache slot i0 = 2j) before the freq-factor division; p[0..3]: the position streams (only p[0] outside MROPE)
 __host__ __device__ inline float rope_theta(const rope_consts & c, const float * p, int j) {

@@ -14,10 +14,9 @@
 #include <cstdint>
 #include <cstring>
 
-namespace b200 {
+#include "b200_op_checks.h"     // SORT_MAX_COLS, SORT_ASC / SORT_DESC
 
-enum { SORT_MAX_COLS = 1024 };          // row length limit (ne0) of the one-CTA network: 1024 items, 8 KB of shared memory
-enum { SORT_ASC = 0, SORT_DESC = 1 };   // enum ggml_sort_order
+namespace b200 {
 
 __host__ __device__ __forceinline__ uint32_t sort_key(float v, int order) {
     if (v != v) return 0xFFFFFFFFu;                                   // NaN: last in both orders

@@ -13,6 +13,7 @@
 // They replace the reference's getrows.cu, binbcast.cu, norm.cu, scale.cu, diagmask.cu, softmax.cu, unary.cu, cpy.cu, mmv.cu, argsort.cu,
 // sumrows.cu, concat.cu (the reference has no SSM kernels).
 #include "b200_internal.h"
+#include "b200_op_checks.h"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
@@ -116,7 +117,7 @@ __device__ __forceinline__ float load_elem(const uint8_t * row, int type, int64_
         case T_IQ1_M: return elem_via_dequant4<T_IQ1_M>(row, i);
         case T_TQ1_0: return elem_via_dequant4<T_TQ1_0>(row, i);
         case T_TQ2_0: return elem_via_dequant4<T_TQ2_0>(row, i);
-        default: return __int_as_float(0x7fc00000);          // unreachable (ggml_b200_op_get_rows rejects unknown types): NaN, never a silent 0
+        default: return __int_as_float(0x7fc00000);          // unreachable (check_get_rows rejects unknown types): NaN, never a silent 0
     }
 }
 
@@ -552,15 +553,14 @@ static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + p
 
 using namespace b200;
 
-#define REQUIRE(cond, msg) do { if (!(cond)) { set_error("%s: %s", __func__, msg); return GGML_B200_EUNSUPPORTED; } } while (0)
+// every launcher below that takes tensor descriptors first applies its acceptance rule from b200_op_checks.h (the one supports_op asks)
+#define CHECK_ARGS(check) do { const op_check r_ = (check); if (!r_.ok()) { set_error("%s: %s", __func__, r_.reason); return r_.code; } } while (0)
 
 extern "C" {
 
 int ggml_b200_op_get_rows(const ggml_b200_tensor * src0, const ggml_b200_tensor * ids, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_get_rows(src0, ids, dst));
     const tdesc s = T(src0), i = T(ids), d = T(dst);
-    REQUIRE(d.type == T_F32 && i.type == 26 /* GGML_TYPE_I32 */, "dst must be f32, ids i32");
-    REQUIRE(s.type == T_F32 || s.type == T_F16 || type_bytes(s.type) != 0, "unsupported row type");
-    REQUIRE(d.nb[0] == 4, "dst rows must be contiguous");
     const int64_t rows = i.ne[0] * i.ne[1] * i.ne[2];
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
     B200_CUDA_TRY(launch_pdl(get_rows_kernel, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream, s, i, d));
@@ -569,26 +569,19 @@ int ggml_b200_op_get_rows(const ggml_b200_tensor * src0, const ggml_b200_tensor 
 }
 
 int ggml_b200_op_bin_bcast(int32_t op, const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_bin_bcast(op, src0, src1, dst));
     const tdesc a = T(src0), b = T(src1), d = T(dst);
-    REQUIRE(a.type == T_F32 && b.type == T_F32 && d.type == T_F32, "f32 only");
     const int64_t n = nelem(d);
     if (n == 0) return GGML_B200_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    const unsigned g = blocks_for(n, 256);
-    switch (op) {
-        case 0: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<0>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
-        case 1: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<1>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
-        case 2: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<2>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
-        case 3: B200_CUDA_TRY(launch_pdl(bin_bcast_kernel<3>, dim3(g), dim3(256), 0, st, a, b, d, n)); break;
-        default: set_error("bin_bcast: bad op %d", op); return GGML_B200_EINVAL;
-    }
+    static void (* const kernel[4])(tdesc, tdesc, tdesc, int64_t) = { bin_bcast_kernel<0>, bin_bcast_kernel<1>, bin_bcast_kernel<2>, bin_bcast_kernel<3> };
+    B200_CUDA_TRY(launch_pdl(kernel[op], dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, a, b, d, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
 int ggml_b200_op_norm(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst, float eps, void * stream) {
+    CHECK_ARGS(check_norm(src, dst));
     const tdesc s = T(src), d = T(dst);
-    REQUIRE(s.type == T_F32 && d.type == T_F32 && s.nb[0] == 4 && d.nb[0] == 4, "f32 rows contiguous along dim 0");
     const int64_t rows = nrows(s);
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
     const int threads = s.ne[0] >= 1024 ? 256 : s.ne[0] >= 256 ? 128 : 32;
@@ -600,9 +593,8 @@ int ggml_b200_op_norm(int32_t rms, const ggml_b200_tensor * src, const ggml_b200
 
 int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const float * gain, const ggml_b200_tensor * dst_mul,
                              const float * bias, const ggml_b200_tensor * dst_add, float eps, void * stream) {
+    CHECK_ARGS(check_norm_affine(src, dst_norm, gain, dst_mul, bias, dst_add));
     const tdesc s = T(src), d1 = T(dst_norm), d2 = T(dst_mul), d3 = T(dst_add);
-    REQUIRE(s.type == T_F32 && d1.type == T_F32 && d2.type == T_F32 && d3.type == T_F32, "f32 only");
-    REQUIRE(s.nb[0] == 4 && d1.nb[0] == 4 && d2.nb[0] == 4 && d3.nb[0] == 4 && gain && bias, "rows contiguous along dim 0");
     const int64_t rows = nrows(s);
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
     const int threads = s.ne[0] >= 1024 ? 256 : s.ne[0] >= 256 ? 128 : 32;
@@ -653,32 +645,26 @@ int ggml_b200_op_soft_max_diag(const float * src, const void * mask, int32_t mas
 }
 
 int ggml_b200_op_cpy(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_cpy(src, dst));
     const tdesc s = T(src), d = T(dst);
     const int64_t n = nelem(s);
-    REQUIRE(n == nelem(d), "element counts differ");
     if (n == 0) return GGML_B200_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    if ((s.type == T_F32 || s.type == T_F16) && (d.type == T_F32 || d.type == T_F16)) {
+    if (d.type == T_F32 || d.type == T_F16) {
         B200_CUDA_TRY(launch_pdl(cpy_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, s, d, s, d, n));
-    } else if (s.type == T_F32 && (d.type == T_Q8_0 || d.type == T_Q4_0)) {
-        REQUIRE(s.nb[0] == 4 && s.ne[0] % 32 == 0 && d.ne[0] % 32 == 0, "f32 -> q needs dim-0 contiguous rows of whole blocks");
+    } else {                                                    // f32 -> Q8_0 / Q4_0
         const int64_t nb = n / 32;
         if (d.type == T_Q8_0) B200_CUDA_TRY(launch_pdl(cpy_f32_q_kernel<T_Q8_0>, dim3(blocks_for(nb, 128)), dim3(128), 0, st, s, d, nb));
         else                  B200_CUDA_TRY(launch_pdl(cpy_f32_q_kernel<T_Q4_0>, dim3(blocks_for(nb, 128)), dim3(128), 0, st, s, d, nb));
-    } else {
-        set_error("cpy: unsupported type pair %d -> %d", s.type, d.type);
-        return GGML_B200_EUNSUPPORTED;
     }
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
 int ggml_b200_op_cpy2(const ggml_b200_tensor * src_a, const ggml_b200_tensor * dst_a, const ggml_b200_tensor * src_b, const ggml_b200_tensor * dst_b, void * stream) {
+    CHECK_ARGS(check_cpy2(src_a, dst_a, src_b, dst_b));
     const tdesc s = T(src_a), d = T(dst_a), s2 = T(src_b), d2 = T(dst_b);
     const int64_t n = nelem(s);
-    REQUIRE(n == nelem(d) && n == nelem(s2) && n == nelem(d2), "element counts differ");
-    auto fl = [](const tdesc & t) { return t.type == T_F32 || t.type == T_F16; };
-    if (!(fl(s) && fl(d) && fl(s2) && fl(d2))) { set_error("cpy2: float tensors only"); return GGML_B200_EUNSUPPORTED; }
     if (n == 0) return GGML_B200_OK;
     B200_CUDA_TRY(launch_pdl(cpy_kernel, dim3(blocks_for(n, 256), 2), dim3(256), 0, (cudaStream_t)stream, s, d, s2, d2, n));
     B200_LAUNCH_CHECK();
@@ -687,17 +673,11 @@ int ggml_b200_op_cpy2(const ggml_b200_tensor * src_a, const ggml_b200_tensor * d
 
 int ggml_b200_op_flash_attn_ext(const ggml_b200_tensor * q, const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * mask,
                                 const ggml_b200_tensor * dst, float scale, float max_bias, float logit_softcap, void * stream) {
+    CHECK_ARGS(check_flash_attn_ext(q, k, v, mask, dst));
     fa_params p;
     p.q = T(q); p.k = T(k); p.v = T(v); p.dst = T(dst);
     if (mask) p.mask = T(mask); else { p.mask = tdesc{}; p.mask.data = nullptr; }
-    auto decodable = [](int t) { return t == T_F32 || t == T_F16 || type_bytes(t) != 0; };
-    REQUIRE(p.q.type == T_F32 && p.dst.type == T_F32 && p.q.nb[0] == 4 && p.dst.nb[0] == 4, "q and dst must be f32 rows");
-    REQUIRE(decodable(p.k.type) && decodable(p.v.type), "unsupported K / V type");
-    REQUIRE(p.q.ne[0] >= 1 && p.q.ne[0] <= 256 && p.k.ne[0] == p.q.ne[0] && p.v.ne[0] == p.q.ne[0] && p.v.ne[1] == p.k.ne[1], "head size must be <= 256 and agree");
-    REQUIRE(p.k.ne[2] > 0 && p.q.ne[2] % p.k.ne[2] == 0 && p.q.ne[3] % p.k.ne[3] == 0 && p.q.ne[2] % p.v.ne[2] == 0 && p.q.ne[3] % p.v.ne[3] == 0, "heads do not broadcast");
-    REQUIRE(!mask || (p.mask.type == T_F16 && p.mask.nb[0] == 2 && p.mask.ne[0] >= p.k.ne[1] && p.mask.ne[1] >= p.q.ne[1]), "mask must be f16 [n_kv, >= n_q]");
     if (p.q.ne[1] == 0 || p.q.ne[2] == 0 || p.q.ne[3] == 0) return GGML_B200_OK;
-    REQUIRE(p.q.ne[2] <= 65535 && p.q.ne[3] <= 65535, "too many heads / batches for one grid");
     p.scale = scale; p.max_bias = max_bias; p.softcap = logit_softcap;
     if (logit_softcap != 0.0f) p.scale /= logit_softcap;
     const uint32_t n_head = (uint32_t)p.q.ne[2];
@@ -710,10 +690,8 @@ int ggml_b200_op_flash_attn_ext(const ggml_b200_tensor * q, const ggml_b200_tens
 }
 
 int ggml_b200_op_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_mul_mat_f(src0, src1, dst));
     const tdesc a = T(src0), b = T(src1), d = T(dst);
-    REQUIRE((a.type == T_F32 || a.type == T_F16) && b.type == T_F32 && d.type == T_F32, "f32/f16 x f32 -> f32");
-    REQUIRE(a.ne[0] == b.ne[0] && d.ne[0] == a.ne[1] && d.ne[1] == b.ne[1] && d.ne[2] == b.ne[2] && d.ne[3] == b.ne[3], "shape mismatch");
-    REQUIRE(b.ne[2] % a.ne[2] == 0 && b.ne[3] % a.ne[3] == 0, "batch dims do not broadcast");
     const int64_t nout = nelem(d);
     if (nout == 0) return GGML_B200_OK;
     B200_CUDA_TRY(launch_pdl(mul_mat_f_kernel, dim3(blocks_for(nout, 4)), dim3(128), 0, (cudaStream_t)stream, a, b, d, nout));
@@ -723,38 +701,13 @@ int ggml_b200_op_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor
 
 int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos, const ggml_b200_tensor * freq_factors, const ggml_b200_tensor * dst,
                       const ggml_b200_rope_params * params, void * stream) {
-    REQUIRE(src && pos && dst && params, "src, pos, dst and params are required");
+    CHECK_ARGS(check_rope(src, pos, freq_factors, dst, params));
     const tdesc s = T(src), p = T(pos), d = T(dst);
-    rope_consts c;
-    c.n_dims = params->n_dims; c.mode = params->mode;
-    for (int i = 0; i < 4; ++i) c.sections[i] = params->sections[i];
-    c.freq_scale = params->freq_scale; c.ext_factor = params->ext_factor; c.mscale = params->mscale; c.theta_scale = params->theta_scale;
-    c.corr_dims[0] = params->corr_dims[0]; c.corr_dims[1] = params->corr_dims[1];
-    REQUIRE((s.type == T_F32 || s.type == T_F16) && d.type == s.type, "src and dst must both be f32 or both f16");
-    const size_t es = s.type == T_F32 ? 4 : 2;
-    REQUIRE(s.nb[0] == es && d.nb[0] == es, "rows must be contiguous along dim 0");
-    REQUIRE(s.ne[0] == d.ne[0] && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "src and dst shapes differ");
-    REQUIRE(c.mode == ROPE_NORM || c.mode == ROPE_NEOX || c.mode == ROPE_MROPE || c.mode == ROPE_VISION, "mode must be 0, 2, 8 or 24");
-    REQUIRE(c.n_dims >= 0 && c.n_dims % 2 == 0 && c.n_dims <= s.ne[0] && s.ne[0] % 2 == 0, "n_dims must be even and <= ne0 (ne0 even)");
-    REQUIRE(c.mode != ROPE_VISION || 2 * (int64_t)c.n_dims == s.ne[0], "VISION mode needs n_dims == ne0/2");
-    if (c.mode & ROPE_MROPE) {
-        REQUIRE(c.sections[0] >= 0 && c.sections[1] >= 0 && c.sections[2] >= 0 && c.sections[3] >= 0, "sections must be >= 0");
-        REQUIRE(c.sections[0] > 0 || c.sections[1] > 0 || c.sections[2] > 0, "MROPE sections must not all be zero");
-        REQUIRE((int64_t)c.sections[0] + c.sections[1] + c.sections[2] + c.sections[3] <= s.ne[0], "MROPE sections exceed ne0");
-    }
-    const int ncache = rope_n_cache(c);
-    REQUIRE(ncache <= ROPE_MAX_CACHE, "n_dims too large (at most 1024 rotated dimensions)");
-    REQUIRE(p.type == 26 /* GGML_TYPE_I32 */ && p.nb[0] == 4 && p.ne[0] >= s.ne[2] * ((c.mode & ROPE_MROPE) ? 4 : 1), "pos must be i32, contiguous, one per position (four in MROPE)");
-    const float * ff = nullptr;
-    if (freq_factors) {
-        const tdesc f = T(freq_factors);
-        REQUIRE(f.type == T_F32 && f.nb[0] == 4 && f.ne[0] >= ncache, "freq_factors must be f32, contiguous, >= n_dims/2 entries (n_dims in VISION mode)");
-        ff = (const float *)f.data;
-    }
+    const rope_consts & c = *params;
+    const float * ff = freq_factors ? (const float *)freq_factors->data : nullptr;
     if (s.ne[0] == 0 || s.ne[1] == 0 || s.ne[2] == 0 || s.ne[3] == 0) return GGML_B200_OK;
-    const int heads_per_cta = (int)std::max<int64_t>(1, 256 / s.ne[0]);
+    const int heads_per_cta = rope_heads_per_cta(s.ne[0]);
     const int64_t hb = (s.ne[1] + heads_per_cta - 1) / heads_per_cta;
-    REQUIRE(s.ne[2] <= 0x7fffffff && hb <= 65535 && s.ne[3] <= 65535, "too many positions / heads / batches for one grid");
     const dim3 grid((unsigned)s.ne[2], (unsigned)hb, (unsigned)s.ne[3]);
     if (s.type == T_F32) B200_CUDA_TRY(launch_pdl(rope_kernel<float>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
     else                 B200_CUDA_TRY(launch_pdl(rope_kernel<__half>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
@@ -763,18 +716,10 @@ int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos
 }
 
 int ggml_b200_op_argsort(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t order, void * stream) {
-    REQUIRE(src && dst, "src and dst are required");
-    if (order != SORT_ASC && order != SORT_DESC) { set_error("argsort: bad order %d (0 ascending, 1 descending)", order); return GGML_B200_EINVAL; }
+    CHECK_ARGS(check_argsort(src, dst, order));
     const tdesc s = T(src), d = T(dst);
-    REQUIRE(s.type == T_F32 && d.type == 26 /* GGML_TYPE_I32 */, "src must be f32, dst i32");
-    REQUIRE(s.nb[0] == 4, "src rows must be contiguous along dim 0");
-    REQUIRE(s.ne[0] == d.ne[0] && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "src and dst shapes differ");
-    size_t nb = 4;
-    for (int i = 0; i < 4; ++i) { REQUIRE(d.ne[i] == 1 || d.nb[i] == nb, "dst must be contiguous"); nb *= (size_t)d.ne[i]; }
-    REQUIRE(s.ne[0] <= SORT_MAX_COLS, "rows longer than 1024 are not supported");
     const int64_t rows = nrows(s);
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
-    REQUIRE(rows <= 0x7fffffff, "too many rows for one grid");
     const int P = sort_width((int)s.ne[0]);
     const int threads = std::max(32, std::min(512, P / 2));
     B200_CUDA_TRY(launch_pdl(argsort_kernel, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, s, (int32_t *)d.data, P, (int)order));
@@ -783,57 +728,30 @@ int ggml_b200_op_argsort(const ggml_b200_tensor * src, const ggml_b200_tensor * 
 }
 
 int ggml_b200_op_sum_rows(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
-    REQUIRE(src && dst, "src and dst are required");
+    CHECK_ARGS(check_sum_rows(src, dst));
     const tdesc s = T(src), d = T(dst);
-    REQUIRE(s.type == T_F32 && d.type == T_F32, "src and dst must be f32");
-    REQUIRE(s.nb[0] == 4 && d.nb[0] == 4, "rows must be contiguous along dim 0");
-    REQUIRE(d.ne[0] == 1 && s.ne[1] == d.ne[1] && s.ne[2] == d.ne[2] && s.ne[3] == d.ne[3], "dst must be [1, ne1, ne2, ne3] of src");
     const int64_t rows = nrows(s);
     if (rows == 0) return GGML_B200_OK;
-    REQUIRE((rows + 3) / 4 <= 0x7fffffff, "too many rows for one grid");
     B200_CUDA_TRY(launch_pdl(sum_rows_kernel, dim3(blocks_for(rows, 4)), dim3(128), 0, (cudaStream_t)stream, s, d, rows));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
-static bool is_contiguous(const tdesc & t) {
-    size_t nb = 4;
-    for (int i = 0; i < 4; ++i) { if (t.ne[i] != 1 && t.nb[i] != nb) return false; nb *= (size_t)t.ne[i]; }
-    return true;
-}
-
 int ggml_b200_op_concat(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, int32_t dim, void * stream) {
-    REQUIRE(src0 && src1 && dst, "src0, src1 and dst are required");
-    if (dim < 0 || dim > 3) { set_error("concat: bad dim %d (0 .. 3)", dim); return GGML_B200_EINVAL; }
+    CHECK_ARGS(check_concat(src0, src1, dst, dim));
     const tdesc a = T(src0), b = T(src1), d = T(dst);
-    REQUIRE((a.type == T_F32 || a.type == 26 /* GGML_TYPE_I32 */) && b.type == a.type && d.type == a.type, "src0, src1 and dst must all be f32 or all i32");
-    REQUIRE(a.nb[0] == 4, "src0 must be contiguous along dim 0");
-    for (int k = 0; k < 4; ++k) {
-        if (k == dim) REQUIRE(d.ne[k] == a.ne[k] + b.ne[k], "dst's extent along dim must be src0's plus src1's");
-        else REQUIRE(a.ne[k] == b.ne[k] && d.ne[k] == a.ne[k], "src0, src1 and dst must agree outside dim");
-    }
     const int64_t n = nelem(d);
     if (n == 0) return GGML_B200_OK;
-    REQUIRE((n + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
     B200_CUDA_TRY(launch_pdl(concat_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, a, b, d, (int)dim, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
 int ggml_b200_op_ssm_conv(const ggml_b200_tensor * sx, const ggml_b200_tensor * c, const ggml_b200_tensor * dst, void * stream) {
-    REQUIRE(sx && c && dst, "sx, c and dst are required");
+    CHECK_ARGS(check_ssm_conv(sx, c, dst));
     const tdesc x = T(sx), w = T(c), d = T(dst);
-    REQUIRE(x.type == T_F32 && w.type == T_F32 && d.type == T_F32, "sx, c and dst must be f32");
-    REQUIRE(x.nb[0] == 4 && w.nb[0] == 4 && d.nb[0] == 4, "sx, c and dst must be contiguous along dim 0");
-    // ggml-cpu reads row i1 of sx at i1 * ne0 (it asserts so) and row i1 of c at i1 * d_conv (whatever c's nb1: only packed rows mean the
-    // same data on both backends)
-    REQUIRE(x.nb[1] == (size_t)x.ne[0] * 4 && w.nb[1] == (size_t)w.ne[0] * 4, "the rows of sx and of c must be packed (nb1 == ne0 * 4)");
-    REQUIRE(x.ne[3] == 1 && w.ne[2] == 1 && w.ne[3] == 1, "sx must be 3-D and c a matrix");
-    REQUIRE(w.ne[1] == x.ne[1] && x.ne[0] - w.ne[0] + 1 >= 0, "c must be [d_conv, d_inner] with d_conv <= ne0 of sx + 1");
-    REQUIRE(d.ne[0] == x.ne[1] && d.ne[1] == x.ne[0] - w.ne[0] + 1 && d.ne[2] == x.ne[2] && d.ne[3] == 1, "dst must be [d_inner, n_t, n_s]");
     const int64_t n = nelem(d);
     if (n == 0) return GGML_B200_OK;
-    REQUIRE((n + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
     B200_CUDA_TRY(launch_pdl(ssm_conv_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, x, w, d, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
@@ -841,24 +759,10 @@ int ggml_b200_op_ssm_conv(const ggml_b200_tensor * sx, const ggml_b200_tensor * 
 
 int ggml_b200_op_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tensor * x, const ggml_b200_tensor * dt, const ggml_b200_tensor * A,
                           const ggml_b200_tensor * B, const ggml_b200_tensor * C, const ggml_b200_tensor * dst, void * stream) {
-    REQUIRE(s && x && dt && A && B && C && dst, "s, x, dt, A, B, C and dst are required");
+    CHECK_ARGS(check_ssm_scan(s, x, dt, A, B, C, dst));
     const tdesc ts = T(s), tx = T(x), tdt = T(dt), ta = T(A), tb = T(B), tc = T(C), d = T(dst);
-    REQUIRE(ts.type == T_F32 && tx.type == T_F32 && tdt.type == T_F32 && ta.type == T_F32 && tb.type == T_F32 && tc.type == T_F32 && d.type == T_F32,
-            "all tensors must be f32");
-    REQUIRE(is_contiguous(ts) && is_contiguous(tx) && is_contiguous(tdt) && is_contiguous(ta) && is_contiguous(d), "s, x, dt, A and dst must be contiguous");
-    REQUIRE(tb.nb[0] == 4 && tc.nb[0] == 4, "B and C must be contiguous along dim 0");
-    const int64_t d_state = ts.ne[0], d_inner = ts.ne[1], n_t = tx.ne[1], n_s = ts.ne[2];
-    REQUIRE(ts.ne[3] == 1 && tx.ne[3] == 1 && tb.ne[3] == 1 && ta.ne[2] == 1 && ta.ne[3] == 1, "s, x and B must be 3-D, A a matrix");
-    // what the CPU backend asserts beyond contiguity (it also holds where a dimension is 1): the strides dst's layout is built from
-    REQUIRE(ts.nb[0] == 4 && tx.nb[0] == 4 && tdt.nb[0] == 4 && ta.nb[0] == 4 && ts.nb[1] == (size_t)d_state * 4 &&
-            ts.nb[2] == (size_t)(d_state * d_inner) * 4 && tx.nb[3] == (size_t)nelem(tx) * 4, "s and x must have packed strides");
-    REQUIRE(tx.ne[0] == d_inner && tx.ne[2] == n_s, "x must be [d_inner, n_t, n_s]");
-    for (int k = 0; k < 4; ++k) REQUIRE(tdt.ne[k] == tx.ne[k] && tc.ne[k] == tb.ne[k], "dt must have x's shape and C B's");
-    REQUIRE(ta.ne[0] == d_state && ta.ne[1] == d_inner, "A must be [d_state, d_inner]");
-    REQUIRE(tb.ne[0] == d_state && tb.ne[1] == n_t && tb.ne[2] == n_s, "B and C must be [d_state, n_t, n_s]");
-    REQUIRE(nelem(d) == nelem(tx) + nelem(ts), "dst must hold y and the final states");
+    const int64_t d_inner = ts.ne[1], n_s = ts.ne[2];
     if (d_inner == 0 || n_s == 0) return GGML_B200_OK;
-    REQUIRE(n_s <= 65535 && (d_inner + 127) / 128 <= 0x7fffffff, "too many rows / sequences for one grid");
     B200_CUDA_TRY(launch_pdl(ssm_scan_kernel, dim3(blocks_for(d_inner, 128), (unsigned)n_s), dim3(128), 0, (cudaStream_t)stream, ts, tx, tdt, ta, tb, tc,
                              (uint8_t *)d.data));
     B200_LAUNCH_CHECK();

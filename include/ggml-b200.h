@@ -58,6 +58,8 @@ enum ggml_b200_type {
     /* grid-codebook i-quants (src/ggml-common.h:330-396; codebooks extracted from it at build time): generic mat-vec, MUL_MAT_ID, dequantize */
     GGML_B200_TYPE_IQ2_XXS = 16, GGML_B200_TYPE_IQ3_XXS = 18, GGML_B200_TYPE_IQ1_S = 19,
     GGML_B200_TYPE_IQ2_XS = 17, GGML_B200_TYPE_IQ3_S = 21, GGML_B200_TYPE_IQ2_S = 22, GGML_B200_TYPE_IQ1_M = 29, GGML_B200_TYPE_TQ1_0 = 34, GGML_B200_TYPE_TQ2_0 = 35,
+    /* indices and positions of the small ops (ggml_b200_tensor) */
+    GGML_B200_TYPE_I32 = 26,
 };
 
 /* ---------------------------------------------------------------------------------------------
@@ -202,7 +204,7 @@ GGML_B200_API int    ggml_b200_quantize_activations(int32_t weight_type, const f
  * ------------------------------------------------------------------------------------------- */
 typedef struct ggml_b200_tensor {
     void *  data;      /* device */
-    int32_t type;      /* enum ggml_type id: 0 f32, 1 f16, 26 i32, or a block-quantized type */
+    int32_t type;      /* enum ggml_b200_type: f32, f16, i32 or a block-quantized type */
     int64_t ne[4];
     size_t  nb[4];
 } ggml_b200_tensor;

@@ -23,7 +23,8 @@ def emu():
     out = EMU / "_build"
     out.mkdir(exist_ok=True)
     so = out / "libsort_emu.so"
-    srcs = [EMU / "sort_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_sort.cuh"]
+    srcs = [EMU / "sort_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_sort.cuh",
+            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h"]
     if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
         cmd = ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
                f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "sort_emu.cpp")]
