@@ -534,3 +534,31 @@ def op_ssm_scan(s, x, dt, A, B, C_):
     d = tensor_desc(out)
     check(L.ggml_b200_op_ssm_scan(*[C.byref(v) for v in t], C.byref(d), _stream()), "ggml_b200_op_ssm_scan")
     return out[: x.numel()].view(x.shape), out[x.numel():].view(s.shape)
+
+
+def _wkv(fn, name, k, s, srcs, extra):
+    """the flat ggml result of RWKV_WKV6 / GATED_LINEAR_ATTN as (y [T, H, S], s_new [n_seqs, H, S, S]) views; s is read as [n_seqs, S S H]"""
+    import torch
+    T, H, S = k.shape
+    n_seqs = s.shape[0]
+    out = torch.empty((T + S * n_seqs, H * S), dtype=torch.float32, device=k.device)
+    t = [strided_desc(v) for v in srcs] + [strided_desc(s.reshape(n_seqs, -1))]
+    check(fn(*[C.byref(v) for v in t], C.byref(tensor_desc(out)), *extra, _stream()), name)
+    return out[:T].view(T, H, S), out[T:].view(n_seqs, H, S, S)
+
+
+def op_rwkv_wkv6(k, v, r, tf, td, s):
+    """GGML_OP_RWKV_WKV6: k, v, r, td f32 [T, H, S], tf f32 [H, S], s f32 [n_seqs, H, S, S] (state[i][j] at [q, h, i, j]), all contiguous;
+    sequence q owns tokens [q T / n_seqs, (q + 1) T / n_seqs).  Returns (y [T, H, S], s_new [n_seqs, H, S, S]): views of the one flat
+    result in ggml's layout (y, then the final states)."""
+    L = lib()
+    L.ggml_b200_op_rwkv_wkv6.argtypes = [C.POINTER(TensorDesc)] * 7 + [C.c_void_p]
+    return _wkv(L.ggml_b200_op_rwkv_wkv6, "ggml_b200_op_rwkv_wkv6", k, s, (k, v, r, tf, td), ())
+
+
+def op_gated_linear_attn(k, v, q, g, s, scale: float):
+    """GGML_OP_GATED_LINEAR_ATTN: k, v, q, g f32 [T, H, S], s f32 [n_seqs, H, S, S], all contiguous; as op_rwkv_wkv6 with the gate g in
+    place of the decay and q * scale in place of r (no bonus term).  Returns (y [T, H, S], s_new [n_seqs, H, S, S])."""
+    L = lib()
+    L.ggml_b200_op_gated_linear_attn.argtypes = [C.POINTER(TensorDesc)] * 6 + [C.c_float, C.c_void_p]
+    return _wkv(L.ggml_b200_op_gated_linear_attn, "ggml_b200_op_gated_linear_attn", k, s, (k, v, q, g), (float(scale),))

@@ -19,6 +19,11 @@ enum { ROPE_NORM = 0, ROPE_NEOX = 2, ROPE_MROPE = 8, ROPE_VISION = 24 };
 enum { ROPE_MAX_CACHE = 512 };              // cos/sin pairs per position held in shared memory: n_dims <= 1024
 enum { SORT_MAX_COLS = 1024 };              // row length limit (ne0) of the one-CTA ARGSORT network: 1024 items, 8 KB of shared memory
 enum { SORT_ASC = 0, SORT_DESC = 1 };       // enum ggml_sort_order
+enum { WKV_COLS = 32 };                     // RWKV_WKV6 / GATED_LINEAR_ATTN: state columns per CTA (one warp, one column per lane)
+enum { WKV_MAX_HEAD = 256 };                // their head size limit: S rows x WKV_COLS columns of state plus four S-vectors, 36 KB of shared memory
+
+// the shared memory of one RWKV_WKV6 / GATED_LINEAR_ATTN CTA for head size S: the state block, then the token's k, r / q, td / g and tf
+inline size_t wkv_smem_bytes(int64_t S) { return (size_t)S * (WKV_COLS + 4) * sizeof(float); }
 
 // number of cos/sin entries a position needs: pairs j < n_dims/2, or j < n_dims (= ne0/2) in VISION mode
 #ifdef __CUDACC__
@@ -239,6 +244,41 @@ inline op_check check_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tenso
     if (d_inner == 0 || n_s == 0) return accepted;
     B200_REQUIRE(n_s <= 65535 && (d_inner + 127) / 128 <= 0x7fffffff, "too many rows / sequences for one grid");
     return accepted;
+}
+
+// what RWKV_WKV6 and GATED_LINEAR_ATTN share: k, v, a (r or q) and b (td or g) f32 [S, H, T], the state s f32 with S S H n_seqs elements
+// (n_seqs = its ne1, as ggml reads it) and dst f32 [S H, T + S n_seqs].  ggml-cpu indexes every one of them flat, whatever its strides,
+// so all must be packed.
+inline op_check check_wkv_common(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * a, const ggml_b200_tensor * b,
+                                 const ggml_b200_tensor * s, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(k && v && a && b && s && dst, "all sources and dst are required");
+    B200_REQUIRE(k->type == F32 && v->type == F32 && a->type == F32 && b->type == F32 && s->type == F32 && dst->type == F32, "all tensors must be f32");
+    B200_REQUIRE(is_packed4(*k) && is_packed4(*v) && is_packed4(*a) && is_packed4(*b) && is_packed4(*s) && is_packed4(*dst), "all tensors must be contiguous");
+    const int64_t S = k->ne[0], H = k->ne[1], T = k->ne[2], n_seqs = s->ne[1];
+    B200_REQUIRE(k->ne[3] == 1 && H >= 1, "k must be [S, H, T] with at least one head");
+    B200_REQUIRE(same_shape(*v, *k) && same_shape(*a, *k) && same_shape(*b, *k), "v and r / q and td / g must have k's shape");
+    B200_REQUIRE(nelem(*s) == S * S * H * n_seqs, "the state must hold S * S * H * n_seqs values (n_seqs = its ne1)");
+    B200_REQUIRE(dst->ne[0] == S * H && dst->ne[1] == T + S * n_seqs && dst->ne[2] == 1 && dst->ne[3] == 1, "dst must be [S * H, T + S * n_seqs]");
+    B200_REQUIRE(S <= WKV_MAX_HEAD, "head size above 256");
+    if (T == 0) return accepted;                           // ggml-cpu writes nothing
+    // ggml-cpu gives each sequence T / n_seqs tokens and divides by that count
+    B200_VALID(n_seqs >= 1 && T % n_seqs == 0, "the tokens must split evenly over the sequences (T % n_seqs == 0)");
+    if (S == 0) return accepted;
+    B200_REQUIRE(H <= 65535 && n_seqs <= 65535, "too many heads / sequences for one grid");
+    return accepted;
+}
+
+inline op_check check_rwkv_wkv6(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * r, const ggml_b200_tensor * tf,
+                                const ggml_b200_tensor * td, const ggml_b200_tensor * s, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(tf, "tf is required");
+    B200_REQUIRE(tf->type == F32 && is_packed4(*tf), "tf must be f32 and contiguous");
+    if (k) B200_REQUIRE(nelem(*tf) == k->ne[0] * k->ne[1], "tf must hold S * H values");
+    return check_wkv_common(k, v, r, td, s, dst);
+}
+
+inline op_check check_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * q, const ggml_b200_tensor * g,
+                                        const ggml_b200_tensor * s, const ggml_b200_tensor * dst) {
+    return check_wkv_common(k, v, q, g, s, dst);
 }
 
 #undef B200_REQUIRE

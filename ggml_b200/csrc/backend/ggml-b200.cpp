@@ -554,6 +554,16 @@ bool supports_checked_op(const ggml_tensor * op) {
             for (int k = 0; k < 6; ++k) t[k] = desc(op->src[k]);
             return b200::check_ssm_scan(&t[0], &t[1], &t[2], &t[3], &t[4], &t[5], &d).ok();
         }
+        case GGML_OP_RWKV_WKV6: {
+            ggml_b200_tensor t[6];
+            for (int k = 0; k < 6; ++k) t[k] = desc(op->src[k]);
+            return b200::check_rwkv_wkv6(&t[0], &t[1], &t[2], &t[3], &t[4], &t[5], &d).ok();
+        }
+        case GGML_OP_GATED_LINEAR_ATTN: {
+            ggml_b200_tensor t[5];
+            for (int k = 0; k < 5; ++k) t[k] = desc(op->src[k]);
+            return b200::check_gated_linear_attn(&t[0], &t[1], &t[2], &t[3], &t[4], &d).ok();
+        }
         default: return false;
     }
 }
@@ -578,7 +588,7 @@ bool device_supports_op(ggml_backend_dev_t dev, const ggml_tensor * op) {
         case GGML_OP_MUL_MAT:    return supports_mul_mat(op) || supports_checked_op(op);
         case GGML_OP_MUL_MAT_ID: return supports_mul_mat_id(op);
         // the launchers that take bare pointers: their layout conditions are the caller's
-        case GGML_OP_SCALE: case GGML_OP_DIAG_MASK_INF:
+        case GGML_OP_SCALE: case GGML_OP_DIAG_MASK_INF: case GGML_OP_SQR: case GGML_OP_SQRT:
             return is_f32_contig(a) && is_f32_contig(op);
         case GGML_OP_SOFT_MAX:
             return is_f32_contig(a) && is_f32_contig(op) && (!b || ((b->type == GGML_TYPE_F32 || b->type == GGML_TYPE_F16) && ggml_is_contiguous(b)));
@@ -810,6 +820,13 @@ void compute_small_op(backend_ctx * ctx, ggml_tensor * node) {
             }
             SHIM_OK(ggml_b200_op_unary(u, (const float *) a->data, (float *) node->data, ggml_nelements(node), st));
         } break;
+        // x * x and sqrtf, correctly rounded on both backends: bit-identical to ggml-cpu
+        case GGML_OP_SQR:
+            SHIM_OK(ggml_b200_op_unary(GGML_B200_UNARY_SQR, (const float *) a->data, (float *) node->data, ggml_nelements(node), st));
+            break;
+        case GGML_OP_SQRT:
+            SHIM_OK(ggml_b200_op_unary(GGML_B200_UNARY_SQRT, (const float *) a->data, (float *) node->data, ggml_nelements(node), st));
+            break;
         case GGML_OP_CPY:  { auto s = desc(a), d = desc(b);    SHIM_OK(ggml_b200_op_cpy(&s, &d, st)); } break;
         case GGML_OP_CONT: case GGML_OP_DUP: { auto s = desc(a), d = desc(node); SHIM_OK(ggml_b200_op_cpy(&s, &d, st)); } break;
         case GGML_OP_ROPE: {
@@ -832,6 +849,20 @@ void compute_small_op(backend_ctx * ctx, ggml_tensor * node) {
             for (int k = 0; k < 6; ++k) t[k] = desc(node->src[k]);
             auto d = desc(node);
             SHIM_OK(ggml_b200_op_ssm_scan(&t[0], &t[1], &t[2], &t[3], &t[4], &t[5], &d, st));
+        } break;
+        case GGML_OP_RWKV_WKV6: {
+            // sources: k, v, r, tf, td, state (ggml_rwkv_wkv6); dst = y, then the final states
+            ggml_b200_tensor t[6];
+            for (int k = 0; k < 6; ++k) t[k] = desc(node->src[k]);
+            auto d = desc(node);
+            SHIM_OK(ggml_b200_op_rwkv_wkv6(&t[0], &t[1], &t[2], &t[3], &t[4], &t[5], &d, st));
+        } break;
+        case GGML_OP_GATED_LINEAR_ATTN: {
+            // sources: k, v, q, g, state (ggml_gated_linear_attn); op_params[0] = scale
+            ggml_b200_tensor t[5];
+            for (int k = 0; k < 5; ++k) t[k] = desc(node->src[k]);
+            auto d = desc(node);
+            SHIM_OK(ggml_b200_op_gated_linear_attn(&t[0], &t[1], &t[2], &t[3], &t[4], &d, ggml_get_op_params_f32(node, 0), st));
         } break;
         default:
             GGML_LOG_ERROR("ggml-b200: op %s is not supported (supports_op must have declined it)\n", ggml_op_desc(node));

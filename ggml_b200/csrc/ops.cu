@@ -8,10 +8,12 @@
 //   diag_mask :9745-9805  soft_max :9810-9925        gelu :6520-6570 (+ fp16 table, ggml-cpu.c:1355)   dup/cpy :3220-4300
 //   rope :9157-9640       argsort :10746-10783       sum_rows :5663-5694 (+ ggml_vec_sum_f32 :2118)
 //   concat :6097-6157     ssm_conv :11379-11445      ssm_scan :11449-11537
+//   rwkv_wkv6 :11865-12044                           gated_linear_attn :12067-12235
 // ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation; CONCAT, SSM_CONV and SSM_SCAN are the
-// rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer.
+// rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer; RWKV_WKV6 and GATED_LINEAR_ATTN are
+// the recurrences of the RWKV-6 time mix and of its gated (RWKV6-Qwen2) form.
 // They replace the reference's getrows.cu, binbcast.cu, norm.cu, scale.cu, diagmask.cu, softmax.cu, unary.cu, cpy.cu, mmv.cu, argsort.cu,
-// sumrows.cu, concat.cu (the reference has no SSM kernels).
+// sumrows.cu, concat.cu, wkv6.cu, gla.cu (the reference has no SSM kernels).
 #include "b200_internal.h"
 #include "b200_op_checks.h"
 #include "b200_quants.cuh"
@@ -20,6 +22,7 @@
 #include "b200_rope.cuh"
 #include "b200_sort.cuh"
 #include "b200_ssm.cuh"
+#include "b200_wkv.cuh"
 
 #include <cfloat>
 
@@ -547,6 +550,70 @@ __global__ void __launch_bounds__(128) ssm_scan_kernel(tdesc s0, tdesc x, tdesc 
     }
 }
 
+// ------------------------------------------------------------------ RWKV_WKV6 / GATED_LINEAR_ATTN (the RWKV-6 recurrence and its gated form)
+// One CTA per (block of WKV_COLS state columns, head h, sequence s); one lane per column j walks the S rows i in order (b200_wkv.cuh), so y[j]
+// keeps the CPU's summation order with no reduction.  The CTA's columns of the state stay in shared memory across the sequence's tokens,
+// lane j touching only column j (conflict-free: the block is stored S x WKV_COLS); it is read from s0 before the first token and written
+// to dst's state part after the last.  The token's k, r / q', td / g are staged in shared memory once per token; the next token's are
+// loaded into registers while the current one is computed.  Each sequence owns n_seq_tok consecutive tokens, as on the CPU.
+// All tensors are packed (check_wkv_common): token t, head h, element i at t * C + h * S + i; state[i][j] of (s, h) at
+// ((s * H + h) * S + i) * S + j; dst: y [C, T], then the final states from T * C.
+template <bool GLA>
+__global__ void __launch_bounds__(WKV_COLS) wkv_kernel(const float * __restrict__ k, const float * __restrict__ v, const float * __restrict__ a,
+                                                       const float * __restrict__ b, const float * __restrict__ tf, const float * __restrict__ s0,
+                                                       float * __restrict__ dst, int S, int H, int64_t T, int64_t n_seq_tok, float scale) {
+    extern __shared__ float wkv_sh[];
+    pdl_trigger();
+    constexpr int PER = WKV_MAX_HEAD / WKV_COLS;                // staged values per lane and vector
+    const int lane = threadIdx.x, j = blockIdx.x * WKV_COLS + lane, h = blockIdx.y, s = blockIdx.z;
+    const bool live = j < S;
+    const int64_t C = (int64_t)S * H;
+    float * st = wkv_sh;                                         // [S][WKV_COLS]
+    float * sk = st + (size_t)S * WKV_COLS, * sa = sk + S, * sb = sa + S, * sf = sb + S;
+
+    const int64_t head_state = ((int64_t)s * H + h) * S * S;
+    for (int i0 = 0; i0 < S; i0 += WKV_COLS) {                  // WKV_COLS rows' loads in flight at once (a decode step is one token)
+        float row[WKV_COLS];
+#pragma unroll
+        for (int u = 0; u < WKV_COLS; ++u) row[u] = live && i0 + u < S ? s0[head_state + (int64_t)(i0 + u) * S + j] : 0.0f;
+#pragma unroll
+        for (int u = 0; u < WKV_COLS; ++u) if (i0 + u < S) st[(i0 + u) * WKV_COLS + lane] = row[u];
+    }
+    if (!GLA) for (int i = lane; i < S; i += WKV_COLS) sf[i] = tf[(int64_t)h * S + i];
+
+    float nk[PER], na[PER], nb[PER], nv = 0.0f;
+    auto fetch = [&](int64_t t) {
+        const int64_t base = t * C + (int64_t)h * S;
+#pragma unroll
+        for (int m = 0; m < PER; ++m) {
+            const int i = lane + m * WKV_COLS;
+            if (i < S) { nk[m] = k[base + i]; na[m] = a[base + i]; nb[m] = b[base + i]; }
+        }
+        if (live) nv = v[base + j];
+    };
+    const int64_t t0 = (int64_t)s * n_seq_tok, t1 = t0 + n_seq_tok;
+    fetch(t0);
+    for (int64_t t = t0; t < t1; ++t) {
+        __syncthreads();                                         // the previous token's k / a / b are no longer read
+#pragma unroll
+        for (int m = 0; m < PER; ++m) {
+            const int i = lane + m * WKV_COLS;
+            if (i < S) { sk[i] = nk[m]; sa[i] = GLA ? gla_scaled_q(na[m], scale) : na[m]; sb[i] = nb[m]; }
+        }
+        const float vj = nv;
+        __syncthreads();
+        if (t + 1 < t1) fetch(t + 1);
+        if (live) {
+            float * col = st + lane;
+            const float y = GLA ? gla_column(sk, sa, sb, vj, col, col, WKV_COLS, S) : wkv6_column(sk, sa, sf, sb, vj, col, col, WKV_COLS, S);
+            dst[t * C + (int64_t)h * S + j] = y;
+        }
+    }
+    if (!live) return;
+    float * out = dst + T * C + head_state;
+    for (int i = 0; i < S; ++i) out[(int64_t)i * S + j] = st[i * WKV_COLS + lane];
+}
+
 static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
 } // namespace b200
@@ -767,6 +834,36 @@ int ggml_b200_op_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tensor * x
                              (uint8_t *)d.data));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
+}
+
+} // extern "C"
+
+// the one launch of RWKV_WKV6 (GLA false: a = r, b = td) and GATED_LINEAR_ATTN (GLA true: a = q, b = g, tf unused), after their check
+template <bool GLA>
+static int launch_wkv(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * a, const ggml_b200_tensor * b,
+                      const ggml_b200_tensor * tf, const ggml_b200_tensor * s, const ggml_b200_tensor * dst, float scale, void * stream) {
+    const int64_t S = k->ne[0], H = k->ne[1], T = k->ne[2], n_seqs = s->ne[1];
+    if (T == 0 || S == 0) return GGML_B200_OK;
+    const dim3 grid(blocks_for(S, WKV_COLS), (unsigned)H, (unsigned)n_seqs);
+    B200_CUDA_TRY(launch_pdl(wkv_kernel<GLA>, grid, dim3(WKV_COLS), wkv_smem_bytes(S), (cudaStream_t)stream, (const float *)k->data, (const float *)v->data,
+                             (const float *)a->data, (const float *)b->data, tf ? (const float *)tf->data : nullptr, (const float *)s->data, (float *)dst->data,
+                             (int)S, (int)H, T, T / n_seqs, scale));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+extern "C" {
+
+int ggml_b200_op_rwkv_wkv6(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * r, const ggml_b200_tensor * tf,
+                           const ggml_b200_tensor * td, const ggml_b200_tensor * s, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_rwkv_wkv6(k, v, r, tf, td, s, dst));
+    return launch_wkv<false>(k, v, r, td, tf, s, dst, 1.0f, stream);
+}
+
+int ggml_b200_op_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * q, const ggml_b200_tensor * g,
+                                   const ggml_b200_tensor * s, const ggml_b200_tensor * dst, float scale, void * stream) {
+    CHECK_ARGS(check_gated_linear_attn(k, v, q, g, s, dst));
+    return launch_wkv<true>(k, v, q, g, nullptr, s, dst, scale, stream);
 }
 
 } // extern "C"

@@ -278,6 +278,17 @@ GGML_B200_API int ggml_b200_op_ssm_conv(const ggml_b200_tensor * sx, const ggml_
  * order and rounding; any d_state (the states are kept in dst, not in registers), n_s <= 65535. */
 GGML_B200_API int ggml_b200_op_ssm_scan(const ggml_b200_tensor * s, const ggml_b200_tensor * x, const ggml_b200_tensor * dt, const ggml_b200_tensor * A,
                                         const ggml_b200_tensor * B, const ggml_b200_tensor * C, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_RWKV_WKV6 (the RWKV-6 time-mix recurrence): k, v, r, td f32 [S, H, T], tf f32 with S * H values, s f32 with S * S * H * n_seqs values
+ * (n_seqs = s->ne[1]), all contiguous -> dst f32 [S * H, T + S * n_seqs], contiguous: y [S * H, T], then the final states in s's layout.
+ * Sequence q owns tokens [q T / n_seqs, (q + 1) T / n_seqs) (T % n_seqs == 0, else GGML_B200_EINVAL) and starts from its state in s.  Per
+ * token, head and state element (i, j): kv = v[j] k[i]; y[j] += (kv tf[i] + state[i][j]) r[i], summed in ascending i; state[i][j] =
+ * state[i][j] td[i] + kv, rounded as the CPU backend's vector path.  S <= 256.  T == 0 writes nothing. */
+GGML_B200_API int ggml_b200_op_rwkv_wkv6(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * r, const ggml_b200_tensor * tf,
+                                         const ggml_b200_tensor * td, const ggml_b200_tensor * s, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_GATED_LINEAR_ATTN: as ggml_b200_op_rwkv_wkv6 with q and g in place of r and td and no tf: temp = state[i][j] g[i] + kv;
+ * y[j] += temp (q[i] scale); state[i][j] = temp. */
+GGML_B200_API int ggml_b200_op_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * q, const ggml_b200_tensor * g,
+                                                 const ggml_b200_tensor * s, const ggml_b200_tensor * dst, float scale, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
