@@ -23,32 +23,12 @@
 //   falcon  FalconMamba form: n_embd 1024, d_inner 2048, d_state 16, d_conv 4, dt_rank 64, RMS_NORM on the dt / B / C views, ssm_x and
 //           ssm_dt Q8_0; one sequence
 //
-// usage: mamba-graph PRESET compare DEVICE [sync]
-//          ggml_backend_compare_graph_backend of ggml-cpu against DEVICE over the prompt and one decode step.  Prints
-//          "node PHASE INDEX OP NAME [ne] nmse E" per contiguous f32 node, then per phase
-//          "summary PHASE sync|free nodes_over_1e-9 N worst W first_over INDEX OP logits L".
-//          With "sync" the device copy of each node result is replaced by the CPU's after the comparison.
-//        mamba-graph PRESET run DEVICE STEPS LOGITS_OUT [FORCE_TOKENS]
-//          ggml_backend_sched over [DEVICE, CPU], the prompt, then STEPS - 1 decode steps; writes per step the logits of each sequence's
-//          last token (STEPS x n_seqs rows of n_vocab f32) and prints "n_splits S", "cpu_nodes C", "tokens t0 t1 ..." (step-major, one per
-//          sequence and step) and "decode_ms_per_step M".  FORCE_TOKENS: i32 tokens in the same order, fed instead of the greedy ones.
-// Devices from $GGML_BACKEND_PATH are loaded with ggml_backend_load_all.
+// usage: mamba-graph PRESET compare DEVICE [sync] | PRESET run DEVICE STEPS LOGITS_OUT [FORCE_TOKENS]  (decoder_harness.h), n_seqs
+// sequences with 7-token prompts.
 
-#include "ggml.h"
-#include "ggml-alloc.h"
-#include "ggml-backend.h"
-#include "ggml-cpu.h"
+#include "decoder_harness.h"
 
-#include <chrono>
-#include <cinttypes>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <random>
-#include <string>
-#include <thread>
-#include <vector>
 
 namespace {
 
@@ -85,6 +65,12 @@ hparams preset(const std::string & name) {
 
 enum fill_kind { FILL_NORMAL, FILL_A, FILL_DT_BIAS };
 
+float fill_special(int kind, int64_t i, int64_t k, std::mt19937 & rng) {
+    if (kind == FILL_A) return -(float) (i % k + 1);                                                    // A[i0, i1] = -(i0 + 1)
+    const double dt = exp(std::uniform_real_distribution<double>(log(1e-3), log(1e-1))(rng));          // softplus^-1(dt) = dt + log(-expm1(-dt))
+    return (float) (dt + log(-expm1(-dt)));
+}
+
 // create the tensors of the model in ctx_w / ctx_s, allocate them in buffers of `bt`, fill the weights from fixed seeds
 void build_model(model & m, ggml_backend_buffer_type_t bt) {
     const hparams & hp = m.hp;
@@ -93,9 +79,7 @@ void build_model(model & m, ggml_backend_buffer_type_t bt) {
     m.ctx_w = ggml_init(ip);
     m.ctx_s = ggml_init(ip);
     ggml_context * c = m.ctx_w;
-    struct fill_job { ggml_tensor * t; float scale, offset; fill_kind kind; };
-    std::vector<fill_job> jobs;
-    auto w = [&](ggml_tensor * t, float scale, float offset, fill_kind kind = FILL_NORMAL) { jobs.push_back({ t, scale, offset, kind }); return t; };
+    weight_fill w;
     const float se = 1.0f / sqrtf((float) hp.n_embd), si = 1.0f / sqrtf((float) hp.d_inner);
     m.tok_embd = w(ggml_new_tensor_2d(c, GGML_TYPE_Q4_K, hp.n_embd, hp.n_vocab), 1.0f, 0.0f);
     m.out_norm = w(ggml_new_tensor_1d(c, GGML_TYPE_F32, hp.n_embd), 0.05f, 1.0f);
@@ -121,35 +105,14 @@ void build_model(model & m, ggml_backend_buffer_type_t bt) {
     ggml_backend_buffer_set_usage(m.buf_w, GGML_BACKEND_BUFFER_USAGE_WEIGHTS);
     ggml_backend_buffer_clear(m.buf_s, 0);
 
-    // tensor j is drawn from its own generator (seed 20240917 + j), so the parallel fill is deterministic
-    std::vector<std::vector<uint8_t>> bytes(jobs.size());
-    auto fill = [&](size_t j) {
-        const ggml_tensor * t = jobs[j].t;
-        std::mt19937 rng(20240917u + (unsigned) j);
-        std::normal_distribution<float> nd(0.0f, 1.0f);
-        std::uniform_real_distribution<double> ud(log(1e-3), log(1e-1));
-        const int64_t n = ggml_nelements(t), k = t->ne[0];
-        std::vector<float> x((size_t) n);
-        for (int64_t i = 0; i < n; ++i) {
-            switch (jobs[j].kind) {
-                case FILL_A: x[(size_t) i] = -(float) (i % k + 1); break;                              // A[i0, i1] = -(i0 + 1)
-                case FILL_DT_BIAS: {
-                    const double dt = exp(ud(rng));                                                     // softplus^-1(dt) = dt + log(-expm1(-dt))
-                    x[(size_t) i] = (float) (dt + log(-expm1(-dt)));
-                } break;
-                default: x[(size_t) i] = jobs[j].offset + jobs[j].scale * nd(rng); break;
-            }
-        }
-        bytes[j].resize(ggml_nbytes(t));
-        if (t->type == GGML_TYPE_F32) memcpy(bytes[j].data(), x.data(), bytes[j].size());
-        else ggml_quantize_chunk(t->type, x.data(), bytes[j].data(), 0, n / k, k, nullptr);
-    };
-    std::vector<std::thread> pool;
-    const size_t n_th = 8;
-    for (size_t th = 0; th < n_th; ++th)
-        pool.emplace_back([&, th] { for (size_t j = th; j < jobs.size(); j += n_th) fill(j); });
-    for (std::thread & t : pool) t.join();
-    for (size_t j = 0; j < jobs.size(); ++j) ggml_backend_tensor_set(jobs[j].t, bytes[j].data(), 0, bytes[j].size());
+    w.run(20240917u, fill_special);
+}
+
+void free_model(model & m) {
+    ggml_backend_buffer_free(m.buf_w);
+    ggml_backend_buffer_free(m.buf_s);
+    ggml_free(m.ctx_w);
+    ggml_free(m.ctx_s);
 }
 
 // the states of one cache for this batch: rows state_copy of s viewed as [n_state, n_seqs], cleared by state_mask on a fresh sequence
@@ -229,171 +192,32 @@ ggml_cgraph * build_graph(const model & m, ggml_context * ctx, int n_t) {
     return gf;
 }
 
-void set_inputs(const hparams & hp, ggml_cgraph * gf, bool first, const std::vector<int32_t> & toks) {
+// the first batch (n_past 0) starts every sequence from a cleared state
+void set_inputs(const hparams & hp, ggml_cgraph * gf, int n_past, const std::vector<int32_t> & toks) {
     ggml_backend_tensor_set(ggml_graph_get_tensor(gf, "inp_tokens"), toks.data(), 0, toks.size() * sizeof(int32_t));
     std::vector<int32_t> copy(hp.n_seqs);
-    std::vector<float> mask(hp.n_seqs, first ? 0.0f : 1.0f);
+    std::vector<float> mask(hp.n_seqs, n_past == 0 ? 0.0f : 1.0f);
     for (int s = 0; s < hp.n_seqs; ++s) copy[s] = s;
     ggml_backend_tensor_set(ggml_graph_get_tensor(gf, "state_copy"), copy.data(), 0, copy.size() * sizeof(int32_t));
     ggml_backend_tensor_set(ggml_graph_get_tensor(gf, "state_mask"), mask.data(), 0, mask.size() * sizeof(float));
 }
 
-// the prompts, sequence-major: n_seqs x 7 tokens
-std::vector<int32_t> prompt_tokens(const hparams & hp) {
-    const std::vector<int32_t> p[2] = { { 1, 417, 2093, 58, 3001, 777, 12 }, { 1, 96, 3333, 1024, 7, 2500, 640 } };
-    std::vector<int32_t> out;
-    for (int s = 0; s < hp.n_seqs; ++s) out.insert(out.end(), p[s % 2].begin(), p[s % 2].end());
-    return out;
-}
-const int PROMPT_LEN = 7;
-
-// ------------------------------------------------------------------ compare
-struct cmp_state { const char * tag; int n_bad; double worst; bool sync; int first_bad; char first_bad_op[64]; double logits; };
-
-double nmse_f32(const float * a, const float * b, size_t n) {       // as tests/test-backend-ops.cpp computes it (a = device, b = cpu)
-    double num = 0.0, den = 0.0;
-    for (size_t i = 0; i < n; ++i) { const double d = (double) a[i] - (double) b[i]; num += d * d; den += (double) a[i] * (double) a[i]; }
-    return den > 0.0 ? num / den : num;
-}
-
-bool on_node(int index, ggml_tensor * t1, ggml_tensor * t2, void * ud) {
-    cmp_state * st = (cmp_state *) ud;
-    if (!ggml_is_contiguous(t1) || t1->type != GGML_TYPE_F32) return true;     // views: compared through their consumers
-    const size_t n = (size_t) ggml_nelements(t1);
-    std::vector<float> a(n), b(n);
-    ggml_backend_tensor_get(t1, b.data(), 0, n * sizeof(float));                    // t1: CPU
-    ggml_backend_tensor_get(t2, a.data(), 0, n * sizeof(float));                    // t2: device
-    const double e = nmse_f32(a.data(), b.data(), n);
-    if (e > st->worst) st->worst = e;
-    if (e > 1e-9) { if (st->n_bad == 0) { st->first_bad = index; snprintf(st->first_bad_op, sizeof(st->first_bad_op), "%s", ggml_op_desc(t1)); } st->n_bad++; }
-    if (strcmp(t1->name, "result_output") == 0) st->logits = e;
-    if (st->sync) ggml_backend_tensor_set(t2, b.data(), 0, n * sizeof(float));
-    printf("node %s %d %s %s [%" PRId64 ",%" PRId64 ",%" PRId64 ",%" PRId64 "] nmse %.3e\n", st->tag, index, ggml_op_desc(t1), t1->name,
-           t1->ne[0], t1->ne[1], t1->ne[2], t1->ne[3], e);
-    return true;
-}
-
-int run_compare(model & m, ggml_backend_t cpu, ggml_backend_t dev, bool sync) {
-    const hparams & hp = m.hp;
-    ggml_gallocr_t allocr = ggml_gallocr_new(ggml_backend_get_default_buffer_type(cpu));
-    int rc = 0;
-    for (int phase = 0; phase < 2 && rc == 0; ++phase) {
-        const int n_t = phase == 0 ? PROMPT_LEN : 1;
-        std::vector<int32_t> toks = prompt_tokens(hp);
-        if (phase == 1) { toks.clear(); for (int s = 0; s < hp.n_seqs; ++s) toks.push_back(99 + 11 * s); }
-        ggml_init_params ip = { ggml_tensor_overhead() * 4096 + ggml_graph_overhead_custom(4096, false), nullptr, true };
-        ggml_context * ctx = ggml_init(ip);
-        ggml_cgraph * gf = build_graph(m, ctx, n_t);
-        ggml_gallocr_alloc_graph(allocr, gf);
-        set_inputs(hp, gf, phase == 0, toks);
-        cmp_state st{ phase == 0 ? "prompt" : "decode", 0, 0.0, sync, -1, "", -1.0 };
-        // the CPU evaluation also advances the CPU-side state caches that the decode phase copies over
-        if (!ggml_backend_compare_graph_backend(cpu, dev, gf, on_node, &st)) { fprintf(stderr, "graph copy failed\n"); rc = 5; }
-        printf("summary %s %s nodes_over_1e-9 %d worst %.3e first_over %d %s logits %.3e\n", st.tag, sync ? "sync" : "free", st.n_bad, st.worst, st.first_bad,
-               st.first_bad_op[0] ? st.first_bad_op : "-", st.logits);
-        ggml_free(ctx);
-    }
-    ggml_gallocr_free(allocr);
-    return rc;
-}
-
-// ------------------------------------------------------------------ run
-int run_decode(model & m, ggml_backend_t dev, ggml_backend_t cpu, int steps, const char * out_path, const char * force_path) {
-    const hparams & hp = m.hp;
-    std::vector<int32_t> force;
-    if (force_path) {
-        FILE * f = fopen(force_path, "rb");
-        if (!f) { fprintf(stderr, "cannot open %s\n", force_path); return 6; }
-        int32_t t;
-        while (fread(&t, sizeof(t), 1, f) == 1) force.push_back(t);
-        fclose(f);
-    }
-    ggml_backend_t backends[2] = { dev, cpu };
-    const int n_be = dev == cpu ? 1 : 2;
-    ggml_backend_sched_t sched = ggml_backend_sched_new(backends, nullptr, n_be, 4096, false);
-    FILE * out = fopen(out_path, "wb");
-    if (!out) { fprintf(stderr, "cannot open %s\n", out_path); return 6; }
-    std::vector<float> logits(hp.n_vocab);
-    std::vector<int32_t> generated;
-    int max_splits = 0, max_cpu_nodes = 0;
-    double decode_s = 0.0;
-    int n_decode = 0;
-    std::vector<int32_t> toks = prompt_tokens(hp);
-    for (int step = 0; step < steps; ++step) {
-        const int n_t = step == 0 ? PROMPT_LEN : 1;
-        ggml_init_params ip = { ggml_tensor_overhead() * 4096 + ggml_graph_overhead_custom(4096, false), nullptr, true };
-        ggml_context * ctx = ggml_init(ip);
-        ggml_cgraph * gf = build_graph(m, ctx, n_t);
-        ggml_backend_sched_reset(sched);
-        if (!ggml_backend_sched_alloc_graph(sched, gf)) { fprintf(stderr, "sched alloc failed\n"); return 7; }
-        set_inputs(hp, gf, step == 0, toks);
-        const auto t0 = std::chrono::steady_clock::now();
-        if (ggml_backend_sched_graph_compute(sched, gf) != GGML_STATUS_SUCCESS) { fprintf(stderr, "compute failed\n"); return 8; }
-        ggml_tensor * res = ggml_graph_get_tensor(gf, "result_output");
-        std::vector<int32_t> next(hp.n_seqs);
-        for (int s = 0; s < hp.n_seqs; ++s) {
-            const size_t row = (size_t) s * n_t + n_t - 1;                         // each sequence's last token
-            ggml_backend_tensor_get(res, logits.data(), row * hp.n_vocab * sizeof(float), hp.n_vocab * sizeof(float));
-            fwrite(logits.data(), sizeof(float), logits.size(), out);
-            int32_t best = 0;
-            for (int i = 1; i < hp.n_vocab; ++i) if (logits[i] > logits[best]) best = i;
-            const size_t k = (size_t) step * hp.n_seqs + s;
-            next[s] = k < force.size() ? force[k] : best;
-        }
-        const double dt = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        if (step >= 2) { decode_s += dt; ++n_decode; }                       // step 0: prompt; step 1: first decode (warm-up)
-        int cpu_nodes = 0;
-        for (int i = 0; i < ggml_graph_n_nodes(gf); ++i)
-            if (n_be == 2 && ggml_backend_sched_get_tensor_backend(sched, ggml_graph_node(gf, i)) == cpu) ++cpu_nodes;
-        if (ggml_backend_sched_get_n_splits(sched) > max_splits) max_splits = ggml_backend_sched_get_n_splits(sched);
-        if (cpu_nodes > max_cpu_nodes) max_cpu_nodes = cpu_nodes;
-        generated.insert(generated.end(), next.begin(), next.end());
-        toks = next;
-        ggml_free(ctx);
-    }
-    fclose(out);
-    printf("n_splits %d\ncpu_nodes %d\ntokens", max_splits, max_cpu_nodes);
-    for (int32_t t : generated) printf(" %d", t);
-    printf("\ndecode_ms_per_step %.4f\n", n_decode ? 1e3 * decode_s / n_decode : -1.0);
-    ggml_backend_sched_free(sched);
-    return 0;
-}
 
 } // namespace
 
 int main(int argc, char ** argv) {
-    if (argc < 4) {
-        fprintf(stderr, "usage: %s PRESET compare DEVICE [sync]\n       %s PRESET run DEVICE STEPS LOGITS_OUT [FORCE_TOKENS]\n", argv[0], argv[0]);
-        return 2;
-    }
-    ggml_backend_load_all();
     model m;
-    m.hp = preset(argv[1]);
-    const std::string mode = argv[2];
-    ggml_backend_t cpu = ggml_backend_init_by_type(GGML_BACKEND_DEVICE_TYPE_CPU, nullptr);
-    ggml_backend_cpu_set_n_threads(cpu, 8);
-    ggml_backend_t dev = cpu;
-    if (strcmp(argv[3], "CPU") != 0) {
-        ggml_backend_dev_t d = ggml_backend_dev_by_name(argv[3]);
-        if (!d) { fprintf(stderr, "no device %s\n", argv[3]); return 3; }
-        dev = ggml_backend_dev_init(d, nullptr);
-    }
-    int rc;
-    if (mode == "compare") {
-        build_model(m, ggml_backend_get_default_buffer_type(cpu));
-        rc = run_compare(m, cpu, dev, argc > 4 && strcmp(argv[4], "sync") == 0);
-    } else if (mode == "run" && argc >= 6) {
-        build_model(m, ggml_backend_get_default_buffer_type(dev));
-        rc = run_decode(m, dev, cpu, atoi(argv[4]), argv[5], argc > 6 ? argv[6] : nullptr);
-    } else {
-        fprintf(stderr, "unknown mode %s\n", mode.c_str());
-        return 2;
-    }
-    ggml_backend_buffer_free(m.buf_w);
-    ggml_backend_buffer_free(m.buf_s);
-    ggml_free(m.ctx_w);
-    ggml_free(m.ctx_s);
-    if (dev != cpu) ggml_backend_free(dev);
-    ggml_backend_free(cpu);
-    return rc;
+    return decoder_main(argc, argv, [&m](const std::string & name) {
+        m.hp = preset(name);
+        const std::vector<int32_t> p[2] = { { 1, 417, 2093, 58, 3001, 777, 12 }, { 1, 96, 3333, 1024, 7, 2500, 640 } };
+        decoder d;
+        d.n_seqs = m.hp.n_seqs;
+        d.n_vocab = m.hp.n_vocab;
+        for (int s = 0; s < m.hp.n_seqs; ++s) d.prompt.insert(d.prompt.end(), p[s % 2].begin(), p[s % 2].end());
+        d.build_model = [&m](ggml_backend_buffer_type_t bt) { build_model(m, bt); };
+        d.free_model = [&m] { free_model(m); };
+        d.build_graph = [&m](ggml_context * ctx, int, int n_t) { return build_graph(m, ctx, n_t); };
+        d.set_inputs = [&m](ggml_cgraph * gf, int n_past, const std::vector<int32_t> & toks) { set_inputs(m.hp, gf, n_past, toks); };
+        return d;
+    });
 }

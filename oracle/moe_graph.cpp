@@ -16,35 +16,15 @@
 //   moe60  Qwen-MoE-like: 60 experts of n_ff_exp 256 (a non-power-of-two sort), top-4, no normalisation, plus a dense shared expert
 //          (SwiGLU, n_ff 1024) gated by SIGMOID(MUL_MAT(gate_inp_shexp, cur)) and added to moe_out
 //
-// usage: moe-graph PRESET compare DEVICE [sync]
-//          ggml_backend_compare_graph_backend of ggml-cpu against DEVICE over a 7-token prompt and one decode step.  Prints
-//          "node PHASE INDEX OP NAME [ne] nmse E" per f32 node, "inode PHASE INDEX OP NAME [ne] mismatches M" per i32 node (M: index
-//          positions that differ), and per ARGSORT row whose top-n_used set differs from the CPU's
-//          "topk PHASE INDEX ROW margin D rms R" (D: the CPU's gap between its n_used-th and (n_used+1)-th probability; R: the RMS
-//          deviation of the device's probabilities from the CPU's over the whole router node), then per phase
-//          "summary PHASE sync|free nodes_over_1e-9 N worst W first_over INDEX OP logits L".
-//          With "sync" the device copy of each node result (f32 and i32) is replaced by the CPU's after the comparison.
-//        moe-graph PRESET run DEVICE STEPS LOGITS_OUT [FORCE_TOKENS]
-//          as llama-graph's run mode: ggml_backend_sched over [DEVICE, CPU], the prompt, then STEPS - 1 decode steps; writes the logits
-//          and prints "n_splits S", "cpu_nodes C", "tokens t0 t1 ..." and "decode_ms_per_step M".
-// Devices from $GGML_BACKEND_PATH are loaded with ggml_backend_load_all.
+// usage: moe-graph PRESET compare DEVICE [sync] | PRESET run DEVICE STEPS LOGITS_OUT [FORCE_TOKENS]  (decoder_harness.h), one sequence
+// with a 7-token prompt, STEPS + 7 <= n_ctx = 64.  In free-running compare mode each ARGSORT row whose top-n_used set differs from the
+// CPU's also prints "topk PHASE INDEX ROW margin D rms R" (D: the CPU's gap between its n_used-th and (n_used+1)-th probability; R: the
+// RMS deviation of the device's probabilities from the CPU's over the whole router node).
 
-#include "ggml.h"
-#include "ggml-alloc.h"
-#include "ggml-backend.h"
-#include "ggml-cpu.h"
+#include "decoder_harness.h"
 
 #include <algorithm>
-#include <chrono>
-#include <cinttypes>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <random>
-#include <string>
-#include <thread>
-#include <vector>
 
 namespace {
 
@@ -90,9 +70,7 @@ void build_model(model & m, ggml_backend_buffer_type_t bt) {
     m.ctx_w = ggml_init(ip);
     m.ctx_kv = ggml_init(ip);
     ggml_context * c = m.ctx_w;
-    struct fill_job { ggml_tensor * t; float scale, offset; };
-    std::vector<fill_job> jobs;
-    auto w = [&](ggml_tensor * t, float scale, float offset) { jobs.push_back({ t, scale, offset }); return t; };
+    weight_fill w;
     const float se = 1.0f / sqrtf((float) hp.n_embd);
     m.tok_embd = w(ggml_new_tensor_2d(c, GGML_TYPE_Q4_K, hp.n_embd, hp.n_vocab), 1.0f, 0.0f);
     m.out_norm = w(ggml_new_tensor_1d(c, GGML_TYPE_F32, hp.n_embd), 0.05f, 1.0f);
@@ -123,26 +101,14 @@ void build_model(model & m, ggml_backend_buffer_type_t bt) {
     if (!m.buf_w || !m.buf_kv) { fprintf(stderr, "model allocation failed\n"); exit(4); }
     ggml_backend_buffer_set_usage(m.buf_w, GGML_BACKEND_BUFFER_USAGE_WEIGHTS);
     ggml_backend_buffer_clear(m.buf_kv, 0);
+    w.run(20240611u);
+}
 
-    // tensor j is drawn from its own generator (seed 20240611 + j), so the parallel fill is deterministic
-    std::vector<std::vector<uint8_t>> bytes(jobs.size());
-    auto fill = [&](size_t j) {
-        const ggml_tensor * t = jobs[j].t;
-        std::mt19937 rng(20240611u + (unsigned) j);
-        std::normal_distribution<float> nd(0.0f, 1.0f);
-        const int64_t n = ggml_nelements(t), k = t->ne[0];
-        std::vector<float> x((size_t) n);
-        for (float & v : x) v = jobs[j].offset + jobs[j].scale * nd(rng);
-        bytes[j].resize(ggml_nbytes(t));
-        if (t->type == GGML_TYPE_F32) memcpy(bytes[j].data(), x.data(), bytes[j].size());
-        else ggml_quantize_chunk(t->type, x.data(), bytes[j].data(), 0, n / k, k, nullptr);
-    };
-    std::vector<std::thread> pool;
-    const size_t n_th = 8;
-    for (size_t th = 0; th < n_th; ++th)
-        pool.emplace_back([&, th] { for (size_t j = th; j < jobs.size(); j += n_th) fill(j); });
-    for (std::thread & t : pool) t.join();
-    for (size_t j = 0; j < jobs.size(); ++j) ggml_backend_tensor_set(jobs[j].t, bytes[j].data(), 0, bytes[j].size());
+void free_model(model & m) {
+    ggml_backend_buffer_free(m.buf_w);
+    ggml_backend_buffer_free(m.buf_kv);
+    ggml_free(m.ctx_w);
+    ggml_free(m.ctx_kv);
 }
 
 // the MoE FFN of layer l on cur [n_embd, N] (llama.cpp's build_moe_ffn with softmax gating and SILU experts)
@@ -230,192 +196,46 @@ void set_inputs(ggml_cgraph * gf, int n_past, const std::vector<int32_t> & toks)
     ggml_backend_tensor_set(ggml_graph_get_tensor(gf, "kq_mask"), mf.data(), 0, mf.size() * sizeof(float));
 }
 
-std::vector<int32_t> prompt_tokens() { return { 1, 417, 2093, 58, 3001, 777, 12 }; }
-
-// ------------------------------------------------------------------ compare
-struct cmp_state { const char * tag; int n_bad; double worst; bool sync; int first_bad; char first_bad_op[64]; double logits; int n_used; };
-
-double nmse_f32(const float * a, const float * b, size_t n) {       // as tests/test-backend-ops.cpp computes it (a = device, b = cpu)
-    double num = 0.0, den = 0.0;
-    for (size_t i = 0; i < n; ++i) { const double d = (double) a[i] - (double) b[i]; num += d * d; den += (double) a[i] * (double) a[i]; }
-    return den > 0.0 ? num / den : num;
-}
-
-void dims(const ggml_tensor * t, char * buf, size_t n) {
-    snprintf(buf, n, "[%" PRId64 ",%" PRId64 ",%" PRId64 ",%" PRId64 "]", t->ne[0], t->ne[1], t->ne[2], t->ne[3]);
-}
-
-// an i32 node: exact index mismatches; for ARGSORT in free-running mode, the rows whose top-n_used set differs and the CPU's margin there
-void on_i32_node(cmp_state * st, int index, ggml_tensor * t1, ggml_tensor * t2) {
-    const size_t n = (size_t) ggml_nelements(t1);
-    std::vector<int32_t> a(n), b(n);
-    ggml_backend_tensor_get(t1, b.data(), 0, n * sizeof(int32_t));                  // t1: CPU
-    ggml_backend_tensor_get(t2, a.data(), 0, n * sizeof(int32_t));                  // t2: device
-    size_t mism = 0;
-    for (size_t i = 0; i < n; ++i) mism += a[i] != b[i];
-    char ne[96];
-    dims(t1, ne, sizeof(ne));
-    printf("inode %s %d %s %s %s mismatches %zu\n", st->tag, index, ggml_op_desc(t1), t1->name, ne, mism);
-    if (t1->op == GGML_OP_ARGSORT && !st->sync && mism) {
-        const ggml_tensor * p1 = t1->src[0], * p2 = t2->src[0];                      // the router probabilities, contiguous [n_expert, N]
-        const int64_t ne0 = t1->ne[0], rows = (int64_t) n / ne0;
-        std::vector<float> pc((size_t) ggml_nelements(p1)), pd(pc.size());
-        ggml_backend_tensor_get(p1, pc.data(), 0, pc.size() * sizeof(float));
-        ggml_backend_tensor_get(p2, pd.data(), 0, pd.size() * sizeof(float));
-        double sq = 0.0;
-        for (size_t i = 0; i < pc.size(); ++i) sq += ((double) pd[i] - pc[i]) * ((double) pd[i] - pc[i]);
-        const double rms = sqrt(sq / (double) pc.size());
-        const int k = std::min<int64_t>(st->n_used, ne0);
-        for (int64_t r = 0; r < rows; ++r) {
-            std::vector<int32_t> sa(a.begin() + r * ne0, a.begin() + r * ne0 + k), sb(b.begin() + r * ne0, b.begin() + r * ne0 + k);
-            std::sort(sa.begin(), sa.end());
-            std::sort(sb.begin(), sb.end());
-            if (sa == sb) continue;
-            const float * pr = pc.data() + r * ne0;
-            const double margin = k < ne0 ? (double) pr[b[r * ne0 + k - 1]] - (double) pr[b[r * ne0 + k]] : 0.0;
-            printf("topk %s %d %" PRId64 " margin %.6e rms %.6e\n", st->tag, index, r, margin, rms);
-        }
+// a differing ARGSORT in free-running mode: the rows whose top-n_used set differs and the CPU's margin there (a: device, b: CPU)
+void report_topk(int n_used, const char * tag, int index, ggml_tensor * t1, ggml_tensor * t2, const std::vector<int32_t> & b,
+                 const std::vector<int32_t> & a) {
+    if (t1->op != GGML_OP_ARGSORT) return;
+    const ggml_tensor * p1 = t1->src[0], * p2 = t2->src[0];                          // the router probabilities, contiguous [n_expert, N]
+    const int64_t ne0 = t1->ne[0], rows = (int64_t) b.size() / ne0;
+    std::vector<float> pc((size_t) ggml_nelements(p1)), pd(pc.size());
+    ggml_backend_tensor_get(p1, pc.data(), 0, pc.size() * sizeof(float));
+    ggml_backend_tensor_get(p2, pd.data(), 0, pd.size() * sizeof(float));
+    double sq = 0.0;
+    for (size_t i = 0; i < pc.size(); ++i) sq += ((double) pd[i] - pc[i]) * ((double) pd[i] - pc[i]);
+    const double rms = sqrt(sq / (double) pc.size());
+    const int k = std::min<int64_t>(n_used, ne0);
+    for (int64_t r = 0; r < rows; ++r) {
+        std::vector<int32_t> sa(a.begin() + r * ne0, a.begin() + r * ne0 + k), sb(b.begin() + r * ne0, b.begin() + r * ne0 + k);
+        std::sort(sa.begin(), sa.end());
+        std::sort(sb.begin(), sb.end());
+        if (sa == sb) continue;
+        const float * pr = pc.data() + r * ne0;
+        const double margin = k < ne0 ? (double) pr[b[r * ne0 + k - 1]] - (double) pr[b[r * ne0 + k]] : 0.0;
+        printf("topk %s %d %" PRId64 " margin %.6e rms %.6e\n", tag, index, r, margin, rms);
     }
-    if (st->sync) ggml_backend_tensor_set(t2, b.data(), 0, n * sizeof(int32_t));
-}
-
-bool on_node(int index, ggml_tensor * t1, ggml_tensor * t2, void * ud) {
-    cmp_state * st = (cmp_state *) ud;
-    if (!ggml_is_contiguous(t1)) return true;                                       // views / f16 cache writes: compared through their consumers
-    if (t1->type == GGML_TYPE_I32) { on_i32_node(st, index, t1, t2); return true; }
-    if (t1->type != GGML_TYPE_F32) return true;
-    const size_t n = (size_t) ggml_nelements(t1);
-    std::vector<float> a(n), b(n);
-    ggml_backend_tensor_get(t1, b.data(), 0, n * sizeof(float));                    // t1: CPU
-    ggml_backend_tensor_get(t2, a.data(), 0, n * sizeof(float));                    // t2: device
-    const double e = nmse_f32(a.data(), b.data(), n);
-    if (e > st->worst) st->worst = e;
-    if (e > 1e-9) { if (st->n_bad == 0) { st->first_bad = index; snprintf(st->first_bad_op, sizeof(st->first_bad_op), "%s", ggml_op_desc(t1)); } st->n_bad++; }
-    if (strcmp(t1->name, "result_output") == 0) st->logits = e;
-    if (st->sync) ggml_backend_tensor_set(t2, b.data(), 0, n * sizeof(float));
-    char ne[96];
-    dims(t1, ne, sizeof(ne));
-    printf("node %s %d %s %s %s nmse %.3e\n", st->tag, index, ggml_op_desc(t1), t1->name, ne, e);
-    return true;
-}
-
-int run_compare(model & m, ggml_backend_t cpu, ggml_backend_t dev, bool sync) {
-    const std::vector<int32_t> prompt = prompt_tokens();
-    ggml_gallocr_t allocr = ggml_gallocr_new(ggml_backend_get_default_buffer_type(cpu));
-    int rc = 0;
-    for (int phase = 0; phase < 2 && rc == 0; ++phase) {
-        const int n_past = phase == 0 ? 0 : (int) prompt.size();
-        const std::vector<int32_t> toks = phase == 0 ? prompt : std::vector<int32_t>{ 99 };
-        ggml_init_params ip = { ggml_tensor_overhead() * 4096 + ggml_graph_overhead_custom(4096, false), nullptr, true };
-        ggml_context * ctx = ggml_init(ip);
-        ggml_cgraph * gf = build_graph(m, ctx, n_past, (int) toks.size());
-        ggml_gallocr_alloc_graph(allocr, gf);
-        set_inputs(gf, n_past, toks);
-        cmp_state st{ phase == 0 ? "prompt" : "decode", 0, 0.0, sync, -1, "", -1.0, m.hp.n_used };
-        // the CPU evaluation also fills the CPU-side KV cache that the decode phase copies over
-        if (!ggml_backend_compare_graph_backend(cpu, dev, gf, on_node, &st)) { fprintf(stderr, "graph copy failed\n"); rc = 5; }
-        printf("summary %s %s nodes_over_1e-9 %d worst %.3e first_over %d %s logits %.3e\n", st.tag, sync ? "sync" : "free", st.n_bad, st.worst, st.first_bad,
-               st.first_bad_op[0] ? st.first_bad_op : "-", st.logits);
-        ggml_free(ctx);
-    }
-    ggml_gallocr_free(allocr);
-    return rc;
-}
-
-// ------------------------------------------------------------------ run
-int run_decode(model & m, ggml_backend_t dev, ggml_backend_t cpu, int steps, const char * out_path, const char * force_path) {
-    const hparams & hp = m.hp;
-    std::vector<int32_t> force;
-    if (force_path) {
-        FILE * f = fopen(force_path, "rb");
-        if (!f) { fprintf(stderr, "cannot open %s\n", force_path); return 6; }
-        int32_t t;
-        while (fread(&t, sizeof(t), 1, f) == 1) force.push_back(t);
-        fclose(f);
-    }
-    const std::vector<int32_t> prompt = prompt_tokens();
-    if ((int) prompt.size() + steps > hp.n_ctx) { fprintf(stderr, "STEPS too large for n_ctx %d\n", hp.n_ctx); return 2; }
-    ggml_backend_t backends[2] = { dev, cpu };
-    const int n_be = dev == cpu ? 1 : 2;
-    ggml_backend_sched_t sched = ggml_backend_sched_new(backends, nullptr, n_be, 4096, false);
-    FILE * out = fopen(out_path, "wb");
-    if (!out) { fprintf(stderr, "cannot open %s\n", out_path); return 6; }
-    std::vector<float> logits(hp.n_vocab);
-    std::vector<int32_t> generated;
-    int n_past = 0, max_splits = 0, max_cpu_nodes = 0;
-    double decode_s = 0.0;
-    int n_decode = 0;
-    std::vector<int32_t> toks = prompt;
-    for (int step = 0; step < steps; ++step) {
-        ggml_init_params ip = { ggml_tensor_overhead() * 4096 + ggml_graph_overhead_custom(4096, false), nullptr, true };
-        ggml_context * ctx = ggml_init(ip);
-        ggml_cgraph * gf = build_graph(m, ctx, n_past, (int) toks.size());
-        ggml_backend_sched_reset(sched);
-        if (!ggml_backend_sched_alloc_graph(sched, gf)) { fprintf(stderr, "sched alloc failed\n"); return 7; }
-        set_inputs(gf, n_past, toks);
-        const auto t0 = std::chrono::steady_clock::now();
-        if (ggml_backend_sched_graph_compute(sched, gf) != GGML_STATUS_SUCCESS) { fprintf(stderr, "compute failed\n"); return 8; }
-        ggml_tensor * res = ggml_graph_get_tensor(gf, "result_output");
-        ggml_backend_tensor_get(res, logits.data(), (size_t) (toks.size() - 1) * hp.n_vocab * sizeof(float), hp.n_vocab * sizeof(float));
-        const double dt = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        if (step >= 2) { decode_s += dt; ++n_decode; }                       // step 0: prompt; step 1: first decode (warm-up)
-        int cpu_nodes = 0;
-        for (int i = 0; i < ggml_graph_n_nodes(gf); ++i)
-            if (n_be == 2 && ggml_backend_sched_get_tensor_backend(sched, ggml_graph_node(gf, i)) == cpu) ++cpu_nodes;
-        if (ggml_backend_sched_get_n_splits(sched) > max_splits) max_splits = ggml_backend_sched_get_n_splits(sched);
-        if (cpu_nodes > max_cpu_nodes) max_cpu_nodes = cpu_nodes;
-        fwrite(logits.data(), sizeof(float), logits.size(), out);
-        int32_t next = 0;
-        for (int i = 1; i < hp.n_vocab; ++i) if (logits[i] > logits[next]) next = i;
-        if (step < (int) force.size()) next = force[step];
-        generated.push_back(next);
-        n_past += (int) toks.size();
-        toks = { next };
-        ggml_free(ctx);
-    }
-    fclose(out);
-    printf("n_splits %d\ncpu_nodes %d\ntokens", max_splits, max_cpu_nodes);
-    for (int32_t t : generated) printf(" %d", t);
-    printf("\ndecode_ms_per_step %.4f\n", n_decode ? 1e3 * decode_s / n_decode : -1.0);
-    ggml_backend_sched_free(sched);
-    return 0;
 }
 
 } // namespace
 
 int main(int argc, char ** argv) {
-    if (argc < 4) {
-        fprintf(stderr, "usage: %s PRESET compare DEVICE [sync]\n       %s PRESET run DEVICE STEPS LOGITS_OUT [FORCE_TOKENS]\n", argv[0], argv[0]);
-        return 2;
-    }
-    ggml_backend_load_all();
     model m;
-    m.hp = preset(argv[1]);
-    const std::string mode = argv[2];
-    ggml_backend_t cpu = ggml_backend_init_by_type(GGML_BACKEND_DEVICE_TYPE_CPU, nullptr);
-    ggml_backend_cpu_set_n_threads(cpu, 8);
-    ggml_backend_t dev = cpu;
-    if (strcmp(argv[3], "CPU") != 0) {
-        ggml_backend_dev_t d = ggml_backend_dev_by_name(argv[3]);
-        if (!d) { fprintf(stderr, "no device %s\n", argv[3]); return 3; }
-        dev = ggml_backend_dev_init(d, nullptr);
-    }
-    int rc;
-    if (mode == "compare") {
-        build_model(m, ggml_backend_get_default_buffer_type(cpu));
-        rc = run_compare(m, cpu, dev, argc > 4 && strcmp(argv[4], "sync") == 0);
-    } else if (mode == "run" && argc >= 6) {
-        build_model(m, ggml_backend_get_default_buffer_type(dev));
-        rc = run_decode(m, dev, cpu, atoi(argv[4]), argv[5], argc > 6 ? argv[6] : nullptr);
-    } else {
-        fprintf(stderr, "unknown mode %s\n", mode.c_str());
-        return 2;
-    }
-    ggml_backend_buffer_free(m.buf_w);
-    ggml_backend_buffer_free(m.buf_kv);
-    ggml_free(m.ctx_w);
-    ggml_free(m.ctx_kv);
-    if (dev != cpu) ggml_backend_free(dev);
-    ggml_backend_free(cpu);
-    return rc;
+    return decoder_main(argc, argv, [&m](const std::string & name) {
+        m.hp = preset(name);
+        decoder d;
+        d.n_vocab = m.hp.n_vocab;
+        d.n_ctx = m.hp.n_ctx;
+        d.prompt = { 1, 417, 2093, 58, 3001, 777, 12 };
+        d.build_model = [&m](ggml_backend_buffer_type_t bt) { build_model(m, bt); };
+        d.free_model = [&m] { free_model(m); };
+        d.build_graph = [&m](ggml_context * ctx, int n_past, int n_t) { return build_graph(m, ctx, n_past, n_t); };
+        d.set_inputs = set_inputs;
+        d.on_i32_mismatch = [&m](const char * tag, int index, ggml_tensor * t1, ggml_tensor * t2, const std::vector<int32_t> & b,
+                                 const std::vector<int32_t> & a) { report_topk(m.hp.n_used, tag, index, t1, t2, b, a); };
+        return d;
+    });
 }

@@ -101,7 +101,7 @@ def _probe_lib():
         O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
         so = O.REF_DIR / "libggml_rope_probe.so"
         if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f llama.mk llama where the reference tree exists)")
+            raise RuntimeError(f"{so} missing (make -C oracle -f decoders.mk llama where the reference tree exists)")
         L = C.CDLL(str(so))
         L.probe_rope.restype = C.c_int
         L.probe_rope.argtypes = [C.c_char_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,

@@ -96,7 +96,7 @@ def _probe_lib():
         O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
         so = O.REF_DIR / "libggml_wkv_probe.so"
         if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f rwkv.mk rwkv where the reference tree exists)")
+            raise RuntimeError(f"{so} missing (make -C oracle -f decoders.mk rwkv where the reference tree exists)")
         L = C.CDLL(str(so))
         L.probe_rwkv_wkv6.restype = C.c_int
         L.probe_rwkv_wkv6.argtypes = [C.c_char_p] + [C.c_int64] * 4 + [C.c_void_p, C.c_void_p]

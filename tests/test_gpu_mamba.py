@@ -8,51 +8,28 @@ ggml_b200_op_concat / _ssm_conv / _ssm_scan and the plug-in), and Mamba decoder 
   (d) the `mamba` (Mamba-130m widths, two sequences) and `falcon` (FalconMamba form) presets: every node matches ggml-cpu on identical inputs,
       free-running logits stay close, the whole graph is one split with no CPU node, teacher-forced logits track ggml-cpu, and fusions /
       CUDA-graph replay change no logit bit (a replayed decode graph reads the states the previous replay wrote)."""
-import re
-import subprocess
-
 import numpy as np
 import pytest
 
+from oracle import decoder
 from oracle import oracle as O
 from oracle import ssm as S
 
 pytestmark = pytest.mark.gpu
 PRESETS = {"mamba": 2, "falcon": 1}          # preset -> sequences decoded side by side
-N_STEPS = 24
-N_VOCAB = 4096
 N_LAYER = 4
+EXE = O.REF_DIR / "mamba-graph"
 
 
 @pytest.fixture(scope="module")
 def plugin():
-    import ggml_b200
-    if not ggml_b200.BACKEND_SO.exists():
-        pytest.fail(f"{ggml_b200.BACKEND_SO} missing: run __graft_entry__.build() where the ggml headers are available")
-    for f in ("test-backend-ops", "mamba-graph", "libggml_ssm_probe.so"):
-        if not (O.REF_DIR / f).exists():
-            pytest.fail(f"oracle/_ref/{f} missing (oracle/Makefile and oracle/mamba.mk in the build container)")
-    ref = O.Ref()
-    assert ref.load_backend(ggml_b200.BACKEND_SO)
-    return ggml_b200.BACKEND_SO
+    return decoder.plugin("test-backend-ops", "mamba-graph", "libggml_ssm_probe.so")
 
 
 # ------------------------------------------------------------------ (a) the reference's test-backend-ops
 @pytest.mark.parametrize("op,n_min", [("CONCAT", 32), ("SSM_CONV", 3), ("SSM_SCAN", 1)])
 def test_reference_test_backend_ops(plugin, op, n_min):
-    env = O.ref_env()
-    env["GGML_BACKEND_PATH"] = str(plugin)
-    p = subprocess.run([str(O.REF_DIR / "test-backend-ops"), "test", "-o", op, "-b", "B2000"], env=env, capture_output=True, text=True, timeout=900)
-    out = p.stdout + p.stderr
-    tail = "\n".join(out.splitlines()[-25:])
-    assert p.returncode == 0 and "FAIL" not in out, tail
-    cases = [l for l in out.splitlines() if l.strip().startswith(op + "(")]
-    declined = [l for l in cases if "not supported" in l]
-    assert not declined, "\n".join(declined[:10])
-    ok = [l for l in cases if "OK" in l]
-    assert len(ok) == len(cases) and len(ok) >= n_min, (len(ok), len(cases), tail)
-    m = re.search(r"(\d+)/(\d+) tests passed", out)
-    assert m and m.group(1) == m.group(2), tail
+    decoder.check_test_backend_ops(plugin, op, n_min)
 
 
 # ------------------------------------------------------------------ (b) probe parity, device vs ggml-cpu
@@ -192,38 +169,10 @@ def test_c_abi_cuda_graph_replay_matches_eager():
 
 
 # ------------------------------------------------------------------ (d) the Mamba presets
-def _run(args, env_extra=None):
-    import ggml_b200
-    env = O.ref_env()
-    env["GGML_BACKEND_PATH"] = str(ggml_b200.BACKEND_SO)
-    env.update(env_extra or {})
-    p = subprocess.run([str(O.REF_DIR / "mamba-graph"), *args], env=env, capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, (p.stdout + p.stderr)[-3000:]
-    return p.stdout
-
-
-def compare(preset, sync):
-    out = _run([preset, "compare", "B2000"] + (["sync"] if sync else []))
-    summary = {}
-    for l in out.splitlines():
-        f = l.split()
-        if f and f[0] == "summary":
-            summary[f[1]] = dict(n_over=int(f[4]), worst=float(f[6]), first=int(f[8]), op=f[9], logits=float(f[11]))
-    nodes = [l.split() for l in out.splitlines() if l.startswith("node ")]
-    return summary, nodes
-
-
-def run(preset, dev, path, force=None, env_extra=None):
-    out = _run([preset, "run", dev, str(N_STEPS), str(path)] + ([str(force)] if force else []), env_extra)
-    kv = {l.split()[0]: l.split()[1:] for l in out.splitlines() if l.strip()}
-    logits = np.fromfile(path, dtype=np.float32).reshape(-1, N_VOCAB)
-    assert logits.shape[0] == N_STEPS * PRESETS[preset]
-    return kv, logits
-
-
 @pytest.mark.parametrize("preset", list(PRESETS))
 def test_mamba_graph_every_node_matches_cpu_on_identical_inputs(plugin, preset):
-    summary, nodes = compare(preset, sync=True)
+    summary, lines = decoder.compare(EXE, preset, sync=True)
+    nodes = lines["node"]
     assert set(summary) == {"prompt", "decode"}, summary
     for n in nodes:
         assert float(n[-1]) <= 1e-9, n
@@ -237,7 +186,7 @@ def test_mamba_graph_every_node_matches_cpu_on_identical_inputs(plugin, preset):
 
 @pytest.mark.parametrize("preset", list(PRESETS))
 def test_mamba_graph_free_running_logits(plugin, preset):
-    summary, _ = compare(preset, sync=False)
+    summary, _ = decoder.compare(EXE, preset, sync=False)
     assert set(summary) == {"prompt", "decode"}, summary
     for phase, s in summary.items():
         assert 0.0 <= s["logits"] <= 5e-3, (phase, s)
@@ -247,49 +196,23 @@ def test_mamba_graph_free_running_logits(plugin, preset):
 @pytest.fixture(scope="module")
 def cpu_runs(plugin, tmp_path_factory):
     d = tmp_path_factory.mktemp("mamba_cpu")
-    return {p: run(p, "CPU", d / f"{p}.logits") for p in PRESETS}
+    return {p: decoder.run(EXE, p, "CPU", d / f"{p}.logits", n) for p, n in PRESETS.items()}
 
 
 @pytest.mark.parametrize("preset", list(PRESETS))
 def test_mamba_graph_runs_in_one_split_on_the_device(plugin, preset, tmp_path):
-    kv, _ = run(preset, "B2000", tmp_path / "l.bin")
+    kv, _ = decoder.run(EXE, preset, "B2000", tmp_path / "l.bin", PRESETS[preset])
     assert int(kv["n_splits"][0]) == 1 and int(kv["cpu_nodes"][0]) == 0, kv
     print(f"mamba graph [{preset}]: one split, no CPU node, decode {kv['decode_ms_per_step'][0]} ms per step")
 
 
 @pytest.mark.parametrize("preset", list(PRESETS))
 def test_mamba_graph_logits_track_cpu_step_by_step(preset, cpu_runs, tmp_path):
-    ckv, cpu_logits = cpu_runs[preset]
-    ctoks = [int(t) for t in ckv["tokens"]]
-    assert ctoks == [int(v) for v in cpu_logits.argmax(1)]
-    force = tmp_path / "force.bin"
-    np.array(ctoks, dtype=np.int32).tofile(force)
-    _, gpu_logits = run(preset, "B2000", tmp_path / "forced.bin", force=force)
-    ties, worst, n_same = [], 0.0, 0
-    for i in range(cpu_logits.shape[0]):
-        c, g_ = cpu_logits[i].astype(np.float64), gpu_logits[i].astype(np.float64)
-        nm = O.nmse(gpu_logits[i], cpu_logits[i])
-        worst = max(worst, nm)
-        assert nm <= 5e-3, (preset, i, nm)
-        rms = float(np.sqrt(np.mean((g_ - c) ** 2)))
-        top2 = np.sort(c)[-2:]
-        margin = float(top2[1] - top2[0])
-        if int(g_.argmax()) != int(c.argmax()):
-            ties.append((i, margin, rms))
-            assert margin <= 6 * rms, f"{preset}: row {i}: argmax differs although the CPU margin {margin:.3e} exceeds 6 x the RMS deviation {rms:.3e}"
-        else:
-            n_same += 1
-    assert n_same >= cpu_logits.shape[0] // 2, (n_same, ties)
-    print(f"mamba graph [{preset}]: {N_STEPS} teacher-forced steps x {PRESETS[preset]} sequences, worst logits NMSE {worst:.2e}, "
-          f"same greedy token at {n_same}/{cpu_logits.shape[0]}, near-ties {ties[:5]}")
+    ties, worst, n_same, ctoks = decoder.check_tracks_cpu(EXE, preset, cpu_runs[preset], tmp_path, PRESETS[preset])
+    print(f"mamba graph [{preset}]: {decoder.N_STEPS} teacher-forced steps x {PRESETS[preset]} sequences, worst logits NMSE {worst:.2e}, "
+          f"same greedy token at {n_same}/{len(ctoks)}, near-ties {ties[:5]}")
 
 
 @pytest.mark.parametrize("preset", list(PRESETS))
 def test_mamba_graph_fusions_and_graph_replay_are_bit_exact(plugin, preset, tmp_path):
-    force = tmp_path / "force.bin"
-    np.arange(100, 100 + N_STEPS * PRESETS[preset], dtype=np.int32).tofile(force)
-    outs = {}
-    for name, env in (("default", {}), ("nofusion", {"GGML_B200_DISABLE_FUSION": "1"}), ("nographs", {"GGML_B200_DISABLE_GRAPHS": "1"})):
-        _, outs[name] = run(preset, "B2000", tmp_path / f"{name}.bin", force=force, env_extra=env)
-    for name in ("nofusion", "nographs"):
-        assert np.array_equal(outs["default"].view(np.uint32), outs[name].view(np.uint32)), (preset, name)
+    decoder.check_fusions_and_graphs_bit_exact(EXE, preset, tmp_path, PRESETS[preset])
