@@ -562,3 +562,63 @@ def op_gated_linear_attn(k, v, q, g, s, scale: float):
     L = lib()
     L.ggml_b200_op_gated_linear_attn.argtypes = [C.POINTER(TensorDesc)] * 6 + [C.c_float, C.c_void_p]
     return _wkv(L.ggml_b200_op_gated_linear_attn, "ggml_b200_op_gated_linear_attn", k, s, (k, v, q, g), (float(scale),))
+
+
+class Im2colParams(C.Structure):
+    """ggml_b200_im2col_params (include/ggml-b200.h)"""
+    _fields_ = [("s0", C.c_int32), ("s1", C.c_int32), ("p0", C.c_int32), ("p1", C.c_int32), ("d0", C.c_int32), ("d1", C.c_int32), ("is_2D", C.c_int32)]
+
+
+def conv_out_size(ins: int, ks: int, s: int, p: int, d: int) -> int:
+    """the output extent of a convolution along one axis (ggml_calc_conv_output_size)"""
+    return (ins + 2 * p - d * (ks - 1) - 1) // s + 1
+
+
+def op_im2col(kernel, x, s0: int, p0: int, d0: int, s1: int = 1, p1: int = 0, d1: int = 1, is_2d: bool = False, dtype=None):
+    """GGML_OP_IM2COL (the first node of ggml_conv_1d / ggml_conv_2d): kernel [OC, IC, KW] (2-D: [OC, IC, KH, KW]; only its shape is read, and
+    its dtype, which must be float16 for a float16 result), x f32 [N, IC, IW] (2-D: [N, IC, IH, IW]; last dim contiguous, any other strides)
+    -> a new contiguous tensor [N, OW, IC KW] (2-D: [N, OH, OW, IC KH KW]) of `dtype` (default float16, as ggml_conv_1d builds it),
+    bit-identical to ggml-cpu"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_im2col.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.POINTER(Im2colParams), C.c_void_p]
+    dtype = torch.float16 if dtype is None else dtype
+    kw, ic = kernel.shape[-1], x.shape[1]
+    ow = conv_out_size(x.shape[-1], kw, s0, p0, d0)
+    if is_2d:
+        kh = kernel.shape[-2]
+        shape = (x.shape[0], conv_out_size(x.shape[-2], kh, s1, p1, d1), ow, ic * kh * kw)
+    else:
+        shape = (x.shape[0], ow, ic * kw)
+    y = torch.empty(shape, dtype=dtype, device=x.device)
+    p = Im2colParams(s0, s1, p0, p1, d0, d1, 1 if is_2d else 0)
+    k, s, d = strided_desc(kernel), strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_im2col(C.byref(k), C.byref(s), C.byref(d), C.byref(p), _stream()), "ggml_b200_op_im2col")
+    return y
+
+
+def mul_mat_f16_f16_workspace_size(M: int, N: int, K: int) -> int:
+    """bytes the tensor-core f16 x f16 GEMM needs for [M, K] x [N, K]; 0 when the shape is not eligible for it"""
+    L = lib()
+    L.ggml_b200_mul_mat_f16_f16_workspace_size.restype = C.c_size_t
+    L.ggml_b200_mul_mat_f16_f16_workspace_size.argtypes = [C.c_int64] * 3
+    return int(L.ggml_b200_mul_mat_f16_f16_workspace_size(M, N, K))
+
+
+def mul_mat_f16_f16(w, x, flags: int = 0, out=None):
+    """f16 w [M, K] x f16 x [N, K] (rows contiguous, any row stride that is a multiple of 16 bytes) -> f32 [N, M] on the tensor cores
+    (ggml_b200_mul_mat_f16_f16); raises when the shape is not eligible (N >= 9, K % 64 == 0)"""
+    import torch
+    L = lib()
+    L.ggml_b200_mul_mat_f16_f16.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
+                                            C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
+    M, K = w.shape
+    N = x.shape[0]
+    need = mul_mat_f16_f16_workspace_size(M, N, K)
+    if need == 0:
+        raise B200Error(f"mul_mat_f16_f16: ({M}, {N}, {K}) is not eligible for the tensor-core path")
+    y = out if out is not None else torch.empty((N, M), dtype=torch.float32, device=w.device)
+    ws = _ws.get(need)
+    check(L.ggml_b200_mul_mat_f16_f16(w.data_ptr(), w.stride(0) * 2, x.data_ptr(), x.stride(0) * 2, y.data_ptr(), M, N, K, ws.data_ptr(), ws.numel(),
+                                      flags, _stream()), "ggml_b200_mul_mat_f16_f16")
+    return y

@@ -233,6 +233,13 @@ int ggml_b200_mul_mat_f16(const void * w, size_t nb01, const float * x, size_t n
     return launch_mmq_f16w(w, nb01, x, nb11, y, M, N, K, workspace, workspace_size, flags, (cudaStream_t)stream);
 }
 
+size_t ggml_b200_mul_mat_f16_f16_workspace_size(int64_t M, int64_t N, int64_t K) { return mmq_f16f16_workspace(M, N, K); }
+int ggml_b200_mul_mat_f16_f16(const void * w, size_t nb01, const void * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * workspace, size_t workspace_size,
+                              uint32_t flags, void * stream) {
+    if (M == 0 || N == 0) return GGML_B200_OK;
+    return launch_mmq_f16f16(w, nb01, x, nb11, y, M, N, K, workspace, workspace_size, flags, (cudaStream_t)stream);
+}
+
 int ggml_b200_mul_mat_fused(const ggml_b200_mul_mat_args * args, const ggml_b200_epilogue * ep, void * stream) {
     int rc = validate(args);
     if (rc != GGML_B200_OK) return rc;

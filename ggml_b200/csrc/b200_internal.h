@@ -101,6 +101,8 @@ bool   plan_dense(const ggml_b200_mul_mat_args & a, dense_plan & pl);   // n >= 
 int    launch_dense(const ggml_b200_mul_mat_args & a, const dense_plan & pl, cudaStream_t st);
 size_t mmq_f16w_workspace(int64_t M, int64_t N, int64_t K);         // dense fp16 weights, n >= 9 (0 = not eligible)
 int    launch_mmq_f16w(const void * w, size_t nb01, const float * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * ws, size_t ws_size, uint32_t flags, cudaStream_t st);
+size_t mmq_f16f16_workspace(int64_t M, int64_t N, int64_t K);       // dense fp16 x fp16, n >= 9, K % 64 == 0 (0 = not eligible)
+int    launch_mmq_f16f16(const void * w, size_t nb01, const void * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * ws, size_t ws_size, uint32_t flags, cudaStream_t st);
 // expert-grouped MUL_MAT_ID on the GEMM kernel (mmq_tc2.cu); the caller checks the workspace
 bool   plan_mmid_grouped(const ggml_b200_mul_mat_id_args & a, mmid_g_plan & pl);
 int    launch_mmid_grouped(const ggml_b200_mul_mat_id_args & a, const mmid_g_plan & pl, cudaStream_t st);

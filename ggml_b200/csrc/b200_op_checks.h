@@ -49,12 +49,16 @@ inline bool same_shape(const ggml_b200_tensor & a, const ggml_b200_tensor & b) {
     return a.ne[0] == b.ne[0] && a.ne[1] == b.ne[1] && a.ne[2] == b.ne[2] && a.ne[3] == b.ne[3];
 }
 inline bool is_float(int32_t t) { return t == GGML_B200_TYPE_F32 || t == GGML_B200_TYPE_F16; }
-// a tensor of 4-byte elements (f32, i32) stored without gaps, in ggml's order
-inline bool is_packed4(const ggml_b200_tensor & t) {
-    size_t nb = 4;
+// a tensor of es-byte elements stored without gaps, in ggml's order
+inline bool is_packed(const ggml_b200_tensor & t, size_t es) {
+    size_t nb = es;
     for (int i = 0; i < 4; ++i) { if (t.ne[i] != 1 && t.nb[i] != nb) return false; nb *= (size_t)t.ne[i]; }
     return true;
 }
+inline bool is_packed4(const ggml_b200_tensor & t) { return is_packed(t, 4); }      // f32, i32
+
+// the output extent of a convolution along one axis (ggml_calc_conv_output_size, src/ggml.c:3770)
+inline int64_t conv_out_size(int64_t ins, int64_t ks, int64_t s, int64_t p, int64_t d) { return (ins + 2 * p - d * (ks - 1) - 1) / s + 1; }
 
 // the block formats this library decodes (every one of them also runs the quantized MUL_MAT / MUL_MAT_ID)
 inline bool is_block_type(int32_t t) {
@@ -133,7 +137,8 @@ inline op_check check_flash_attn_ext(const ggml_b200_tensor * q, const ggml_b200
 
 inline op_check check_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst) {
     const ggml_b200_tensor & a = *src0, & b = *src1, & d = *dst;
-    B200_REQUIRE(is_float(a.type) && b.type == F32 && d.type == F32, "f32/f16 x f32 -> f32");
+    // an f16 src1 only with an f16 src0: the CPU backend's vec_dot type for f16 weights, used as is (any other pair it converts first)
+    B200_REQUIRE(is_float(a.type) && (b.type == F32 || (b.type == F16 && a.type == F16)) && d.type == F32, "f32/f16 x f32 or f16 x f16 -> f32");
     B200_REQUIRE(a.ne[0] == b.ne[0] && d.ne[0] == a.ne[1] && d.ne[1] == b.ne[1] && d.ne[2] == b.ne[2] && d.ne[3] == b.ne[3], "shape mismatch");
     B200_REQUIRE(b.ne[2] % a.ne[2] == 0 && b.ne[3] % a.ne[3] == 0, "batch dims do not broadcast");
     return accepted;
@@ -279,6 +284,30 @@ inline op_check check_rwkv_wkv6(const ggml_b200_tensor * k, const ggml_b200_tens
 inline op_check check_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * q, const ggml_b200_tensor * g,
                                         const ggml_b200_tensor * s, const ggml_b200_tensor * dst) {
     return check_wkv_common(k, v, q, g, s, dst);
+}
+
+// IM2COL: src0 the conv kernel (its extents), src1 the f32 input, dst [IC KH KW, OW, OH, N] (1-D: [IC KW, OW, N, 1]), f32 or f16
+inline op_check check_im2col(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, const ggml_b200_im2col_params * params) {
+    B200_REQUIRE(src0 && src1 && dst && params, "src0, src1, dst and params are required");
+    const ggml_b200_tensor & k = *src0, & x = *src1, & d = *dst;
+    const ggml_b200_im2col_params & c = *params;
+    B200_VALID(c.is_2D == 0 || c.is_2D == 1, "is_2D must be 0 or 1");
+    B200_VALID(c.s0 >= 1 && c.d0 >= 1 && (!c.is_2D || (c.s1 >= 1 && c.d1 >= 1)), "strides and dilations must be >= 1");
+    B200_REQUIRE(x.type == F32 && x.nb[0] == 4, "src1 must be f32, contiguous along dim 0");
+    // ggml-cpu writes dst as if it were packed, whatever its strides
+    B200_REQUIRE(is_float(d.type) && is_packed(d, d.type == F32 ? 4 : 2), "dst must be f32 or f16 and packed");
+    B200_REQUIRE(d.type == F32 || (k.type == F16 && k.nb[0] == 2), "an f16 dst needs an f16 src0");
+    B200_REQUIRE(c.is_2D || x.ne[3] == 1, "the 1-D input must be 3-D");
+    const bool two = c.is_2D == 1;
+    const int64_t KW = k.ne[0], KH = two ? k.ne[1] : 1, IC = two ? x.ne[2] : x.ne[1], N = two ? x.ne[3] : x.ne[2];
+    const int64_t OW = conv_out_size(x.ne[0], KW, c.s0, c.p0, c.d0), OH = two ? conv_out_size(x.ne[1], KH, c.s1, c.p1, c.d1) : 1;
+    B200_REQUIRE(d.ne[0] == IC * KH * KW && d.ne[1] == OW && d.ne[2] == (two ? OH : N) && d.ne[3] == (two ? N : 1),
+                 "dst must be [IC KH KW, OW, OH, N] (1-D: [IC KW, OW, N, 1]) of the input and params");
+    // ggml-cpu keeps the image and channel offsets of src1 in an int: beyond INT32_MAX the two backends would read different data
+    B200_REQUIRE((two ? x.nb[3] : x.nb[2]) <= 0x7fffffff && (two ? x.nb[2] : x.nb[1]) <= 0x7fffffff, "src1 image / channel strides above INT32_MAX bytes");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
 }
 
 #undef B200_REQUIRE

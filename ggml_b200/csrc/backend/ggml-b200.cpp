@@ -506,6 +506,14 @@ ggml_b200_rope_params rope_params(const ggml_tensor * node) {
     return rp;
 }
 
+// the strides, paddings, dilations and form of an IM2COL node: op_params as ggml_im2col writes them (read back at ggml-cpu.c:9886-9892)
+ggml_b200_im2col_params im2col_params(const ggml_tensor * node) {
+    const int32_t * ip = (const int32_t *) node->op_params;
+    ggml_b200_im2col_params p;
+    p.s0 = ip[0]; p.s1 = ip[1]; p.p0 = ip[2]; p.p1 = ip[3]; p.d0 = ip[4]; p.d1 = ip[5]; p.is_2D = ip[6];
+    return p;
+}
+
 // the ops whose launcher takes descriptors: its check, on the descriptors compute_nodes passes, plus what the launcher does not see
 bool supports_checked_op(const ggml_tensor * op) {
     const ggml_tensor * a = op->src[0], * b = op->src[1];
@@ -549,6 +557,11 @@ bool supports_checked_op(const ggml_tensor * op) {
         case GGML_OP_SUM_ROWS: return b200::check_sum_rows(&x, &d).ok();
         case GGML_OP_CONCAT: { const ggml_b200_tensor y = desc(b); return b200::check_concat(&x, &y, &d, ggml_get_op_params_i32(op, 0)).ok(); }
         case GGML_OP_SSM_CONV: { const ggml_b200_tensor c = desc(b); return b200::check_ssm_conv(&x, &c, &d).ok(); }
+        case GGML_OP_IM2COL: {                             // GGML_OP_IM2COL_BACK (training) stays declined
+            const ggml_b200_tensor y = desc(b);
+            const ggml_b200_im2col_params p = im2col_params(op);
+            return b200::check_im2col(&x, &y, &d, &p).ok();
+        }
         case GGML_OP_SSM_SCAN: {
             ggml_b200_tensor t[6];
             for (int k = 0; k < 6; ++k) t[k] = desc(op->src[k]);
@@ -843,6 +856,11 @@ void compute_small_op(backend_ctx * ctx, ggml_tensor * node) {
             SHIM_OK(ggml_b200_op_concat(&x, &y, &d, ggml_get_op_params_i32(node, 0), st));
         } break;
         case GGML_OP_SSM_CONV: { auto x = desc(a), c = desc(b), d = desc(node); SHIM_OK(ggml_b200_op_ssm_conv(&x, &c, &d, st)); } break;
+        case GGML_OP_IM2COL: {
+            auto k = desc(a), x = desc(b), d = desc(node);
+            const ggml_b200_im2col_params p = im2col_params(node);
+            SHIM_OK(ggml_b200_op_im2col(&k, &x, &d, &p, st));
+        } break;
         case GGML_OP_SSM_SCAN: {
             // sources: s, x, dt, A, B, C (ggml_ssm_scan); dst = y, then the final states
             ggml_b200_tensor t[6];
@@ -964,6 +982,17 @@ bool f16_weights_on_tensor_cores(const ggml_tensor * node) {
     return ggml_b200_mul_mat_f16_workspace_size(a->ne[1], b->ne[1], a->ne[0]) > 0;
 }
 
+// f16 x f16 with a batch (the conv mat-mul of ggml_conv_1d / _2d: src0 the IM2COL result, src1 the conv kernel): the tensor-core kernel
+// with both operands read by TMA (plain 2-D operands, rows 16-byte aligned, K % 64 == 0); every other f16 x f16 node takes mul_mat_f
+bool f16_f16_on_tensor_cores(const ggml_tensor * node) {
+    const ggml_tensor * a = node->src[0], * b = node->src[1];
+    if (a->type != GGML_TYPE_F16 || b->type != GGML_TYPE_F16 || node->type != GGML_TYPE_F32) return false;
+    if (a->ne[2] != 1 || a->ne[3] != 1 || b->ne[2] != 1 || b->ne[3] != 1 || b->ne[1] < 9) return false;
+    if (a->nb[0] != 2 || b->nb[0] != 2 || (a->nb[1] % 16) != 0 || (b->nb[1] % 16) != 0 || a->nb[1] < 2 * (size_t) a->ne[0] || b->nb[1] < 2 * (size_t) b->ne[0]) return false;
+    if (((uintptr_t) a->data % 16) != 0 || ((uintptr_t) b->data % 16) != 0 || !ggml_is_contiguous(node)) return false;
+    return ggml_b200_mul_mat_f16_f16_workspace_size(a->ne[1], b->ne[1], a->ne[0]) > 0;
+}
+
 size_t node_scratch_need(const ggml_tensor * node) {
     if (node->op == GGML_OP_MUL_MAT && is_b200_weight_type(node->src[0]->type)) {
         // the flags the launch will pass (SRC0_STATIC) select neither the kernel nor the workspace size
@@ -971,6 +1000,7 @@ size_t node_scratch_need(const ggml_tensor * node) {
         return ggml_b200_mul_mat_workspace_size(&args);
     }
     if (node->op == GGML_OP_MUL_MAT && f16_weights_on_tensor_cores(node)) return ggml_b200_mul_mat_f16_workspace_size(node->src[0]->ne[1], node->src[1]->ne[1], node->src[0]->ne[0]);
+    if (node->op == GGML_OP_MUL_MAT && f16_f16_on_tensor_cores(node)) return ggml_b200_mul_mat_f16_f16_workspace_size(node->src[0]->ne[1], node->src[1]->ne[1], node->src[0]->ne[0]);
     if (node->op == GGML_OP_MUL_MAT_ID) {
         const ggml_b200_mul_mat_id_args args = mul_mat_id_args(node);
         return ggml_b200_mul_mat_id_workspace_size(&args);
@@ -1103,6 +1133,12 @@ void compute_nodes(backend_ctx * ctx, ggml_cgraph * cgraph) {
                     void * ws = ctx->scratch(need);
                     SHIM_OK(ggml_b200_mul_mat_f16(a->data, a->nb[1], (const float *) b->data, b->nb[1], (float *) node->data, a->ne[1], b->ne[1], a->ne[0], ws, ctx->workspace_size,
                                                   src0_flags(ctx, node->src[0]), ctx->stream));
+                } else if (f16_f16_on_tensor_cores(node)) {
+                    const ggml_tensor * a = node->src[0], * b = node->src[1];
+                    const size_t need = ggml_b200_mul_mat_f16_f16_workspace_size(a->ne[1], b->ne[1], a->ne[0]);
+                    void * ws = ctx->scratch(need);
+                    SHIM_OK(ggml_b200_mul_mat_f16_f16(a->data, a->nb[1], b->data, b->nb[1], (float *) node->data, a->ne[1], b->ne[1], a->ne[0], ws, ctx->workspace_size,
+                                                      src0_flags(ctx, node->src[0]), ctx->stream));
                 } else { auto x = desc(node->src[0]), y = desc(node->src[1]), d = desc(node); SHIM_OK(ggml_b200_op_mul_mat_f(&x, &y, &d, ctx->stream)); }
                 break;
             case GGML_OP_MUL_MAT_ID: compute_mul_mat_id(ctx, node); break;

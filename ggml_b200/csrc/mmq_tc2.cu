@@ -10,7 +10,8 @@
 // codes convert to fp16 with two packed-half instructions per two weights and carry 11 instead of 8 significant bits.  NMSE against
 // the CPU backend ~1e-7 .. 1e-6 (the reference's gate is 5e-4, tests/test-backend-ops.cpp:1915-1917).  T_F16: the A operand already
 // is fp16 (dense f16 weights, or a format without an operand decoder dequantized into the workspace first, launch_dense) and
-// arrives by TMA like X.
+// arrives by TMA like X.  f16 x f16 (launch_mmq_f16f16, the conv mat-mul of ggml_conv_1d / _2d): X already is fp16 and comes by TMA straight
+// from src1, with no conversion kernel and no row scale.
 //
 // Warp roles (12 warps, three warpgroups; setmaxnreg moves the producer's registers to the consumers):
 //   warps 0-7   two consumer warpgroups; thread t owns W row t of the tile.  Per K-step (64 weights) each thread dequantizes its
@@ -284,7 +285,7 @@ mmq_tc2_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     // inv_scale of the tile's columns -> shared memory
     for (int c = tid; c < p.BN; c += T2_CONSUMERS) {
         const int64_t n = GROUPED ? (int64_t)gn0 + c : (int64_t)tn * p.BN + c;
-        s_inv[c] = (GROUPED ? c < gcols : n < p.N) ? __ldcg(p.inv_scale + n) : 0.0f;
+        s_inv[c] = (GROUPED ? c < gcols : n < p.N) ? (p.inv_scale ? __ldcg(p.inv_scale + n) : 1.0f) : 0.0f;     // null: fp16 activations, unscaled
     }
     if (p.splitk > 1 && tid == 0) { while (atomicAdd(&p.flags[tile], 0u) < (unsigned)(p.splitk - 1)) __nanosleep(64); __threadfence(); }
     consumers_sync();
@@ -374,17 +375,23 @@ static bool tc2_smem_plan(int BN, int raw, int & nstages, int & smem) {
     return true;
 }
 
-bool plan_wgmma(const ggml_b200_mul_mat_args & a, tc2_plan & pl) {
-    const bool dense = a.type == T_F16;                            // fp16 A tiles (launch_dense / launch_mmq_f16w)
+// x_f16: src1 already is fp16 (f16 x f16, launch_mmq_f16f16): its B tiles come by TMA straight from src1, so its rows must be 16-byte
+// aligned, and nothing is converted or scaled.  Its K rule is the dense form's own granularity, one 64-wide K-step per unit (split-K
+// divides units, at most one split per unit); the other routes keep theirs.
+static bool plan_tc2(const ggml_b200_mul_mat_args & a, bool x_f16, tc2_plan & pl) {
+    const bool dense = a.type == T_F16;                            // fp16 A tiles (launch_dense / launch_mmq_f16w / launch_mmq_f16f16)
     int raw = 0, ksteps = 1;                                       // T_F16: no raw ring, one K-step per unit
+    if (x_f16 && !dense) return false;
     if (!dense && !tc2_unit_geometry(a.type, raw, ksteps)) return false;
     if (a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
     // n >= 9: every batch the mat-vec kernels do not take (the reference's mul_mat_q threshold, ggml-cuda.cu:1852-1875); also 5 <= n <= 8
     // when the mat-vec kernel cannot hold that many activation records next to its weight stages (very long rows: api.cu decides);
     // columns beyond n in the 64-wide minimum tile are zero-filled by the TMA box and never stored
-    if (a.N < (dense ? 9 : 5) || a.M < 1 || a.K % 256 != 0 || a.K < 256) return false;
+    const int64_t k_unit = x_f16 ? T2_BK : 256;
+    if (a.N < (dense ? 9 : 5) || a.M < 1 || a.K % k_unit != 0 || a.K < k_unit) return false;
     const size_t rb = dense ? (size_t)a.K * 2 : row_bytes(a.type, a.K);
     if ((dense ? (a.nb01 < rb || (a.nb01 % 16) != 0) : a.nb01 != rb) || (rb % 16) != 0 || ((uintptr_t)a.src0 & 15) != 0 || ((uintptr_t)a.src1 & 3) != 0 || (a.nb11 & 3) != 0) return false;
+    if (x_f16 && (a.nb11 < rb || (a.nb11 % 16) != 0 || ((uintptr_t)a.src1 & 15) != 0)) return false;
     if (a.M >= (1ll << 31) || a.N >= (1ll << 31) || rb >= (1ull << 31)) return false;
     if (!tc_get_encode()) return false;
     static const int env_bn = getenv("GGML_B200_TC2_BN") ? atoi(getenv("GGML_B200_TC2_BN")) : 0;
@@ -402,12 +409,14 @@ bool plan_wgmma(const ggml_b200_mul_mat_args & a, tc2_plan & pl) {
     pl.splitk = splitk;
     if (!tc2_smem_plan(BN, raw, pl.nstages, pl.smem)) return false;
     pl.grid = tiles * splitk;
-    pl.xb_bytes = ((size_t)a.N * a.K * 2 + 255) & ~(size_t)255;
+    pl.xb_bytes = x_f16 ? 0 : ((size_t)a.N * a.K * 2 + 255) & ~(size_t)255;
     pl.partial_bytes = splitk > 1 ? (size_t)tiles * (splitk - 1) * BN * T2_BM * 4 : 0;
-    pl.scale_bytes = ((size_t)a.N * 4 + 255) & ~(size_t)255;
+    pl.scale_bytes = x_f16 ? 0 : ((size_t)a.N * 4 + 255) & ~(size_t)255;
     pl.workspace = pl.xb_bytes + pl.partial_bytes + pl.scale_bytes + 1024;
     return true;
 }
+
+bool plan_wgmma(const ggml_b200_mul_mat_args & a, tc2_plan & pl) { return plan_tc2(a, false, pl); }
 
 // 2-D tensor map over a row-major matrix (dims and box innermost first, row stride in bytes); false with the error set on failure
 static bool encode_2d(CUtensorMap * map, CUtensorMapDataType dtype, const void * base, uint64_t cols, uint64_t rows, uint64_t row_stride,
@@ -422,16 +431,18 @@ static bool encode_2d(CUtensorMap * map, CUtensorMapDataType dtype, const void *
     return true;
 }
 
-template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const tc2_plan & pl, cudaStream_t st) {
+// x_f16 (plan_tc2 with x_f16, T_F16 only): the fp16 activations [N][K] with row stride a.nb11, read by TMA as they are; no conversion
+// kernel runs in front and the epilogue scales nothing (inv_scale null)
+template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const tc2_plan & pl, cudaStream_t st, const void * x_f16 = nullptr) {
     if (!a.workspace || a.workspace_size < pl.workspace) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, pl.workspace); return GGML_B200_EWORKSPACE; }
     uint8_t * ws = (uint8_t *)(((uintptr_t)a.workspace + 255) & ~(uintptr_t)255);
     __half * xb = (__half *)ws;
     float * partials = pl.partial_bytes ? (float *)(ws + pl.xb_bytes) : nullptr;
-    float * inv_scale = (float *)(ws + pl.xb_bytes + pl.partial_bytes);
+    float * inv_scale = x_f16 ? nullptr : (float *)(ws + pl.xb_bytes + pl.partial_bytes);
     unsigned int * flags = tc_flag_slot();
     if (!flags) return GGML_B200_ECUDA;
 
-    { const int rc = tc_launch_x_to_f16(a.src1, a.nb11, xb, inv_scale, a.K, a.N, st); if (rc != GGML_B200_OK) return rc; }
+    if (!x_f16) { const int rc = tc_launch_x_to_f16(a.src1, a.nb11, xb, inv_scale, a.K, a.N, st); if (rc != GGML_B200_OK) return rc; }
     const size_t rb = T == T_F16 ? (size_t)a.K * 2 : row_bytes(a.type, a.K);
     alignas(64) CUtensorMap map_w, map_x;
     bool ok;
@@ -439,7 +450,9 @@ template <int T> static int launch_tc2(const ggml_b200_mul_mat_args & a, const t
         ok = encode_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a.src0, a.K, a.M, a.nb01, T2_BK, T2_BM, CU_TENSOR_MAP_SWIZZLE_128B, "W fp16");
     else
         ok = encode_2d(&map_w, CU_TENSOR_MAP_DATA_TYPE_UINT32, a.src0, rb / 4, a.M, rb, tc2fmt<T>::RAW / 4, T2_BM, CU_TENSOR_MAP_SWIZZLE_NONE, "W");
-    if (!ok || !encode_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, xb, a.K, a.N, a.K * 2, T2_BK, pl.BN, CU_TENSOR_MAP_SWIZZLE_128B, "X")) return GGML_B200_ECUDA;
+    if (ok) ok = x_f16 ? encode_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, x_f16, a.K, a.N, a.nb11, T2_BK, pl.BN, CU_TENSOR_MAP_SWIZZLE_128B, "X fp16")
+                       : encode_2d(&map_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, xb, a.K, a.N, a.K * 2, T2_BK, pl.BN, CU_TENSOR_MAP_SWIZZLE_128B, "X");
+    if (!ok) return GGML_B200_ECUDA;
     tc2_params p{};
     p.y = a.dst; p.partials = partials; p.flags = flags; p.inv_scale = inv_scale; p.M = a.M; p.N = a.N;
     p.BN = pl.BN; p.m_tiles = pl.m_tiles; p.n_tiles = pl.n_tiles; p.splitk = pl.splitk; p.units_total = pl.chunks; p.nstages = pl.nstages;
@@ -511,6 +524,21 @@ int launch_mmq_f16w(const void * w, size_t nb01, const float * x, size_t nb11, f
     if (!make_f16w_args(w, nb01, x, nb11, y, M, N, K, flags, b) || !plan_wgmma(b, pl)) { set_error("mul_mat_f16: shape not eligible for the tensor-core path"); return GGML_B200_EUNSUPPORTED; }
     b.workspace = ws; b.workspace_size = ws_size;
     return launch_tc2<T_F16>(b, pl, st);
+}
+
+// dense fp16 x fp16 (the conv mat-mul of ggml_conv_1d / _2d: A the IM2COL result, B the conv kernel), n >= 9, K % 64 == 0: both operands
+// by TMA, the workspace holds only the split-K partials.  Ordering: the producer's griddepcontrol.wait comes before its first TMA of
+// either tile (DENSE issues no load ahead of it), so a predecessor that wrote A or B (the IM2COL kernel) has completed before any read.
+size_t mmq_f16f16_workspace(int64_t M, int64_t N, int64_t K) {
+    ggml_b200_mul_mat_args b; tc2_plan pl;
+    make_f16w_args((const void *)(uintptr_t)256, (size_t)K * 2, (const float *)(uintptr_t)256, (size_t)K * 2, (float *)(uintptr_t)256, M, N, K, 0, b);
+    return plan_tc2(b, true, pl) ? pl.workspace : 0;
+}
+int launch_mmq_f16f16(const void * w, size_t nb01, const void * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K, void * ws, size_t ws_size, uint32_t flags, cudaStream_t st) {
+    ggml_b200_mul_mat_args b; tc2_plan pl;
+    if (!make_f16w_args(w, nb01, (const float *)x, nb11, y, M, N, K, flags, b) || !plan_tc2(b, true, pl)) { set_error("mul_mat_f16_f16: shape not eligible for the tensor-core path"); return GGML_B200_EUNSUPPORTED; }
+    b.workspace = ws; b.workspace_size = ws_size;
+    return launch_tc2<T_F16>(b, pl, st, x);
 }
 
 // ----------------------------------------------------------------------------- MUL_MAT_ID, expert-grouped (batched tokens)

@@ -8,7 +8,8 @@
 //   diag_mask :9745-9805  soft_max :9810-9925        gelu :6520-6570 (+ fp16 table, ggml-cpu.c:1355)   dup/cpy :3220-4300
 //   rope :9157-9640       argsort :10746-10783       sum_rows :5663-5694 (+ ggml_vec_sum_f32 :2118)
 //   concat :6097-6157     ssm_conv :11379-11445      ssm_scan :11449-11537
-//   rwkv_wkv6 :11865-12044                           gated_linear_attn :12067-12235
+//   rwkv_wkv6 :11865-12044                           gated_linear_attn :12067-12235   im2col :9875-10041
+// IM2COL is the first node of ggml_conv_1d / ggml_conv_2d (the convolutional front end of Whisper-style encoders).
 // ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation; CONCAT, SSM_CONV and SSM_SCAN are the
 // rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer; RWKV_WKV6 and GATED_LINEAR_ATTN are
 // the recurrences of the RWKV-6 time mix and of its gated (RWKV6-Qwen2) form.
@@ -16,6 +17,7 @@
 // sumrows.cu, concat.cu, wkv6.cu, gla.cu (the reference has no SSM kernels).
 #include "b200_internal.h"
 #include "b200_op_checks.h"
+#include "b200_conv.cuh"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
@@ -331,6 +333,9 @@ __global__ void __launch_bounds__(128) mul_mat_f_kernel(tdesc a, tdesc b, tdesc 
     float acc = 0.0f;
     if (a.type == T_F32) {
         for (int64_t k = lane; k < a.ne[0]; k += 32) acc += *(const float *)(ar + k * a.nb[0]) * *(const float *)(br + k * b.nb[0]);
+    } else if (b.type == T_F16) {                                // f16 x f16 (the conv mat-mul of ggml_conv_1d / _2d): src1 read as is
+        for (int64_t k = lane; k < a.ne[0]; k += 32)
+            acc += __half2float(*(const __half *)(ar + k * a.nb[0])) * __half2float(*(const __half *)(br + k * b.nb[0]));
     } else {
         for (int64_t k = lane; k < a.ne[0]; k += 32)
             acc += __half2float(*(const __half *)(ar + k * a.nb[0])) * __half2float(__float2half_rn(*(const float *)(br + k * b.nb[0])));
@@ -455,6 +460,16 @@ template <typename T> __global__ void __launch_bounds__(128) rope_kernel(tdesc s
         rope_rotate(x0, x1, cache[slot].x, cache[slot].y, y0, y1);
         rope_st<T>(dr + e0 * sizeof(T), y0); rope_st<T>(dr + e1 * sizeof(T), y1);
     }
+}
+
+// ------------------------------------------------------------------ IM2COL (f32 input -> f32 / f16 columns, dst packed)
+// One thread per dst element, in dst's order, so the stores coalesce; b200_conv.cuh locates the input element (or the padding) of each.
+template <typename T> __global__ void im2col_kernel(im2col_geom g, const uint8_t * __restrict__ src1, T * __restrict__ dst, int64_t n) {
+    pdl_trigger();
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const float v = im2col_value(g, src1, e);
+    if constexpr (sizeof(T) == 4) dst[e] = v; else dst[e] = __float2half_rn(v);
 }
 
 // ------------------------------------------------------------------ ARGSORT (f32 rows of ne0 <= 1024 -> i32 indices, dst contiguous)
@@ -778,6 +793,19 @@ int ggml_b200_op_rope(const ggml_b200_tensor * src, const ggml_b200_tensor * pos
     const dim3 grid((unsigned)s.ne[2], (unsigned)hb, (unsigned)s.ne[3]);
     if (s.type == T_F32) B200_CUDA_TRY(launch_pdl(rope_kernel<float>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
     else                 B200_CUDA_TRY(launch_pdl(rope_kernel<__half>, grid, dim3(128), 0, (cudaStream_t)stream, s, (const int32_t *)p.data, ff, d, c, heads_per_cta));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_im2col(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, const ggml_b200_im2col_params * params,
+                        void * stream) {
+    CHECK_ARGS(check_im2col(src0, src1, dst, params));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    const im2col_geom g = im2col_geometry(*src0, *src1, *dst, *params);
+    const uint8_t * x = (const uint8_t *)src1->data;
+    if (dst->type == T_F32) B200_CUDA_TRY(launch_pdl(im2col_kernel<float>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, x, (float *)dst->data, n));
+    else                    B200_CUDA_TRY(launch_pdl(im2col_kernel<__half>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, x, (__half *)dst->data, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

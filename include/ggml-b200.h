@@ -121,6 +121,13 @@ typedef struct ggml_b200_epilogue {
 GGML_B200_API size_t ggml_b200_mul_mat_f16_workspace_size(int64_t M, int64_t N, int64_t K);
 GGML_B200_API int    ggml_b200_mul_mat_f16(const void * w, size_t nb01, const float * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K,
                                            void * workspace, size_t workspace_size, uint32_t flags, void * stream);
+/* dense fp16 [M][K] (row stride nb01 bytes) x fp16 [N][K] (row stride nb11 bytes) -> f32 [N][M] on the tensor cores: both operands go
+   straight into the GEMM by TMA, with no conversion pass.  This is GGML_OP_MUL_MAT with f16 src0 and f16 src1, the product ggml_conv_1d /
+   ggml_conv_2d build (w: the IM2COL result, x: the conv kernel).  Eligible: N >= 9, K % 64 == 0, both row strides multiples of 16 bytes.
+   workspace_size = 0 from the size function: shape not eligible. */
+GGML_B200_API size_t ggml_b200_mul_mat_f16_f16_workspace_size(int64_t M, int64_t N, int64_t K);
+GGML_B200_API int    ggml_b200_mul_mat_f16_f16(const void * w, size_t nb01, const void * x, size_t nb11, float * y, int64_t M, int64_t N, int64_t K,
+                                               void * workspace, size_t workspace_size, uint32_t flags, void * stream);
 GGML_B200_API int    ggml_b200_mul_mat_fused(const ggml_b200_mul_mat_args * args, const ggml_b200_epilogue * epilogue, void * stream);
 
 /* MUL_MAT with HOST activations / results: copies src1 (host, contiguous [N][K]) to the device, runs
@@ -236,7 +243,8 @@ GGML_B200_API int ggml_b200_op_cpy2(const ggml_b200_tensor * src_a, const ggml_b
  * library decodes (quantized KV caches), mask f16 [n_kv, >= n_q] or NULL -> dst f32 [d, n_head, n_q, b]; d <= 256.  Replaces src/ggml-cuda/fattn*.cu. */
 GGML_B200_API int ggml_b200_op_flash_attn_ext(const ggml_b200_tensor * q, const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * mask,
                                               const ggml_b200_tensor * dst, float scale, float max_bias, float logit_softcap, void * stream);
-/* float mat-mul: src0 f32/f16 [K, M, ne02, ne03] (any strides) x src1 f32 [K, N, ne12, ne13] -> dst f32 */
+/* float mat-mul: src0 f32/f16 [K, M, ne02, ne03] (any strides) x src1 f32 [K, N, ne12, ne13] -> dst f32; src1 may also be f16 when src0
+ * is f16 (read as is: the CPU backend rounds an f32 src1 to f16 for an f16 src0, and takes an f16 src1 unchanged) */
 GGML_B200_API int ggml_b200_op_mul_mat_f(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream);
 /* GGML_OP_ROPE, forward (ggml_rope_ext / ggml_rope_multi): src f32 or f16 [ne0, n_head, n_pos, b] -> dst of the same type and shape (any row
  * strides, dim 0 contiguous; dst may be src itself).  pos i32 [n_pos] (MROPE / VISION: [4 * n_pos]) is read on the device.  freq_factors: NULL or
@@ -289,6 +297,20 @@ GGML_B200_API int ggml_b200_op_rwkv_wkv6(const ggml_b200_tensor * k, const ggml_
  * y[j] += temp (q[i] scale); state[i][j] = temp. */
 GGML_B200_API int ggml_b200_op_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * q, const ggml_b200_tensor * g,
                                                  const ggml_b200_tensor * s, const ggml_b200_tensor * dst, float scale, void * stream);
+/* GGML_OP_IM2COL (ggml_im2col; the first node of ggml_conv_1d / ggml_conv_2d): the op_params of the node, in their order */
+typedef struct ggml_b200_im2col_params {
+    int32_t s0, s1;        /* stride along the width / height, >= 1 (s1, p1, d1: 2-D only) */
+    int32_t p0, p1;        /* padding (zeros) */
+    int32_t d0, d1;        /* dilation, >= 1 */
+    int32_t is_2D;         /* 0: 1-D, 1: 2-D */
+} ggml_b200_im2col_params;
+/* src0: the conv kernel (only its extents are read: KW = ne0, 2-D KH = ne1), src1: the input f32 [IW, IC, N, 1] (1-D) or [IW, IH, IC, N] (2-D),
+ * contiguous along dim 0 -> dst f32 or f16, packed, [IC KW, OW, N, 1] (1-D) or [IC KH KW, OW, OH, N] (2-D), OW and OH the output sizes
+ * (in + 2 p - d (k - 1) - 1) / s + 1; an f16 dst needs an f16 src0, as the CPU backend asserts.  Bit-identical to the CPU backend in both dst
+ * types; a channel's rows are read as packed, as the CPU backend reads them.  src1 offsets of an image / a channel beyond INT32_MAX bytes:
+ * GGML_B200_EUNSUPPORTED (the CPU backend keeps them in an int). */
+GGML_B200_API int ggml_b200_op_im2col(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst,
+                                      const ggml_b200_im2col_params * params, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
