@@ -1,8 +1,9 @@
 // b200_op_checks.h — what each descriptor-taking op launcher of ops.cu accepts, decided in one place.  Every ggml_b200_op_* below returns
-// the verdict of its check before it launches anything, and the backend's supports_op asks the same check for each such node, so that a
-// node the plug-in accepts is one its launcher runs.  The checks read only the descriptors and the op's scalars: what the launcher cannot
-// see (graph structure, ggml-cpu's own layout assumptions) stays with the caller.  Conditions that matter only for a launch (the grid
-// limits) come after the empty-tensor early return, in the order the launchers have always applied them.
+// the verdict of its check before it launches anything, and the backend's supports_op asks the same check for each such node, on descriptors
+// built by the same code that builds the launch's (bound_op in backend/ggml-b200.cpp), so that a node the plug-in accepts is one its
+// launcher runs.  The checks read only the descriptors and the op's scalars: what the launcher cannot see (graph structure, ggml-cpu's
+// own layout assumptions) stays with the caller.  Conditions that matter only for a launch (the grid limits) come after the empty-tensor
+// early return, in the order the launchers have always applied them.
 //
 // Host-only C++: the ABI header and the standard library, no CUDA and no ggml headers, so the plug-in, the launchers and the CPU tests
 // compile the same rules.
