@@ -297,7 +297,7 @@ def tensor_desc(t) -> TensorDesc:
     import torch
     d = TensorDesc()
     d.data = t.data_ptr()
-    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26}[t.dtype]
+    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30}[t.dtype]
     shape = list(t.shape)[::-1] + [1] * (4 - t.dim())
     es = t.element_size()
     nb = es
@@ -485,7 +485,7 @@ def strided_desc(t) -> TensorDesc:
     import torch
     d = TensorDesc()
     d.data = t.data_ptr()
-    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26}[t.dtype]
+    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30}[t.dtype]
     es = t.element_size()
     shape, strides = list(t.shape)[::-1], list(t.stride())[::-1]
     for i in range(4):
@@ -621,4 +621,71 @@ def mul_mat_f16_f16(w, x, flags: int = 0, out=None):
     ws = _ws.get(need)
     check(L.ggml_b200_mul_mat_f16_f16(w.data_ptr(), w.stride(0) * 2, x.data_ptr(), x.stride(0) * 2, y.data_ptr(), M, N, K, ws.data_ptr(), ws.numel(),
                                       flags, _stream()), "ggml_b200_mul_mat_f16_f16")
+    return y
+
+
+class PoolParams(C.Structure):
+    """ggml_b200_pool_params (include/ggml-b200.h)"""
+    _fields_ = [("op", C.c_int32), ("k0", C.c_int32), ("k1", C.c_int32), ("s0", C.c_int32), ("s1", C.c_int32), ("p0", C.c_int32), ("p1", C.c_int32)]
+
+
+POOL_MAX, POOL_AVG = 0, 1
+
+
+def pool_out_size(ins: int, ks: int, s: int, p: float) -> int:
+    """the output extent of a pool along one axis as ggml_calc_pool_output_size computes it: in float, from the float padding"""
+    import numpy as np
+    f = np.float32
+    return int((f(ins) + f(2) * f(p) - f(ks)) / f(s) + f(1))
+
+
+def op_pool_2d(x, op: int, k0: int, k1: int, s0: int, s1: int, p0: float = 0.0, p1: float = 0.0):
+    """GGML_OP_POOL_2D (ggml_pool_2d): x f32 [N, C, IH, IW] (last dim contiguous, any other strides), op POOL_MAX or POOL_AVG, window k0 x k1
+    (width x height), stride s0 / s1, paddings p0 / p1 as ggml_pool_2d takes them (float: they size the output, and the kernel uses them
+    truncated, as ggml-cpu does) -> a new contiguous f32 tensor [N, C, OH, OW], bit-identical to ggml-cpu"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_pool_2d.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.POINTER(PoolParams), C.c_void_p]
+    oh, ow = pool_out_size(x.shape[-2], k1, s1, p1), pool_out_size(x.shape[-1], k0, s0, p0)
+    y = torch.empty(tuple(x.shape[:-2]) + (oh, ow), dtype=torch.float32, device=x.device)
+    p = PoolParams(int(op), k0, k1, s0, s1, int(p0), int(p1))
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_pool_2d(C.byref(s), C.byref(d), C.byref(p), _stream()), "ggml_b200_op_pool_2d")
+    return y
+
+
+def op_upscale(x, shape):
+    """GGML_OP_UPSCALE (nearest; ggml_upscale_ext): x f32 of rank <= 4, any strides -> a new contiguous f32 tensor of `shape` (same rank,
+    every extent >= x's; torch order), element i = x[i * x.shape / shape] per dim with ggml-cpu's float factors, bit-identical.
+    ggml_upscale(x, f) is shape = x.shape with the last two dims times f."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_upscale.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_void_p]
+    y = torch.empty(tuple(shape), dtype=torch.float32, device=x.device)
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_upscale(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_upscale")
+    return y
+
+
+def op_leaky_relu(x, slope: float, inplace: bool = False):
+    """GGML_OP_LEAKY_RELU of an f32 torch tensor (last dim contiguous, any other strides): ((x > 0) ? x : 0) + slope ((x < 0) ? x : 0),
+    bit-identical to ggml-cpu (NaN and -0 give +0).  inplace: the result is written into x."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_leaky_relu.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_float, C.c_void_p]
+    y = x if inplace else torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    s, d = strided_desc(x), strided_desc(y)
+    check(L.ggml_b200_op_leaky_relu(C.byref(s), C.byref(d), float(slope), _stream()), "ggml_b200_op_leaky_relu")
+    return y
+
+
+def op_repeat(x, shape):
+    """GGML_OP_REPEAT: x (float32, int32, float16, bfloat16 or int16; last dim contiguous, any other strides) tiled into a new contiguous
+    tensor of `shape` (torch order, each extent a whole multiple of x's), copied as raw words: every bit pattern is kept"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_repeat.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_void_p]
+    y = torch.empty(tuple(shape), dtype=x.dtype, device=x.device)
+    s, d = strided_desc(x), strided_desc(y)
+    check(L.ggml_b200_op_repeat(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_repeat")
     return y

@@ -311,6 +311,73 @@ inline op_check check_im2col(const ggml_b200_tensor * src0, const ggml_b200_tens
     return accepted;
 }
 
+// POOL_2D: src f32 [IW, IH, C, N] (elements packed along dim 0), dst f32 [OW, OH, C, N] packed; OW / OH are dst's (ggml_pool_2d derives them
+// from float paddings), so only C and N are compared with src
+inline op_check check_pool_2d(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, const ggml_b200_pool_params * params) {
+    B200_REQUIRE(src && dst && params, "src, dst and params are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    const ggml_b200_pool_params & p = *params;
+    B200_VALID(p.op == 0 || p.op == 1, "op must be 0 (MAX) or 1 (AVG): ggml-cpu aborts on POOL_COUNT");
+    B200_VALID(p.k0 >= 1 && p.k1 >= 1 && p.s0 >= 1 && p.s1 >= 1, "window and stride must be >= 1");
+    B200_REQUIRE(s.type == F32 && d.type == F32, "src and dst must be f32");
+    B200_REQUIRE(s.nb[0] == 4, "src must be contiguous along dim 0");
+    // ggml-cpu writes dst as if it were packed, whatever its strides
+    B200_REQUIRE(is_packed4(d), "dst must be packed");
+    B200_VALID(d.ne[2] == s.ne[2] && d.ne[3] == s.ne[3] && d.ne[0] >= 0 && d.ne[1] >= 0, "dst must be [OW, OH, C, N] of src's C and N");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
+// UPSCALE (nearest): src and dst f32, any strides; ggml_upscale_ext asserts dst extents >= src's
+inline op_check check_upscale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == F32 && d.type == F32, "src and dst must be f32");
+    if (nelem(d) == 0) return accepted;
+    B200_VALID(s.ne[0] >= 1 && s.ne[1] >= 1 && s.ne[2] >= 1 && s.ne[3] >= 1, "src must not be empty");
+    B200_VALID(d.ne[0] >= s.ne[0] && d.ne[1] >= s.ne[1] && d.ne[2] >= s.ne[2] && d.ne[3] >= s.ne[3], "dst extents must be >= src's");
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
+// LEAKY_RELU: src and dst f32 of one shape, elements packed along dim 0 (dst may be src: in place)
+inline op_check check_leaky_relu(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == F32 && d.type == F32, "src and dst must be f32");
+    B200_REQUIRE(s.nb[0] == 4 && d.nb[0] == 4, "src and dst must be contiguous along dim 0");
+    B200_VALID(same_shape(s, d), "src and dst shapes differ");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
+// the element size of a type REPEAT moves as raw words, 0 for any other: the types ggml-cpu repeats
+inline size_t repeat_elem_size(int32_t t) {
+    switch (t) {
+        case GGML_B200_TYPE_F32: case GGML_B200_TYPE_I32: return 4;
+        case GGML_B200_TYPE_F16: case GGML_B200_TYPE_BF16: case GGML_B200_TYPE_I16: return 2;
+        default: return 0;
+    }
+}
+
+// REPEAT: src and dst of one 4- or 2-byte type, both contiguous along dim 0 (ggml-cpu asserts so), dst a whole repeat of src
+inline op_check check_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    const size_t es = repeat_elem_size(s.type);
+    B200_REQUIRE(es && d.type == s.type, "src and dst must be one type of f32, i32, f16, bf16 or i16");
+    B200_REQUIRE(s.nb[0] == es && d.nb[0] == es, "src and dst must be contiguous along dim 0");
+    // ggml_can_repeat: an empty src repeats only into an empty dst
+    if (nelem(s) == 0) { B200_VALID(nelem(d) == 0, "an empty src repeats only into an empty dst"); return accepted; }
+    B200_VALID(d.ne[0] % s.ne[0] == 0 && d.ne[1] % s.ne[1] == 0 && d.ne[2] % s.ne[2] == 0 && d.ne[3] % s.ne[3] == 0,
+               "dst extents must be whole multiples of src's");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((nelem(d) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
 #undef B200_REQUIRE
 #undef B200_VALID
 

@@ -608,6 +608,32 @@ int bound_op(const ggml_tensor * node, bool launch, void * stream) {
             const ggml_b200_im2col_params p = im2col_params(node);
             return launch ? ggml_b200_op_im2col(&k, &x, &d, &p, stream) : b200::check_im2col(&k, &x, &d, &p).code;
         }
+        case GGML_OP_POOL_2D: {                            // GGML_OP_POOL_2D_BACK (training) stays declined
+            // ggml-cpu steps from plane to plane by nb2 until ggml_nbytes(src) is used up (ggml-cpu.c:10336-10375): it reads the planes
+            // the descriptors name only when they are evenly spaced and a plane's rows end within nb2
+            if (!launch && ggml_nelements(a) > 0 && ((a->ne[3] > 1 && a->nb[3] != a->ne[2] * a->nb[2]) ||
+                                                     (a->ne[1] - 1) * (int64_t) a->nb[1] + a->ne[0] * (int64_t) sizeof(float) > (int64_t) a->nb[2]))
+                return GGML_B200_EUNSUPPORTED;
+            const int32_t * ip = (const int32_t *) node->op_params;
+            const ggml_b200_pool_params p = { ip[0], ip[1], ip[2], ip[3], ip[4], ip[5], ip[6] };
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_pool_2d(&x, &d, &p, stream) : b200::check_pool_2d(&x, &d, &p).code;
+        }
+        case GGML_OP_UPSCALE: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_upscale(&x, &d, stream) : b200::check_upscale(&x, &d).code;
+        }
+        case GGML_OP_LEAKY_RELU: {
+            // ggml-cpu walks nrows rows at i*nb1 (ggml-cpu.c:6712-6716): only evenly spaced rows mean the same data on both backends
+            if (!launch && (a->nb[2] != a->ne[1] * a->nb[1] || a->nb[3] != a->ne[2] * a->nb[2] ||
+                            node->nb[2] != node->ne[1] * node->nb[1] || node->nb[3] != node->ne[2] * node->nb[2])) return GGML_B200_EUNSUPPORTED;
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_leaky_relu(&x, &d, ggml_get_op_params_f32(node, 0), stream) : b200::check_leaky_relu(&x, &d).code;
+        }
+        case GGML_OP_REPEAT: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_repeat(&x, &d, stream) : b200::check_repeat(&x, &d).code;
+        }
         case GGML_OP_SSM_SCAN: {
             // sources: s, x, dt, A, B, C (ggml_ssm_scan); dst = y, then the final states
             ggml_b200_tensor t[6];

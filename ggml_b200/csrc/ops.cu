@@ -9,7 +9,9 @@
 //   rope :9157-9640       argsort :10746-10783       sum_rows :5663-5694 (+ ggml_vec_sum_f32 :2118)
 //   concat :6097-6157     ssm_conv :11379-11445      ssm_scan :11449-11537
 //   rwkv_wkv6 :11865-12044                           gated_linear_attn :12067-12235   im2col :9875-10041
-// IM2COL is the first node of ggml_conv_1d / ggml_conv_2d (the convolutional front end of Whisper-style encoders).
+//   pool_2d :10305-10377  upscale :10503-10540       leaky_relu :6689-6717            repeat :5901-6015
+// IM2COL is the first node of ggml_conv_1d / ggml_conv_2d (the convolutional front end of Whisper-style encoders); POOL_2D, UPSCALE,
+// LEAKY_RELU and REPEAT (the batch norm's per-channel vectors) are the ops around the convs of YOLO-style networks.
 // ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation; CONCAT, SSM_CONV and SSM_SCAN are the
 // rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer; RWKV_WKV6 and GATED_LINEAR_ATTN are
 // the recurrences of the RWKV-6 time mix and of its gated (RWKV6-Qwen2) form.
@@ -18,6 +20,7 @@
 #include "b200_internal.h"
 #include "b200_op_checks.h"
 #include "b200_conv.cuh"
+#include "b200_pool.cuh"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
@@ -472,6 +475,44 @@ template <typename T> __global__ void im2col_kernel(im2col_geom g, const uint8_t
     if constexpr (sizeof(T) == 4) dst[e] = v; else dst[e] = __float2half_rn(v);
 }
 
+// ------------------------------------------------------------------ POOL_2D, UPSCALE, LEAKY_RELU, REPEAT (around the convs of YOLO-style nets)
+// One thread per dst element, in dst's order, so the stores coalesce; b200_pool.cuh holds each element's logic.
+__global__ void pool2d_kernel(pool2d_geom g, const uint8_t * __restrict__ src, float * __restrict__ dst, int64_t n) {
+    pdl_trigger();
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    dst[e] = pool2d_value(g, src, e);
+}
+
+__global__ void upscale_kernel(upscale_geom g, const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int64_t n) {
+    pdl_trigger();
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    int64_t dofs;
+    const int64_t sofs = upscale_offsets(g, e, dofs);
+    *(float *)(dst + dofs) = *(const float *)(src + sofs);
+}
+
+// in place when dst is src: each thread reads its element before it writes it
+__global__ void leaky_relu_kernel(tdesc s, tdesc d, float slope, int64_t n) {
+    pdl_trigger();
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const int64_t i0 = e % d.ne[0], i1 = (e / d.ne[0]) % d.ne[1], i2 = (e / (d.ne[0] * d.ne[1])) % d.ne[2], i3 = e / (d.ne[0] * d.ne[1] * d.ne[2]);
+    const float x = *(const float *)(s.data + i0 * 4 + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
+    *(float *)(d.data + i0 * 4 + i1 * d.nb[1] + i2 * d.nb[2] + i3 * d.nb[3]) = leaky_relu_value(x, slope);
+}
+
+// W: the element as a raw word (uint32_t: f32 / i32, uint16_t: f16 / bf16 / i16), never converted
+template <typename W> __global__ void repeat_kernel(repeat_geom g, const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int64_t n) {
+    pdl_trigger();
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    int64_t dofs;
+    const int64_t sofs = repeat_offsets(g, e, dofs);
+    *(W *)(dst + dofs) = *(const W *)(src + sofs);
+}
+
 // ------------------------------------------------------------------ ARGSORT (f32 rows of ne0 <= 1024 -> i32 indices, dst contiguous)
 // One CTA per row: the row's (key, index) items (b200_sort.cuh), padded to P = the next power of two, are sorted by the bitonic network in
 // shared memory, one compare-exchange per thread and step.  The order is a strict total order (ties by index, NaNs last), so each output
@@ -806,6 +847,49 @@ int ggml_b200_op_im2col(const ggml_b200_tensor * src0, const ggml_b200_tensor * 
     const uint8_t * x = (const uint8_t *)src1->data;
     if (dst->type == T_F32) B200_CUDA_TRY(launch_pdl(im2col_kernel<float>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, x, (float *)dst->data, n));
     else                    B200_CUDA_TRY(launch_pdl(im2col_kernel<__half>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, x, (__half *)dst->data, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_pool_2d(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, const ggml_b200_pool_params * params, void * stream) {
+    CHECK_ARGS(check_pool_2d(src, dst, params));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    const pool2d_geom g = pool2d_geometry(*src, *dst, *params);
+    B200_CUDA_TRY(launch_pdl(pool2d_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, (const uint8_t *)src->data, (float *)dst->data, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_upscale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_upscale(src, dst));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    const upscale_geom g = upscale_geometry(*src, *dst);
+    B200_CUDA_TRY(launch_pdl(upscale_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, (const uint8_t *)src->data, (uint8_t *)dst->data, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_leaky_relu(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, float slope, void * stream) {
+    CHECK_ARGS(check_leaky_relu(src, dst));
+    const tdesc s = T(src), d = T(dst);
+    const int64_t n = nelem(d);
+    if (n == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(leaky_relu_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, s, d, slope, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_repeat(src, dst));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    const repeat_geom g = repeat_geometry(*src, *dst);
+    const uint8_t * s = (const uint8_t *)src->data;
+    uint8_t * d = (uint8_t *)dst->data;
+    if (repeat_elem_size(src->type) == 4) B200_CUDA_TRY(launch_pdl(repeat_kernel<uint32_t>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, s, d, n));
+    else                                  B200_CUDA_TRY(launch_pdl(repeat_kernel<uint16_t>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, s, d, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

@@ -60,6 +60,8 @@ enum ggml_b200_type {
     GGML_B200_TYPE_IQ2_XS = 17, GGML_B200_TYPE_IQ3_S = 21, GGML_B200_TYPE_IQ2_S = 22, GGML_B200_TYPE_IQ1_M = 29, GGML_B200_TYPE_TQ1_0 = 34, GGML_B200_TYPE_TQ2_0 = 35,
     /* indices and positions of the small ops (ggml_b200_tensor) */
     GGML_B200_TYPE_I32 = 26,
+    /* the 2-byte element types GGML_OP_REPEAT moves besides f16 */
+    GGML_B200_TYPE_I16 = 25, GGML_B200_TYPE_BF16 = 30,
 };
 
 /* ---------------------------------------------------------------------------------------------
@@ -311,6 +313,31 @@ typedef struct ggml_b200_im2col_params {
  * GGML_B200_EUNSUPPORTED (the CPU backend keeps them in an int). */
 GGML_B200_API int ggml_b200_op_im2col(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst,
                                       const ggml_b200_im2col_params * params, void * stream);
+/* GGML_OP_POOL_2D (ggml_pool_2d): the op_params of the node, in their order */
+typedef struct ggml_b200_pool_params {
+    int32_t op;            /* 0 MAX, 1 AVG (2, COUNT: GGML_B200_EINVAL, as the CPU backend aborts on it) */
+    int32_t k0, k1;        /* window width / height, >= 1 */
+    int32_t s0, s1;        /* stride, >= 1 */
+    int32_t p0, p1;        /* padding, as stored in op_params: ggml_pool_2d's float paddings truncated */
+} ggml_b200_pool_params;
+/* src f32 [IW, IH, C, N] (elements packed along dim 0, any row / channel / image strides) -> dst f32 [OW, OH, C, N], packed.  OW and OH are
+ * dst's own extents: ggml_pool_2d computes them from its float paddings, so they are never re-derived here.  Window (ox, oy) starts at
+ * (ox s0 - p0, oy s1 - p1); taps outside the input are skipped.  MAX starts at -FLT_MAX and takes a tap only when it is greater (NaN taps are
+ * ignored, a window of padding or NaN gives -FLT_MAX); AVG sums the in-range taps in row order and divides by k0 k1.  Bit-identical to the
+ * CPU backend.  dst C or N different from src's: GGML_B200_EINVAL. */
+GGML_B200_API int ggml_b200_op_pool_2d(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, const ggml_b200_pool_params * params, void * stream);
+/* GGML_OP_UPSCALE (nearest; ggml_upscale / ggml_upscale_ext): src f32 (any strides) -> dst f32 (any strides), dst extents >= src's (else
+ * GGML_B200_EINVAL).  dst (i0, i1, i2, i3) = src (i0 / sf0, ...) truncated, sf_i = (float) dst ne_i / src ne_i, computed here from the two
+ * descriptors in float as the CPU backend computes them: bit-identical. */
+GGML_B200_API int ggml_b200_op_upscale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_LEAKY_RELU: src and dst f32 of the same shape (else GGML_B200_EINVAL), both contiguous along dim 0, any other strides; dst may be
+ * src itself (in place).  dst = ((x > 0) ? x : 0) + slope ((x < 0) ? x : 0), each step rounded as the CPU backend rounds it: NaN and -0 give
+ * +0.  Bit-identical. */
+GGML_B200_API int ggml_b200_op_leaky_relu(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, float slope, void * stream);
+/* GGML_OP_REPEAT: src and dst of one type with 4-byte (f32, i32) or 2-byte (f16, bf16, i16) elements, both contiguous along dim 0, any other
+ * strides; every dst extent a whole multiple of src's (else GGML_B200_EINVAL).  dst (i0, i1, i2, i3) = src (i0 % ne00, i1 % ne01, ...), moved
+ * as raw words: every bit pattern (NaN payloads included) is kept. */
+GGML_B200_API int ggml_b200_op_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
