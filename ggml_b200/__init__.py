@@ -324,6 +324,9 @@ def mul_mat_fused(t, W, X, M, K, bias, gelu: bool, residual=None):
     return Y.view(-1), Y2, Y3
 
 
+UNARY_SIN, UNARY_COS = 11, 12                  # GGML_B200_UNARY_SIN / _COS (GGML_OP_SIN / GGML_OP_COS): sinf / cosf
+
+
 def op_unary(uop: int, x):
     import torch
     L = lib()
@@ -688,4 +691,71 @@ def op_repeat(x, shape):
     y = torch.empty(tuple(shape), dtype=x.dtype, device=x.device)
     s, d = strided_desc(x), strided_desc(y)
     check(L.ggml_b200_op_repeat(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_repeat")
+    return y
+
+
+def op_win_part(x, w: int):
+    """GGML_OP_WIN_PART (ggml_win_part): x f32 [H0, W0, C] (packed; torch order of ggml's [C, W0, H0]) -> a new f32 tensor
+    [npx npy, w, w, C], window py npx + px holding pixels (px w + i1, py w + i2), zeros past the image; raw words, bit-identical to ggml-cpu"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_win_part.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_int32] * 3 + [C.c_void_p]
+    h0, w0, c = x.shape[-3:]
+    npx, npy = -(-w0 // w), -(-h0 // w)
+    y = torch.empty((npx * npy, w, w, c), dtype=torch.float32, device=x.device)
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_win_part(C.byref(s), C.byref(d), npx, npy, w, _stream()), "ggml_b200_op_win_part")
+    return y
+
+
+def op_win_unpart(x, w0: int, h0: int, w: int):
+    """GGML_OP_WIN_UNPART (ggml_win_unpart): x f32 [np, w, w, C] (packed, np >= ceil(w0 / w) ceil(h0 / w)) -> a new f32 tensor [h0, w0, C],
+    the inverse of op_win_part without its padding; raw words, bit-identical to ggml-cpu"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_win_unpart.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_int32, C.c_void_p]
+    y = torch.empty((h0, w0, x.shape[-1]), dtype=torch.float32, device=x.device)
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_win_unpart(C.byref(s), C.byref(d), w, _stream()), "ggml_b200_op_win_unpart")
+    return y
+
+
+def op_get_rel_pos(x):
+    """GGML_OP_GET_REL_POS (ggml_get_rel_pos): x f16 [2w - 1, C] (packed) -> a new f16 tensor [w, w, C], y[i2, i1] = x[(w - 1 - i1) + i2];
+    raw 2-byte words, bit-identical to ggml-cpu"""
+    import torch
+    L = lib()
+    L.ggml_b200_op_get_rel_pos.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_void_p]
+    w = (x.shape[-2] + 1) // 2
+    y = torch.empty((w, w, x.shape[-1]), dtype=x.dtype, device=x.device)
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_get_rel_pos(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_get_rel_pos")
+    return y
+
+
+def op_add_rel_pos(a, pw, ph, inplace: bool = False):
+    """GGML_OP_ADD_REL_POS (ggml_add_rel_pos[_inplace]): a f32 [P, A B, L L], pw and ph f32 [P, B, A, L] (all packed) ->
+    a[p, q, kh L + kw] + ph[p, q, kh] + pw[p, q, kw] with ggml-cpu's order of the two adds (ph first when kh <= kw): bit-identical.
+    inplace: the result is written into a."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_add_rel_pos.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.c_void_p]
+    y = a if inplace else torch.empty(a.shape, dtype=torch.float32, device=a.device)
+    s, w, h, d = strided_desc(a), strided_desc(pw), strided_desc(ph), strided_desc(y)
+    check(L.ggml_b200_op_add_rel_pos(C.byref(s), C.byref(w), C.byref(h), C.byref(d), _stream()), "ggml_b200_op_add_rel_pos")
+    return y
+
+
+def op_conv_transpose_2d(kernel, x, stride: int):
+    """GGML_OP_CONV_TRANSPOSE_2D (ggml_conv_transpose_2d_p0): kernel f16 [Cin, Cout, Kh, Kw] (packed Kh x Kw planes), x f32 [Cin, H, W] or
+    [1, Cin, H, W] (last dim contiguous) -> a new f32 tensor [(1,) Cout, (H-1) s + Kh, (W-1) s + Kw], padding 0.  x is rounded to fp16 as
+    ggml-cpu rounds it; each tap's dot over Cin is summed in f32 and the taps are added in ggml-cpu's order."""
+    import torch
+    L = lib()
+    L.ggml_b200_op_conv_transpose_2d.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_int32, C.c_void_p]
+    cout, kh, kw = kernel.shape[1:]
+    h, w = x.shape[-2:]
+    y = torch.empty(tuple(x.shape[:-3]) + (cout, (h - 1) * stride + kh, (w - 1) * stride + kw), dtype=torch.float32, device=x.device)
+    k, s, d = strided_desc(kernel), strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_conv_transpose_2d(C.byref(k), C.byref(s), C.byref(d), stride, _stream()), "ggml_b200_op_conv_transpose_2d")
     return y

@@ -378,6 +378,96 @@ inline op_check check_repeat(const ggml_b200_tensor * src, const ggml_b200_tenso
     return accepted;
 }
 
+// WIN_PART / WIN_UNPART / GET_REL_POS / ADD_REL_POS (b200_sam.cuh): one CTA row of threads per row of ne0 elements, rows on grid x (32-bit
+// row indices), blocks of a row on grid y
+inline bool rows_fit_grid(int64_t rows, int64_t row_len) { return rows <= 0x7fffffff && (row_len + 255) / 256 <= 65535; }
+inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// WIN_PART: src f32 [C, W0, H0, 1] -> dst f32 [C, w, w, npx npy], both packed (ggml-cpu indexes them as packed); op_params npx, npy, w as
+// ggml_win_part derives them
+inline op_check check_win_part(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t npx, int32_t npy, int32_t w) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == GGML_B200_TYPE_F32 && d.type == GGML_B200_TYPE_F32, "src and dst must be f32");
+    B200_REQUIRE(is_packed4(s) && is_packed4(d), "src and dst must be packed");
+    B200_VALID(w >= 1, "the window must be >= 1");
+    B200_VALID(s.ne[3] == 1, "src must be one image [C, W0, H0, 1]");
+    B200_VALID(npx == ceil_div(s.ne[1], w) && npy == ceil_div(s.ne[2], w), "npx / npy must be ceil(W0 / w) / ceil(H0 / w)");
+    B200_VALID(d.ne[0] == s.ne[0] && d.ne[1] == w && d.ne[2] == w && d.ne[3] == (int64_t)npx * npy, "dst must be [C, w, w, npx npy]");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE(rows_fit_grid(nrows(d), d.ne[0]) && s.ne[1] * s.ne[2] <= 0x7fffffff, "too many rows for one grid");
+    return accepted;
+}
+
+// WIN_UNPART: src f32 [C, w, w, np] -> dst f32 [C, W0, H0, 1], both packed; np must hold every window of the image, or the reads leave src
+inline op_check check_win_unpart(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t w) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == GGML_B200_TYPE_F32 && d.type == GGML_B200_TYPE_F32, "src and dst must be f32");
+    B200_REQUIRE(is_packed4(s) && is_packed4(d), "src and dst must be packed");
+    B200_VALID(w >= 1, "the window must be >= 1");
+    B200_VALID(d.ne[0] == s.ne[0] && d.ne[3] == 1 && s.ne[1] == w && s.ne[2] == w, "src must be [C, w, w, np] and dst [C, W0, H0, 1]");
+    B200_VALID(s.ne[3] >= ceil_div(d.ne[1], w) * ceil_div(d.ne[2], w), "src must hold ceil(W0 / w) ceil(H0 / w) windows");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE(rows_fit_grid(nrows(d), d.ne[0]) && nrows(s) <= 0x7fffffff, "too many rows for one grid");
+    return accepted;
+}
+
+// GET_REL_POS: src f16 [C, 2w - 1] -> dst f16 [C, w, w], both packed (ggml-cpu reads src row p at p ne0).  ggml-cpu also runs a BF16 src
+// into its F16 dst as raw bits; nothing builds that, and it is declined.
+inline op_check check_get_rel_pos(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == GGML_B200_TYPE_F16 && d.type == GGML_B200_TYPE_F16, "src and dst must be f16");
+    B200_REQUIRE(is_packed(s, 2) && is_packed(d, 2), "src and dst must be packed");
+    const int64_t w = d.ne[1];
+    B200_VALID(w >= 1 && d.ne[2] == w && d.ne[3] == 1 && d.ne[0] == s.ne[0] && s.ne[1] == 2 * w - 1 && s.ne[2] == 1 && s.ne[3] == 1,
+               "src must be [C, 2w - 1] and dst [C, w, w]");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE(rows_fit_grid(nrows(d), d.ne[0]), "too many rows for one grid");
+    return accepted;
+}
+
+// ADD_REL_POS: src0 and dst f32 [L L, A B, P, 1], pw = src1 and ph = src2 f32 [L, A, B, P], all packed (ggml_add_rel_pos asserts it, and
+// ggml-cpu indexes them so); dst may be src0 (in place).  ggml-cpu touches only the first slice of a src0 with ne3 > 1: declined.
+inline op_check check_add_rel_pos(const ggml_b200_tensor * src0, const ggml_b200_tensor * pw, const ggml_b200_tensor * ph, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src0 && pw && ph && dst, "src0, pw, ph and dst are required");
+    const ggml_b200_tensor & a = *src0, & w = *pw, & h = *ph, & d = *dst;
+    B200_REQUIRE(a.type == GGML_B200_TYPE_F32 && w.type == GGML_B200_TYPE_F32 && h.type == GGML_B200_TYPE_F32 && d.type == GGML_B200_TYPE_F32,
+                 "src0, pw, ph and dst must be f32");
+    B200_REQUIRE(is_packed4(a) && is_packed4(w) && is_packed4(h) && is_packed4(d), "src0, pw, ph and dst must be packed");
+    B200_REQUIRE(a.ne[3] == 1, "src0 must have ne3 == 1 (ggml-cpu adds to its first slice only)");
+    B200_VALID(same_shape(w, h) && same_shape(a, d), "pw and ph, src0 and dst must have one shape each");
+    const int64_t L = w.ne[0];
+    B200_VALID(a.ne[0] == L * L && a.ne[1] == w.ne[1] * w.ne[2] && a.ne[2] == w.ne[3], "src0 must be [L L, A B, P] of pw's [L, A, B, P]");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE(rows_fit_grid(nrows(d), d.ne[0]), "too many rows for one grid");
+    return accepted;
+}
+
+// CONV_TRANSPOSE_2D (ggml_conv_transpose_2d_p0): kernel f16 [Kw, Kh, Cout, Cin] with packed Kw x Kh planes, input f32 [W, H, Cin, 1]
+// contiguous along dim 0, dst f32 [(W-1) s + Kw, (H-1) s + Kh, Cout, 1] packed: the layouts ggml-cpu reads.  ggml-cpu computes only the
+// first image of a batch (and leaves the rest zero): ne3 > 1 is declined.
+inline op_check check_conv_transpose_2d(const ggml_b200_tensor * kernel, const ggml_b200_tensor * input, const ggml_b200_tensor * dst, int32_t stride) {
+    B200_REQUIRE(kernel && input && dst, "kernel, input and dst are required");
+    const ggml_b200_tensor & k = *kernel, & x = *input, & d = *dst;
+    B200_REQUIRE(k.type == GGML_B200_TYPE_F16 && x.type == GGML_B200_TYPE_F32 && d.type == GGML_B200_TYPE_F32, "kernel f16, input and dst f32");
+    B200_REQUIRE(k.nb[0] == 2 && k.nb[1] == (size_t)(2 * k.ne[0]), "the kernel's Kw x Kh planes must be packed");
+    B200_REQUIRE(x.nb[0] == 4, "input must be contiguous along dim 0");
+    B200_REQUIRE(is_packed4(d), "dst must be packed");
+    B200_REQUIRE(x.ne[3] == 1 && d.ne[3] == 1, "one image only (ggml-cpu computes the first image of a batch)");
+    B200_VALID(stride >= 1, "stride must be >= 1");
+    B200_VALID(k.ne[3] == x.ne[2] && d.ne[2] == k.ne[2], "kernel must be [Kw, Kh, Cout, Cin] of input's Cin and dst's Cout");
+    B200_VALID(d.ne[0] == (x.ne[0] - 1) * stride + k.ne[0] && d.ne[1] == (x.ne[1] - 1) * stride + k.ne[1],
+               "dst must be [(W-1) s + Kw, (H-1) s + Kh, Cout]");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE(stride <= 255, "stride must be <= 255 (one grid z per stride phase)");
+    B200_REQUIRE(d.ne[0] <= 0x7fffffff && d.ne[1] <= 0x7fffffff && k.ne[2] <= 0x7fffffff && k.ne[3] <= 0x7fffffff, "extents must fit 32 bits");
+    B200_REQUIRE(ceil_div(ceil_div(d.ne[0], stride), 32) * ceil_div(ceil_div(d.ne[1], stride), 2) <= 0x7fffffff && ceil_div(k.ne[2], 32) <= 65535,
+                 "too many tiles for one grid");
+    return accepted;
+}
+
 #undef B200_REQUIRE
 #undef B200_VALID
 

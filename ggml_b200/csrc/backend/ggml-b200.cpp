@@ -634,6 +634,33 @@ int bound_op(const ggml_tensor * node, bool launch, void * stream) {
             const auto x = desc(a), d = desc(node);
             return launch ? ggml_b200_op_repeat(&x, &d, stream) : b200::check_repeat(&x, &d).code;
         }
+        // the ops of SAM-style image encoders and mask decoders; ggml-cpu indexes all their operands as packed, and the checks require it
+        case GGML_OP_WIN_PART: {
+            const int32_t * ip = (const int32_t *) node->op_params;            // npx, npy, w (ggml_win_part)
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_win_part(&x, &d, ip[0], ip[1], ip[2], stream) : b200::check_win_part(&x, &d, ip[0], ip[1], ip[2]).code;
+        }
+        case GGML_OP_WIN_UNPART: {
+            const int32_t w = ggml_get_op_params_i32(node, 0);
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_win_unpart(&x, &d, w, stream) : b200::check_win_unpart(&x, &d, w).code;
+        }
+        case GGML_OP_GET_REL_POS: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_get_rel_pos(&x, &d, stream) : b200::check_get_rel_pos(&x, &d).code;
+        }
+        case GGML_OP_ADD_REL_POS: {                        // sources: a, pw, ph; in place (op_params[0]) dst is a view of a
+            const ggml_tensor * ph = node->src[2];
+            if (!launch && (!b || !ph)) return GGML_B200_EUNSUPPORTED;
+            const auto x = desc(a), w = desc(b), h = desc(ph), d = desc(node);
+            return launch ? ggml_b200_op_add_rel_pos(&x, &w, &h, &d, stream) : b200::check_add_rel_pos(&x, &w, &h, &d).code;
+        }
+        case GGML_OP_CONV_TRANSPOSE_2D: {                  // sources: the kernel, the input; op_params[0] = stride
+            if (!launch && !b) return GGML_B200_EUNSUPPORTED;
+            const int32_t s = ggml_get_op_params_i32(node, 0);
+            const auto k = desc(a), x = desc(b), d = desc(node);
+            return launch ? ggml_b200_op_conv_transpose_2d(&k, &x, &d, s, stream) : b200::check_conv_transpose_2d(&k, &x, &d, s).code;
+        }
         case GGML_OP_SSM_SCAN: {
             // sources: s, x, dt, A, B, C (ggml_ssm_scan); dst = y, then the final states
             ggml_b200_tensor t[6];
@@ -667,9 +694,11 @@ int bound_op(const ggml_tensor * node, bool launch, void * stream) {
             if (!launch) return verdict(is_f32_contig(a) && is_f32_contig(node) && (!b || ((b->type == GGML_TYPE_F32 || b->type == GGML_TYPE_F16) && ggml_is_contiguous(b))));
             return ggml_b200_op_soft_max((const float *) a->data, b ? b->data : nullptr, b ? (int32_t) b->type : 0, (float *) node->data,
                                          node->ne[0], node->ne[1], node->ne[2], node->ne[3], ggml_get_op_params_f32(node, 0), ggml_get_op_params_f32(node, 1), stream);
-        // SQR and SQRT: x * x and sqrtf, correctly rounded on both backends: bit-identical to ggml-cpu
-        case GGML_OP_UNARY: case GGML_OP_SQR: case GGML_OP_SQRT: {
-            const int u = node->op == GGML_OP_SQR ? GGML_B200_UNARY_SQR : node->op == GGML_OP_SQRT ? GGML_B200_UNARY_SQRT : unary_code(node);
+        // SQR and SQRT: x * x and sqrtf, correctly rounded on both backends: bit-identical to ggml-cpu.  SIN and COS: the device's sinf / cosf
+        // (within 2 ulp), not bit-identical to glibc's
+        case GGML_OP_UNARY: case GGML_OP_SQR: case GGML_OP_SQRT: case GGML_OP_SIN: case GGML_OP_COS: {
+            const int u = node->op == GGML_OP_SQR ? GGML_B200_UNARY_SQR : node->op == GGML_OP_SQRT ? GGML_B200_UNARY_SQRT
+                        : node->op == GGML_OP_SIN ? GGML_B200_UNARY_SIN : node->op == GGML_OP_COS ? GGML_B200_UNARY_COS : unary_code(node);
             if (!launch) return verdict(u >= 0 && is_f32_contig(a) && is_f32_contig(node));
             return ggml_b200_op_unary(u, (const float *) a->data, (float *) node->data, ggml_nelements(node), stream);
         }

@@ -10,8 +10,12 @@
 //   concat :6097-6157     ssm_conv :11379-11445      ssm_scan :11449-11537
 //   rwkv_wkv6 :11865-12044                           gated_linear_attn :12067-12235   im2col :9875-10041
 //   pool_2d :10305-10377  upscale :10503-10540       leaky_relu :6689-6717            repeat :5901-6015
+//   win_part :11541-11582 win_unpart :11604-11640    get_rel_pos :11737-11760         add_rel_pos :11784-11842
+//   conv_transpose_2d :10140-10230                   sin / cos :1733-1734
 // IM2COL is the first node of ggml_conv_1d / ggml_conv_2d (the convolutional front end of Whisper-style encoders); POOL_2D, UPSCALE,
-// LEAKY_RELU and REPEAT (the batch norm's per-channel vectors) are the ops around the convs of YOLO-style networks.
+// LEAKY_RELU and REPEAT (the batch norm's per-channel vectors) are the ops around the convs of YOLO-style networks.  WIN_PART / WIN_UNPART
+// (windowed attention), GET_REL_POS / ADD_REL_POS (the decomposed relative-position bias), CONV_TRANSPOSE_2D (the mask decoder's output
+// upscaling) and SIN / COS (the random-Fourier positional encoding) are the ops of Segment-Anything-style image encoders and mask decoders.
 // ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation; CONCAT, SSM_CONV and SSM_SCAN are the
 // rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer; RWKV_WKV6 and GATED_LINEAR_ATTN are
 // the recurrences of the RWKV-6 time mix and of its gated (RWKV6-Qwen2) form.
@@ -21,6 +25,7 @@
 #include "b200_op_checks.h"
 #include "b200_conv.cuh"
 #include "b200_pool.cuh"
+#include "b200_sam.cuh"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
@@ -220,7 +225,8 @@ __global__ void diag_mask_inf_kernel(const float * x, float * y, int64_t ne0, in
     const int64_t c = i % ne0, r = (i / ne0) % ne1;
     y[i] = c > n_past + r ? -INFINITY : x[i];
 }
-enum { U_GELU = 0, U_SILU = 1, U_RELU = 2, U_TANH = 3, U_NEG = 4, U_ABS = 5, U_GELU_QUICK = 6, U_SIGMOID = 7, U_EXP = 8, U_SQR = 9, U_SQRT = 10 };
+enum { U_GELU = 0, U_SILU = 1, U_RELU = 2, U_TANH = 3, U_NEG = 4, U_ABS = 5, U_GELU_QUICK = 6, U_SIGMOID = 7, U_EXP = 8, U_SQR = 9, U_SQRT = 10,
+       U_SIN = 11, U_COS = 12 };
 __global__ void unary_kernel(int uop, const float * x, float * y, int64_t n) {
     pdl_trigger();
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -238,7 +244,10 @@ __global__ void unary_kernel(int uop, const float * x, float * y, int64_t n) {
         case U_SIGMOID: r = 1.0f / (1.0f + expf(-v)); break;
         case U_EXP: r = expf(v); break;
         case U_SQR: r = v * v; break;
-        default: r = sqrtf(v); break;
+        case U_SQRT: r = sqrtf(v); break;
+        // the library sinf / cosf (within 2 ulp everywhere), never the __sinf / __cosf intrinsics
+        case U_SIN: r = sinf(v); break;
+        default: r = cosf(v); break;
     }
     y[i] = r;
 }
@@ -513,6 +522,120 @@ template <typename W> __global__ void repeat_kernel(repeat_geom g, const uint8_t
     *(W *)(dst + dofs) = *(const W *)(src + sofs);
 }
 
+// ------------------------------------------------------------------ WIN_PART, WIN_UNPART, GET_REL_POS, ADD_REL_POS (SAM-style image encoders)
+// One row of threads per dst row of ne0 words: the row on grid x, blocks of the row on grid y.  The row's source is decided once per thread
+// in 32-bit arithmetic (b200_sam.cuh), and loads and stores coalesce along dim 0.  The data ops move raw words.
+__global__ void win_part_kernel(win_geom g, const uint32_t * __restrict__ src, uint32_t * __restrict__ dst, int64_t ne0) {
+    pdl_trigger();
+    const int64_t i0 = (int64_t)blockIdx.y * blockDim.x + threadIdx.x;
+    if (i0 >= ne0) return;
+    const int32_t sr = win_part_src_row(g, blockIdx.x);
+    dst[(int64_t)blockIdx.x * ne0 + i0] = sr < 0 ? 0u : src[(int64_t)sr * ne0 + i0];          // 0u: the +0.0f ggml-cpu writes
+}
+
+__global__ void win_unpart_kernel(win_geom g, const uint32_t * __restrict__ src, uint32_t * __restrict__ dst, int64_t ne0) {
+    pdl_trigger();
+    const int64_t i0 = (int64_t)blockIdx.y * blockDim.x + threadIdx.x;
+    if (i0 >= ne0) return;
+    dst[(int64_t)blockIdx.x * ne0 + i0] = src[(int64_t)win_unpart_src_row(g, blockIdx.x) * ne0 + i0];
+}
+
+__global__ void get_rel_pos_kernel(uint32_t w, const uint16_t * __restrict__ src, uint16_t * __restrict__ dst, int64_t ne0) {
+    pdl_trigger();
+    const int64_t i0 = (int64_t)blockIdx.y * blockDim.x + threadIdx.x;
+    if (i0 >= ne0) return;
+    dst[(int64_t)blockIdx.x * ne0 + i0] = src[(int64_t)get_rel_pos_src_row(w, blockIdx.x) * ne0 + i0];
+}
+
+// V consecutive keys per thread (V = 4: float4 loads and stores, when L L % 4 == 0 and src / dst are 16-byte aligned).  In place when dst is
+// src: each thread reads its elements before it writes them.
+template <int V> __global__ void add_rel_pos_kernel(const float * src, const float * __restrict__ pw, const float * __restrict__ ph, float * dst,
+                                                    uint32_t L, uint32_t LL) {
+    pdl_trigger();
+    const uint32_t c0 = (blockIdx.y * blockDim.x + threadIdx.x) * V;
+    if (c0 >= LL) return;
+    const int64_t r = blockIdx.x, e = r * LL + c0;
+    const float * pwr = pw + r * L, * phr = ph + r * L;
+    float v[V];
+    if constexpr (V == 4) { const float4 t = *(const float4 *)(src + e); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w; }
+    else v[0] = src[e];
+    uint32_t kh = c0 / L, kw = c0 - kh * L;
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+        v[j] = add_rel_pos_value(v[j], pwr[kw], phr[kh], kh, kw);
+        if (++kw == L) { kw = 0; ++kh; }
+    }
+    if constexpr (V == 4) *(float4 *)(dst + e) = make_float4(v[0], v[1], v[2], v[3]);
+    else dst[e] = v[0];
+}
+
+// ------------------------------------------------------------------ CONV_TRANSPOSE_2D (the mask decoder's output upscaling)
+// Output (ox, oy) = (px + s qx, py + s qy) of stride phase (px, py) takes taps kx = px + s mx, ky = py + s my from input (qx - mx, qy - my):
+// every output of one phase has the same taps.  A CTA owns CT2D_TQX x CT2D_TQY outputs (qx, qy) of the phase blockIdx.z and CT2D_CO output
+// channels; each thread one output pixel x CT2D_COT channels, accumulated in f32 registers.  The taps run in descending (my, mx), which is
+// ascending input row, then column: ggml-cpu's order.  For each tap the dot over Cin runs in chunks of CT2D_CI channels, each staged in shared
+// memory as the fp16-rounded input tile and the kernel slice (as f32).  No workspace; every output is written once (phases without taps,
+// s > K, write +0).  Three CTAs per SM: 80 registers without spills (a bare 256-thread bound lets ptxas squeeze to 64 and spill).
+__global__ void __launch_bounds__(CT2D_THREADS, 3) ct2d_kernel(ct2d_geom g, const uint8_t * __restrict__ k, const uint8_t * __restrict__ x,
+                                                            float * __restrict__ dst) {
+    pdl_trigger();
+    constexpr int NP = CT2D_TQX * CT2D_TQY;
+    __shared__ float sx[CT2D_CI][NP];
+    __shared__ __align__(16) float sk[CT2D_CI][CT2D_CO];
+    const int s = g.s, py = (int)blockIdx.z / s, px = (int)blockIdx.z - py * s;
+    const int nqx = px < g.OW ? (g.OW - px + s - 1) / s : 0, nqy = py < g.OH ? (g.OH - py + s - 1) / s : 0;   // this phase's outputs
+    const int tiles_x = ((g.OW + s - 1) / s + CT2D_TQX - 1) / CT2D_TQX;
+    const int ty = (int)blockIdx.x / tiles_x, tx = (int)blockIdx.x - ty * tiles_x;
+    const int qx0 = tx * CT2D_TQX, qy0 = ty * CT2D_TQY;
+    if (qx0 >= nqx || qy0 >= nqy) return;                                   // the whole CTA: a tile beyond this phase's outputs
+    const int p = threadIdx.x % NP, grp = threadIdx.x / NP;                 // grp is warp-uniform: sk reads broadcast
+    const int qx = qx0 + p % CT2D_TQX, qy = qy0 + p / CT2D_TQX;
+    const int co0 = blockIdx.y * CT2D_CO;
+    const int Mx = px < g.Kw ? (g.Kw - px + s - 1) / s : 0, My = py < g.Kh ? (g.Kh - py + s - 1) / s : 0;
+    float out[CT2D_COT];
+#pragma unroll
+    for (int j = 0; j < CT2D_COT; ++j) out[j] = 0.0f;
+    for (int my = My - 1; my >= 0; --my) {
+        for (int mx = Mx - 1; mx >= 0; --mx) {
+            const int ky = py + my * s, kx = px + mx * s;
+            float dot[CT2D_COT];
+#pragma unroll
+            for (int j = 0; j < CT2D_COT; ++j) dot[j] = 0.0f;
+            for (int ci0 = 0; ci0 < g.Cin; ci0 += CT2D_CI) {
+                const int n = min(CT2D_CI, g.Cin - ci0);
+                __syncthreads();                                            // the previous chunk's readers are done
+                for (int i = threadIdx.x; i < CT2D_CI * NP; i += CT2D_THREADS) {
+                    const int c = i / NP, pp = i % NP;
+                    const int ix = qx0 + pp % CT2D_TQX - mx, iy = qy0 + pp / CT2D_TQX - my;
+                    sx[c][pp] = c < n && ix >= 0 && ix < g.W && iy >= 0 && iy < g.H ? ct2d_input(g, x, ix, iy, ci0 + c) : 0.0f;
+                }
+                for (int i = threadIdx.x; i < CT2D_CI * CT2D_CO; i += CT2D_THREADS) {
+                    const int c = i / CT2D_CO, o = i % CT2D_CO;
+                    sk[c][o] = c < n && co0 + o < g.Cout ? ct2d_kernel(g, k, kx, ky, co0 + o, ci0 + c) : 0.0f;
+                }
+                __syncthreads();
+                for (int c = 0; c < n; ++c) {
+                    const float xv = sx[c][p];
+#pragma unroll
+                    for (int j = 0; j < CT2D_COT; ++j) dot[j] = ct2d_dot_step(dot[j], xv, sk[c][grp * CT2D_COT + j]);
+                }
+            }
+            const int ix = qx - mx, iy = qy - my;
+            if (ix >= 0 && ix < g.W && iy >= 0 && iy < g.H) {               // a tap ggml-cpu has: add it
+#pragma unroll
+                for (int j = 0; j < CT2D_COT; ++j) out[j] = pool_add(out[j], dot[j]);
+            }
+        }
+    }
+    if (qx >= nqx || qy >= nqy) return;
+    const int64_t ox = px + (int64_t)s * qx, oy = py + (int64_t)s * qy;
+#pragma unroll
+    for (int j = 0; j < CT2D_COT; ++j) {
+        const int co = co0 + grp * CT2D_COT + j;
+        if (co < g.Cout) dst[((int64_t)co * g.OH + oy) * g.OW + ox] = out[j];
+    }
+}
+
 // ------------------------------------------------------------------ ARGSORT (f32 rows of ne0 <= 1024 -> i32 indices, dst contiguous)
 // One CTA per row: the row's (key, index) items (b200_sort.cuh), padded to P = the next power of two, are sorted by the bitonic network in
 // shared memory, one compare-exchange per thread and step.  The order is a strict total order (ties by index, NaNs last), so each output
@@ -743,7 +866,7 @@ int ggml_b200_op_diag_mask_inf(const float * src, float * dst, int64_t ne0, int6
 
 int ggml_b200_op_unary(int32_t uop, const float * src, float * dst, int64_t n, void * stream) {
     if (n <= 0) return GGML_B200_OK;
-    if (uop < 0 || uop > U_SQRT) { set_error("unary: bad op %d", uop); return GGML_B200_EINVAL; }
+    if (uop < 0 || uop > U_COS) { set_error("unary: bad op %d", uop); return GGML_B200_EINVAL; }
     B200_CUDA_TRY(launch_pdl(unary_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, uop, src, dst, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
@@ -890,6 +1013,78 @@ int ggml_b200_op_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * d
     uint8_t * d = (uint8_t *)dst->data;
     if (repeat_elem_size(src->type) == 4) B200_CUDA_TRY(launch_pdl(repeat_kernel<uint32_t>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, s, d, n));
     else                                  B200_CUDA_TRY(launch_pdl(repeat_kernel<uint16_t>, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, g, s, d, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+// the row kernels' block: ne0 threads rounded up to a warp, at most 256 (the checks bound the row's blocks by 65535)
+static inline int row_threads(int64_t ne0) { return (int)std::min<int64_t>(256, (ne0 + 31) / 32 * 32); }
+
+int ggml_b200_op_win_part(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t npx, int32_t npy, int32_t w, void * stream) {
+    CHECK_ARGS(check_win_part(src, dst, npx, npy, w));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    const win_geom g{ w, npx, (int32_t)src->ne[1], (int32_t)src->ne[2] };
+    const int64_t ne0 = dst->ne[0];
+    const int th = row_threads(ne0);
+    B200_CUDA_TRY(launch_pdl(win_part_kernel, dim3((unsigned)nrows(*dst), blocks_for(ne0, th)), dim3(th), 0, (cudaStream_t)stream, g,
+                             (const uint32_t *)src->data, (uint32_t *)dst->data, ne0));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_win_unpart(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t w, void * stream) {
+    CHECK_ARGS(check_win_unpart(src, dst, w));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    const win_geom g{ w, (int32_t)((dst->ne[1] + w - 1) / w), (int32_t)dst->ne[1], (int32_t)dst->ne[2] };
+    const int64_t ne0 = dst->ne[0];
+    const int th = row_threads(ne0);
+    B200_CUDA_TRY(launch_pdl(win_unpart_kernel, dim3((unsigned)nrows(*dst), blocks_for(ne0, th)), dim3(th), 0, (cudaStream_t)stream, g,
+                             (const uint32_t *)src->data, (uint32_t *)dst->data, ne0));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_get_rel_pos(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_get_rel_pos(src, dst));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    const int64_t ne0 = dst->ne[0];
+    const int th = row_threads(ne0);
+    B200_CUDA_TRY(launch_pdl(get_rel_pos_kernel, dim3((unsigned)nrows(*dst), blocks_for(ne0, th)), dim3(th), 0, (cudaStream_t)stream,
+                             (uint32_t)dst->ne[1], (const uint16_t *)src->data, (uint16_t *)dst->data, ne0));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_add_rel_pos(const ggml_b200_tensor * src0, const ggml_b200_tensor * pw, const ggml_b200_tensor * ph, const ggml_b200_tensor * dst,
+                             void * stream) {
+    CHECK_ARGS(check_add_rel_pos(src0, pw, ph, dst));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    const uint32_t L = (uint32_t)pw->ne[0], LL = (uint32_t)dst->ne[0];
+    const float * s = (const float *)src0->data, * w = (const float *)pw->data, * h = (const float *)ph->data;
+    float * d = (float *)dst->data;
+    const dim3 rows((unsigned)nrows(*dst));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (LL % 4 == 0 && ((uintptr_t)s % 16) == 0 && ((uintptr_t)d % 16) == 0) {
+        const int th = row_threads(LL / 4);
+        B200_CUDA_TRY(launch_pdl(add_rel_pos_kernel<4>, dim3(rows.x, blocks_for(LL / 4, th)), dim3(th), 0, st, s, w, h, d, L, LL));
+    } else {
+        const int th = row_threads(LL);
+        B200_CUDA_TRY(launch_pdl(add_rel_pos_kernel<1>, dim3(rows.x, blocks_for(LL, th)), dim3(th), 0, st, s, w, h, d, L, LL));
+    }
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_conv_transpose_2d(const ggml_b200_tensor * kernel, const ggml_b200_tensor * input, const ggml_b200_tensor * dst, int32_t stride,
+                                   void * stream) {
+    CHECK_ARGS(check_conv_transpose_2d(kernel, input, dst, stride));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    const ct2d_geom g = ct2d_geometry(*kernel, *input, *dst, stride);
+    const int64_t nq_x = (g.OW + stride - 1) / stride, nq_y = (g.OH + stride - 1) / stride;      // outputs of the largest phase
+    const unsigned tiles = blocks_for(nq_x, CT2D_TQX) * blocks_for(nq_y, CT2D_TQY);
+    const dim3 grid(tiles, blocks_for(g.Cout, CT2D_CO), (unsigned)(stride * stride));
+    B200_CUDA_TRY(launch_pdl(ct2d_kernel, grid, dim3(CT2D_THREADS), 0, (cudaStream_t)stream, g, (const uint8_t *)kernel->data,
+                             (const uint8_t *)input->data, (float *)dst->data));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

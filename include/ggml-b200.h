@@ -220,7 +220,9 @@ typedef struct ggml_b200_tensor {
 
 enum ggml_b200_unary { GGML_B200_UNARY_GELU = 0, GGML_B200_UNARY_SILU = 1, GGML_B200_UNARY_RELU = 2, GGML_B200_UNARY_TANH = 3,
                        GGML_B200_UNARY_NEG = 4, GGML_B200_UNARY_ABS = 5, GGML_B200_UNARY_GELU_QUICK = 6, GGML_B200_UNARY_SIGMOID = 7,
-                       GGML_B200_UNARY_EXP = 8, GGML_B200_UNARY_SQR = 9, GGML_B200_UNARY_SQRT = 10 };
+                       GGML_B200_UNARY_EXP = 8, GGML_B200_UNARY_SQR = 9, GGML_B200_UNARY_SQRT = 10,
+                       /* GGML_OP_SIN / GGML_OP_COS: sinf / cosf (within 2 ulp, not the fast intrinsics) */
+                       GGML_B200_UNARY_SIN = 11, GGML_B200_UNARY_COS = 12 };
 
 GGML_B200_API int ggml_b200_op_get_rows(const ggml_b200_tensor * src0, const ggml_b200_tensor * ids, const ggml_b200_tensor * dst, void * stream);
 /* op: 0 add, 1 mul, 2 sub, 3 div; src1 broadcasts into dst's shape; dst may alias src0 */
@@ -338,6 +340,28 @@ GGML_B200_API int ggml_b200_op_leaky_relu(const ggml_b200_tensor * src, const gg
  * strides; every dst extent a whole multiple of src's (else GGML_B200_EINVAL).  dst (i0, i1, i2, i3) = src (i0 % ne00, i1 % ne01, ...), moved
  * as raw words: every bit pattern (NaN payloads included) is kept. */
 GGML_B200_API int ggml_b200_op_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_WIN_PART (ggml_win_part): src f32 [C, W0, H0, 1] -> dst f32 [C, w, w, npx npy], both packed; npx, npy, w the node's op_params.
+ * Window py npx + px holds the image pixels (px w + i1, py w + i2), zeros where it runs past the image.  Raw 4-byte words: bit-identical
+ * (NaN payloads and -0 kept).  npx != ceil(W0 / w), npy != ceil(H0 / w), w < 1 or dst extents that disagree: GGML_B200_EINVAL. */
+GGML_B200_API int ggml_b200_op_win_part(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t npx, int32_t npy, int32_t w, void * stream);
+/* GGML_OP_WIN_UNPART (ggml_win_unpart): src f32 [C, w, w, np] -> dst f32 [C, W0, H0, 1], both packed; the inverse of WIN_PART, dropping the
+ * padding.  Raw words: bit-identical.  np < ceil(W0 / w) ceil(H0 / w) (the reads would leave src), w < 1: GGML_B200_EINVAL. */
+GGML_B200_API int ggml_b200_op_win_unpart(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t w, void * stream);
+/* GGML_OP_GET_REL_POS (ggml_get_rel_pos): src f16 [C, 2w - 1] -> dst f16 [C, w, w], both packed: dst[i2, i1, :] = src[(w - 1 - i1) + i2, :],
+ * raw 2-byte words (bit-identical).  Other types (BF16 included): GGML_B200_EUNSUPPORTED. */
+GGML_B200_API int ggml_b200_op_get_rel_pos(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_ADD_REL_POS (ggml_add_rel_pos[_inplace]): src0 f32 [L L, A B, P, 1], pw and ph f32 [L, A, B, P], dst like src0, all packed; dst may
+ * be src0 (in place).  dst[r, kh L + kw] = src0[r, kh L + kw] + ph[r, kh] + pw[r, kw], the two adds in the CPU backend's order (ph first when
+ * kh <= kw, pw first otherwise): bit-identical.  src0 with ne3 > 1: GGML_B200_EUNSUPPORTED; extents that disagree: GGML_B200_EINVAL. */
+GGML_B200_API int ggml_b200_op_add_rel_pos(const ggml_b200_tensor * src0, const ggml_b200_tensor * pw, const ggml_b200_tensor * ph, const ggml_b200_tensor * dst,
+                                           void * stream);
+/* GGML_OP_CONV_TRANSPOSE_2D (ggml_conv_transpose_2d_p0): kernel f16 [Kw, Kh, Cout, Cin] (Kw x Kh planes packed), input f32 [W, H, Cin, 1]
+ * (contiguous along dim 0) -> dst f32 [(W-1) s + Kw, (H-1) s + Kh, Cout, 1] packed, padding 0.  The input is rounded to fp16 (to nearest even,
+ * as the CPU backend rounds it); each tap's dot over Cin is an f32 sum of exact fp16 x fp16 products; the taps are added from +0.0 in the CPU
+ * backend's order (ascending input row, then column).  Only the order inside a dot differs from the CPU backend.  A batch (ne3 > 1):
+ * GGML_B200_EUNSUPPORTED; stride < 1 or extents that disagree: GGML_B200_EINVAL. */
+GGML_B200_API int ggml_b200_op_conv_transpose_2d(const ggml_b200_tensor * kernel, const ggml_b200_tensor * input, const ggml_b200_tensor * dst,
+                                                 int32_t stride, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
