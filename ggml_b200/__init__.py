@@ -297,7 +297,7 @@ def tensor_desc(t) -> TensorDesc:
     import torch
     d = TensorDesc()
     d.data = t.data_ptr()
-    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30}[t.dtype]
+    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30, torch.int64: 27}[t.dtype]
     shape = list(t.shape)[::-1] + [1] * (4 - t.dim())
     es = t.element_size()
     nb = es
@@ -325,6 +325,7 @@ def mul_mat_fused(t, W, X, M, K, bias, gelu: bool, residual=None):
 
 
 UNARY_SIN, UNARY_COS = 11, 12                  # GGML_B200_UNARY_SIN / _COS (GGML_OP_SIN / GGML_OP_COS): sinf / cosf
+UNARY_STEP = 13                                # GGML_B200_UNARY_STEP (GGML_UNARY_OP_STEP): x > 0 ? 1 : 0
 
 
 def op_unary(uop: int, x):
@@ -488,7 +489,7 @@ def strided_desc(t) -> TensorDesc:
     import torch
     d = TensorDesc()
     d.data = t.data_ptr()
-    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30}[t.dtype]
+    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30, torch.int64: 27}[t.dtype]
     es = t.element_size()
     shape, strides = list(t.shape)[::-1], list(t.stride())[::-1]
     for i in range(4):
@@ -758,4 +759,80 @@ def op_conv_transpose_2d(kernel, x, stride: int):
     y = torch.empty(tuple(x.shape[:-3]) + (cout, (h - 1) * stride + kh, (w - 1) * stride + kw), dtype=torch.float32, device=x.device)
     k, s, d = strided_desc(kernel), strided_desc(x), tensor_desc(y)
     check(L.ggml_b200_op_conv_transpose_2d(C.byref(k), C.byref(s), C.byref(d), stride, _stream()), "ggml_b200_op_conv_transpose_2d")
+    return y
+
+
+def _launch(name: str, *descs):
+    L = lib()
+    fn = getattr(L, name)
+    fn.argtypes = [C.POINTER(TensorDesc)] * len(descs) + [C.c_void_p]
+    check(fn(*(C.byref(d) for d in descs), _stream()), name)
+
+
+def op_out_prod(a, b):
+    """GGML_OP_OUT_PROD (ggml_out_prod): a f32 torch [(b3,) (b2,) K, M] with its last dim contiguous, b f32 torch [(B3,) (B2,) K, N] with any
+    strides (b.t() of a contiguous [N, K] is the gradient's form) -> a new f32 tensor [(B3,) (B2,) N, M], out[.., n, m] = sum_k a[.., k, m]
+    b[.., k, n]: one fused multiply-add per term in ascending k; a's batch dims broadcast over b's as in MUL_MAT"""
+    import torch
+    y = torch.empty(tuple(b.shape[:-2]) + (b.shape[-1], a.shape[-1]), dtype=torch.float32, device=a.device)
+    _launch("ggml_b200_op_out_prod", strided_desc(a), strided_desc(b), tensor_desc(y))
+    return y
+
+
+def op_cross_entropy_loss(logits, labels):
+    """GGML_OP_CROSS_ENTROPY_LOSS: logits and labels f32 of one shape (rows = the last dim, contiguous) -> a new f32 tensor [1]:
+    -1/nr sum of labels * log_softmax(logits), reduced in one fixed order"""
+    import torch
+    y = torch.empty((1,), dtype=torch.float32, device=logits.device)
+    _launch("ggml_b200_op_cross_entropy_loss", strided_desc(logits), strided_desc(labels), tensor_desc(y))
+    return y
+
+
+def op_cross_entropy_loss_back(grad, logits, labels):
+    """GGML_OP_CROSS_ENTROPY_LOSS_BACK: grad f32 [1] (read on the device), logits and labels f32 of one shape, contiguous -> a new tensor
+    (softmax(logits) - labels) * grad / nr, row by row"""
+    import torch
+    y = torch.empty_like(logits)
+    _launch("ggml_b200_op_cross_entropy_loss_back", tensor_desc(grad), tensor_desc(logits), tensor_desc(labels), tensor_desc(y))
+    return y
+
+
+def op_opt_step_adamw(w, g, m, v, params):
+    """GGML_OP_OPT_STEP_ADAMW, in place on w, m and v (f32, contiguous, one shape) with the gradient g; params f32 [7] on the device =
+    alpha, beta1, beta2, eps, wd, beta1h, beta2h, read by the kernel; bit-identical to ggml-cpu.  Returns w."""
+    _launch("ggml_b200_op_opt_step_adamw", tensor_desc(w), tensor_desc(g), tensor_desc(m), tensor_desc(v), tensor_desc(params))
+    return w
+
+
+def op_argmax(x):
+    """GGML_OP_ARGMAX: x f32 [rows, n] (last dim contiguous) -> a new i32 tensor [rows], ggml-cpu's rule: the last index of the maximum,
+    a NaN restarting the search, a trailing run of NaNs ignored, 0 for a row of NaNs"""
+    import torch
+    y = torch.empty((x.shape[0],), dtype=torch.int32, device=x.device)
+    _launch("ggml_b200_op_argmax", strided_desc(x), tensor_desc(y))
+    return y
+
+
+def op_count_equal(a, b):
+    """GGML_OP_COUNT_EQUAL: a and b i32 of one shape, at most 2-D (any strides) -> a new i64 tensor [1], the number of equal pairs"""
+    import torch
+    y = torch.empty((1,), dtype=torch.int64, device=a.device)
+    _launch("ggml_b200_op_count_equal", strided_desc(a), strided_desc(b), tensor_desc(y))
+    return y
+
+
+def op_sum(x):
+    """GGML_OP_SUM: x f32 (last dim contiguous) -> a new f32 tensor [1], the sum in double rounded once"""
+    import torch
+    y = torch.empty((1,), dtype=torch.float32, device=x.device)
+    _launch("ggml_b200_op_sum", strided_desc(x), tensor_desc(y))
+    return y
+
+
+def op_repeat_back(x, shape):
+    """GGML_OP_REPEAT_BACK: x f32 (last dim contiguous, any other strides) -> a new f32 tensor of `shape` (torch order), each of whose
+    extents divides x's: the sum over the repeats, in ggml-cpu's order (bit-identical)"""
+    import torch
+    y = torch.empty(tuple(shape), dtype=torch.float32, device=x.device)
+    _launch("ggml_b200_op_repeat_back", strided_desc(x), tensor_desc(y))
     return y

@@ -468,6 +468,107 @@ inline op_check check_conv_transpose_2d(const ggml_b200_tensor * kernel, const g
     return accepted;
 }
 
+// ------------------------------------------------------------------ the ops of ggml_opt's backward and optimizer graphs (b200_train.cuh)
+
+// OUT_PROD: src0 f32 [ne0, K, ne02, ne03] contiguous along dim 0, src1 f32 [ne1, K, ne2, ne3] any strides, dst f32 packed (ggml-cpu zeroes it
+// as packed); ne2 % ne02 == 0, ne3 % ne03 == 0.  ggml-cpu's f16 and quantized src0 forms are declined.
+inline op_check check_out_prod(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src0 && src1 && dst, "src0, src1 and dst are required");
+    const ggml_b200_tensor & a = *src0, & b = *src1, & d = *dst;
+    B200_REQUIRE(a.type == F32 && b.type == F32 && d.type == F32, "src0, src1 and dst must be f32");
+    B200_REQUIRE(a.nb[0] == 4, "src0 must be contiguous along dim 0");
+    B200_REQUIRE(is_packed4(d), "dst must be packed");
+    B200_VALID(d.ne[0] == a.ne[0] && d.ne[1] == b.ne[0] && a.ne[1] == b.ne[1] && d.ne[2] == b.ne[2] && d.ne[3] == b.ne[3],
+               "dst must be [src0 ne0, src1 ne0, src1 ne2, src1 ne3] and src0, src1 share K");
+    B200_VALID(a.ne[2] >= 1 && a.ne[3] >= 1 && d.ne[2] % a.ne[2] == 0 && d.ne[3] % a.ne[3] == 0, "src0's batch dims must divide dst's");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE((d.ne[1] + 127) / 128 <= 65535 && d.ne[2] * d.ne[3] <= 65535 && (d.ne[0] + 127) / 128 <= 0x7fffffff, "too many tiles for one grid");
+    return accepted;
+}
+
+// CROSS_ENTROPY_LOSS: logits and labels f32 of one shape, rows contiguous along dim 0 (ggml-cpu reads row i1 at i1 nb1: evenly spaced rows
+// are the caller's condition), dst an f32 scalar
+inline op_check check_cross_entropy_loss(const ggml_b200_tensor * logits, const ggml_b200_tensor * labels, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(logits && labels && dst, "logits, labels and dst are required");
+    const ggml_b200_tensor & x = *logits, & l = *labels, & d = *dst;
+    B200_REQUIRE(x.type == F32 && l.type == F32 && d.type == F32, "logits, labels and dst must be f32");
+    B200_REQUIRE(x.nb[0] == 4 && l.nb[0] == 4, "rows must be contiguous along dim 0");
+    B200_VALID(same_shape(x, l), "logits and labels must have one shape");
+    B200_VALID(nelem(d) == 1, "dst must be a scalar");
+    return accepted;
+}
+
+// CROSS_ENTROPY_LOSS_BACK: grad an f32 scalar, logits, labels and dst f32 of one shape, all packed (ggml-cpu asserts it)
+inline op_check check_cross_entropy_loss_back(const ggml_b200_tensor * grad, const ggml_b200_tensor * logits, const ggml_b200_tensor * labels,
+                                              const ggml_b200_tensor * dst) {
+    B200_REQUIRE(grad && logits && labels && dst, "grad, logits, labels and dst are required");
+    const ggml_b200_tensor & g = *grad, & x = *logits, & l = *labels, & d = *dst;
+    B200_REQUIRE(g.type == F32 && x.type == F32 && l.type == F32 && d.type == F32, "grad, logits, labels and dst must be f32");
+    B200_REQUIRE(is_packed4(x) && is_packed4(l) && is_packed4(d), "logits, labels and dst must be packed");
+    B200_VALID(nelem(g) == 1, "grad must be a scalar");
+    B200_VALID(same_shape(x, l) && same_shape(x, d), "logits, labels and dst must have one shape");
+    if (nelem(d) == 0) return accepted;
+    B200_REQUIRE(nrows(d) <= 0x7fffffff, "too many rows for one grid");
+    return accepted;
+}
+
+// OPT_STEP_ADAMW: w, g, m, v f32 of one shape, all packed (ggml-cpu addresses g, m and v with w's offsets), params f32 with 7 elements
+inline op_check check_opt_step_adamw(const ggml_b200_tensor * w, const ggml_b200_tensor * g, const ggml_b200_tensor * m, const ggml_b200_tensor * v,
+                                     const ggml_b200_tensor * params) {
+    B200_REQUIRE(w && g && m && v && params, "w, g, m, v and params are required");
+    B200_REQUIRE(w->type == F32 && g->type == F32 && m->type == F32 && v->type == F32 && params->type == F32, "w, g, m, v and params must be f32");
+    B200_REQUIRE(is_packed4(*w) && is_packed4(*g) && is_packed4(*m) && is_packed4(*v) && is_packed4(*params), "w, g, m, v and params must be packed");
+    B200_VALID(same_shape(*w, *g) && same_shape(*w, *m) && same_shape(*w, *v), "w, g, m and v must have one shape");
+    B200_VALID(nelem(*params) == 7, "params must hold 7 values");
+    return accepted;
+}
+
+// ARGMAX: src f32 [ne0, ne1] rows contiguous along dim 0, dst i32 [ne1] contiguous along dim 0
+inline op_check check_argmax(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == F32 && d.type == I32, "src must be f32, dst i32");
+    B200_REQUIRE(s.nb[0] == 4 && d.nb[0] == 4, "src rows and dst must be contiguous along dim 0");
+    B200_VALID(s.ne[2] == 1 && s.ne[3] == 1 && d.ne[0] == s.ne[1] && d.ne[1] == 1 && d.ne[2] == 1 && d.ne[3] == 1, "src must be a matrix, dst [ne1]");
+    if (s.ne[1] == 0) return accepted;
+    B200_VALID(s.ne[0] >= 1, "rows must not be empty");
+    B200_REQUIRE(s.ne[0] <= 0x7fffffff && s.ne[1] <= 0x7fffffff, "extents must fit 32 bits");
+    return accepted;
+}
+
+// COUNT_EQUAL: src0 and src1 i32 of one shape, any strides, dst an i64 scalar.  ggml-cpu's row walk (ggml-cpu.c:5850-5853) names the right
+// row only when ne2 == ne3 == 1: others are declined.
+inline op_check check_count_equal(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src0 && src1 && dst, "src0, src1 and dst are required");
+    const ggml_b200_tensor & a = *src0, & b = *src1, & d = *dst;
+    B200_REQUIRE(a.type == I32 && b.type == I32 && d.type == GGML_B200_TYPE_I64, "src0 and src1 must be i32, dst i64");
+    B200_VALID(same_shape(a, b), "src0 and src1 must have one shape");
+    B200_VALID(nelem(d) == 1, "dst must be a scalar");
+    B200_REQUIRE(a.ne[2] == 1 && a.ne[3] == 1, "ne2 and ne3 must be 1 (the CPU backend's row walk)");
+    return accepted;
+}
+
+// SUM: src f32 contiguous along dim 0 (ggml-cpu asserts it), any other strides, dst an f32 scalar
+inline op_check check_sum(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    B200_REQUIRE(src->type == F32 && dst->type == F32, "src and dst must be f32");
+    B200_REQUIRE(src->nb[0] == 4, "src must be contiguous along dim 0");
+    B200_VALID(nelem(*dst) == 1, "dst must be a scalar");
+    return accepted;
+}
+
+// REPEAT_BACK: src and dst f32, both contiguous along dim 0 (ggml-cpu asserts nb0 == nb00 == 4 and honours every other stride), every src
+// extent a whole multiple of dst's.  ggml-cpu has no other type (it aborts on I32 / I16): declined.
+inline op_check check_repeat_back(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    const ggml_b200_tensor & s = *src, & d = *dst;
+    B200_REQUIRE(s.type == F32 && d.type == F32, "src and dst must be f32");
+    B200_REQUIRE(s.nb[0] == 4 && d.nb[0] == 4, "src and dst must be contiguous along dim 0");
+    if (nelem(d) == 0) return accepted;
+    for (int i = 0; i < 4; ++i) B200_VALID(s.ne[i] % d.ne[i] == 0, "every src extent must be a whole multiple of dst's");
+    return accepted;
+}
+
 #undef B200_REQUIRE
 #undef B200_VALID
 

@@ -527,6 +527,7 @@ int unary_code(const ggml_tensor * node) {
         case GGML_UNARY_OP_GELU_QUICK: return GGML_B200_UNARY_GELU_QUICK;
         case GGML_UNARY_OP_SIGMOID:    return GGML_B200_UNARY_SIGMOID;
         case GGML_UNARY_OP_EXP:        return GGML_B200_UNARY_EXP;
+        case GGML_UNARY_OP_STEP:       return GGML_B200_UNARY_STEP;
         default:                       return -1;
     }
 }
@@ -661,6 +662,54 @@ int bound_op(const ggml_tensor * node, bool launch, void * stream) {
             const auto k = desc(a), x = desc(b), d = desc(node);
             return launch ? ggml_b200_op_conv_transpose_2d(&k, &x, &d, s, stream) : b200::check_conv_transpose_2d(&k, &x, &d, s).code;
         }
+        // the ops of ggml_opt's backward and optimizer graphs
+        case GGML_OP_OUT_PROD: {
+            if (!launch && !b) return GGML_B200_EUNSUPPORTED;
+            const auto x = desc(a), y = desc(b), d = desc(node);
+            return launch ? ggml_b200_op_out_prod(&x, &y, &d, stream) : b200::check_out_prod(&x, &y, &d).code;
+        }
+        case GGML_OP_CROSS_ENTROPY_LOSS: {
+            // ggml-cpu walks nrows rows at i*nb1 (ggml-cpu.c:12484-12486): only evenly spaced rows mean the same data on both backends
+            if (!launch && (!b || a->nb[2] != a->ne[1] * a->nb[1] || a->nb[3] != a->ne[2] * a->nb[2] ||
+                            b->nb[2] != b->ne[1] * b->nb[1] || b->nb[3] != b->ne[2] * b->nb[2])) return GGML_B200_EUNSUPPORTED;
+            const auto x = desc(a), l = desc(b), d = desc(node);
+            return launch ? ggml_b200_op_cross_entropy_loss(&x, &l, &d, stream) : b200::check_cross_entropy_loss(&x, &l, &d).code;
+        }
+        case GGML_OP_CROSS_ENTROPY_LOSS_BACK: {            // sources: the loss's gradient, the logits, the labels
+            const ggml_tensor * c = node->src[2];
+            if (!launch && (!b || !c)) return GGML_B200_EUNSUPPORTED;
+            const auto gr = desc(a), x = desc(b), l = desc(c), d = desc(node);
+            return launch ? ggml_b200_op_cross_entropy_loss_back(&gr, &x, &l, &d, stream) : b200::check_cross_entropy_loss_back(&gr, &x, &l, &d).code;
+        }
+        case GGML_OP_OPT_STEP_ADAMW: {                     // sources: w, grad, m, v, params; dst is a view of w, updated in place
+            const ggml_tensor * m = node->src[2], * v = node->src[3], * pr = node->src[4];
+            if (!launch && (!b || !m || !v || !pr)) return GGML_B200_EUNSUPPORTED;
+            // the kernel reads the hyper-parameters on the device: a source still in a host buffer (device_supports_op lets one through for
+            // the scheduler to copy in) is an error here, never a read of a host pointer
+            if (launch && !buffer_is_b200(pr->view_src ? pr->view_src->buffer : pr->buffer)) {
+                GGML_LOG_ERROR("ggml-b200: OPT_STEP_ADAMW's hyper-parameters (%s) are not in a device buffer\n", pr->name);
+                return GGML_B200_EINVAL;
+            }
+            const auto w = desc(node), gr = desc(b), tm = desc(m), tv = desc(v), tp = desc(pr);
+            return launch ? ggml_b200_op_opt_step_adamw(&w, &gr, &tm, &tv, &tp, stream) : b200::check_opt_step_adamw(&w, &gr, &tm, &tv, &tp).code;
+        }
+        case GGML_OP_ARGMAX: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_argmax(&x, &d, stream) : b200::check_argmax(&x, &d).code;
+        }
+        case GGML_OP_COUNT_EQUAL: {
+            if (!launch && !b) return GGML_B200_EUNSUPPORTED;
+            const auto x = desc(a), y = desc(b), d = desc(node);
+            return launch ? ggml_b200_op_count_equal(&x, &y, &d, stream) : b200::check_count_equal(&x, &y, &d).code;
+        }
+        case GGML_OP_SUM: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_sum(&x, &d, stream) : b200::check_sum(&x, &d).code;
+        }
+        case GGML_OP_REPEAT_BACK: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_repeat_back(&x, &d, stream) : b200::check_repeat_back(&x, &d).code;
+        }
         case GGML_OP_SSM_SCAN: {
             // sources: s, x, dt, A, B, C (ggml_ssm_scan); dst = y, then the final states
             ggml_b200_tensor t[6];
@@ -720,8 +769,14 @@ bool device_supports_op(ggml_backend_dev_t dev, const ggml_tensor * op) {
         if (a->ne[2] != 1 || a->ne[3] != 1 || b->ne[2] != 1 || b->ne[3] != 1 || !ggml_is_contiguous(a)) return false;
         return supports_mul_mat(op) && tensor_on_device(b, device);
     }
-    for (int i = 0; i < GGML_MAX_SRC; ++i)
-        if (op->src[i] && !tensor_on_device(op->src[i], device)) return false;
+    // OPT_STEP_ADAMW's hyper-parameters live in a host buffer (ggml_opt rewrites them every step): ggml_backend_sched copies such a source
+    // into this device before the split runs.  Only a host buffer is let through; a graph computed on this backend directly must hold them
+    // on the device (the launch refuses a host tensor, bound_op)
+    for (int i = 0; i < GGML_MAX_SRC; ++i) {
+        if (!op->src[i] || tensor_on_device(op->src[i], device)) continue;
+        const ggml_tensor * s = op->src[i]->view_src ? op->src[i]->view_src : op->src[i];
+        if (!(op->op == GGML_OP_OPT_STEP_ADAMW && i == 4 && ggml_backend_buffer_is_host(s->buffer))) return false;
+    }
     switch (op->op) {
         case GGML_OP_NONE: case GGML_OP_RESHAPE: case GGML_OP_VIEW: case GGML_OP_PERMUTE: case GGML_OP_TRANSPOSE:
             return true;

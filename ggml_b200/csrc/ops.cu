@@ -12,10 +12,15 @@
 //   pool_2d :10305-10377  upscale :10503-10540       leaky_relu :6689-6717            repeat :5901-6015
 //   win_part :11541-11582 win_unpart :11604-11640    get_rel_pos :11737-11760         add_rel_pos :11784-11842
 //   conv_transpose_2d :10140-10230                   sin / cos :1733-1734
+//   out_prod :7788-7905   cross_entropy_loss :12449-12525                    cross_entropy_loss_back :12545-12605
+//   opt_step_adamw :12626-12685                      argmax :5773-5795          count_equal :5821-5878   sum :5537-5565
+//   repeat_back :6019-6075                           step :1737
 // IM2COL is the first node of ggml_conv_1d / ggml_conv_2d (the convolutional front end of Whisper-style encoders); POOL_2D, UPSCALE,
 // LEAKY_RELU and REPEAT (the batch norm's per-channel vectors) are the ops around the convs of YOLO-style networks.  WIN_PART / WIN_UNPART
 // (windowed attention), GET_REL_POS / ADD_REL_POS (the decomposed relative-position bias), CONV_TRANSPOSE_2D (the mask decoder's output
 // upscaling) and SIN / COS (the random-Fourier positional encoding) are the ops of Segment-Anything-style image encoders and mask decoders.
+// OUT_PROD (the gradient of MUL_MAT), CROSS_ENTROPY_LOSS and its gradient, OPT_STEP_ADAMW, ARGMAX, COUNT_EQUAL, SUM, REPEAT_BACK (the
+// gradient of a broadcast ADD / MUL) and STEP (the gradient of RELU) are the ops ggml_opt's backward and optimizer graphs add.
 // ARGSORT and SUM_ROWS are the mixture-of-experts router's top-k and weight normalisation; CONCAT, SSM_CONV and SSM_SCAN are the
 // rolling conv state, the causal depthwise convolution and the selective scan of the Mamba-1 layer; RWKV_WKV6 and GATED_LINEAR_ATTN are
 // the recurrences of the RWKV-6 time mix and of its gated (RWKV6-Qwen2) form.
@@ -26,6 +31,7 @@
 #include "b200_conv.cuh"
 #include "b200_pool.cuh"
 #include "b200_sam.cuh"
+#include "b200_train.cuh"
 #include "b200_quants.cuh"
 #include "b200_dequant.cuh"
 #include "b200_ptx.cuh"
@@ -226,7 +232,7 @@ __global__ void diag_mask_inf_kernel(const float * x, float * y, int64_t ne0, in
     y[i] = c > n_past + r ? -INFINITY : x[i];
 }
 enum { U_GELU = 0, U_SILU = 1, U_RELU = 2, U_TANH = 3, U_NEG = 4, U_ABS = 5, U_GELU_QUICK = 6, U_SIGMOID = 7, U_EXP = 8, U_SQR = 9, U_SQRT = 10,
-       U_SIN = 11, U_COS = 12 };
+       U_SIN = 11, U_COS = 12, U_STEP = 13 };
 __global__ void unary_kernel(int uop, const float * x, float * y, int64_t n) {
     pdl_trigger();
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -247,7 +253,8 @@ __global__ void unary_kernel(int uop, const float * x, float * y, int64_t n) {
         case U_SQRT: r = sqrtf(v); break;
         // the library sinf / cosf (within 2 ulp everywhere), never the __sinf / __cosf intrinsics
         case U_SIN: r = sinf(v); break;
-        default: r = cosf(v); break;
+        case U_COS: r = cosf(v); break;
+        default: r = step_value(v); break;
     }
     y[i] = r;
 }
@@ -636,6 +643,265 @@ __global__ void __launch_bounds__(CT2D_THREADS, 3) ct2d_kernel(ct2d_geom g, cons
     }
 }
 
+// ------------------------------------------------------------------ OUT_PROD (the gradient of MUL_MAT): a tiled FP32 SIMT GEMM
+// dst[i0, i1] = sum_k a[i0, k] b[i1, k] for one (i2, i3) per grid z.  A CTA owns OP_BM x OP_BN outputs and walks K in slices of OP_BK:
+// each slice of a (coalesced along i0) and of b (coalesced along whichever of i1 / k is contiguous, b_k_contig) is staged in shared
+// memory, then every thread updates its OP_TM x OP_TN accumulators with one fused multiply-add per term, in ascending k (b200_train.cuh).
+// A thread's outputs are two groups of 4 along i0 (tx*4 and 64 + tx*4) by two of 4 along i1, so its shared-memory reads are float4s
+// without bank conflicts and a warp's stores cover 64 consecutive i0.  No workspace; K == 0 writes zeros.
+struct out_prod_geom {
+    int64_t M, N, K;                // dst ne0, ne1; the shared dim
+    int64_t ne2, dps2, dps3;        // dst ne2; dst per src0 along dims 2 and 3
+    int64_t anb1, anb2, anb3;       // src0 strides (nb0 == 4), bytes
+    int64_t bnb0, bnb1, bnb2, bnb3; // src1 strides, bytes
+    int64_t dnb1, dnb2, dnb3;       // dst strides, bytes
+    int b_k_contig;                 // src1 is contiguous along k (ggml_transpose(grad)): stage it k-fastest
+};
+
+__global__ void __launch_bounds__(OP_THREADS, 1) out_prod_kernel(out_prod_geom g, const uint8_t * __restrict__ a, const uint8_t * __restrict__ b,
+                                                                 uint8_t * __restrict__ dst) {
+    pdl_trigger();
+    __shared__ __align__(16) float sa[OP_BK][OP_BM];
+    __shared__ __align__(16) float sb[OP_BK][OP_BN + 4];       // +4: the k-fastest staging writes without bank conflicts
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int64_t m0 = (int64_t)blockIdx.x * OP_BM, n0 = (int64_t)blockIdx.y * OP_BN;
+    const int64_t i2 = blockIdx.z % g.ne2, i3 = blockIdx.z / g.ne2;
+    const uint8_t * ab = a + (i2 / g.dps2) * g.anb2 + (i3 / g.dps3) * g.anb3;
+    const uint8_t * bb = b + i2 * g.bnb2 + i3 * g.bnb3;
+    float acc[OP_TM][OP_TN];
+#pragma unroll
+    for (int r = 0; r < OP_TM; ++r)
+#pragma unroll
+        for (int c = 0; c < OP_TN; ++c) acc[r][c] = 0.0f;
+    for (int64_t k0 = 0; k0 < g.K; k0 += OP_BK) {
+        const int kn = (int)min((int64_t)OP_BK, g.K - k0);
+#pragma unroll
+        for (int j = 0; j < OP_BK * OP_BM / OP_THREADS; ++j) {
+            const int e = tid + j * OP_THREADS, k = e / OP_BM, m = e % OP_BM;
+            sa[k][m] = k < kn && m0 + m < g.M ? *(const float *)(ab + (m0 + m) * 4 + (k0 + k) * g.anb1) : 0.0f;
+        }
+#pragma unroll
+        for (int j = 0; j < OP_BK * OP_BN / OP_THREADS; ++j) {
+            const int e = tid + j * OP_THREADS;
+            const int k = g.b_k_contig ? e % OP_BK : e / OP_BN, n = g.b_k_contig ? e / OP_BK : e % OP_BN;
+            sb[k][n] = k < kn && n0 + n < g.N ? *(const float *)(bb + (n0 + n) * g.bnb0 + (k0 + k) * g.bnb1) : 0.0f;
+        }
+        __syncthreads();
+        if (kn == OP_BK) {
+#pragma unroll
+            for (int k = 0; k < OP_BK; ++k) {
+                const float4 a0 = *(const float4 *)&sa[k][tx * 4], a1 = *(const float4 *)&sa[k][64 + tx * 4];
+                const float4 b0 = *(const float4 *)&sb[k][ty * 4], b1 = *(const float4 *)&sb[k][64 + ty * 4];
+                const float av[OP_TM] = { a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w };
+                const float bv[OP_TN] = { b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w };
+#pragma unroll
+                for (int r = 0; r < OP_TM; ++r)
+#pragma unroll
+                    for (int c = 0; c < OP_TN; ++c) acc[r][c] = out_prod_step(acc[r][c], av[r], bv[c]);
+            }
+        } else {                                              // the last, partial slice: only the kn terms K has
+            for (int k = 0; k < kn; ++k) {
+                const float4 a0 = *(const float4 *)&sa[k][tx * 4], a1 = *(const float4 *)&sa[k][64 + tx * 4];
+                const float4 b0 = *(const float4 *)&sb[k][ty * 4], b1 = *(const float4 *)&sb[k][64 + ty * 4];
+                const float av[OP_TM] = { a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w };
+                const float bv[OP_TN] = { b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w };
+#pragma unroll
+                for (int r = 0; r < OP_TM; ++r)
+#pragma unroll
+                    for (int c = 0; c < OP_TN; ++c) acc[r][c] = out_prod_step(acc[r][c], av[r], bv[c]);
+            }
+        }
+        __syncthreads();
+    }
+    uint8_t * db = dst + i2 * g.dnb2 + i3 * g.dnb3;
+#pragma unroll
+    for (int c = 0; c < OP_TN; ++c) {
+        const int64_t n = n0 + (c < 4 ? ty * 4 + c : 64 + ty * 4 + c - 4);
+        if (n >= g.N) continue;
+#pragma unroll
+        for (int r = 0; r < OP_TM; ++r) {
+            const int64_t m = m0 + (r < 4 ? tx * 4 + r : 64 + tx * 4 + r - 4);
+            if (m < g.M) *(float *)(db + n * g.dnb1 + m * 4) = acc[r][c];
+        }
+    }
+}
+
+// ------------------------------------------------------------------ reductions of one CTA (CROSS_ENTROPY_LOSS, SUM, COUNT_EQUAL)
+// A block-wide sum of doubles / int64s in one fixed order: lane-strided butterflies, then the warp partials in warp order.  Every thread
+// gets the result.  blockDim is a multiple of 32.
+template <typename V> __device__ __forceinline__ V block_sum_fixed(V v, V * sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    __syncthreads();
+    if (lane == 0) sh[warp] = v;
+    __syncthreads();
+    V r = 0;
+    for (int w = 0; w < nw; ++w) r += sh[w];
+    return r;
+}
+
+// CROSS_ENTROPY_LOSS: warp w takes rows w, w + nw, ...; per row the max and the double sum of expf(x - max) by the warp, then the row's
+// value (b200_train.cuh, ce_term) summed in double across the lanes and rounded to f32 as ggml_vec_sum_f32 rounds it.  Each warp adds its
+// row values in double in row order, the warps' sums are added in warp order and the total is rounded once: a fixed order, no atomics.
+__global__ void __launch_bounds__(RED_THREADS) cross_entropy_loss_kernel(tdesc x, tdesc l, float * dst) {
+    pdl_trigger();
+    __shared__ double sh[RED_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int64_t nc = x.ne[0], nr = x.ne[1] * x.ne[2] * x.ne[3];
+    double wsum = 0.0;
+    for (int64_t r = warp; r < nr; r += nw) {
+        const int64_t i1 = r % x.ne[1], i2 = (r / x.ne[1]) % x.ne[2], i3 = r / (x.ne[1] * x.ne[2]);
+        const float * xr = (const float *)(x.data + i1 * x.nb[1] + i2 * x.nb[2] + i3 * x.nb[3]);
+        const float * lr = (const float *)(l.data + i1 * l.nb[1] + i2 * l.nb[2] + i3 * l.nb[3]);
+        float mx = -INFINITY;
+        for (int64_t i = lane; i < nc; i += 32) mx = fmaxf(mx, xr[i]);
+        mx = warp_max(mx);
+        double se = 0.0;
+        for (int64_t i = lane; i < nc; i += 32) se += (double)expf(pool_add(xr[i], -mx));
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+        const float neg_lse = -logf((float)se);
+        double rs = 0.0;
+        for (int64_t i = lane; i < nc; i += 32) rs += (double)ce_term(xr[i], mx, neg_lse, lr[i]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) rs += __shfl_xor_sync(0xffffffffu, rs, o);
+        wsum += (double)(float)rs;
+    }
+    const double total = block_sum_fixed(lane == 0 ? wsum : 0.0, sh);         // every lane holds its warp's sum: count it once
+    if (threadIdx.x == 0) *dst = pool_mul((float)total, -1.0f / (float)nr);
+}
+
+// SUM: each thread adds its elements (lane-strided along dim 0, rows in order) in double; the block adds the threads' sums in a fixed order
+// and rounds once, as ggml-cpu's one double accumulator rounds once.
+__global__ void __launch_bounds__(RED_THREADS) sum_kernel(tdesc s, float * dst) {
+    pdl_trigger();
+    __shared__ double sh[RED_THREADS / 32];
+    const int64_t ne0 = s.ne[0], nr = s.ne[1] * s.ne[2] * s.ne[3];
+    double acc = 0.0;
+    if (ne0 >= 32) {
+        for (int64_t r = threadIdx.x >> 5; r < nr; r += blockDim.x >> 5) {          // a warp per row
+            const int64_t i1 = r % s.ne[1], i2 = (r / s.ne[1]) % s.ne[2], i3 = r / (s.ne[1] * s.ne[2]);
+            const float * xr = (const float *)(s.data + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
+            for (int64_t i = threadIdx.x & 31; i < ne0; i += 32) acc += (double)xr[i];
+        }
+    } else {                                                                         // short rows: a thread per element
+        for (int64_t e = threadIdx.x; e < ne0 * nr; e += blockDim.x) {
+            const int64_t i0 = e % ne0, r = e / ne0, i1 = r % s.ne[1], i2 = (r / s.ne[1]) % s.ne[2], i3 = r / (s.ne[1] * s.ne[2]);
+            acc += (double)*(const float *)(s.data + i0 * 4 + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
+        }
+    }
+    const double total = block_sum_fixed(acc, sh);
+    if (threadIdx.x == 0) *dst = (float)total;
+}
+
+// COUNT_EQUAL (ne2 == ne3 == 1): the number of equal i32 pairs, counted per thread and added in a fixed order
+__global__ void __launch_bounds__(RED_THREADS) count_equal_kernel(tdesc a, tdesc b, int64_t * dst) {
+    pdl_trigger();
+    __shared__ long long sh[RED_THREADS / 32];
+    const int64_t ne0 = a.ne[0], n = ne0 * a.ne[1];
+    long long cnt = 0;
+    for (int64_t e = threadIdx.x; e < n; e += blockDim.x) {
+        const int64_t i0 = e % ne0, i1 = e / ne0;
+        cnt += *(const int32_t *)(a.data + i0 * a.nb[0] + i1 * a.nb[1]) == *(const int32_t *)(b.data + i0 * b.nb[0] + i1 * b.nb[1]);
+    }
+    const long long total = block_sum_fixed(cnt, sh);
+    if (threadIdx.x == 0) *dst = (int64_t)total;
+}
+
+// ------------------------------------------------------------------ CROSS_ENTROPY_LOSS_BACK (packed rows): one CTA per row
+// max, then s = the double sum of e = expf(x - max), inv = (float)(1.0 / s), and dst = (e inv - l) grad[0] / nr (b200_train.cuh).  grad is
+// read on the device.
+__global__ void cross_entropy_loss_back_kernel(const float * grad, const float * x, const float * l, float * dst, int64_t nc, int64_t nr) {
+    pdl_trigger();
+    __shared__ float shf[32];
+    __shared__ double shd[32];
+    const int64_t r = blockIdx.x;
+    const float * xr = x + r * nc, * lr = l + r * nc;
+    float * yr = dst + r * nc;
+    float mx = -INFINITY;
+    for (int64_t i = threadIdx.x; i < nc; i += blockDim.x) mx = fmaxf(mx, xr[i]);
+    mx = block_reduce<true>(mx, shf);
+    double se = 0.0;
+    for (int64_t i = threadIdx.x; i < nc; i += blockDim.x) se += (double)expf(pool_add(xr[i], -mx));
+    se = block_sum_fixed(se, shd);
+    const float inv = (float)(1.0 / se), d_by_nr = pool_div(*grad, (float)nr);
+    for (int64_t i = threadIdx.x; i < nc; i += blockDim.x) yr[i] = ce_back_value(expf(pool_add(xr[i], -mx)), inv, lr[i], d_by_nr);
+}
+
+// ------------------------------------------------------------------ OPT_STEP_ADAMW (packed, in place): one thread per element
+// The seven hyper-parameters are read from device memory by every thread: a captured graph replays with the values of its step.
+__global__ void opt_step_adamw_kernel(float * __restrict__ w, const float * __restrict__ g, float * __restrict__ m, float * __restrict__ v,
+                                      const float * __restrict__ params, int64_t n) {
+    pdl_trigger();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float p[ADAMW_NPARAMS];
+#pragma unroll
+    for (int j = 0; j < ADAMW_NPARAMS; ++j) p[j] = params[j];
+    float wi = w[i], mi = m[i], vi = v[i];
+    adamw_update(wi, g[i], mi, vi, p);
+    w[i] = wi; m[i] = mi; v[i] = vi;
+}
+
+// ------------------------------------------------------------------ ARGMAX (f32 rows -> i32): one CTA per row, the closed form of
+// b200_train.cuh in three block-wide passes: the last element that is not NaN, the last NaN before it, then the last-tie argmax between.
+__device__ __forceinline__ int32_t block_max_i32(int32_t v, int32_t * sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    __syncthreads();
+    if (lane == 0) sh[warp] = v;
+    __syncthreads();
+    int32_t r = -1;
+    for (int k = 0; k < nw; ++k) r = max(r, sh[k]);
+    return r;
+}
+
+__global__ void __launch_bounds__(256) argmax_kernel(const uint8_t * __restrict__ src, int64_t nb1, int32_t * __restrict__ dst, int64_t dnb0_words,
+                                                     int32_t ne0) {
+    pdl_trigger();
+    __shared__ int32_t shi[8];
+    __shared__ float shv[8];
+    const float * x = (const float *)(src + (int64_t)blockIdx.x * nb1);
+    int32_t last = -1;
+    for (int32_t i = threadIdx.x; i < ne0; i += blockDim.x) if (!isnan(x[i])) last = i;
+    last = block_max_i32(last, shi);
+    int32_t nan_before = -1;
+    for (int32_t i = threadIdx.x; i < last; i += blockDim.x) if (isnan(x[i])) nan_before = i;
+    nan_before = block_max_i32(nan_before, shi);
+    float bv = 0.0f;
+    int32_t bi = -1;
+    for (int32_t i = nan_before + 1 + threadIdx.x; i <= last; i += blockDim.x) if (argmax_beats(x[i], i, bv, bi)) { bv = x[i]; bi = i; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int32_t oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (argmax_beats(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    __syncthreads();
+    if (lane == 0) { shv[warp] = bv; shi[warp] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float rv = shv[0];
+        int32_t ri = shi[0];
+        for (int k = 1; k < nw; ++k) if (argmax_beats(shv[k], shi[k], rv, ri)) { rv = shv[k]; ri = shi[k]; }
+        dst[(int64_t)blockIdx.x * dnb0_words] = last < 0 ? 0 : ri;
+    }
+}
+
+// ------------------------------------------------------------------ REPEAT_BACK (f32): one thread per dst element, the repeats in
+// ggml-cpu's order (b200_train.cuh)
+__global__ void repeat_back_kernel(repeat_back_geom g, const uint8_t * __restrict__ src, uint8_t * __restrict__ dst, int64_t n) {
+    pdl_trigger();
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    float v;
+    const int64_t off = repeat_back_value(g, src, e, &v);
+    *(float *)(dst + off) = v;
+}
+
 // ------------------------------------------------------------------ ARGSORT (f32 rows of ne0 <= 1024 -> i32 indices, dst contiguous)
 // One CTA per row: the row's (key, index) items (b200_sort.cuh), padded to P = the next power of two, are sorted by the bitonic network in
 // shared memory, one compare-exchange per thread and step.  The order is a strict total order (ties by index, NaNs last), so each output
@@ -866,7 +1132,7 @@ int ggml_b200_op_diag_mask_inf(const float * src, float * dst, int64_t ne0, int6
 
 int ggml_b200_op_unary(int32_t uop, const float * src, float * dst, int64_t n, void * stream) {
     if (n <= 0) return GGML_B200_OK;
-    if (uop < 0 || uop > U_COS) { set_error("unary: bad op %d", uop); return GGML_B200_EINVAL; }
+    if (uop < 0 || uop > U_STEP) { set_error("unary: bad op %d", uop); return GGML_B200_EINVAL; }
     B200_CUDA_TRY(launch_pdl(unary_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, uop, src, dst, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
@@ -1171,6 +1437,87 @@ int ggml_b200_op_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_t
                                    const ggml_b200_tensor * s, const ggml_b200_tensor * dst, float scale, void * stream) {
     CHECK_ARGS(check_gated_linear_attn(k, v, q, g, s, dst));
     return launch_wkv<true>(k, v, q, g, nullptr, s, dst, scale, stream);
+}
+
+// ------------------------------------------------------------------ the ops of ggml_opt's backward and optimizer graphs
+int ggml_b200_op_out_prod(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_out_prod(src0, src1, dst));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    out_prod_geom g;
+    g.M = dst->ne[0]; g.N = dst->ne[1]; g.K = src0->ne[1];
+    g.ne2 = dst->ne[2]; g.dps2 = dst->ne[2] / src0->ne[2]; g.dps3 = dst->ne[3] / src0->ne[3];
+    g.anb1 = (int64_t)src0->nb[1]; g.anb2 = (int64_t)src0->nb[2]; g.anb3 = (int64_t)src0->nb[3];
+    g.bnb0 = (int64_t)src1->nb[0]; g.bnb1 = (int64_t)src1->nb[1]; g.bnb2 = (int64_t)src1->nb[2]; g.bnb3 = (int64_t)src1->nb[3];
+    g.dnb1 = (int64_t)dst->nb[1]; g.dnb2 = (int64_t)dst->nb[2]; g.dnb3 = (int64_t)dst->nb[3];
+    g.b_k_contig = src1->nb[0] != 4 && src1->nb[1] == 4;
+    const dim3 grid(blocks_for(g.M, OP_BM), blocks_for(g.N, OP_BN), (unsigned)(dst->ne[2] * dst->ne[3]));
+    B200_CUDA_TRY(launch_pdl(out_prod_kernel, grid, dim3(OP_THREADS), 0, (cudaStream_t)stream, g, (const uint8_t *)src0->data,
+                             (const uint8_t *)src1->data, (uint8_t *)dst->data));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_cross_entropy_loss(const ggml_b200_tensor * logits, const ggml_b200_tensor * labels, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_cross_entropy_loss(logits, labels, dst));
+    B200_CUDA_TRY(launch_pdl(cross_entropy_loss_kernel, dim3(1), dim3(RED_THREADS), 0, (cudaStream_t)stream, T(logits), T(labels), (float *)dst->data));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_cross_entropy_loss_back(const ggml_b200_tensor * grad, const ggml_b200_tensor * logits, const ggml_b200_tensor * labels,
+                                         const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_cross_entropy_loss_back(grad, logits, labels, dst));
+    if (nelem(*dst) == 0) return GGML_B200_OK;
+    const int64_t nc = dst->ne[0], nr = nrows(*dst);
+    const int threads = (int)std::min<int64_t>(1024, std::max<int64_t>(32, (nc + 31) / 32 * 32));
+    B200_CUDA_TRY(launch_pdl(cross_entropy_loss_back_kernel, dim3((unsigned)nr), dim3(threads), 0, (cudaStream_t)stream, (const float *)grad->data,
+                             (const float *)logits->data, (const float *)labels->data, (float *)dst->data, nc, nr));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_opt_step_adamw(const ggml_b200_tensor * w, const ggml_b200_tensor * g, const ggml_b200_tensor * m, const ggml_b200_tensor * v,
+                                const ggml_b200_tensor * params, void * stream) {
+    CHECK_ARGS(check_opt_step_adamw(w, g, m, v, params));
+    const int64_t n = nelem(*w);
+    if (n == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(opt_step_adamw_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (float *)w->data,
+                             (const float *)g->data, (float *)m->data, (float *)v->data, (const float *)params->data, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_argmax(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_argmax(src, dst));
+    if (src->ne[1] == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(argmax_kernel, dim3((unsigned)src->ne[1]), dim3(256), 0, (cudaStream_t)stream, (const uint8_t *)src->data,
+                             (int64_t)src->nb[1], (int32_t *)dst->data, (int64_t)(dst->nb[0] / 4), (int32_t)src->ne[0]));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_count_equal(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_count_equal(src0, src1, dst));
+    B200_CUDA_TRY(launch_pdl(count_equal_kernel, dim3(1), dim3(RED_THREADS), 0, (cudaStream_t)stream, T(src0), T(src1), (int64_t *)dst->data));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_sum(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_sum(src, dst));
+    B200_CUDA_TRY(launch_pdl(sum_kernel, dim3(1), dim3(RED_THREADS), 0, (cudaStream_t)stream, T(src), (float *)dst->data));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
+}
+
+int ggml_b200_op_repeat_back(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_repeat_back(src, dst));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(repeat_back_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, repeat_back_geometry(*src, *dst),
+                             (const uint8_t *)src->data, (uint8_t *)dst->data, n));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
 }
 
 } // extern "C"

@@ -62,6 +62,8 @@ enum ggml_b200_type {
     GGML_B200_TYPE_I32 = 26,
     /* the 2-byte element types GGML_OP_REPEAT moves besides f16 */
     GGML_B200_TYPE_I16 = 25, GGML_B200_TYPE_BF16 = 30,
+    /* GGML_OP_COUNT_EQUAL's scalar result */
+    GGML_B200_TYPE_I64 = 27,
 };
 
 /* ---------------------------------------------------------------------------------------------
@@ -222,7 +224,9 @@ enum ggml_b200_unary { GGML_B200_UNARY_GELU = 0, GGML_B200_UNARY_SILU = 1, GGML_
                        GGML_B200_UNARY_NEG = 4, GGML_B200_UNARY_ABS = 5, GGML_B200_UNARY_GELU_QUICK = 6, GGML_B200_UNARY_SIGMOID = 7,
                        GGML_B200_UNARY_EXP = 8, GGML_B200_UNARY_SQR = 9, GGML_B200_UNARY_SQRT = 10,
                        /* GGML_OP_SIN / GGML_OP_COS: sinf / cosf (within 2 ulp, not the fast intrinsics) */
-                       GGML_B200_UNARY_SIN = 11, GGML_B200_UNARY_COS = 12 };
+                       GGML_B200_UNARY_SIN = 11, GGML_B200_UNARY_COS = 12,
+                       /* GGML_UNARY_OP_STEP: x > 0 ? 1 : 0 (NaN gives 0); the gradient of RELU */
+                       GGML_B200_UNARY_STEP = 13 };
 
 GGML_B200_API int ggml_b200_op_get_rows(const ggml_b200_tensor * src0, const ggml_b200_tensor * ids, const ggml_b200_tensor * dst, void * stream);
 /* op: 0 add, 1 mul, 2 sub, 3 div; src1 broadcasts into dst's shape; dst may alias src0 */
@@ -362,6 +366,40 @@ GGML_B200_API int ggml_b200_op_add_rel_pos(const ggml_b200_tensor * src0, const 
  * GGML_B200_EUNSUPPORTED; stride < 1 or extents that disagree: GGML_B200_EINVAL. */
 GGML_B200_API int ggml_b200_op_conv_transpose_2d(const ggml_b200_tensor * kernel, const ggml_b200_tensor * input, const ggml_b200_tensor * dst,
                                                  int32_t stride, void * stream);
+
+/* The ops ggml_opt's backward and optimizer graphs add (ggml_build_backward_expand, ggml_opt_step_adamw), all f32 unless stated.
+ * GGML_OP_OUT_PROD (the gradient of MUL_MAT): src0 [ne0, K, ne02, ne03] contiguous along dim 0, src1 [ne1, K, ne2, ne3] with any strides
+ * (ggml_transpose(grad) is the common case) -> dst [ne0, ne1, ne2, ne3] packed; ne2 % ne02 == 0 and ne3 % ne03 == 0 (broadcast as MUL_MAT).
+ * dst[i0, i1] = sum over k of src0[i0, k] src1[i1, k], one fused multiply-add per term in ascending k from +0: the CPU backend's chain on
+ * the elements of its SIMD body (i0 below ne0 rounded down to 32), within NMSE 1e-12 elsewhere.  K = 0 gives zeros.  f16 or quantized
+ * src0: GGML_B200_EUNSUPPORTED. */
+GGML_B200_API int ggml_b200_op_out_prod(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_CROSS_ENTROPY_LOSS: logits and labels of one shape, rows contiguous along dim 0 -> dst, a scalar:
+ * -1/nr sum over rows and i of labels_i (x_i - max - log sum_j exp(x_j - max)), with the CPU backend's per-row rounding.  The rows are
+ * reduced in one fixed order (no atomics): passes repeat bit for bit. */
+GGML_B200_API int ggml_b200_op_cross_entropy_loss(const ggml_b200_tensor * logits, const ggml_b200_tensor * labels, const ggml_b200_tensor * dst,
+                                                  void * stream);
+/* GGML_OP_CROSS_ENTROPY_LOSS_BACK: grad a scalar (read on the device), logits, labels and dst of one shape, all packed:
+ * dst = (softmax(logits) - labels) grad[0] / nr, row by row. */
+GGML_B200_API int ggml_b200_op_cross_entropy_loss_back(const ggml_b200_tensor * grad, const ggml_b200_tensor * logits, const ggml_b200_tensor * labels,
+                                                       const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_OPT_STEP_ADAMW, in place: w (the node's dst, a view of the weight), its gradient g and moments m and v, all of one shape and
+ * packed; params f32 [7] = alpha, beta1, beta2, eps, wd, beta1h, beta2h, read on the device by every launch (a replayed CUDA graph sees
+ * the values of the step it replays).  w, m and v are updated with the CPU backend's expressions in its order: bit-identical. */
+GGML_B200_API int ggml_b200_op_opt_step_adamw(const ggml_b200_tensor * w, const ggml_b200_tensor * g, const ggml_b200_tensor * m, const ggml_b200_tensor * v,
+                                              const ggml_b200_tensor * params, void * stream);
+/* GGML_OP_ARGMAX: src [ne0, ne1] (rows contiguous along dim 0) -> dst i32 [ne1] (dim 0 contiguous): the CPU backend's rule (the last index
+ * of the maximum; a NaN restarts the search after it; a trailing run of NaNs is ignored; all NaN gives 0).  Exact. */
+GGML_B200_API int ggml_b200_op_argmax(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_COUNT_EQUAL: src0 and src1 i32 of one shape [ne0, ne1, 1, 1] (any strides) -> dst i64 scalar, the number of equal pairs.  Exact.
+ * ne2 or ne3 > 1: GGML_B200_EUNSUPPORTED (the CPU backend's row walk reads other rows then). */
+GGML_B200_API int ggml_b200_op_count_equal(const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_SUM: src (contiguous along dim 0, any other strides) -> dst a scalar: the sum in double, rounded once, in one fixed order. */
+GGML_B200_API int ggml_b200_op_sum(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* GGML_OP_REPEAT_BACK: src -> dst, both contiguous along dim 0 (any other strides), every src extent a whole multiple of dst's:
+ * dst (k) = the sum over the repeats of src into dst's shape, added in the CPU backend's loop order: bit-identical.  Other types than f32:
+ * GGML_B200_EUNSUPPORTED. */
+GGML_B200_API int ggml_b200_op_repeat_back(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Introspection
