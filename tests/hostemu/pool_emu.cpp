@@ -1,19 +1,15 @@
 // pool_emu.cpp — TEST INFRASTRUCTURE ONLY: ggml_b200/csrc/b200_pool.cuh (the per-element logic of POOL_2D, UPSCALE, LEAKY_RELU and REPEAT)
 // compiled for the host through tests/hostemu/shim and driven the way ops.cu's pool2d_kernel / upscale_kernel / leaky_relu_kernel /
-// repeat_kernel drive it (one dst element at a time, in dst's order, with the launchers' arguments), plus the four checks of
-// b200_op_checks.h, exported with a C ABI for tests/test_hostemu_pool.py.
+// repeat_kernel drive it (one dst element at a time, in dst's order, with the launchers' arguments), exported with a C ABI for
+// tests/test_hostemu_pool.py.
 #define B200_HOST_EMU 1
 #include "cuda_shim.h"
 #include "../../ggml_b200/csrc/b200_pool.cuh"
-#include "../../ggml_b200/csrc/b200_op_checks.h"
+#include "check_code.h"
 
 #include <cstring>
 
 using namespace b200;
-
-namespace {
-int code(const op_check & r) { return r.ok() || r.reason ? r.code : 1; }       // 1: a refusal without a reason
-}
 
 extern "C" {
 
@@ -66,11 +62,5 @@ int emu_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
     }
     return 0;
 }
-
-// the checks alone (no data is touched)
-int emu_check_pool_2d(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, const ggml_b200_pool_params * params) { return code(check_pool_2d(src, dst, params)); }
-int emu_check_upscale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) { return code(check_upscale(src, dst)); }
-int emu_check_leaky_relu(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) { return code(check_leaky_relu(src, dst)); }
-int emu_check_repeat(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) { return code(check_repeat(src, dst)); }
 
 } // extern "C"

@@ -1,19 +1,14 @@
 // sam_emu.cpp — TEST INFRASTRUCTURE ONLY: ggml_b200/csrc/b200_sam.cuh (the per-row / per-element logic of WIN_PART, WIN_UNPART, GET_REL_POS,
 // ADD_REL_POS and CONV_TRANSPOSE_2D) compiled for the host through tests/hostemu/shim and driven the way ops.cu's kernels drive it (one dst row
-// or element at a time, with the launchers' arguments), plus the five checks of b200_op_checks.h, exported with a C ABI for
-// tests/test_hostemu_sam.py.
+// or element at a time, with the launchers' arguments), exported with a C ABI for tests/test_hostemu_sam.py.
 #define B200_HOST_EMU 1
 #include "cuda_shim.h"
 #include "../../ggml_b200/csrc/b200_sam.cuh"
-#include "../../ggml_b200/csrc/b200_op_checks.h"
+#include "check_code.h"
 
 #include <cstring>
 
 using namespace b200;
-
-namespace {
-int code(const op_check & r) { return r.ok() || r.reason ? r.code : 1; }       // 1: a refusal without a reason
-}
 
 extern "C" {
 
@@ -81,17 +76,6 @@ int emu_conv_transpose_2d(const ggml_b200_tensor * kernel, const ggml_b200_tenso
             for (int32_t ox = 0; ox < g.OW; ++ox)
                 d[((int64_t)co * g.OH + oy) * g.OW + ox] = ct2d_value(g, (const uint8_t *)kernel->data, (const uint8_t *)input->data, ox, oy, co);
     return 0;
-}
-
-// the checks alone (no data is touched)
-int emu_check_win_part(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t npx, int32_t npy, int32_t w) { return code(check_win_part(src, dst, npx, npy, w)); }
-int emu_check_win_unpart(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t w) { return code(check_win_unpart(src, dst, w)); }
-int emu_check_get_rel_pos(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) { return code(check_get_rel_pos(src, dst)); }
-int emu_check_add_rel_pos(const ggml_b200_tensor * src0, const ggml_b200_tensor * pw, const ggml_b200_tensor * ph, const ggml_b200_tensor * dst) {
-    return code(check_add_rel_pos(src0, pw, ph, dst));
-}
-int emu_check_conv_transpose_2d(const ggml_b200_tensor * kernel, const ggml_b200_tensor * input, const ggml_b200_tensor * dst, int32_t stride) {
-    return code(check_conv_transpose_2d(kernel, input, dst, stride));
 }
 
 } // extern "C"

@@ -1,16 +1,12 @@
 // train_emu.cpp — TEST INFRASTRUCTURE ONLY: ggml_b200/csrc/b200_train.cuh (the per-element logic of OUT_PROD, OPT_STEP_ADAMW, ARGMAX,
 // REPEAT_BACK, STEP and the cross-entropy pair) compiled for the host through tests/hostemu/shim and driven the way ops.cu's kernels drive it,
-// plus the eight checks of b200_op_checks.h, exported with a C ABI for tests/test_hostemu_train.py.
+// exported with a C ABI for tests/test_hostemu_train.py.
 #define B200_HOST_EMU 1
 #include "cuda_shim.h"
 #include "../../ggml_b200/csrc/b200_train.cuh"
-#include "../../ggml_b200/csrc/b200_op_checks.h"
+#include "check_code.h"
 
 using namespace b200;
-
-namespace {
-int code(const op_check & r) { return r.ok() || r.reason ? r.code : 1; }       // 1: a refusal without a reason
-}
 
 extern "C" {
 
@@ -57,21 +53,5 @@ int emu_repeat_back(const ggml_b200_tensor * s, const ggml_b200_tensor * d) {
 }
 
 void emu_step(const float * x, float * y, int64_t n) { for (int64_t i = 0; i < n; ++i) y[i] = step_value(x[i]); }
-
-int emu_check_out_prod(const ggml_b200_tensor * a, const ggml_b200_tensor * b, const ggml_b200_tensor * d) { return code(check_out_prod(a, b, d)); }
-int emu_check_cross_entropy_loss(const ggml_b200_tensor * x, const ggml_b200_tensor * l, const ggml_b200_tensor * d) {
-    return code(check_cross_entropy_loss(x, l, d));
-}
-int emu_check_cross_entropy_loss_back(const ggml_b200_tensor * g, const ggml_b200_tensor * x, const ggml_b200_tensor * l, const ggml_b200_tensor * d) {
-    return code(check_cross_entropy_loss_back(g, x, l, d));
-}
-int emu_check_opt_step_adamw(const ggml_b200_tensor * w, const ggml_b200_tensor * g, const ggml_b200_tensor * m, const ggml_b200_tensor * v,
-                             const ggml_b200_tensor * p) {
-    return code(check_opt_step_adamw(w, g, m, v, p));
-}
-int emu_check_argmax(const ggml_b200_tensor * s, const ggml_b200_tensor * d) { return code(check_argmax(s, d)); }
-int emu_check_count_equal(const ggml_b200_tensor * a, const ggml_b200_tensor * b, const ggml_b200_tensor * d) { return code(check_count_equal(a, b, d)); }
-int emu_check_sum(const ggml_b200_tensor * s, const ggml_b200_tensor * d) { return code(check_sum(s, d)); }
-int emu_check_repeat_back(const ggml_b200_tensor * s, const ggml_b200_tensor * d) { return code(check_repeat_back(s, d)); }
 
 } // extern "C"

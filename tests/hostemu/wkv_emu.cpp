@@ -1,11 +1,9 @@
 // wkv_emu.cpp — TEST INFRASTRUCTURE ONLY: ggml_b200/csrc/b200_wkv.cuh (the per-element math of RWKV_WKV6 and GATED_LINEAR_ATTN) compiled
 // for the host through tests/hostemu/shim and driven the way ops.cu's wkv_kernel drives it (per sequence, head and column, the sequence's
-// tokens in order, q * scale rounded once per token and row), plus the two acceptance rules of b200_op_checks.h, exported with a C ABI for
-// tests/test_hostemu_wkv.py.
+// tokens in order, q * scale rounded once per token and row), exported with a C ABI for tests/test_hostemu_wkv.py.
 #define B200_HOST_EMU 1
 #include "cuda_shim.h"
 #include "../../ggml_b200/csrc/b200_wkv.cuh"
-#include "../../ggml_b200/csrc/b200_op_checks.h"
 
 #include <vector>
 
@@ -33,8 +31,6 @@ void emu_wkv(bool gla, const float * k, const float * v, const float * a, const 
         }
 }
 
-int code(const op_check & r) { return r.ok() || r.reason ? r.code : 1; }
-
 } // namespace
 
 extern "C" {
@@ -47,15 +43,6 @@ void emu_rwkv_wkv6(const float * k, const float * v, const float * r, const floa
 void emu_gated_linear_attn(const float * k, const float * v, const float * q, const float * g, const float * s0, float * dst,
                            int64_t S, int64_t H, int64_t T, int64_t n_seqs, float scale) {
     emu_wkv(true, k, v, q, nullptr, g, s0, dst, S, H, T, n_seqs, scale);
-}
-
-int emu_check_rwkv_wkv6(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * r, const ggml_b200_tensor * tf,
-                        const ggml_b200_tensor * td, const ggml_b200_tensor * s, const ggml_b200_tensor * d) {
-    return code(check_rwkv_wkv6(k, v, r, tf, td, s, d));
-}
-int emu_check_gated_linear_attn(const ggml_b200_tensor * k, const ggml_b200_tensor * v, const ggml_b200_tensor * q, const ggml_b200_tensor * g,
-                                const ggml_b200_tensor * s, const ggml_b200_tensor * d) {
-    return code(check_gated_linear_attn(k, v, q, g, s, d));
 }
 
 } // extern "C"

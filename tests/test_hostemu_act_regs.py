@@ -3,30 +3,17 @@ of an activation task in registers, lane pairs combine their integer sums, the t
 8, 4, 2 with the rows exchanged at the first step), emulated in one warp on the host (tests/hostemu/areg_emu.cpp) and compared bit for bit
 with the task-per-lane consume it replaces."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+from hostemu.emu import load
 from oracle import oracle as O
-
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libareg_emu.so"
-    srcs = [EMU / "areg_emu.cpp", EMU / "shim" / "cuda_shim.h"] + [ROOT / "ggml_b200" / "csrc" / f for f in ("b200_quants.cuh", "b200_sb_tasks.cuh")]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable", "-Wno-unknown-pragmas",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "areg_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("areg_emu")
     L.emu_sb_areg_rows.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     return L
 

@@ -8,55 +8,33 @@ packed), values that round to fp16 ties, subnormals and infinity, and the Whispe
 check_im2col (b200_op_checks.h), which both ggml_b200_op_im2col and the plug-in's supports_op apply, is pinned here too, with the f16 x f16
 form of check_mul_mat_f."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import ggml_b200 as g
+from hostemu.emu import EINVAL, EUNSUPPORTED, OK, desc, load
 from oracle import conv as V
 
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
-OK, EUNSUPPORTED, EINVAL = 0, -1, -2
 F32, F16 = 0, 1
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libconv_emu.so"
-    srcs = [EMU / "conv_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_conv.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h", ROOT / "include" / "ggml-b200.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "conv_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
-    for fn in (L.emu_im2col, L.emu_check_im2col):
-        fn.restype = C.c_int
-        fn.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.POINTER(g.Im2colParams)]
-    L.emu_check_mul_mat_f.restype = C.c_int
-    L.emu_check_mul_mat_f.argtypes = [C.POINTER(g.TensorDesc)] * 3
+    L = load("conv_emu")
+    L.emu_im2col.restype = C.c_int
+    L.emu_im2col.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.POINTER(g.Im2colParams)]
     return L
 
 
-def desc(type_, ne, nb=None, data=4096):
-    """a ggml tensor descriptor: ne in ggml order, nb in bytes (packed when None)"""
-    d = g.TensorDesc()
-    d.data, d.type = data, type_
-    es = 4 if type_ == F32 else 2
-    ne = list(ne) + [1] * (4 - len(ne))
-    if nb is None:
-        nb = [es]
-        for i in range(1, 4):
-            nb.append(nb[-1] * ne[i - 1])
-    for i in range(4):
-        d.ne[i], d.nb[i] = ne[i], nb[i]
-    return d
+@pytest.fixture(scope="module")
+def checks():
+    L = load("op_checks_emu")
+    L.emu_check_im2col.restype = C.c_int
+    L.emu_check_im2col.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.POINTER(g.Im2colParams)]
+    L.emu_check_mul_mat_f.restype = C.c_int
+    L.emu_check_mul_mat_f.argtypes = [C.POINTER(g.TensorDesc)] * 3
+    return L
 
 
 def params(case: V.Im2colCase) -> g.Im2colParams:
@@ -93,10 +71,10 @@ def test_host_compiled_im2col_is_bit_identical_to_ggml_cpu(case, emu, ref):
     assert got.shape == want.shape and np.array_equal(got.view(u), want.view(u)), (str(case), int((got.view(u) != want.view(u)).sum()))
 
 
-def test_check_im2col_codes(emu):
+def test_check_im2col_codes(checks):
     def chk(k, x, d, p):
-        return emu.emu_check_im2col(C.byref(k), C.byref(x), C.byref(d), C.byref(p)) if k is not None else \
-            emu.emu_check_im2col(None, C.byref(x), C.byref(d), C.byref(p))
+        return checks.emu_check_im2col(C.byref(k), C.byref(x), C.byref(d), C.byref(p)) if k is not None else \
+            checks.emu_check_im2col(None, C.byref(x), C.byref(d), C.byref(p))
     P = lambda s0=1, s1=0, p0=1, p1=0, d0=1, d1=0, two=0: g.Im2colParams(s0, s1, p0, p1, d0, d1, two)
     k, x = desc(F16, (3, 4, 6)), desc(F32, (17, 4, 2))
     d16, d32 = desc(F16, (12, 17, 2)), desc(F32, (12, 17, 2))
@@ -133,8 +111,8 @@ def test_check_im2col_codes(emu):
     assert chk(k2, desc(F32, (11, 9, 3, 2), (4, 60, 600, 1800)), desc(F32, (18, 9, 8, 2)), P2()) == OK                    # rows spread
 
 
-def test_check_mul_mat_f_takes_f16_src1_with_f16_src0_only(emu):
-    chk = lambda a, b, d: emu.emu_check_mul_mat_f(C.byref(a), C.byref(b), C.byref(d))
+def test_check_mul_mat_f_takes_f16_src1_with_f16_src0_only(checks):
+    chk = lambda a, b, d: checks.emu_check_mul_mat_f(C.byref(a), C.byref(b), C.byref(d))
     assert chk(desc(F16, (64, 16)), desc(F16, (64, 9)), desc(F32, (16, 9))) == OK
     assert chk(desc(F16, (64, 16)), desc(F32, (64, 9)), desc(F32, (16, 9))) == OK
     assert chk(desc(F32, (64, 16)), desc(F16, (64, 9)), desc(F32, (16, 9))) == EUNSUPPORTED

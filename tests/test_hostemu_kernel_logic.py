@@ -3,30 +3,20 @@ ggml_b200/csrc/b200_quants.cuh / b200_dequant.cuh) compiled for the HOST through
 Catches indexing / bit-twiddling mistakes in a block format without a GPU; the `-m gpu` parity tests remain the gate for the
 kernels themselves (scheduling, memory movement, PTX-level instructions)."""
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 import pytest
 
+from hostemu.emu import load
 from oracle import oracle as O
 
 ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libhostemu.so"
-    srcs = [EMU / "hostemu.cpp", EMU / "shim" / "cuda_shim.h"] + [ROOT / "ggml_b200" / "csrc" / f for f in ("b200_quants.cuh", "b200_dequant.cuh", "b200_sb_tasks.cuh", "b200_tc_dequant.cuh", "b200_iq.cuh", "b200_sb_mma.cuh", "generated/iq_grids.h")]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable", "-Wno-unknown-pragmas",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "hostemu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("hostemu")
     L.emu_row_dot.restype = C.c_float
     L.emu_row_dot.argtypes = [C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     L.emu_dequant.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64]

@@ -9,61 +9,36 @@ against the reference's own ggml-cpu ops, one-node graphs through oracle/pool_pr
 The EUNSUPPORTED / EINVAL codes of check_pool_2d, check_upscale, check_leaky_relu and check_repeat (b200_op_checks.h), which the C ABI
 launchers and the plug-in's supports_op apply, are pinned here too."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import ggml_b200 as g
+from hostemu.emu import EINVAL, EUNSUPPORTED, OK, bits, desc, load, view_desc
 from oracle import pool as P
 
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
-OK, EUNSUPPORTED, EINVAL = 0, -1, -2
 F32, F16, I16, I32, BF16 = P.F32, P.F16, P.I16, P.I32, P.BF16
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libpool_emu.so"
-    srcs = [EMU / "pool_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_pool.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h", ROOT / "include" / "ggml-b200.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "pool_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("pool_emu")
     TD = C.POINTER(g.TensorDesc)
-    for fn in (L.emu_pool_2d, L.emu_check_pool_2d):
-        fn.restype, fn.argtypes = C.c_int, [TD, TD, C.POINTER(g.PoolParams)]
-    for fn in (L.emu_upscale, L.emu_check_upscale, L.emu_repeat, L.emu_check_repeat, L.emu_check_leaky_relu):
+    L.emu_pool_2d.restype, L.emu_pool_2d.argtypes = C.c_int, [TD, TD, C.POINTER(g.PoolParams)]
+    for fn in (L.emu_upscale, L.emu_repeat):
         fn.restype, fn.argtypes = C.c_int, [TD, TD]
     L.emu_leaky_relu.restype, L.emu_leaky_relu.argtypes = C.c_int, [TD, TD, C.c_float]
     return L
 
 
-def desc(type_, ne, nb=None, data=4096):
-    """a ggml tensor descriptor: ne in ggml order, nb in bytes (packed when None)"""
-    d = g.TensorDesc()
-    d.data, d.type = data, type_
-    ne = tuple(ne) + (1,) * (4 - len(ne))
-    nb = nb or P.packed_nb(ne, P.ES[type_])
-    for i in range(4):
-        d.ne[i], d.nb[i] = ne[i], nb[i]
-    return d
-
-
-def src_desc(src: P.Source, parent: np.ndarray):
-    ne, nb = src.view()
-    return desc(src.type, ne, nb, parent.ctypes.data + src.offs)
-
-
-def bits(a):
-    return a.view(np.uint32 if a.itemsize == 4 else np.uint16)
+@pytest.fixture(scope="module")
+def checks():
+    L = load("op_checks_emu")
+    TD = C.POINTER(g.TensorDesc)
+    L.emu_check_pool_2d.restype, L.emu_check_pool_2d.argtypes = C.c_int, [TD, TD, C.POINTER(g.PoolParams)]
+    for fn in (L.emu_check_upscale, L.emu_check_repeat, L.emu_check_leaky_relu):
+        fn.restype, fn.argtypes = C.c_int, [TD, TD]
+    return L
 
 
 def nan_equal(got, want):
@@ -90,7 +65,7 @@ def test_host_compiled_pool_2d_is_bit_identical_to_ggml_cpu(case, emu, ref):
     parent = case.src.parent()
     got = np.zeros(case.ne_dst[::-1], dtype=np.float32)
     p = g.PoolParams(*case.params)
-    assert emu.emu_pool_2d(C.byref(src_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), C.byref(p)) == OK
+    assert emu.emu_pool_2d(C.byref(view_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), C.byref(p)) == OK
     want = P.pool_2d("CPU", case, parent)
     assert nan_equal(got, want), (str(case), int((bits(got) != bits(want)).sum()))
     if case.op == P.POOL_MAX:                                  # MAX moves input values: no arithmetic, no NaN result, every bit equal
@@ -114,7 +89,7 @@ def test_pool_2d_corner_semantics(emu, ref):
 def test_host_compiled_upscale_is_bit_identical_to_ggml_cpu(case, emu, ref):
     parent = case.src.parent()
     got = np.zeros(tuple(case.ne_dst)[::-1], dtype=np.float32)
-    assert emu.emu_upscale(C.byref(src_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data))) == OK
+    assert emu.emu_upscale(C.byref(view_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data))) == OK
     want = P.upscale("CPU", case, parent)
     assert np.array_equal(bits(got), bits(want)), str(case)
 
@@ -126,12 +101,12 @@ def test_host_compiled_leaky_relu_is_bit_identical_to_ggml_cpu(case, emu, ref):
     ne, nb = case.src.view()
     if case.inplace:
         work = parent.copy()
-        s = src_desc(case.src, work)
+        s = view_desc(case.src, work)
         assert emu.emu_leaky_relu(C.byref(s), C.byref(s), case.slope) == OK
         got = work.reshape(-1)[: want.size]
     else:
         got = np.zeros(ne[::-1], dtype=np.float32)
-        assert emu.emu_leaky_relu(C.byref(src_desc(case.src, parent)), C.byref(desc(F32, ne, data=got.ctypes.data)), case.slope) == OK
+        assert emu.emu_leaky_relu(C.byref(view_desc(case.src, parent)), C.byref(desc(F32, ne, data=got.ctypes.data)), case.slope) == OK
     assert nan_equal(got, want), str(case)
     ne, nb = case.src.view()
     x = np.lib.stride_tricks.as_strided(parent.reshape(-1)[case.src.offs // 4:], ne[::-1], nb[::-1])
@@ -145,16 +120,16 @@ def test_host_compiled_leaky_relu_is_bit_identical_to_ggml_cpu(case, emu, ref):
 def test_host_compiled_repeat_is_bit_identical_to_ggml_cpu(case, emu, ref):
     parent = case.src.parent()
     got = np.zeros(tuple(case.ne_dst)[::-1], dtype=np.uint32 if P.ES[case.src.type] == 4 else np.uint16)
-    assert emu.emu_repeat(C.byref(src_desc(case.src, parent)), C.byref(desc(case.src.type, case.ne_dst, data=got.ctypes.data))) == OK
+    assert emu.emu_repeat(C.byref(view_desc(case.src, parent)), C.byref(desc(case.src.type, case.ne_dst, data=got.ctypes.data))) == OK
     want = P.repeat("CPU", case, parent)
     assert np.array_equal(got, want.view(got.dtype)), str(case)
 
 
 # ------------------------------------------------------------------ the checks' codes
-def test_check_pool_2d_codes(emu):
+def test_check_pool_2d_codes(checks):
     def chk(s, d, *params):
         p = g.PoolParams(*params)
-        return emu.emu_check_pool_2d(C.byref(s) if s else None, C.byref(d), C.byref(p))
+        return checks.emu_check_pool_2d(C.byref(s) if s else None, C.byref(d), C.byref(p))
     x, y = desc(F32, (13, 13, 16, 2)), desc(F32, (6, 6, 16, 2))
     assert chk(x, y, 0, 2, 2, 2, 2, 0, 0) == OK and chk(x, y, 1, 2, 2, 2, 2, 0, 0) == OK
     assert chk(x, y, 2, 2, 2, 2, 2, 0, 0) == EINVAL                                   # POOL_COUNT: ggml-cpu aborts
@@ -173,8 +148,8 @@ def test_check_pool_2d_codes(emu):
     assert chk(desc(F32, (13, 13, 0, 2)), desc(F32, (6, 6, 0, 2)), 0, 2, 2, 2, 2, 0, 0) == OK             # empty
 
 
-def test_check_upscale_codes(emu):
-    chk = lambda s, d: emu.emu_check_upscale(C.byref(s) if s else None, C.byref(d))
+def test_check_upscale_codes(checks):
+    chk = lambda s, d: checks.emu_check_upscale(C.byref(s) if s else None, C.byref(d))
     x = desc(F32, (13, 13, 128, 1))
     assert chk(x, desc(F32, (26, 26, 128, 1))) == OK and chk(x, desc(F32, (13, 13, 128, 1))) == OK
     assert chk(desc(F32, (2, 5, 7, 11)), desc(F32, (5, 7, 11, 13))) == OK                 # fractional factors
@@ -186,8 +161,8 @@ def test_check_upscale_codes(emu):
     assert chk(None, desc(F32, (26, 26, 128, 1))) == EUNSUPPORTED
 
 
-def test_check_leaky_relu_codes(emu):
-    chk = lambda s, d: emu.emu_check_leaky_relu(C.byref(s) if s else None, C.byref(d))
+def test_check_leaky_relu_codes(checks):
+    chk = lambda s, d: checks.emu_check_leaky_relu(C.byref(s) if s else None, C.byref(d))
     x = desc(F32, (10, 5, 4, 3))
     assert chk(x, x) == OK and chk(x, desc(F32, (10, 5, 4, 3))) == OK
     assert chk(x, desc(F32, (10, 5, 4, 2))) == EINVAL                                     # shapes differ
@@ -198,8 +173,8 @@ def test_check_leaky_relu_codes(emu):
     assert chk(None, x) == EUNSUPPORTED
 
 
-def test_check_repeat_codes(emu):
-    chk = lambda s, d: emu.emu_check_repeat(C.byref(s) if s else None, C.byref(d))
+def test_check_repeat_codes(checks):
+    chk = lambda s, d: checks.emu_check_repeat(C.byref(s) if s else None, C.byref(d))
     for t in (F32, I32, F16, BF16, I16):
         assert chk(desc(t, (1, 1, 16, 1)), desc(t, (13, 13, 16, 2))) == OK
     assert chk(desc(8, (32, 1), (34, 34, 34, 34)), desc(8, (32, 4), (34, 34, 136, 136))) == EUNSUPPORTED                         # Q8_0: ggml-cpu aborts

@@ -4,33 +4,19 @@ graphs through oracle/rope_probe.cpp.  Covers the four modes (NORM, NEOX, MROPE,
 YaRN, freq_scale, positions up to 4095, strided views and the in-place form: pair-index, section and tail mistakes show up here without
 a device.  The constants are derived by ggml_b200.rope_params, the Python mirror of what the plug-in passes to the kernel."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import ggml_b200 as g
+from hostemu.emu import load
 from oracle import oracle as O
 from oracle import rope as R
-
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "librope_emu.so"
-    srcs = [EMU / "rope_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_rope.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "rope_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("rope_emu")
     L.emu_rope.restype = C.c_int
     L.emu_rope.argtypes = [C.c_int] + [C.c_void_p] * 8
     return L

@@ -12,69 +12,38 @@ and checked against the reference's own ggml-cpu ops, one-node graphs through or
 The EUNSUPPORTED / EINVAL codes of the five checks (b200_op_checks.h), which the C ABI launchers and the plug-in's supports_op apply, are
 pinned here too."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import ggml_b200 as g
+from hostemu.emu import EINVAL, EUNSUPPORTED, OK, bits, desc, load, view_desc
 from oracle import oracle as O
 from oracle import pool as P
 from oracle import sam as S
 
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
-OK, EUNSUPPORTED, EINVAL = 0, -1, -2
 F32, F16, BF16 = P.F32, P.F16, P.BF16
 CONV_NMSE = 1e-10
 
 
-@pytest.fixture(scope="module")
-def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libsam_emu.so"
-    srcs = [EMU / "sam_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_sam.cuh", ROOT / "ggml_b200" / "csrc" / "b200_pool.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h", ROOT / "include" / "ggml-b200.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "sam_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+def signatures(L, prefix):
+    """the ctypes signatures of the five ops' entries <prefix><op>: the emus (emu_) and their checks (emu_check_) take the same arguments"""
     TD = C.POINTER(g.TensorDesc)
-    for fn in (L.emu_win_part, L.emu_check_win_part):
-        fn.restype, fn.argtypes = C.c_int, [TD, TD, C.c_int32, C.c_int32, C.c_int32]
-    for fn in (L.emu_win_unpart, L.emu_check_win_unpart):
-        fn.restype, fn.argtypes = C.c_int, [TD, TD, C.c_int32]
-    for fn in (L.emu_get_rel_pos, L.emu_check_get_rel_pos):
-        fn.restype, fn.argtypes = C.c_int, [TD, TD]
-    for fn in (L.emu_add_rel_pos, L.emu_check_add_rel_pos):
-        fn.restype, fn.argtypes = C.c_int, [TD] * 4
-    for fn in (L.emu_conv_transpose_2d, L.emu_check_conv_transpose_2d):
-        fn.restype, fn.argtypes = C.c_int, [TD] * 3 + [C.c_int32]
+    for op, args in (("win_part", [TD, TD, C.c_int32, C.c_int32, C.c_int32]), ("win_unpart", [TD, TD, C.c_int32]), ("get_rel_pos", [TD, TD]),
+                     ("add_rel_pos", [TD] * 4), ("conv_transpose_2d", [TD] * 3 + [C.c_int32])):
+        fn = getattr(L, prefix + op)
+        fn.restype, fn.argtypes = C.c_int, args
     return L
 
 
-def desc(type_, ne, nb=None, data=4096):
-    """a ggml tensor descriptor: ne in ggml order, nb in bytes (packed when None)"""
-    d = g.TensorDesc()
-    d.data, d.type = data, type_
-    ne = tuple(ne) + (1,) * (4 - len(ne))
-    nb = nb or P.packed_nb(ne, P.ES[type_])
-    for i in range(4):
-        d.ne[i], d.nb[i] = ne[i], nb[i]
-    return d
+@pytest.fixture(scope="module")
+def emu():
+    return signatures(load("sam_emu"), "emu_")
 
 
-def src_desc(src: P.Source, parent: np.ndarray):
-    ne, nb = src.view()
-    return desc(src.type, ne, nb, parent.ctypes.data + src.offs)
-
-
-def bits(a):
-    return a.view(np.uint32 if a.itemsize == 4 else np.uint16)
+@pytest.fixture(scope="module")
+def checks():
+    return signatures(load("op_checks_emu"), "emu_check_")
 
 
 WIN_PARTS, WIN_UNPARTS, RELPOS, ADDS, CONVS = S.win_part_grid(), S.win_unpart_grid(), S.rel_pos_grid(), S.add_rel_pos_grid(), S.conv_transpose_grid()
@@ -96,7 +65,7 @@ def test_host_compiled_win_part_is_bit_identical_to_ggml_cpu(case, emu, ref):
     parent = case.src.parent()
     got = np.full(case.ne_dst[::-1], 0xdeadbeef, dtype=np.uint32)
     npx, npy = S.cdiv(case.src.ne[1], case.w), S.cdiv(case.src.ne[2], case.w)
-    assert emu.emu_win_part(C.byref(src_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), npx, npy, case.w) == OK
+    assert emu.emu_win_part(C.byref(view_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), npx, npy, case.w) == OK
     want = S.win_part("CPU", case, parent)
     assert np.array_equal(got, want), str(case)
     assert np.isnan(parent).any() and (want == 0x80000000).any()              # NaN and -0 words among the moved ones
@@ -106,7 +75,7 @@ def test_host_compiled_win_part_is_bit_identical_to_ggml_cpu(case, emu, ref):
 def test_host_compiled_win_unpart_is_bit_identical_to_ggml_cpu(case, emu, ref):
     parent = case.src.parent()
     got = np.full(case.ne_dst[::-1], 0xdeadbeef, dtype=np.uint32)
-    assert emu.emu_win_unpart(C.byref(src_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), case.w) == OK
+    assert emu.emu_win_unpart(C.byref(view_desc(case.src, parent)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), case.w) == OK
     assert np.array_equal(got, S.win_unpart("CPU", case, parent)), str(case)
 
 
@@ -122,7 +91,7 @@ def test_win_unpart_inverts_win_part(ref):
 def test_host_compiled_get_rel_pos_is_bit_identical_to_ggml_cpu(case, emu, ref):
     parent = case.src.parent()
     got = np.full(case.ne_dst[::-1], 0xdead, dtype=np.uint16)
-    assert emu.emu_get_rel_pos(C.byref(src_desc(case.src, parent)), C.byref(desc(F16, case.ne_dst, data=got.ctypes.data))) == OK
+    assert emu.emu_get_rel_pos(C.byref(view_desc(case.src, parent)), C.byref(desc(F16, case.ne_dst, data=got.ctypes.data))) == OK
     want = S.get_rel_pos("CPU", case, parent)
     assert np.array_equal(got, want), str(case)
     w, rows = case.w, parent.reshape(2 * case.w - 1, -1)
@@ -136,11 +105,11 @@ def test_host_compiled_add_rel_pos_is_bit_identical_to_ggml_cpu(case, emu, ref):
     sa, sw, sh = case.sources()
     if case.inplace:
         got = a.copy()
-        d = src_desc(sa, got)
-        assert emu.emu_add_rel_pos(C.byref(d), C.byref(src_desc(sw, pw)), C.byref(src_desc(sh, ph)), C.byref(d)) == OK
+        d = view_desc(sa, got)
+        assert emu.emu_add_rel_pos(C.byref(d), C.byref(view_desc(sw, pw)), C.byref(view_desc(sh, ph)), C.byref(d)) == OK
     else:
         got = np.zeros(case.ne_dst[::-1], dtype=np.float32)
-        assert emu.emu_add_rel_pos(C.byref(src_desc(sa, a)), C.byref(src_desc(sw, pw)), C.byref(src_desc(sh, ph)),
+        assert emu.emu_add_rel_pos(C.byref(view_desc(sa, a)), C.byref(view_desc(sw, pw)), C.byref(view_desc(sh, ph)),
                                    C.byref(desc(F32, case.ne_dst, data=got.ctypes.data))) == OK
     nan = np.isnan(want)
     assert np.array_equal(nan, np.isnan(got)) and np.array_equal(bits(got)[~nan], bits(want)[~nan]), str(case)
@@ -156,7 +125,7 @@ def test_host_compiled_add_rel_pos_is_bit_identical_to_ggml_cpu(case, emu, ref):
 def conv_emu(emu, case, k, x):
     ks, xs = case.sources()
     got = np.zeros(case.ne_dst[::-1], dtype=np.float32)
-    rc = emu.emu_conv_transpose_2d(C.byref(src_desc(ks, k)), C.byref(src_desc(xs, x)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), case.s)
+    rc = emu.emu_conv_transpose_2d(C.byref(view_desc(ks, k)), C.byref(view_desc(xs, x)), C.byref(desc(F32, case.ne_dst, data=got.ctypes.data)), case.s)
     return rc, got
 
 
@@ -213,8 +182,8 @@ def test_ggml_cpu_sin_cos_are_within_one_ulp(case, ref):
 
 
 # ------------------------------------------------------------------ the checks' codes
-def test_check_win_part_codes(emu):
-    chk = lambda s, d, npx, npy, w: emu.emu_check_win_part(C.byref(s) if s else None, C.byref(d), npx, npy, w)
+def test_check_win_part_codes(checks):
+    chk = lambda s, d, npx, npy, w: checks.emu_check_win_part(C.byref(s) if s else None, C.byref(d), npx, npy, w)
     x = desc(F32, (768, 64, 64, 1))
     assert chk(x, desc(F32, (768, 14, 14, 25)), 5, 5, 14) == OK
     assert chk(desc(F32, (6, 32, 32, 1)), desc(F32, (6, 14, 14, 9)), 3, 3, 14) == OK
@@ -231,8 +200,8 @@ def test_check_win_part_codes(emu):
     assert chk(desc(F32, (0, 64, 64, 1)), desc(F32, (0, 14, 14, 25)), 5, 5, 14) == OK   # empty
 
 
-def test_check_win_unpart_codes(emu):
-    chk = lambda s, d, w: emu.emu_check_win_unpart(C.byref(s) if s else None, C.byref(d), w)
+def test_check_win_unpart_codes(checks):
+    chk = lambda s, d, w: checks.emu_check_win_unpart(C.byref(s) if s else None, C.byref(d), w)
     y = desc(F32, (768, 64, 64, 1))
     assert chk(desc(F32, (768, 14, 14, 25)), y, 14) == OK and chk(desc(F32, (768, 14, 14, 26)), y, 14) == OK
     assert chk(desc(F32, (768, 14, 14, 24)), y, 14) == EINVAL                          # the reads would leave src
@@ -243,8 +212,8 @@ def test_check_win_unpart_codes(emu):
     assert chk(None, y, 14) == EUNSUPPORTED
 
 
-def test_check_get_rel_pos_codes(emu):
-    chk = lambda s, d: emu.emu_check_get_rel_pos(C.byref(s) if s else None, C.byref(d))
+def test_check_get_rel_pos_codes(checks):
+    chk = lambda s, d: checks.emu_check_get_rel_pos(C.byref(s) if s else None, C.byref(d))
     assert chk(desc(F16, (64, 127)), desc(F16, (64, 64, 64))) == OK and chk(desc(F16, (3, 1)), desc(F16, (3, 1, 1))) == OK
     assert chk(desc(F16, (64, 125)), desc(F16, (64, 64, 64))) == EINVAL                # 2w - 1 rows
     assert chk(desc(F16, (64, 127)), desc(F16, (64, 64, 63))) == EINVAL and chk(desc(F16, (64, 127)), desc(F16, (32, 64, 64))) == EINVAL
@@ -254,8 +223,8 @@ def test_check_get_rel_pos_codes(emu):
     assert chk(None, desc(F16, (64, 64, 64))) == EUNSUPPORTED
 
 
-def test_check_add_rel_pos_codes(emu):
-    chk = lambda a, w, h, d: emu.emu_check_add_rel_pos(*(C.byref(t) if t else None for t in (a, w, h, d)))
+def test_check_add_rel_pos_codes(checks):
+    chk = lambda a, w, h, d: checks.emu_check_add_rel_pos(*(C.byref(t) if t else None for t in (a, w, h, d)))
     a, p = desc(F32, (4096, 4096, 12, 1)), desc(F32, (64, 64, 64, 12))
     assert chk(a, p, p, a) == OK and chk(desc(F32, (196, 196, 300)), desc(F32, (14, 14, 14, 300)), desc(F32, (14, 14, 14, 300)), desc(F32, (196, 196, 300))) == OK
     assert chk(a, p, desc(F32, (64, 64, 64, 11)), a) == EINVAL                         # pw and ph differ
@@ -269,8 +238,8 @@ def test_check_add_rel_pos_codes(emu):
     assert chk(None, p, p, a) == EUNSUPPORTED and chk(a, p, None, a) == EUNSUPPORTED
 
 
-def test_check_conv_transpose_2d_codes(emu):
-    chk = lambda k, x, d, s: emu.emu_check_conv_transpose_2d(*(C.byref(t) if t else None for t in (k, x, d)), s)
+def test_check_conv_transpose_2d_codes(checks):
+    chk = lambda k, x, d, s: checks.emu_check_conv_transpose_2d(*(C.byref(t) if t else None for t in (k, x, d)), s)
     k, x = desc(F16, (2, 2, 64, 256)), desc(F32, (64, 64, 256, 1))
     assert chk(k, x, desc(F32, (128, 128, 64, 1)), 2) == OK
     assert chk(desc(F16, (3, 3, 4, 5)), desc(F32, (6, 5, 5, 1)), desc(F32, (8, 7, 4, 1)), 1) == OK

@@ -6,31 +6,17 @@ oracle/moe_probe.cpp.  Row lengths 1 to 1024 (powers of two and not), both order
     in an order of its own; DESIGN.md §3);
   * rows with +-inf and NaNs: a permutation, the numbers in order before every NaN."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+from hostemu.emu import load
 from oracle import moe as M
-
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libsort_emu.so"
-    srcs = [EMU / "sort_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_sort.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "sort_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("sort_emu")
     L.emu_argsort.restype = C.c_int
     L.emu_argsort.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p]
     return L

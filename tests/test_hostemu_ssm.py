@@ -5,16 +5,12 @@ BIT-IDENTICAL to ggml-cpu: that pins the order of every sum and the separate rou
 The grid covers d_conv 2 / 4 / 8, n_t 1 / 5 / 64, n_s 1 / 3, d_state 1 / 16 / 64 / 256, dt on both sides of the softplus cut-off at 20,
 strided conv inputs and B / C as strided views of one x_db, as in the Mamba layer."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+from hostemu.emu import load
 from oracle import ssm as S
-
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
 
 
 class EmuTensor(C.Structure):
@@ -31,16 +27,7 @@ def emu_tensor(v: S.View) -> EmuTensor:
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libssm_emu.so"
-    srcs = [EMU / "ssm_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_ssm.cuh"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "ssm_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("ssm_emu")
     L.emu_ssm_conv.restype = None
     L.emu_ssm_conv.argtypes = [C.POINTER(EmuTensor), C.POINTER(EmuTensor), C.c_void_p, C.c_int64]
     L.emu_ssm_scan.restype = None

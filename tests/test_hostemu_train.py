@@ -12,67 +12,41 @@ The EUNSUPPORTED / EINVAL codes of the eight checks (b200_op_checks.h), which th
 pinned here too."""
 import ctypes as C
 import itertools
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import ggml_b200 as g
+from hostemu.emu import EINVAL, EUNSUPPORTED, I64, OK, desc, load, view_desc
 from oracle import oracle as O
 from oracle import train as TR
 from oracle.pool import F32, I32, Source
 
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
-OK, EUNSUPPORTED, EINVAL = 0, -1, -2
-I64 = 27
 OUT_PROD_NMSE = 1e-12
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libtrain_emu.so"
-    srcs = [EMU / "train_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_train.cuh", ROOT / "ggml_b200" / "csrc" / "b200_pool.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h", ROOT / "include" / "ggml-b200.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-pthread", "-mf16c", "-mavx", "-ffp-contract=off", "-Wno-unused-variable",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "train_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("train_emu")
     TD, vp = C.POINTER(g.TensorDesc), C.c_void_p
     L.emu_adamw.restype, L.emu_adamw.argtypes = None, [C.c_int64, vp, vp, vp, vp, vp]
     for fn in (L.emu_argmax_closed, L.emu_argmax_seq):
         fn.restype, fn.argtypes = C.c_int32, [vp, C.c_int64]
     L.emu_step.restype, L.emu_step.argtypes = None, [vp, vp, C.c_int64]
-    for name, n in (("emu_out_prod", 3), ("emu_repeat_back", 2), ("emu_check_out_prod", 3), ("emu_check_cross_entropy_loss", 3),
-                    ("emu_check_cross_entropy_loss_back", 4), ("emu_check_opt_step_adamw", 5), ("emu_check_argmax", 2),
-                    ("emu_check_count_equal", 3), ("emu_check_sum", 2), ("emu_check_repeat_back", 2)):
-        fn = getattr(L, name)
+    for fn, n in ((L.emu_out_prod, 3), (L.emu_repeat_back, 2)):
         fn.restype, fn.argtypes = C.c_int, [TD] * n
     return L
 
 
-def desc(type_, ne, nb=None, data=4096):
-    d = g.TensorDesc()
-    d.data, d.type = data, type_
-    ne = list(ne) + [1] * (4 - len(ne))
-    es = 8 if type_ == I64 else 4
-    if nb is None:
-        nb = [es]
-        for i in range(3):
-            nb.append(nb[-1] * ne[i])
-    for i in range(4):
-        d.ne[i], d.nb[i] = ne[i], nb[i]
-    return d
-
-
-def view_desc(src: Source, parent: np.ndarray):
-    ne, nb = src.view()
-    return desc(src.type, ne, nb, data=parent.ctypes.data + src.offs)
+@pytest.fixture(scope="module")
+def checks():
+    L = load("op_checks_emu")
+    TD = C.POINTER(g.TensorDesc)
+    for name, n in (("out_prod", 3), ("cross_entropy_loss", 3), ("cross_entropy_loss_back", 4), ("opt_step_adamw", 5), ("argmax", 2),
+                    ("count_equal", 3), ("sum", 2), ("repeat_back", 2)):
+        fn = getattr(L, "emu_check_" + name)
+        fn.restype, fn.argtypes = C.c_int, [TD] * n
+    return L
 
 
 def u32(a):
@@ -227,53 +201,53 @@ def test_step_specials(emu):
 
 
 # ------------------------------------------------------------------ the checks' codes
-def test_check_codes(emu):
+def test_check_codes(checks):
     b = C.byref
     # OUT_PROD
     a, y, d = desc(F32, (8, 4, 2, 1)), desc(F32, (5, 4, 4, 1)), desc(F32, (8, 5, 4, 1))
-    assert emu.emu_check_out_prod(b(a), b(y), b(d)) == OK
-    assert emu.emu_check_out_prod(b(a), b(desc(F32, (5, 4, 4, 1), nb=(16, 4, 80, 320))), b(d)) == OK       # transposed src1
-    assert emu.emu_check_out_prod(b(desc(1, (8, 4, 2, 1))), b(y), b(d)) == EUNSUPPORTED                    # f16 src0
-    assert emu.emu_check_out_prod(b(desc(F32, (8, 4, 2, 1), nb=(16, 4, 128, 256))), b(y), b(d)) == EUNSUPPORTED
-    assert emu.emu_check_out_prod(b(a), b(y), b(desc(F32, (8, 5, 4, 1), nb=(4, 64, 320, 1280)))) == EUNSUPPORTED
-    assert emu.emu_check_out_prod(b(a), b(desc(F32, (5, 3, 4, 1))), b(d)) == EINVAL                        # K differs
-    assert emu.emu_check_out_prod(b(desc(F32, (8, 4, 3, 1))), b(y), b(d)) == EINVAL                        # 4 % 3
+    assert checks.emu_check_out_prod(b(a), b(y), b(d)) == OK
+    assert checks.emu_check_out_prod(b(a), b(desc(F32, (5, 4, 4, 1), nb=(16, 4, 80, 320))), b(d)) == OK       # transposed src1
+    assert checks.emu_check_out_prod(b(desc(1, (8, 4, 2, 1))), b(y), b(d)) == EUNSUPPORTED                    # f16 src0
+    assert checks.emu_check_out_prod(b(desc(F32, (8, 4, 2, 1), nb=(16, 4, 128, 256))), b(y), b(d)) == EUNSUPPORTED
+    assert checks.emu_check_out_prod(b(a), b(y), b(desc(F32, (8, 5, 4, 1), nb=(4, 64, 320, 1280)))) == EUNSUPPORTED
+    assert checks.emu_check_out_prod(b(a), b(desc(F32, (5, 3, 4, 1))), b(d)) == EINVAL                        # K differs
+    assert checks.emu_check_out_prod(b(desc(F32, (8, 4, 3, 1))), b(y), b(d)) == EINVAL                        # 4 % 3
     # CROSS_ENTROPY_LOSS / _BACK
     x, s = desc(F32, (10, 5)), desc(F32, (1,))
-    assert emu.emu_check_cross_entropy_loss(b(x), b(x), b(s)) == OK
-    assert emu.emu_check_cross_entropy_loss(b(x), b(desc(F32, (10, 4))), b(s)) == EINVAL
-    assert emu.emu_check_cross_entropy_loss(b(x), b(x), b(desc(F32, (2,)))) == EINVAL
-    assert emu.emu_check_cross_entropy_loss(b(desc(F32, (10, 5), nb=(20, 4, 200, 200))), b(x), b(s)) == EUNSUPPORTED
-    assert emu.emu_check_cross_entropy_loss(b(desc(1, (10, 5))), b(x), b(s)) == EUNSUPPORTED
-    assert emu.emu_check_cross_entropy_loss_back(b(s), b(x), b(x), b(x)) == OK
-    assert emu.emu_check_cross_entropy_loss_back(b(desc(F32, (2,))), b(x), b(x), b(x)) == EINVAL
-    assert emu.emu_check_cross_entropy_loss_back(b(s), b(x), b(x), b(desc(F32, (10, 5), nb=(4, 48, 240, 240)))) == EUNSUPPORTED
+    assert checks.emu_check_cross_entropy_loss(b(x), b(x), b(s)) == OK
+    assert checks.emu_check_cross_entropy_loss(b(x), b(desc(F32, (10, 4))), b(s)) == EINVAL
+    assert checks.emu_check_cross_entropy_loss(b(x), b(x), b(desc(F32, (2,)))) == EINVAL
+    assert checks.emu_check_cross_entropy_loss(b(desc(F32, (10, 5), nb=(20, 4, 200, 200))), b(x), b(s)) == EUNSUPPORTED
+    assert checks.emu_check_cross_entropy_loss(b(desc(1, (10, 5))), b(x), b(s)) == EUNSUPPORTED
+    assert checks.emu_check_cross_entropy_loss_back(b(s), b(x), b(x), b(x)) == OK
+    assert checks.emu_check_cross_entropy_loss_back(b(desc(F32, (2,))), b(x), b(x), b(x)) == EINVAL
+    assert checks.emu_check_cross_entropy_loss_back(b(s), b(x), b(x), b(desc(F32, (10, 5), nb=(4, 48, 240, 240)))) == EUNSUPPORTED
     # OPT_STEP_ADAMW
     w, p = desc(F32, (10, 5, 4, 3)), desc(F32, (7,))
-    assert emu.emu_check_opt_step_adamw(b(w), b(w), b(w), b(w), b(p)) == OK
-    assert emu.emu_check_opt_step_adamw(b(w), b(w), b(w), b(w), b(desc(F32, (6,)))) == EINVAL
-    assert emu.emu_check_opt_step_adamw(b(w), b(desc(F32, (10, 5, 4, 2))), b(w), b(w), b(p)) == EINVAL
-    assert emu.emu_check_opt_step_adamw(b(w), b(w), b(desc(F32, (10, 5, 4, 3), nb=(4, 48, 240, 960))), b(w), b(p)) == EUNSUPPORTED
-    assert emu.emu_check_opt_step_adamw(b(desc(1, (10, 5, 4, 3))), b(w), b(w), b(w), b(p)) == EUNSUPPORTED
+    assert checks.emu_check_opt_step_adamw(b(w), b(w), b(w), b(w), b(p)) == OK
+    assert checks.emu_check_opt_step_adamw(b(w), b(w), b(w), b(w), b(desc(F32, (6,)))) == EINVAL
+    assert checks.emu_check_opt_step_adamw(b(w), b(desc(F32, (10, 5, 4, 2))), b(w), b(w), b(p)) == EINVAL
+    assert checks.emu_check_opt_step_adamw(b(w), b(w), b(desc(F32, (10, 5, 4, 3), nb=(4, 48, 240, 960))), b(w), b(p)) == EUNSUPPORTED
+    assert checks.emu_check_opt_step_adamw(b(desc(1, (10, 5, 4, 3))), b(w), b(w), b(w), b(p)) == EUNSUPPORTED
     # ARGMAX
-    assert emu.emu_check_argmax(b(desc(F32, (100, 10))), b(desc(I32, (10,)))) == OK
-    assert emu.emu_check_argmax(b(desc(F32, (100, 10))), b(desc(F32, (10,)))) == EUNSUPPORTED
-    assert emu.emu_check_argmax(b(desc(F32, (100, 10), nb=(40, 4, 400, 400))), b(desc(I32, (10,)))) == EUNSUPPORTED
-    assert emu.emu_check_argmax(b(desc(F32, (100, 10, 2))), b(desc(I32, (10,)))) == EINVAL
-    assert emu.emu_check_argmax(b(desc(F32, (100, 10))), b(desc(I32, (9,)))) == EINVAL
-    assert emu.emu_check_argmax(b(desc(F32, (0, 10))), b(desc(I32, (10,)))) == EINVAL
+    assert checks.emu_check_argmax(b(desc(F32, (100, 10))), b(desc(I32, (10,)))) == OK
+    assert checks.emu_check_argmax(b(desc(F32, (100, 10))), b(desc(F32, (10,)))) == EUNSUPPORTED
+    assert checks.emu_check_argmax(b(desc(F32, (100, 10), nb=(40, 4, 400, 400))), b(desc(I32, (10,)))) == EUNSUPPORTED
+    assert checks.emu_check_argmax(b(desc(F32, (100, 10, 2))), b(desc(I32, (10,)))) == EINVAL
+    assert checks.emu_check_argmax(b(desc(F32, (100, 10))), b(desc(I32, (9,)))) == EINVAL
+    assert checks.emu_check_argmax(b(desc(F32, (0, 10))), b(desc(I32, (10,)))) == EINVAL
     # COUNT_EQUAL
     ci, c64 = desc(I32, (4, 500)), desc(I64, (1,))
-    assert emu.emu_check_count_equal(b(ci), b(ci), b(c64)) == OK
-    assert emu.emu_check_count_equal(b(ci), b(desc(I32, (4, 499))), b(c64)) == EINVAL
-    assert emu.emu_check_count_equal(b(ci), b(ci), b(desc(I32, (1,)))) == EUNSUPPORTED
-    assert emu.emu_check_count_equal(b(desc(I32, (4, 5, 3))), b(desc(I32, (4, 5, 3))), b(c64)) == EUNSUPPORTED
+    assert checks.emu_check_count_equal(b(ci), b(ci), b(c64)) == OK
+    assert checks.emu_check_count_equal(b(ci), b(desc(I32, (4, 499))), b(c64)) == EINVAL
+    assert checks.emu_check_count_equal(b(ci), b(ci), b(desc(I32, (1,)))) == EUNSUPPORTED
+    assert checks.emu_check_count_equal(b(desc(I32, (4, 5, 3))), b(desc(I32, (4, 5, 3))), b(c64)) == EUNSUPPORTED
     # SUM
-    assert emu.emu_check_sum(b(desc(F32, (10, 5, 4, 3))), b(s)) == OK
-    assert emu.emu_check_sum(b(desc(F32, (10, 5), nb=(20, 4, 200, 200))), b(s)) == EUNSUPPORTED
-    assert emu.emu_check_sum(b(desc(F32, (10, 5))), b(desc(F32, (2,)))) == EINVAL
+    assert checks.emu_check_sum(b(desc(F32, (10, 5, 4, 3))), b(s)) == OK
+    assert checks.emu_check_sum(b(desc(F32, (10, 5), nb=(20, 4, 200, 200))), b(s)) == EUNSUPPORTED
+    assert checks.emu_check_sum(b(desc(F32, (10, 5))), b(desc(F32, (2,)))) == EINVAL
     # REPEAT_BACK
-    assert emu.emu_check_repeat_back(b(desc(F32, (16, 6, 4, 2))), b(desc(F32, (8, 6, 4, 2)))) == OK
-    assert emu.emu_check_repeat_back(b(desc(I32, (16, 6, 4, 2))), b(desc(I32, (8, 6, 4, 2)))) == EUNSUPPORTED
-    assert emu.emu_check_repeat_back(b(desc(F32, (16, 6), nb=(8, 128, 768, 768))), b(desc(F32, (8, 6)))) == EUNSUPPORTED
-    assert emu.emu_check_repeat_back(b(desc(F32, (15, 6))), b(desc(F32, (8, 6)))) == EINVAL
+    assert checks.emu_check_repeat_back(b(desc(F32, (16, 6, 4, 2))), b(desc(F32, (8, 6, 4, 2)))) == OK
+    assert checks.emu_check_repeat_back(b(desc(I32, (16, 6, 4, 2))), b(desc(I32, (8, 6, 4, 2)))) == EUNSUPPORTED
+    assert checks.emu_check_repeat_back(b(desc(F32, (16, 6), nb=(8, 128, 768, 768))), b(desc(F32, (8, 6)))) == EUNSUPPORTED
+    assert checks.emu_check_repeat_back(b(desc(F32, (15, 6))), b(desc(F32, (8, 6)))) == EINVAL

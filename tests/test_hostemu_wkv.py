@@ -11,39 +11,30 @@ the reference's own ggml-cpu ops, one-node graphs through oracle/wkv_probe.cpp.
   * The acceptance rules check_rwkv_wkv6 / check_gated_linear_attn (b200_op_checks.h), which the launchers and supports_op share: the
     codes are pinned, and the WKV6 / GLA nodes of the rwkv6 and qrwkv presets of oracle/rwkv_graph.cpp are accepted."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 import torch
 
 import ggml_b200 as g
+from hostemu.emu import EINVAL, EUNSUPPORTED, OK, bits, load
 from oracle import oracle as O
 from oracle import wkv as W
-
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "hostemu"
-OK, EUNSUPPORTED, EINVAL = 0, -1, -2
 
 
 @pytest.fixture(scope="module")
 def emu():
-    out = EMU / "_build"
-    out.mkdir(exist_ok=True)
-    so = out / "libwkv_emu.so"
-    srcs = [EMU / "wkv_emu.cpp", EMU / "shim" / "cuda_shim.h", ROOT / "ggml_b200" / "csrc" / "b200_wkv.cuh",
-            ROOT / "ggml_b200" / "csrc" / "b200_op_checks.h", ROOT / "include" / "ggml-b200.h"]
-    if not so.exists() or so.stat().st_mtime < max(p.stat().st_mtime for p in srcs):
-        cmd = ["g++", "-std=c++17", "-O2", "-fPIC", "-shared", "-ffp-contract=off", "-Wall", "-Werror",
-               f"-I{EMU / 'shim'}", "-o", str(so), str(EMU / "wkv_emu.cpp")]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    L = C.CDLL(str(so))
+    L = load("wkv_emu")
     L.emu_rwkv_wkv6.restype = None
     L.emu_rwkv_wkv6.argtypes = [C.c_void_p] * 7 + [C.c_int64] * 4
     L.emu_gated_linear_attn.restype = None
     L.emu_gated_linear_attn.argtypes = [C.c_void_p] * 6 + [C.c_int64] * 4 + [C.c_float]
+    return L
+
+
+@pytest.fixture(scope="module")
+def checks():
+    L = load("op_checks_emu")
     L.emu_check_rwkv_wkv6.argtypes = [C.POINTER(g.TensorDesc)] * 7
     L.emu_check_gated_linear_attn.argtypes = [C.POINTER(g.TensorDesc)] * 6
     return L
@@ -57,10 +48,6 @@ def emu_wkv(L, case: W.WkvCase, srcs):
     else:
         L.emu_rwkv_wkv6(*p, case.S, case.H, case.T, case.n_seqs)
     return case.split(out)
-
-
-def bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
 
 
 def ulps(a, b):
@@ -125,8 +112,8 @@ def codes(L, src, tf, s, d):
             L.emu_check_gated_linear_attn(C.byref(k), C.byref(v), C.byref(a), C.byref(b), C.byref(s), C.byref(d)))
 
 
-def test_wkv_check_codes(emu):
-    L = emu
+def test_wkv_check_codes(checks):
+    L = checks
     assert codes(L, *wkv_descs(64, 32, 1, 1)) == (OK, OK)
     assert codes(L, *wkv_descs(64, 32, 0, 2)) == (OK, OK)                       # T = 0: nothing to do, as on the CPU
     assert codes(L, *wkv_descs(256, 2, 3, 1)) == (OK, OK)                       # the head-size limit
@@ -153,8 +140,8 @@ def test_wkv_check_codes(emu):
 
 
 @pytest.mark.parametrize("preset,H,n_seqs", [("rwkv6", 32, 2), ("qrwkv", 32, 1)])
-def test_wkv_nodes_of_the_presets_are_accepted(emu, preset, H, n_seqs):
+def test_wkv_nodes_of_the_presets_are_accepted(checks, preset, H, n_seqs):
     # oracle/rwkv_graph.cpp: head size 64, a 7-token prompt per sequence, then one token per sequence per decode step
     for n_t in (7, 1):
-        c = codes(emu, *wkv_descs(64, H, n_t * n_seqs, n_seqs))
+        c = codes(checks, *wkv_descs(64, H, n_t * n_seqs, n_seqs))
         assert c[1 if preset == "qrwkv" else 0] == OK, (preset, n_t, c)
