@@ -13,7 +13,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from . import oracle as O
+from .probe import probe_lib, ptrs, result
 from .ssm import View, _nb
 
 F32, F16 = 0, 1
@@ -99,48 +99,26 @@ def im2col_grid() -> list:
 
 
 # ------------------------------------------------------------------ the probe
-_lib = None
+SIGNATURES = {
+    "probe_im2col": [C.c_char_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_mul_mat_f16": [C.c_char_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_conv_1d": [C.c_char_p] + [C.c_int64] * 4 + [C.c_int] * 3 + [C.c_void_p, C.c_void_p],
+}
 
 
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_conv_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f whisper.mk whisper where the reference tree exists)")
-        L = C.CDLL(str(so))
-        L.probe_im2col.restype = C.c_int
-        L.probe_im2col.argtypes = [C.c_char_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-        L.probe_mul_mat_f16.restype = C.c_int
-        L.probe_mul_mat_f16.argtypes = [C.c_char_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
-        L.probe_conv_1d.restype = C.c_int
-        L.probe_conv_1d.argtypes = [C.c_char_p] + [C.c_int64] * 4 + [C.c_int] * 3 + [C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
-
-
-def _ptrs(arrays):
-    return (C.c_void_p * len(arrays))(*[a.ctypes.data for a in arrays])
-
-
-def _result(rc, raw, what, value):
-    if raw:
-        return rc
-    if rc != 0:
-        raise RuntimeError(f"{what} returned {rc}")
-    return value
+def _lib():
+    return probe_lib("conv", "make -C oracle -f whisper.mk whisper", SIGNATURES)
 
 
 def im2col(dev: str, case: Im2colCase, view: View | None = None, raw: bool = False):
     """IM2COL of `case` on ggml device `dev`: dst contiguous, ggml dims reversed (float32 or float16).  raw: the probe's code"""
-    L = _probe_lib()
+    L = _lib()
     v = view or case.view_of_input()
     out = np.zeros(case.ne_dst[::-1], dtype=np.float16 if case.dst_type == F16 else np.float32)
     ne_k, ne_x = np.array(case.ne_kernel, dtype=np.int64), np.array(case.ne_input, dtype=np.int64)
     rc = L.probe_im2col(dev.encode(), case.kernel_type, ne_k.ctypes.data, ne_x.ctypes.data, case.view, case.params.ctypes.data, case.dst_type,
-                        _ptrs([v.parent]), out.ctypes.data)
-    return _result(rc, raw, f"probe_im2col({dev}, {case})", out)
+                        ptrs([v.parent]), out.ctypes.data)
+    return result(rc, raw, f"probe_im2col({dev}, {case})", out)
 
 
 def f16_operands(M: int, N: int, K: int, b_view: int, seed: int = 0):
@@ -154,11 +132,11 @@ def f16_operands(M: int, N: int, K: int, b_view: int, seed: int = 0):
 
 def mul_mat_f16(dev: str, M: int, N: int, K: int, b_view: int = 0, operands=None, raw: bool = False):
     """MUL_MAT(a f16 [K, M], b f16 [K, N]) on `dev`: f32 [N, M]"""
-    L = _probe_lib()
+    L = _lib()
     a, b = operands if operands is not None else f16_operands(M, N, K, b_view)
     out = np.zeros((N, M), dtype=np.float32)
-    rc = L.probe_mul_mat_f16(dev.encode(), M, N, K, b_view, _ptrs([a, b]), out.ctypes.data)
-    return _result(rc, raw, f"probe_mul_mat_f16({dev}, {M}, {N}, {K}, view {b_view})", out)
+    rc = L.probe_mul_mat_f16(dev.encode(), M, N, K, b_view, ptrs([a, b]), out.ctypes.data)
+    return result(rc, raw, f"probe_mul_mat_f16({dev}, {M}, {N}, {K}, view {b_view})", out)
 
 
 def mul_mat_f16_reference(a: np.ndarray, b: np.ndarray, b_view: int) -> np.ndarray:
@@ -169,10 +147,10 @@ def mul_mat_f16_reference(a: np.ndarray, b: np.ndarray, b_view: int) -> np.ndarr
 
 def conv_1d(dev: str, KW: int, IC: int, OC: int, L_: int, s: int, p: int, d: int, seed: int = 0, raw: bool = False):
     """ggml_conv_1d(kernel f16 [OC, IC, KW], x f32 [IC, L]) on `dev`: f32 [OC, OL]"""
-    L = _probe_lib()
+    L = _lib()
     rng = np.random.default_rng(13000 + seed)
     k = (rng.standard_normal((OC, IC, KW)) / np.sqrt(IC * KW)).astype(np.float16)
     x = rng.standard_normal((IC, L_)).astype(np.float32)
     out = np.zeros((OC, conv_out(L_, KW, s, p, d)), dtype=np.float32)
-    rc = L.probe_conv_1d(dev.encode(), KW, IC, OC, L_, s, p, d, _ptrs([k, x]), out.ctypes.data)
-    return _result(rc, raw, f"probe_conv_1d({dev}, KW={KW} IC={IC} OC={OC} L={L_} s={s} p={p} d={d})", out)
+    rc = L.probe_conv_1d(dev.encode(), KW, IC, OC, L_, s, p, d, ptrs([k, x]), out.ctypes.data)
+    return result(rc, raw, f"probe_conv_1d({dev}, KW={KW} IC={IC} OC={OC} L={L_} s={s} p={p} d={d})", out)

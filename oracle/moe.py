@@ -12,7 +12,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from . import oracle as O
+from .probe import probe_lib, result
 
 ASC, DESC = 0, 1
 KINDS = ("tiefree", "ties", "special")
@@ -95,46 +95,31 @@ def check_sorted_row(x: np.ndarray, got: np.ndarray, order: int, want: np.ndarra
             assert np.array_equal(got, want), "indices differ from ggml-cpu's on a tie-free row"
 
 
-_lib = None
+SIGNATURES = {
+    "probe_argsort": [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_sum_rows": [C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
+}
 
 
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_moe_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f decoders.mk moe where the reference tree exists)")
-        L = C.CDLL(str(so))
-        L.probe_argsort.restype = C.c_int
-        L.probe_argsort.argtypes = [C.c_char_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        L.probe_sum_rows.restype = C.c_int
-        L.probe_sum_rows.argtypes = [C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
+def _lib():
+    return probe_lib("moe", "make -C oracle -f decoders.mk moe", SIGNATURES)
 
 
 def argsort(dev: str, case: Case, order: int, parent: np.ndarray | None = None, raw: bool = False):
     """ARGSORT of `case` on ggml device `dev`: i32 rows [ne1 * ne2 * ne3, ne0].  raw: return the probe's code instead of raising"""
-    L = _probe_lib()
+    L = _lib()
     x = np.ascontiguousarray(case.parent() if parent is None else parent, dtype=np.float32)
     ne = np.array(case.ne, dtype=np.int64)
     out = np.empty(int(np.prod(case.ne)), dtype=np.int32)
     rc = L.probe_argsort(dev.encode(), ne.ctypes.data, case.view, order, x.ctypes.data, out.ctypes.data)
-    if raw:
-        return rc
-    if rc != 0:
-        raise RuntimeError(f"probe_argsort({dev}, {case}, {order}) returned {rc}")
-    return out.reshape(-1, case.ne[0])
+    return result(rc, raw, f"probe_argsort({dev}, {case}, {order})", out.reshape(-1, case.ne[0]))
 
 
 def sum_rows(dev: str, case: Case, parent: np.ndarray | None = None) -> np.ndarray:
     """SUM_ROWS of `case` on ggml device `dev`: f32 [ne1 * ne2 * ne3]"""
-    L = _probe_lib()
+    L = _lib()
     x = np.ascontiguousarray(case.parent() if parent is None else parent, dtype=np.float32)
     ne = np.array(case.ne, dtype=np.int64)
     out = np.empty(int(np.prod(case.ne[1:])), dtype=np.float32)
     rc = L.probe_sum_rows(dev.encode(), ne.ctypes.data, case.view, x.ctypes.data, out.ctypes.data)
-    if rc != 0:
-        raise RuntimeError(f"probe_sum_rows({dev}, {case}) returned {rc}")
-    return out
+    return result(rc, False, f"probe_sum_rows({dev}, {case})", out)

@@ -5,10 +5,7 @@
 // from Python with ctypes (oracle/moe.py).  On "CPU" it is ggml-cpu's op; on "B2000" (the plug-in, loaded beforehand with
 // probe_load_backend of libggml_probe.so) it is this repository's kernel.  Nothing here is on the product path.
 
-#include "ggml.h"
-#include "ggml-alloc.h"
-#include "ggml-backend.h"
-#include "ggml-cpu.h"
+#include "probe_harness.h"
 
 namespace {
 
@@ -23,53 +20,26 @@ ggml_tensor * source(ggml_context * ctx, const int64_t * ne, int view, ggml_tens
     return ggml_view_4d(ctx, *parent, ne[0], ne[1], ne[2], ne[3], p->nb[1], p->nb[2], p->nb[3], 0);
 }
 
-// build the one-node graph of `r` and run it on `dev`; x fills the parent, out receives r (contiguous)
-int run(const char * dev, ggml_context * ctx, ggml_tensor * parent, ggml_tensor * r, const float * x, void * out) {
-    ggml_backend_dev_t d = ggml_backend_dev_by_name(dev);
-    ggml_backend_t be = d ? ggml_backend_dev_init(d, nullptr) : nullptr;
-    if (!be) { ggml_free(ctx); return -1; }
-    if (ggml_backend_is_cpu(be)) ggml_backend_cpu_set_n_threads(be, 4);
-    ggml_cgraph * gf = ggml_new_graph(ctx);
-    ggml_build_forward_expand(gf, r);
-    int rc = 0;
-    ggml_backend_buffer_t buf = nullptr;
-    if (!ggml_backend_supports_op(be, r)) rc = -2;
-    else if (!(buf = ggml_backend_alloc_ctx_tensors(ctx, be))) rc = -3;
-    else {
-        ggml_backend_tensor_set(parent, x, 0, ggml_nbytes(parent));
-        ggml_backend_graph_compute(be, gf);
-        ggml_backend_tensor_get(r, out, 0, ggml_nbytes(r));
-    }
-    if (buf) ggml_backend_buffer_free(buf);
-    ggml_free(ctx);
-    ggml_backend_free(be);
-    return rc;
-}
-
-ggml_context * new_ctx() {
-    ggml_init_params ip = { ggml_tensor_overhead() * 8 + ggml_graph_overhead(), nullptr, true };
-    return ggml_init(ip);
-}
-
 } // namespace
 
 extern "C" {
 
-// out (i32, ne0*ne1*ne2*ne3) = ARGSORT(x, order) on device `dev`; x holds the parent tensor (see source()).
-// Returns 0, -1 (no such device), -2 (the device declines the node), -3 (allocation failed).
+// Every probe returns probe_run's code (probe_harness.h).
+
+// out (i32, ne0*ne1*ne2*ne3) = ARGSORT(x, order) on device `dev`; x holds the parent tensor (see source())
 int probe_argsort(const char * dev, const int64_t * ne, int view, int order, const float * x, int32_t * out) {
-    ggml_context * ctx = new_ctx();
+    ggml_context * ctx = probe_ctx();
     ggml_tensor * parent;
-    ggml_tensor * a = source(ctx, ne, view, &parent);
-    return run(dev, ctx, parent, ggml_argsort(ctx, a, (ggml_sort_order) order), x, out);
+    ggml_tensor * r = ggml_argsort(ctx, source(ctx, ne, view, &parent), (ggml_sort_order) order);
+    return probe_run(dev, ctx, r, { { parent, x } }, { { r, out } });
 }
 
 // out (f32, ne1*ne2*ne3) = SUM_ROWS(x) on device `dev`; as probe_argsort
 int probe_sum_rows(const char * dev, const int64_t * ne, int view, const float * x, float * out) {
-    ggml_context * ctx = new_ctx();
+    ggml_context * ctx = probe_ctx();
     ggml_tensor * parent;
-    ggml_tensor * a = source(ctx, ne, view, &parent);
-    return run(dev, ctx, parent, ggml_sum_rows(ctx, a), x, out);
+    ggml_tensor * r = ggml_sum_rows(ctx, source(ctx, ne, view, &parent));
+    return probe_run(dev, ctx, r, { { parent, x } }, { { r, out } });
 }
 
 } // extern "C"

@@ -13,7 +13,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import oracle as O
+from .probe import probe_lib, result
 
 F32, F16, I16, I32, BF16 = 0, 1, 25, 26, 30
 ES = {F32: 4, I32: 4, F16: 2, BF16: 2, I16: 2}
@@ -196,35 +196,16 @@ def repeat_grid() -> list:
 
 
 # ------------------------------------------------------------------ the probe
-_lib = None
+SIGNATURES = {
+    "probe_pool_2d": [C.c_char_p, C.c_void_p] + [C.c_int] * 5 + [C.c_float] * 2 + [C.c_void_p, C.c_void_p],
+    "probe_upscale": [C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+    "probe_leaky_relu": [C.c_char_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_repeat": [C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+}
 
 
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_pool_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f yolo.mk yolo where the reference tree exists)")
-        L = C.CDLL(str(so))
-        L.probe_pool_2d.restype = C.c_int
-        L.probe_pool_2d.argtypes = [C.c_char_p, C.c_void_p] + [C.c_int] * 5 + [C.c_float] * 2 + [C.c_void_p, C.c_void_p]
-        L.probe_upscale.restype = C.c_int
-        L.probe_upscale.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.probe_leaky_relu.restype = C.c_int
-        L.probe_leaky_relu.argtypes = [C.c_char_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
-        L.probe_repeat.restype = C.c_int
-        L.probe_repeat.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
-
-
-def _result(rc, raw, what, value):
-    if raw:
-        return rc
-    if rc != 0:
-        raise RuntimeError(f"{what} returned {rc}")
-    return value
+def _lib():
+    return probe_lib("pool", "make -C oracle -f yolo.mk yolo", SIGNATURES)
 
 
 def _dtype(t):
@@ -238,39 +219,39 @@ def nbytes(ne, nb, es):
 
 def pool_2d(dev: str, case: PoolCase, parent=None, raw: bool = False):
     """POOL_2D of `case` on `dev`: f32, ggml dims reversed"""
-    L = _probe_lib()
+    L = _lib()
     parent = case.src.parent() if parent is None else parent
     out = np.zeros(case.ne_dst[::-1], dtype=np.float32)
     rc = L.probe_pool_2d(dev.encode(), case.src.spec().ctypes.data, case.op, case.k0, case.k1, case.s0, case.s1, case.p0, case.p1,
                          parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_pool_2d({dev}, {case})", out)
+    return result(rc, raw, f"probe_pool_2d({dev}, {case})", out)
 
 
 def upscale(dev: str, case: UpscaleCase, parent=None, raw: bool = False):
-    L = _probe_lib()
+    L = _lib()
     parent = case.src.parent() if parent is None else parent
     out = np.zeros(tuple(case.ne_dst)[::-1], dtype=np.float32)
     ne = np.array(case.ne_dst, dtype=np.int64)
     rc = L.probe_upscale(dev.encode(), case.src.spec().ctypes.data, ne.ctypes.data, parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_upscale({dev}, {case})", out)
+    return result(rc, raw, f"probe_upscale({dev}, {case})", out)
 
 
 def leaky_relu(dev: str, case: LeakyCase, parent=None, raw: bool = False):
     """LEAKY_RELU of `case` on `dev`: not in place, the packed result (ggml dims reversed); in place, the bytes of the source view (its
     ggml_nbytes from its first element), as f32"""
-    L = _probe_lib()
+    L = _lib()
     parent = case.src.parent() if parent is None else parent
     ne, nb = case.src.view()
     out = np.zeros(ne[::-1], dtype=np.float32) if not case.inplace else np.zeros(nbytes(ne, nb, 4) // 4, dtype=np.float32)
     rc = L.probe_leaky_relu(dev.encode(), case.src.spec().ctypes.data, case.slope, int(case.inplace), parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_leaky_relu({dev}, {case})", out)
+    return result(rc, raw, f"probe_leaky_relu({dev}, {case})", out)
 
 
 def repeat(dev: str, case: RepeatCase, parent=None, raw: bool = False):
     """REPEAT of `case` on `dev`: raw words (uint32 / uint16), ggml dims reversed"""
-    L = _probe_lib()
+    L = _lib()
     parent = case.src.parent() if parent is None else parent
     out = np.zeros(tuple(case.ne_dst)[::-1], dtype=_dtype(case.src.type) if case.src.type != F32 else np.uint32)
     ne = np.array(case.ne_dst, dtype=np.int64)
     rc = L.probe_repeat(dev.encode(), case.src.spec().ctypes.data, ne.ctypes.data, parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_repeat({dev}, {case})", out)
+    return result(rc, raw, f"probe_repeat({dev}, {case})", out)

@@ -11,6 +11,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import oracle as O
+from .probe import probe_lib, result
 
 ROPE_NORM, ROPE_NEOX, ROPE_MROPE, ROPE_VISION = 0, 2, 8, 24
 MODE_NAMES = {ROPE_NORM: "norm", ROPE_NEOX: "neox", ROPE_MROPE: "mrope", ROPE_VISION: "vision"}
@@ -92,27 +93,15 @@ def grid(inplace: bool = False) -> list:
     return out
 
 
-_lib = None
-
-
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_rope_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f decoders.mk llama where the reference tree exists)")
-        L = C.CDLL(str(so))
-        L.probe_rope.restype = C.c_int
-        L.probe_rope.argtypes = [C.c_char_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                 C.c_int, C.c_int, C.c_void_p, C.c_int] + [C.c_float] * 6 + [C.c_void_p]
-        _lib = L
-    return _lib
+SIGNATURES = {
+    "probe_rope": [C.c_char_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                   C.c_int] + [C.c_float] * 6 + [C.c_void_p],
+}
 
 
 def probe(dev: str, case: Case) -> np.ndarray:
     """ROPE of `case` on ggml device `dev`: the result, contiguous, in ggml order (flat)"""
-    L = _probe_lib()
+    L = probe_lib("rope", "make -C oracle -f decoders.mk llama", SIGNATURES)
     x, pos, ff = case.inputs()
     ne = np.array(case.ne, dtype=np.int64)
     sec = np.array(case.sections, dtype=np.int32)
@@ -121,6 +110,4 @@ def probe(dev: str, case: Case) -> np.ndarray:
                       ff.ctypes.data if ff is not None else None, 0 if ff is None else ff.size, case.n_dims, case.mode, sec.ctypes.data,
                       case.n_ctx_orig, case.freq_base, case.freq_scale, case.ext_factor, case.attn_factor, case.beta_fast, case.beta_slow,
                       out.ctypes.data)
-    if rc != 0:
-        raise RuntimeError(f"probe_rope({dev}, {case}) returned {rc}")
-    return out
+    return result(rc, False, f"probe_rope({dev}, {case})", out)

@@ -13,8 +13,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from . import oracle as O
-from .pool import F16, F32, Source, _result
+from .pool import F16, F32, Source
+from .probe import probe_lib, result
 
 SIN, COS = 0, 1
 
@@ -258,26 +258,18 @@ def sin_cos_grid():
 
 
 # ------------------------------------------------------------------ the probe
-_lib = None
+SIGNATURES = {
+    "probe_win_part": [C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_win_unpart": [C.c_char_p, C.c_void_p] + [C.c_int] * 3 + [C.c_void_p, C.c_void_p],
+    "probe_get_rel_pos": [C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_add_rel_pos": [C.c_char_p] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 4,
+    "probe_conv_transpose_2d": [C.c_char_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p],
+    "probe_sin_cos": [C.c_char_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
+}
 
 
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_sam_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f sam.mk sam where the reference tree exists)")
-        L = C.CDLL(str(so))
-        vp, i = C.c_void_p, C.c_int
-        for name, args in (("probe_win_part", [C.c_char_p, vp, i, vp, vp]), ("probe_win_unpart", [C.c_char_p, vp, i, i, i, vp, vp]),
-                           ("probe_get_rel_pos", [C.c_char_p, vp, i, vp, vp]),
-                           ("probe_add_rel_pos", [C.c_char_p, vp, vp, vp, i, vp, vp, vp, vp]),
-                           ("probe_conv_transpose_2d", [C.c_char_p, vp, vp, i, vp, vp, vp]), ("probe_sin_cos", [C.c_char_p, vp, i, vp, vp])):
-            fn = getattr(L, name)
-            fn.restype, fn.argtypes = C.c_int, args
-        _lib = L
-    return _lib
+def _lib():
+    return probe_lib("sam", "make -C oracle -f sam.mk sam", SIGNATURES)
 
 
 def win_part(dev: str, case: WinPartCase, parent=None, raw: bool = False):
@@ -285,16 +277,16 @@ def win_part(dev: str, case: WinPartCase, parent=None, raw: bool = False):
     parent = case.src.parent() if parent is None else parent
     out = np.zeros(case.ne_dst[::-1], dtype=np.uint32)
     spec = case.src.spec()
-    rc = _probe_lib().probe_win_part(dev.encode(), spec.ctypes.data, case.w, parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_win_part({dev}, {case})", out)
+    rc = _lib().probe_win_part(dev.encode(), spec.ctypes.data, case.w, parent.ctypes.data, out.ctypes.data)
+    return result(rc, raw, f"probe_win_part({dev}, {case})", out)
 
 
 def win_unpart(dev: str, case: WinUnpartCase, parent=None, raw: bool = False):
     parent = case.src.parent() if parent is None else parent
     out = np.zeros(case.ne_dst[::-1], dtype=np.uint32)
     spec = case.src.spec()
-    rc = _probe_lib().probe_win_unpart(dev.encode(), spec.ctypes.data, case.w0, case.h0, case.w, parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_win_unpart({dev}, {case})", out)
+    rc = _lib().probe_win_unpart(dev.encode(), spec.ctypes.data, case.w0, case.h0, case.w, parent.ctypes.data, out.ctypes.data)
+    return result(rc, raw, f"probe_win_unpart({dev}, {case})", out)
 
 
 def get_rel_pos(dev: str, case: RelPosCase, parent=None, raw: bool = False):
@@ -302,8 +294,8 @@ def get_rel_pos(dev: str, case: RelPosCase, parent=None, raw: bool = False):
     parent = case.src.parent() if parent is None else parent
     out = np.zeros(case.ne_dst[::-1], dtype=np.uint16)
     spec = case.src.spec()
-    rc = _probe_lib().probe_get_rel_pos(dev.encode(), spec.ctypes.data, case.w, parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_get_rel_pos({dev}, {case})", out)
+    rc = _lib().probe_get_rel_pos(dev.encode(), spec.ctypes.data, case.w, parent.ctypes.data, out.ctypes.data)
+    return result(rc, raw, f"probe_get_rel_pos({dev}, {case})", out)
 
 
 def add_rel_pos(dev: str, case: AddRelPosCase, parents=None, raw: bool = False):
@@ -311,9 +303,9 @@ def add_rel_pos(dev: str, case: AddRelPosCase, parents=None, raw: bool = False):
     a, pw, ph = case.parents() if parents is None else parents
     specs = [s.spec() for s in case.sources()]                     # held: the probe reads them through raw pointers
     out = np.zeros(case.ne_dst[::-1], dtype=np.float32)
-    rc = _probe_lib().probe_add_rel_pos(dev.encode(), *(s.ctypes.data for s in specs), int(case.inplace),
-                                        a.ctypes.data, pw.ctypes.data, ph.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_add_rel_pos({dev}, {case})", out)
+    rc = _lib().probe_add_rel_pos(dev.encode(), *(s.ctypes.data for s in specs), int(case.inplace),
+                                  a.ctypes.data, pw.ctypes.data, ph.ctypes.data, out.ctypes.data)
+    return result(rc, raw, f"probe_add_rel_pos({dev}, {case})", out)
 
 
 def conv_transpose_2d(dev: str, case: ConvT2dCase, parents=None, raw: bool = False):
@@ -321,14 +313,14 @@ def conv_transpose_2d(dev: str, case: ConvT2dCase, parents=None, raw: bool = Fal
     k, x = case.parents() if parents is None else parents
     sk, sx = (s.spec() for s in case.sources())                    # held: the probe reads them through raw pointers
     out = np.zeros(case.ne_dst[::-1], dtype=np.float32)
-    rc = _probe_lib().probe_conv_transpose_2d(dev.encode(), sk.ctypes.data, sx.ctypes.data, case.s, k.ctypes.data, x.ctypes.data,
-                                              out.ctypes.data)
-    return _result(rc, raw, f"probe_conv_transpose_2d({dev}, {case})", out)
+    rc = _lib().probe_conv_transpose_2d(dev.encode(), sk.ctypes.data, sx.ctypes.data, case.s, k.ctypes.data, x.ctypes.data,
+                                        out.ctypes.data)
+    return result(rc, raw, f"probe_conv_transpose_2d({dev}, {case})", out)
 
 
 def sin_cos(dev: str, case: SinCosCase, parent=None, raw: bool = False):
     parent = sin_cos_parent(case) if parent is None else parent
     out = np.zeros(case.src.ne[::-1], dtype=np.float32)
     spec = case.src.spec()
-    rc = _probe_lib().probe_sin_cos(dev.encode(), spec.ctypes.data, case.op, parent.ctypes.data, out.ctypes.data)
-    return _result(rc, raw, f"probe_sin_cos({dev}, {case})", out)
+    rc = _lib().probe_sin_cos(dev.encode(), spec.ctypes.data, case.op, parent.ctypes.data, out.ctypes.data)
+    return result(rc, raw, f"probe_sin_cos({dev}, {case})", out)

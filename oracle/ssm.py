@@ -13,7 +13,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from . import oracle as O
+from .probe import probe_lib, ptrs, result
 
 F32, I32, F16 = 0, 1, 2
 NP_TYPES = {F32: np.float32, I32: np.int32, F16: np.float16}
@@ -204,67 +204,44 @@ def concat_grid() -> list:
 
 
 # ------------------------------------------------------------------ the probe
-_lib = None
+SIGNATURES = {
+    "probe_concat": [C.c_char_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_ssm_conv": [C.c_char_p] + [C.c_int64] * 4 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p],
+    "probe_ssm_scan": [C.c_char_p] + [C.c_int64] * 5 + [C.c_void_p, C.c_void_p],
+}
 
 
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_ssm_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f decoders.mk mamba where the reference tree exists)")
-        L = C.CDLL(str(so))
-        L.probe_concat.restype = C.c_int
-        L.probe_concat.argtypes = [C.c_char_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        L.probe_ssm_conv.restype = C.c_int
-        L.probe_ssm_conv.argtypes = [C.c_char_p] + [C.c_int64] * 4 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-        L.probe_ssm_scan.restype = C.c_int
-        L.probe_ssm_scan.argtypes = [C.c_char_p] + [C.c_int64] * 5 + [C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
-
-
-def _ptrs(arrays):
-    return (C.c_void_p * len(arrays))(*[a.ctypes.data for a in arrays])
-
-
-def _result(rc, raw, what, value):
-    """the probe's code when raw, else value (raising when the probe failed)"""
-    if raw:
-        return rc
-    if rc != 0:
-        raise RuntimeError(f"{what} returned {rc}")
-    return value
+def _lib():
+    return probe_lib("ssm", "make -C oracle -f decoders.mk mamba", SIGNATURES)
 
 
 def concat(dev: str, case: ConcatCase, raw: bool = False):
     """CONCAT of `case` on ggml device `dev`: the result, contiguous, ggml dims reversed.  raw: return the probe's code"""
-    L = _probe_lib()
+    L = _lib()
     parents = case.parents()
     out = np.zeros(case.ne_dst[::-1], dtype=NP_TYPES[case.type])
     ne_a, ne_b = np.array(case.ne_a, dtype=np.int64), np.array(case.ne_b, dtype=np.int64)
-    rc = L.probe_concat(dev.encode(), case.type, ne_a.ctypes.data, case.view_a, ne_b.ctypes.data, case.view_b, case.dim, _ptrs(parents), out.ctypes.data)
-    return _result(rc, raw, f"probe_concat({dev}, {case})", out)
+    rc = L.probe_concat(dev.encode(), case.type, ne_a.ctypes.data, case.view_a, ne_b.ctypes.data, case.view_b, case.dim, ptrs(parents), out.ctypes.data)
+    return result(rc, raw, f"probe_concat({dev}, {case})", out)
 
 
 def ssm_conv(dev: str, case: ConvCase, views=None, raw: bool = False):
     """SSM_CONV of `case` on `dev`: f32 [n_s, n_t, d_inner]"""
-    L = _probe_lib()
+    L = _lib()
     sx, c = views or case.views()
     out = np.zeros((case.n_s, case.n_t, case.d_inner), dtype=np.float32)
-    rc = L.probe_ssm_conv(dev.encode(), case.d_conv, case.d_inner, case.n_t, case.n_s, case.view_sx, case.view_c, _ptrs([sx.parent, c.parent]), out.ctypes.data)
-    return _result(rc, raw, f"probe_ssm_conv({dev}, {case})", out)
+    rc = L.probe_ssm_conv(dev.encode(), case.d_conv, case.d_inner, case.n_t, case.n_s, case.view_sx, case.view_c, ptrs([sx.parent, c.parent]), out.ctypes.data)
+    return result(rc, raw, f"probe_ssm_conv({dev}, {case})", out)
 
 
 def ssm_scan(dev: str, case: ScanCase, views=None, raw: bool = False):
     """SSM_SCAN of `case` on `dev`: (y f32 [n_s, n_t, d_inner], final states f32 [n_s, d_inner, d_state])"""
-    L = _probe_lib()
+    L = _lib()
     v = views or case.views()
     parents = [w.parent for w in v[:4]] + ([v[4].parent, v[5].parent] if case.bc_rank < 0 else [v[4].parent])
     out = np.zeros(case.n_y + case.d_state * case.d_inner * case.n_s, dtype=np.float32)
-    rc = L.probe_ssm_scan(dev.encode(), case.d_state, case.d_inner, case.n_t, case.n_s, case.bc_rank, _ptrs(parents), out.ctypes.data)
-    return _result(rc, raw, f"probe_ssm_scan({dev}, {case})",
+    rc = L.probe_ssm_scan(dev.encode(), case.d_state, case.d_inner, case.n_t, case.n_s, case.bc_rank, ptrs(parents), out.ctypes.data)
+    return result(rc, raw, f"probe_ssm_scan({dev}, {case})",
                    (out[: case.n_y].reshape(case.n_s, case.n_t, case.d_inner), out[case.n_y:].reshape(case.n_s, case.d_inner, case.d_state)))
 
 

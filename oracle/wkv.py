@@ -13,6 +13,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import oracle as O
+from .probe import probe_lib, ptrs, result
 
 GLA_SCALES = (1.0, 64 ** -0.5)
 
@@ -87,35 +88,21 @@ def cpu_vector_width() -> int:
 
 
 # ------------------------------------------------------------------ the probe
-_lib = None
+SIGNATURES = {
+    "probe_rwkv_wkv6": [C.c_char_p] + [C.c_int64] * 4 + [C.c_void_p, C.c_void_p],
+    "probe_gated_linear_attn": [C.c_char_p] + [C.c_int64] * 4 + [C.c_float, C.c_void_p, C.c_void_p],
+    "probe_sqr_sqrt": [C.c_char_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p],
+}
 
 
-def _probe_lib():
-    global _lib
-    if _lib is None:
-        O.Ref()                                            # loads the reference libraries (and the shared backend registry) globally
-        so = O.REF_DIR / "libggml_wkv_probe.so"
-        if not so.exists():
-            raise RuntimeError(f"{so} missing (make -C oracle -f decoders.mk rwkv where the reference tree exists)")
-        L = C.CDLL(str(so))
-        L.probe_rwkv_wkv6.restype = C.c_int
-        L.probe_rwkv_wkv6.argtypes = [C.c_char_p] + [C.c_int64] * 4 + [C.c_void_p, C.c_void_p]
-        L.probe_gated_linear_attn.restype = C.c_int
-        L.probe_gated_linear_attn.argtypes = [C.c_char_p] + [C.c_int64] * 4 + [C.c_float, C.c_void_p, C.c_void_p]
-        L.probe_sqr_sqrt.restype = C.c_int
-        L.probe_sqr_sqrt.argtypes = [C.c_char_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]
-        _lib = L
-    return _lib
-
-
-def _ptrs(arrays):
-    return (C.c_void_p * len(arrays))(*[a.ctypes.data for a in arrays])
+def _lib():
+    return probe_lib("wkv", "make -C oracle -f decoders.mk rwkv", SIGNATURES)
 
 
 def wkv(dev: str, case: WkvCase, srcs=None, raw: bool = False, T: int | None = None):
     """the node of `case` on `dev`: (y, final states), or the probe's code when raw.  T overrides the token count (raw only: a T that
     is not a multiple of n_seqs, which ggml-cpu cannot run)"""
-    L = _probe_lib()
+    L = _lib()
     srcs = srcs if srcs is not None else case.sources()
     T = case.T if T is None else T
     out = np.zeros((T + case.S * case.n_seqs) * case.S * case.H, dtype=np.float32)
@@ -123,24 +110,16 @@ def wkv(dev: str, case: WkvCase, srcs=None, raw: bool = False, T: int | None = N
         assert raw
         srcs = [np.zeros(max(1, T * case.H * case.S), np.float32) if a.shape[0] == case.T and a.ndim == 3 else a for a in srcs]
     if case.gla:
-        rc = L.probe_gated_linear_attn(dev.encode(), case.S, case.H, T, case.n_seqs, case.scale, _ptrs(srcs), out.ctypes.data)
+        rc = L.probe_gated_linear_attn(dev.encode(), case.S, case.H, T, case.n_seqs, case.scale, ptrs(srcs), out.ctypes.data)
     else:
-        rc = L.probe_rwkv_wkv6(dev.encode(), case.S, case.H, T, case.n_seqs, _ptrs(srcs), out.ctypes.data)
-    if raw:
-        return rc
-    if rc != 0:
-        raise RuntimeError(f"probe({dev}, {case}) returned {rc}")
-    return case.split(out)
+        rc = L.probe_rwkv_wkv6(dev.encode(), case.S, case.H, T, case.n_seqs, ptrs(srcs), out.ctypes.data)
+    return rc if raw else case.split(result(rc, raw, f"probe({dev}, {case})", out))
 
 
 def sqr_sqrt(dev: str, op: int, x: np.ndarray, raw: bool = False):
     """SQR (op 0) or SQRT (op 1) of the f32 vector x on `dev`"""
-    L = _probe_lib()
+    L = _lib()
     x = np.ascontiguousarray(x, dtype=np.float32)
     out = np.zeros_like(x)
-    rc = L.probe_sqr_sqrt(dev.encode(), op, x.size, _ptrs([x]), out.ctypes.data)
-    if raw:
-        return rc
-    if rc != 0:
-        raise RuntimeError(f"probe_sqr_sqrt({dev}, {op}) returned {rc}")
-    return out
+    rc = L.probe_sqr_sqrt(dev.encode(), op, x.size, ptrs([x]), out.ctypes.data)
+    return result(rc, raw, f"probe_sqr_sqrt({dev}, {op})", out)
