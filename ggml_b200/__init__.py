@@ -378,21 +378,26 @@ def op_diag_mask_inf(x, n_past: int):
     return y
 
 
-def op_soft_max(x, scale: float = 1.0, diag_n_past: int = -1):
-    """row softmax of a contiguous f32 [ne3?, ne2, ne1, ne0] tensor; diag_n_past >= 0: the fused SCALE -> DIAG_MASK_INF -> SOFT_MAX pass"""
+def op_soft_max(x, scale: float = 1.0, diag_n_past: int = -1, mask=None, max_bias: float = 0.0, inplace: bool = False):
+    """row softmax of a contiguous f32 [ne3?, ne2, ne1, ne0] tensor; diag_n_past >= 0: the fused SCALE -> DIAG_MASK_INF -> SOFT_MAX pass.
+    mask: a contiguous f16 or f32 [ne01 >= ne1, ne0] added (times the ALiBi slope of head i2 when max_bias > 0) to row i1 of every matrix,
+    as ggml_soft_max_ext broadcasts it.  inplace: the result is written into x."""
     import torch
     L = lib()
     L.ggml_b200_op_soft_max_diag.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int64] * 4 + [C.c_float, C.c_float, C.c_int32, C.c_void_p]
     sh = [1] * (4 - x.dim()) + list(x.shape)
-    y = torch.empty_like(x)
-    check(L.ggml_b200_op_soft_max_diag(x.data_ptr(), None, 0, y.data_ptr(), sh[3], sh[2], sh[1], sh[0], scale, 0.0, diag_n_past, _stream()), "ggml_b200_op_soft_max_diag")
+    y = x if inplace else torch.empty_like(x)
+    mp, mt = (None, 0) if mask is None else (mask.data_ptr(), {torch.float32: F32, torch.float16: F16}[mask.dtype])
+    check(L.ggml_b200_op_soft_max_diag(x.data_ptr(), mp, mt, y.data_ptr(), sh[3], sh[2], sh[1], sh[0], scale, max_bias, diag_n_past, _stream()),
+          "ggml_b200_op_soft_max_diag")
     return y
 
 
 def op_cpy(src, dst):
+    """GGML_OP_CPY: src and dst torch tensors (any views) or TensorDescs (bytes_desc: a view into a quantized cache)"""
     L = lib()
     L.ggml_b200_op_cpy.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p]
-    s, d = tensor_desc(src), tensor_desc(dst)
+    s, d = (t if isinstance(t, TensorDesc) else strided_desc(t) for t in (src, dst))
     check(L.ggml_b200_op_cpy(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_cpy")
 
 
@@ -496,6 +501,43 @@ def strided_desc(t) -> TensorDesc:
         d.ne[i] = shape[i] if i < len(shape) else 1
         d.nb[i] = strides[i] * es if i < len(shape) else (d.nb[i - 1] * d.ne[i - 1] if i else es)
     return d
+
+
+def bytes_desc(buf, type_: int, ne, nb, offset: int = 0) -> TensorDesc:
+    """descriptor of `type_` elements (block-quantized rows too) in the raw bytes of a cuda uint8 tensor, from byte `offset`, with ne[4]
+    and nb[4] in ggml order given explicitly: a view into a KV cache, as a graph's ggml_view_4d makes it"""
+    d = TensorDesc()
+    d.data, d.type = buf.data_ptr() + offset, type_
+    for i in range(4):
+        d.ne[i], d.nb[i] = ne[i], nb[i]
+    return d
+
+
+def op_flash_attn_ext(q, k, v, mask, scale: float, max_bias: float = 0.0, softcap: float = 0.0):
+    """GGML_OP_FLASH_ATTN_EXT: q f32 [ne3, n_head, n_q, D] (torch order of ggml's [D, n_q, n_head, ne3]; any view with the last dim
+    contiguous, e.g. a permuted one); k and v [nk3, n_head_kv, n_kv, D], torch tensors or TensorDescs (bytes_desc: block rows of a cache
+    view); mask None or f16 [>= n_q, n_kv'] with n_kv' >= n_kv (row i for query i).  Returns a new f32 tensor [ne3, n_q, n_head, D]
+    (ggml's [D, n_head, n_q, ne3])."""
+    import torch
+    ne3, n_head, n_q, D = q.shape
+    y = torch.empty((ne3, n_q, n_head, D), dtype=torch.float32, device=q.device)
+    descs = [strided_desc(q)] + [t if isinstance(t, TensorDesc) else strided_desc(t) for t in (k, v)]
+    L = lib()
+    L.ggml_b200_op_flash_attn_ext.argtypes = [C.POINTER(TensorDesc)] * 5 + [C.c_float] * 3 + [C.c_void_p]
+    m = C.byref(strided_desc(mask)) if mask is not None else None
+    check(L.ggml_b200_op_flash_attn_ext(*(C.byref(d) for d in descs), m, C.byref(tensor_desc(y)), scale, max_bias, softcap, _stream()),
+          "ggml_b200_op_flash_attn_ext")
+    return y
+
+
+def op_mul_mat_f(a, b, out=None):
+    """the float GGML_OP_MUL_MAT (KQ and KQV of non-flash attention): a f32 or f16 [a3, a2, M, K], b f32 (f16 with an f16 a) [b3, b2, N, K],
+    both any views (a transposed V: nb0 != the element size); a's batch dims broadcast over b's.  out: None (a new contiguous tensor) or an
+    f32 tensor [b3, b2, N, M] of any strides.  out[.., n, m] = sum_k a[.., m, k] b[.., n, k], b rounded to f16 first when a is f16 and b f32."""
+    import torch
+    y = out if out is not None else torch.empty(tuple(b.shape[:-1]) + (a.shape[-2],), dtype=torch.float32, device=a.device)
+    _launch("ggml_b200_op_mul_mat_f", strided_desc(a), strided_desc(b), strided_desc(y))
+    return y
 
 
 def op_concat(a, b, dim: int):

@@ -324,10 +324,12 @@ template <int QT> __global__ void cpy_f32_q_kernel(tdesc s, tdesc d, int64_t nbl
     float amax = 0.0f, vmax = 0.0f;
     for (int i = 0; i < 32; ++i) if (amax < fabsf(x[i])) { amax = fabsf(x[i]); vmax = x[i]; }
     if (QT == T_Q8_0) {
-        const float dd = __fdiv_rn(amax, 127.0f), id = dd != 0.0f ? __fdiv_rn(1.0f, dd) : 0.0f;
+        // what ggml-cpu's CPY writes on x86 (quantize_row_q8_0, AVX branch, src/ggml-cpu/ggml-cpu-quants.c:786-830): id = 127 / amax, codes
+        // rounded half to even.  The _ref formula (id = 1 / d, roundf) differs in a few codes per million, more on half-integer inputs.
+        const float dd = __fdiv_rn(amax, 127.0f), id = amax != 0.0f ? __fdiv_rn(127.0f, amax) : 0.0f;
         *(__half *)o = __float2half_rn(dd);
-        for (int i = 0; i < 32; ++i) o[2 + i] = (uint8_t)(int8_t)roundf(__fmul_rn(x[i], id));
-    } else {
+        for (int i = 0; i < 32; ++i) o[2 + i] = (uint8_t)(int8_t)__float2int_rn(__fmul_rn(x[i], id));
+    } else {                                                    // Q4_0: quantize_row_q4_0_ref, which ggml-cpu's CPY calls as well
         const float dd = __fdiv_rn(vmax, -8.0f), id = dd != 0.0f ? __fdiv_rn(1.0f, dd) : 0.0f;
         *(__half *)o = __float2half_rn(dd);
         for (int i = 0; i < 16; ++i) {

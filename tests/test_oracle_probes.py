@@ -1,14 +1,15 @@
-"""CPU-only: the ctypes fronts of the one-node op probes (oracle/{conv,moe,pool,rope,sam,ssm,train,wkv}.py) against their libraries
+"""CPU-only: the ctypes fronts of the one-node op probes (oracle/{attn,conv,moe,pool,rope,sam,ssm,train,wkv}.py) against their libraries
 (oracle/_ref/libggml_<family>_probe.so, over oracle/probe_harness.h).
   - each module's SIGNATURES names exactly the probe_* symbols its library exports, so a signature table cannot drift from the library;
   - every public probe function reports -1 for a device that does not exist ("NOPE"): with raw=True as its code, otherwise as a
-    RuntimeError.  This is the harness's first exit path in all eight libraries; no device is needed for it."""
+    RuntimeError.  This is the harness's first exit path in all nine libraries; no device is needed for it."""
 import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
+from oracle import attn as A
 from oracle import conv as V
 from oracle import moe as M
 from oracle import oracle as O
@@ -19,7 +20,7 @@ from oracle import ssm as SS
 from oracle import train as TR
 from oracle import wkv as W
 
-MODULES = {"conv": V, "moe": M, "pool": P, "rope": R, "sam": S, "ssm": SS, "train": TR, "wkv": W}
+MODULES = {"attn": A, "conv": V, "moe": M, "pool": P, "rope": R, "sam": S, "ssm": SS, "train": TR, "wkv": W}
 
 
 def need(family):
@@ -49,6 +50,10 @@ def _train_source():
 
 # (family, the probe_* symbol it reaches, a call on "NOPE" with a small valid input: its code, or "raises" for the functions without raw)
 CALLS = [
+    ("attn", "probe_flash_attn_ext", lambda: A.flash_attn_ext("NOPE", A.FaCase(32, 3, 1, 2, 1, O.F16, O.F16, mask="causal"), raw=True)),
+    ("attn", "probe_soft_max", lambda: A.soft_max("NOPE", A.SoftMaxCase((8, 2, 3, 1), P.F16, 4, max_bias=8.0), raw=True)),
+    ("attn", "probe_cpy", lambda: A.cpy("NOPE", A.CpyCase(P.Source(P.F32, (32, 2)), O.Q8_0, (32, 2), 4, 1), _f32(2, 32), np.zeros(136, np.uint8),
+                                        raw=True)),
     ("conv", "probe_im2col", lambda: V.im2col("NOPE", V.im2col_grid()[0], raw=True)),
     ("conv", "probe_mul_mat_f16", lambda: V.mul_mat_f16("NOPE", 4, 2, 8, raw=True)),
     ("conv", "probe_conv_1d", lambda: V.conv_1d("NOPE", 3, 2, 2, 8, 1, 0, 1, raw=True)),
