@@ -338,11 +338,12 @@ def op_unary(uop: int, x):
 
 
 def op_norm(x, eps: float, rms: bool = False):
+    """GGML_OP_NORM / RMS_NORM along the last dim of an f32 x (any view with that dim contiguous) -> a new contiguous tensor"""
     import torch
     L = lib()
     L.ggml_b200_op_norm.argtypes = [C.c_int32, C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_float, C.c_void_p]
-    y = torch.empty_like(x)
-    s, d = tensor_desc(x), tensor_desc(y)
+    y = torch.empty(x.shape, dtype=x.dtype, device=x.device)
+    s, d = strided_desc(x), tensor_desc(y)
     check(L.ggml_b200_op_norm(int(rms), C.byref(s), C.byref(d), eps, _stream()), "ggml_b200_op_norm")
     return y
 
@@ -801,6 +802,26 @@ def op_conv_transpose_2d(kernel, x, stride: int):
     y = torch.empty(tuple(x.shape[:-3]) + (cout, (h - 1) * stride + kh, (w - 1) * stride + kw), dtype=torch.float32, device=x.device)
     k, s, d = strided_desc(kernel), strided_desc(x), tensor_desc(y)
     check(L.ggml_b200_op_conv_transpose_2d(C.byref(k), C.byref(s), C.byref(d), stride, _stream()), "ggml_b200_op_conv_transpose_2d")
+    return y
+
+
+def op_get_rows(src, ids, out):
+    """GGML_OP_GET_ROWS: out[i12, i11, i10, :] = row ids[i12, i11, i10] of src's matrix (i11, i12), decoded to f32.  src a torch tensor
+    (any view with packed rows) or a TensorDesc (bytes_desc: block-quantized rows), ggml [ne0, rows, ne11, ne12]; ids i32 [ne12, ne11, n],
+    any view; out f32 [ne12, ne11, n, ne0], any view with packed rows (a padded row stride)"""
+    _launch("ggml_b200_op_get_rows", src if isinstance(src, TensorDesc) else strided_desc(src), strided_desc(ids), strided_desc(out))
+    return out
+
+
+def op_bin_bcast(op: int, a, b, out=None):
+    """GGML_OP_ADD / MUL / SUB / DIV (op 0 / 1 / 2 / 3) of f32 a and b, b's dims dividing a's (ggml's whole-repeat broadcast); a, b and out
+    any views (out = a: in place).  out None: a new contiguous tensor"""
+    import torch
+    y = out if out is not None else torch.empty(a.shape, dtype=torch.float32, device=a.device)
+    L = lib()
+    L.ggml_b200_op_bin_bcast.argtypes = [C.c_int32] + [C.POINTER(TensorDesc)] * 3 + [C.c_void_p]
+    s0, s1, d = strided_desc(a), strided_desc(b), strided_desc(y)
+    check(L.ggml_b200_op_bin_bcast(op, C.byref(s0), C.byref(s1), C.byref(d), _stream()), "ggml_b200_op_bin_bcast")
     return y
 
 

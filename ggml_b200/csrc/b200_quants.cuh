@@ -112,6 +112,12 @@ __device__ __forceinline__ float gelu_ggml(float v) {
     const float g = 0.5f * xh * (1.0f + tanhf(0.79788456080286535587989211986876f * xh * (1.0f + 0.044715f * xh * xh)));
     return __half2float(__float2half_rn(g));
 }
+// GELU_QUICK likewise through ggml-cpu's fp16 -> fp16 table of x * (1 / (1 + expf(-1.702 x))) (ggml_vec_gelu_quick_f32, ggml-cpu.c:1797).
+// It has no cut-offs: |x| >= 65520 reads the table at +-inf, which gives +inf above and NaN (-inf * 0) below.
+__device__ __forceinline__ float gelu_quick_ggml(float v) {
+    const float xh = __half2float(__float2half_rn(v));
+    return __half2float(__float2half_rn(xh * (1.0f / (1.0f + expf(-1.702f * xh)))));
+}
 __device__ __forceinline__ float h2f(uint32_t bits16) { return __half2float(__ushort_as_half((unsigned short)bits16)); }
 
 // n consecutive 32-bit words starting at a 2-byte aligned address (generic/global/shared)

@@ -170,31 +170,54 @@ template <int OP> __global__ void bin_bcast_kernel(tdesc a, tdesc b, tdesc d, in
 }
 
 // ------------------------------------------------------------------ NORM / RMS_NORM (rows contiguous along dim 0)
+// block-wide sum of one double per thread (blockDim multiple of 32, <= 1024); result broadcast to all threads
+__device__ __forceinline__ double block_sum_f64(double v, double * sh) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (nw == 1) return v;
+    __syncthreads();
+    if (lane == 0) sh[warp] = v;
+    __syncthreads();
+    double r = lane < nw ? sh[lane] : 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+    return r;
+}
+
+// A row's mean (0 for RMS_NORM) and scale as ggml-cpu computes them (ggml_compute_forward_norm_f32 / _rms_norm_f32): the sums of x and of
+// the f32 squares in double, the mean and the variance rounded to f32, scale = 1.0f / sqrtf(variance + eps).  Sums in f32 put rows with a
+// common offset of 30 .. 1e4 up to 4340x (in NMSE against f64) further from the true result than ggml-cpu's.
+template <bool RMS> __device__ __forceinline__ void norm_row_stats(const float * x, int64_t n, float eps, double * sh, float & mean, float & scale) {
+    mean = 0.0f;
+    if (!RMS) {
+        double sum = 0.0;
+        for (int64_t i = threadIdx.x; i < n; i += blockDim.x) sum += (double)x[i];
+        mean = (float)(block_sum_f64(sum, sh) / (double)n);
+    }
+    double sq = 0.0;
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i] - mean; sq += (double)(v * v); }
+    const float var = (float)(block_sum_f64(sq, sh) / (double)n);
+    scale = 1.0f / sqrtf(var + eps);
+}
+
 template <bool RMS> __global__ void norm_kernel(tdesc s, tdesc d, float eps) {
     pdl_trigger();
-    __shared__ float sh[32];
+    __shared__ double sh[32];
     const int64_t r = blockIdx.x;
     const int64_t i1 = r % s.ne[1], i2 = (r / s.ne[1]) % s.ne[2], i3 = r / (s.ne[1] * s.ne[2]);
     const float * x = (const float *)(s.data + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
     float * y = (float *)(d.data + i1 * d.nb[1] + i2 * d.nb[2] + i3 * d.nb[3]);
     const int64_t n = s.ne[0];
-    float mean = 0.0f;
-    if (!RMS) {
-        float sum = 0.0f;
-        for (int64_t i = threadIdx.x; i < n; i += blockDim.x) sum += x[i];
-        mean = block_reduce<false>(sum, sh) / (float)n;
-    }
-    float sq = 0.0f;
-    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i] - mean; sq += v * v; }
-    const float var = block_reduce<false>(sq, sh) / (float)n;
-    const float scale = 1.0f / sqrtf(var + eps);
+    float mean, scale;
+    norm_row_stats<RMS>(x, n, eps, sh, mean, scale);
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) y[i] = (x[i] - mean) * scale;
 }
 
 // NORM -> MUL(gain) -> ADD(bias) in one pass; every intermediate tensor of the three ggml nodes is still written
 template <bool RMS> __global__ void norm_affine_kernel(tdesc s, tdesc d1, const float * gain, tdesc d2, const float * bias, tdesc d3, float eps) {
     pdl_trigger();
-    __shared__ float sh[32];
+    __shared__ double sh[32];
     const int64_t r = blockIdx.x;
     const int64_t i1 = r % s.ne[1], i2 = (r / s.ne[1]) % s.ne[2], i3 = r / (s.ne[1] * s.ne[2]);
     const float * x = (const float *)(s.data + i1 * s.nb[1] + i2 * s.nb[2] + i3 * s.nb[3]);
@@ -202,16 +225,8 @@ template <bool RMS> __global__ void norm_affine_kernel(tdesc s, tdesc d1, const 
     float * y2 = (float *)(d2.data + i1 * d2.nb[1] + i2 * d2.nb[2] + i3 * d2.nb[3]);
     float * y3 = (float *)(d3.data + i1 * d3.nb[1] + i2 * d3.nb[2] + i3 * d3.nb[3]);
     const int64_t n = s.ne[0];
-    float mean = 0.0f;
-    if (!RMS) {
-        float sum = 0.0f;
-        for (int64_t i = threadIdx.x; i < n; i += blockDim.x) sum += x[i];
-        mean = block_reduce<false>(sum, sh) / (float)n;
-    }
-    float sq = 0.0f;
-    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i] - mean; sq += v * v; }
-    const float var = block_reduce<false>(sq, sh) / (float)n;
-    const float scale = 1.0f / sqrtf(var + eps);
+    float mean, scale;
+    norm_row_stats<RMS>(x, n, eps, sh, mean, scale);
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
         const float a = (x[i] - mean) * scale, b = __fmul_rn(a, gain[i]), c = __fadd_rn(b, bias[i]);   // separately rounded, like the three ggml ops
         y1[i] = a; y2[i] = b; y3[i] = c;
@@ -246,7 +261,7 @@ __global__ void unary_kernel(int uop, const float * x, float * y, int64_t n) {
         case U_TANH: r = tanhf(v); break;
         case U_NEG: r = -v; break;
         case U_ABS: r = fabsf(v); break;
-        case U_GELU_QUICK: r = v * (1.0f / (1.0f + expf(-1.702f * v))); break;
+        case U_GELU_QUICK: r = gelu_quick_ggml(v); break;
         case U_SIGMOID: r = 1.0f / (1.0f + expf(-v)); break;
         case U_EXP: r = expf(v); break;
         case U_SQR: r = v * v; break;

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY: what the ctypes fronts of the one-node op probes (oracle/{attn,conv,moe,pool,rope,sam,ssm,train,wkv}.py over
+"""TEST INFRASTRUCTURE ONLY: what the ctypes fronts of the one-node op probes (oracle/{attn,conv,core,moe,pool,rope,sam,ssm,train,wkv}.py over
 oracle/_ref/libggml_<family>_probe.so) share: loading a family's library with its signatures, and turning a probe's code into a result."""
 from __future__ import annotations
 

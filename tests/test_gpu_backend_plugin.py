@@ -60,10 +60,12 @@ def test_plugin_vs_cpu_backend_large(plugin):
         assert O.nmse(Yg, Yc) < 1e-10, (O.TYPE_NAMES[t], M, N, K)
 
 
-@pytest.mark.parametrize("op", ["GET_ROWS", "ADD", "MUL", "NORM", "RMS_NORM", "SCALE", "DIAG_MASK_INF", "SOFT_MAX", "GELU", "SILU", "CPY", "CONT", "DUP", "FLASH_ATTN_EXT"])
+@pytest.mark.parametrize("op", ["GET_ROWS", "ADD", "MUL", "NORM", "RMS_NORM", "SCALE", "DIAG_MASK_INF", "SOFT_MAX", "GELU", "SILU", "CPY", "CONT", "DUP",
+                                "FLASH_ATTN_EXT", "DIV", "TANH", "NEG", "ABS", "GELU_QUICK", "SIGMOID", "EXP", "RELU", "STEP"])
 def test_reference_test_backend_ops_small_ops(plugin, op):
-    """the ops either side of the mat-mul in the gpt-2 graph (SURVEY.md §8f-1), gated by the reference's own
-    per-op tolerances (default NMSE 1e-7; CPY/SOFT_MAX 1e-6)"""
+    """the ops either side of the mat-mul in the gpt-2 graph (SURVEY.md §8f-1) and the other binary and unary ops the plug-in accepts
+    (SQR, SQRT, SIN and COS run in tests/test_gpu_rwkv.py and tests/test_gpu_sam.py; the reference's sweep has no SUB case, which
+    tests/test_gpu_core_ops.py covers), gated by the reference's own per-op tolerances (default NMSE 1e-7; CPY/SOFT_MAX 1e-6)"""
     rc, out = run_tbo(plugin, "test", "-o", op, "-b", "B2000")
     tail = "\n".join(out.splitlines()[-25:])
     assert rc == 0 and "FAIL" not in out, tail

@@ -1,8 +1,8 @@
-"""CPU-only: the ctypes fronts of the one-node op probes (oracle/{attn,conv,moe,pool,rope,sam,ssm,train,wkv}.py) against their libraries
+"""CPU-only: the ctypes fronts of the one-node op probes (oracle/{attn,conv,core,moe,pool,rope,sam,ssm,train,wkv}.py) against their libraries
 (oracle/_ref/libggml_<family>_probe.so, over oracle/probe_harness.h).
   - each module's SIGNATURES names exactly the probe_* symbols its library exports, so a signature table cannot drift from the library;
   - every public probe function reports -1 for a device that does not exist ("NOPE"): with raw=True as its code, otherwise as a
-    RuntimeError.  This is the harness's first exit path in all nine libraries; no device is needed for it."""
+    RuntimeError.  This is the harness's first exit path in all ten libraries; no device is needed for it."""
 import shutil
 import subprocess
 
@@ -11,6 +11,7 @@ import pytest
 
 from oracle import attn as A
 from oracle import conv as V
+from oracle import core as K
 from oracle import moe as M
 from oracle import oracle as O
 from oracle import pool as P
@@ -20,7 +21,7 @@ from oracle import ssm as SS
 from oracle import train as TR
 from oracle import wkv as W
 
-MODULES = {"attn": A, "conv": V, "moe": M, "pool": P, "rope": R, "sam": S, "ssm": SS, "train": TR, "wkv": W}
+MODULES = {"attn": A, "conv": V, "core": K, "moe": M, "pool": P, "rope": R, "sam": S, "ssm": SS, "train": TR, "wkv": W}
 
 
 def need(family):
@@ -54,6 +55,15 @@ CALLS = [
     ("attn", "probe_soft_max", lambda: A.soft_max("NOPE", A.SoftMaxCase((8, 2, 3, 1), P.F16, 4, max_bias=8.0), raw=True)),
     ("attn", "probe_cpy", lambda: A.cpy("NOPE", A.CpyCase(P.Source(P.F32, (32, 2)), O.Q8_0, (32, 2), 4, 1), _f32(2, 32), np.zeros(136, np.uint8),
                                         raw=True)),
+    ("core", "probe_get_rows", lambda: K.get_rows("NOPE", K.block_source(O.Q4_0, (32, 3)), np.zeros(54, np.uint8), np.zeros((1, 1, 2), np.int32),
+                                                 raw=True)),
+    ("core", "probe_binary", lambda: K.binary("NOPE", K.ADD, P.Source(P.F32, (4, 3)), _f32(3, 4), P.Source(P.F32, (4, 1)), _f32(1, 4), raw=True)),
+    ("core", "probe_norm", lambda: K.norm("NOPE", True, 1e-6, P.Source(P.F32, (8, 2)), _f32(2, 8), raw=True)),
+    ("core", "probe_unary", lambda: K.unary("NOPE", K.GELU_QUICK, _f32(5), raw=True)),
+    ("core", "probe_scale_mask", lambda: K.scale_mask("NOPE", _f32(2, 3, 4), 0.5, 1, raw=True)),
+    ("core", "probe_cpy", lambda: K.cpy("NOPE", 1, P.Source(P.F32, (4, 3), transpose=True), _f32(4, 3), raw=True)),
+    ("core", "probe_norm_affine", lambda: K.norm_affine("NOPE", False, 1e-5, _f32(2, 8), _f32(8), _f32(8), raw=True)),
+    ("core", "probe_scale_mask_softmax", lambda: K.scale_mask_softmax("NOPE", _f32(2, 3, 4), 0.5, 1, raw=True)),
     ("conv", "probe_im2col", lambda: V.im2col("NOPE", V.im2col_grid()[0], raw=True)),
     ("conv", "probe_mul_mat_f16", lambda: V.mul_mat_f16("NOPE", 4, 2, 8, raw=True)),
     ("conv", "probe_conv_1d", lambda: V.conv_1d("NOPE", 3, 2, 2, 8, 1, 0, 1, raw=True)),
@@ -93,7 +103,15 @@ def test_every_probe_is_called():
     assert {sym for _, sym, _ in CALLS} == {sym for m in MODULES.values() for sym in m.SIGNATURES}
 
 
-@pytest.mark.parametrize("family, symbol, call", CALLS, ids=[sym for _, sym, _ in CALLS])
+def _call_ids():
+    """each call's id: its symbol, prefixed by its family where an earlier family exports the same symbol (attn's and core's probe_cpy)"""
+    ids = []
+    for fam, sym, _ in CALLS:
+        ids.append(f"{fam}-{sym}" if sym in ids else sym)
+    return ids
+
+
+@pytest.mark.parametrize("family, symbol, call", CALLS, ids=_call_ids())
 def test_unknown_device_returns_minus_one(family, symbol, call):
     need(family)
     if symbol in RAISES:
