@@ -76,12 +76,10 @@ static int validate(const ggml_b200_mul_mat_args * a) {
 
 // the int8 mma.sync consume path (mmvq_mma.cu): default for 2 <= n <= 8, and for n = 1 when the rows are very long (K >= 12288: the dp4a kernel's
 // chunks shrink to a few rows there; at K = 8192 the dp4a kernel is still the faster one; threshold chosen on a Blackwell part, not re-measured
-// on the H100).
-// GGML_B200_MMA = 0 never, 2 always; per call GGML_B200_MM_GEMV_MMA / GGML_B200_MM_GEMV_DP4A select explicitly
+// on the H100).  Per call GGML_B200_MM_GEMV_MMA / GGML_B200_MM_GEMV_DP4A select explicitly.
 static bool mma_wanted(const ggml_b200_mul_mat_args & a, mma_plan & pl) {
-    static const int env = getenv("GGML_B200_MMA") ? atoi(getenv("GGML_B200_MMA")) : 1;
     if (a.flags & (GGML_B200_MM_GEMV_V1 | GGML_B200_MM_GEMV_DP4A)) return false;
-    if (!(a.flags & GGML_B200_MM_GEMV_MMA) && (env == 0 || (a.N < 2 && env != 2 && a.K < 12288))) return false;
+    if (!(a.flags & GGML_B200_MM_GEMV_MMA) && a.N < 2 && a.K < 12288) return false;
     return plan_mma(a, pl);
 }
 
@@ -164,8 +162,6 @@ const char * ggml_b200_version(void) { return "ggml-b200 0.1 (sm_90a)"; }
 uint64_t ggml_b200_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 int ggml_b200_sm_count(void) { return sm_count(); }
 int ggml_b200_prepare(void) { return control_block() ? GGML_B200_OK : GGML_B200_ECUDA; }
-// the GEMM records no per-CTA stamp trace
-int ggml_b200_debug_gemm_trace(uint64_t * host_dst, int32_t max_ctas) { (void)host_dst; (void)max_ctas; return 0; }
 int ggml_b200_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -266,8 +262,6 @@ int ggml_b200_mul_mat_gather_supported(const ggml_b200_mul_mat_args * args) {
     sb_plan pl;
     return validate(args) == GGML_B200_OK && args->N == 1 && plan_sb(*args, pl) ? 1 : 0;
 }
-
-int ggml_b200_debug_trace(unsigned long long * out256) { return debug_read_trace(out256); }
 
 int ggml_b200_gather_wait(const uint32_t * flags_local, int32_t world, uint32_t epoch, void * stream) {
     if (!flags_local || world < 1 || world > 8) { set_error("gather_wait: bad arguments"); return GGML_B200_EINVAL; }

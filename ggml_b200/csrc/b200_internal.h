@@ -8,7 +8,6 @@
 
 #include <atomic>
 #include <cstdio>
-#include <cstdlib>
 
 #include "../../include/ggml-b200.h"
 
@@ -21,17 +20,12 @@ int  sm_count();
 // Per-device control block, zeroed once, in 4-byte words:
 //   [0, 64)                    global control words of the mat-vec kernels
 //   [64, 64 + 64 * 8)          64 per-launch scheduling slots of the mat-vec kernels (sb_next_slot)
-//   [1024, 1536)               mat-vec stamp trace (GGML_B200_SB_DEBUG): 32 records of 8 x u64
 //   [2048, 2048 + 64 * 256)    64 slots of 256 self-cleaning split-K flags of the GEMM (tc_flag_slot)
 constexpr int CTL_SPLITK_FLAGS = 2048, TC_FLAG_SLOTS = 64, TC_FLAGS_PER_SLOT = 256;
 unsigned int * control_block();   // nullptr on error (set_error called)
 
 // Programmatic dependent launch: kernels launched through launch_pdl may become resident while their predecessor on the stream still
-// runs; each one orders itself against it with griddepcontrol.wait.  The environment knob read below (= 1) launches them plainly.
-inline bool pdl_enabled() {
-    static const bool on = !(getenv("GGML_B200_NO_PDL") && atoi(getenv("GGML_B200_NO_PDL")) != 0);
-    return on;
-}
+// runs; each one orders itself against it with griddepcontrol.wait.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, const Args &... args) {
     cudaLaunchConfig_t cfg = {};
@@ -39,7 +33,7 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
@@ -85,10 +79,12 @@ int    launch_tma(const ggml_b200_mul_mat_args & a, const tma_plan & pl, cudaStr
 // mmvq_sb.cu (n = 1 bandwidth path)
 bool   plan_sb(const ggml_b200_mul_mat_args & a, sb_plan & pl);
 int    launch_sb(const ggml_b200_mul_mat_args & a, const sb_plan & pl, cudaStream_t st, const ggml_b200_gather * ga = nullptr, const ggml_b200_epilogue * ep = nullptr);
-int    debug_read_trace(unsigned long long * out);
 int    launch_gather_wait(const uint32_t * flags, int world, uint32_t epoch, cudaStream_t st);
 unsigned int * sb_next_slot(unsigned int * ctl);   // the next of the 64 self-resetting scheduling slots
-int64_t l2_prefetch_cap();                         // bytes of W a dependent mat-vec launch pulls into L2 ahead of its predecessor's output
+// bytes of W a dependent mat-vec launch (mmvq_sb and mmvq_mma) pulls into L2 ahead of its predecessor's output: 8 MB of the H100's 50 MB L2
+// (scripts/gemv_sweep.py on an H100, sweeping the cap: q4_K n = 1 and n = 8 dependent launches 12-17 % faster than with 48 MB, within a few
+// % of no prefetch)
+constexpr int64_t L2_PREFETCH_CAP = (int64_t)8 << 20;
 
 // mmvq_mma.cu (bandwidth path, int8 mma.sync consume phase: 2 <= n <= 8, n = 1 on request); workspace: the quantized activation records
 bool   plan_mma(const ggml_b200_mul_mat_args & a, mma_plan & pl);

@@ -40,7 +40,7 @@ struct sb_params {
     int64_t M, K;
     int32_t row_bytes, rows_per_chunk, nchunks, stage_bytes, nstages, ntasks_row;
     unsigned int * counters;      // this launch's scheduling slot: [0] next chunk, [1] finished producers, [2] finished CTAs (all return to 0)
-    unsigned int * ctl;           // device-global control words: [0] exchange epoch, [1] trace launch index
+    unsigned int * ctl;           // device-global control words: [0] exchange epoch
     int32_t ncols; int64_t x_stride;   // activation columns (1..8) and the distance between them in floats; y is [ncols][M]
     int32_t src1_static;          // activations are not produced by the preceding kernel either: never wait for it (independent ops overlap)
     int32_t src0_static;          // weights are not produced by the preceding kernel: prefetch them before griddepcontrol.wait
@@ -49,7 +49,6 @@ struct sb_params {
     // row-sharded multi-GPU: every result is stored straight into each peer's full-length y over NVLink (world == 0: off)
     // fused epilogue (bias add and GELU of the following ggml nodes): y2 = y + bias, y3 = gelu(y2); null = off
     const float * ep_bias; float * ep_y2; float * ep_y3; const float * ep_res;    // ep_res: y3 = y2 + residual instead of gelu(y2)
-    unsigned long long * dbg;     // optional %globaltimer trace (GGML_B200_SB_DEBUG=1): 32 launches x 8 stamps
     int32_t world, rank;
     int64_t row_offset;
     uint32_t epoch;
@@ -66,7 +65,6 @@ struct mma_params {
     const uint8_t * w; const float * x; float * y;
     int64_t M, K;
     int32_t row_bytes, ntiles, nslices, ks, ntask_row, pitch, stage_bytes, nstages;
-    unsigned int * counters;      // null: tiles dealt round-robin; else this launch's scheduling slot: [0] next tile, [1] finished producers
     int32_t ncols; int64_t x_stride;
     int32_t src1_static, src0_static;
     int64_t l2_prefetch_bytes;
@@ -74,7 +72,7 @@ struct mma_params {
     mma_act A;
 };
 
-struct mma_plan { mma_params p; int grid, smem, ng; size_t workspace; };
+struct mma_plan { mma_params p; int grid, smem; size_t workspace; };
 
 // ----------------------------------------------------------------------------- wgmma GEMM (mmq_tc2.cu)
 struct tc2_plan {

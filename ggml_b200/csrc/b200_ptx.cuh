@@ -1,5 +1,5 @@
 // b200_ptx.cuh — device primitives shared by the kernel files (sm_90a): mbarriers, 1-D bulk copies (TMA) and the L2 bulk prefetch,
-// the async-proxy fence, programmatic dependent launch, %globaltimer, warp reductions.
+// the async-proxy fence, programmatic dependent launch, warp reductions.
 #pragma once
 #include <stdint.h>
 
@@ -46,8 +46,6 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 // ---- programmatic dependent launch: let the next kernel's prologue start / wait for the previous kernel's results
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-__device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 
 // ---- warp reductions (butterfly: every lane gets the result)
 __device__ __forceinline__ float warp_sum(float v) {

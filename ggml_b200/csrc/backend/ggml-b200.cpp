@@ -1348,9 +1348,8 @@ static ggml_status graph_compute_impl(backend_ctx * ctx, ggml_cgraph * cgraph, i
 ggml_status backend_graph_compute(ggml_backend_t backend, ggml_cgraph * cgraph) {
     backend_ctx * ctx = (backend_ctx *) backend->context;
     scoped_device sd(ctx->device);
-    static const bool profile = getenv("GGML_B200_PROFILE") && atoi(getenv("GGML_B200_PROFILE")) != 0;
     int mode = 3, n_real = 0;
-    if (!profile) return graph_compute_impl(ctx, cgraph, mode, n_real);
+    if (!profile_on()) return graph_compute_impl(ctx, cgraph, mode, n_real);
     const auto t0 = std::chrono::steady_clock::now();
     const ggml_status st = graph_compute_impl(ctx, cgraph, mode, n_real);
     const double us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count();

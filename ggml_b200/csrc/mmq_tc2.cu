@@ -364,12 +364,10 @@ static bool tc2_unit_geometry(int type, int & raw, int & ksteps) {
 // shared memory: the raw ring (2 units of 256 rows) first, then as many operand stages (>= 2: a stage is rewritten two steps after
 // its MMAs were issued, and wait_group 1 has completed them by then) as fit the 227 KB an H100 block may use
 static bool tc2_smem_plan(int BN, int raw, int & nstages, int & smem) {
-    static const int env_stages = getenv("GGML_B200_TC2_STAGES") ? atoi(getenv("GGML_B200_TC2_STAGES")) : 0;
     const int stage = T2_BM * T2_BK * 2 + BN * T2_BK * 2;
     const int tail = 2 * T2_BM * raw + (2 * T2_MAX_STAGES + 4) * 8 + BN * 4 + 1024;       // + 1024: alignment of the ring
     int ns = (227 * 1024 - tail) / stage;
     if (ns > T2_MAX_STAGES) ns = T2_MAX_STAGES;
-    if (env_stages >= 2 && env_stages < ns) ns = env_stages;
     if (ns < 2) return false;
     nstages = ns; smem = ns * stage + tail;
     return true;
@@ -394,17 +392,13 @@ static bool plan_tc2(const ggml_b200_mul_mat_args & a, bool x_f16, tc2_plan & pl
     if (x_f16 && (a.nb11 < rb || (a.nb11 % 16) != 0 || ((uintptr_t)a.src1 & 15) != 0)) return false;
     if (a.M >= (1ll << 31) || a.N >= (1ll << 31) || rb >= (1ull << 31)) return false;
     if (!tc_get_encode()) return false;
-    static const int env_bn = getenv("GGML_B200_TC2_BN") ? atoi(getenv("GGML_B200_TC2_BN")) : 0;
-    int BN = a.N > 64 ? 128 : 64;                                  // 2 x 128 rows x 128 columns of f32 accumulators: 128 registers per thread
-    if (env_bn == 64 || env_bn == 128) BN = env_bn;
+    const int BN = a.N > 64 ? 128 : 64;                            // 2 x 128 rows x 128 columns of f32 accumulators: 128 registers per thread
     pl.BN = BN;
     pl.n_tiles = (int)((a.N + BN - 1) / BN);
     pl.m_tiles = (int)((a.M + T2_BM - 1) / T2_BM);
     pl.chunks = (int)(a.K / (T2_BK * ksteps));                     // units along K
     const int tiles = pl.m_tiles * pl.n_tiles;
     int splitk = sm_count() / tiles; if (splitk < 1) splitk = 1; if (splitk > 8) splitk = 8; if (splitk > pl.chunks) splitk = pl.chunks;
-    static const int env_splitk = getenv("GGML_B200_TC_SPLITK") ? atoi(getenv("GGML_B200_TC_SPLITK")) : 0;
-    if (env_splitk > 0 && env_splitk <= pl.chunks) splitk = env_splitk;
     if (splitk > 1 && tiles > TC_FLAGS_PER_SLOT) splitk = 1;
     pl.splitk = splitk;
     if (!tc2_smem_plan(BN, raw, pl.nstages, pl.smem)) return false;
@@ -481,8 +475,7 @@ static bool dense_source_type(int t) {
     }
 }
 bool plan_dense(const ggml_b200_mul_mat_args & a, dense_plan & pl) {
-    static const bool env_off = getenv("GGML_B200_TC_DENSE") && atoi(getenv("GGML_B200_TC_DENSE")) == 0;
-    if (env_off || !dense_source_type(a.type) || a.N < 9 || a.K % 256 != 0) return false;
+    if (!dense_source_type(a.type) || a.N < 9 || a.K % 256 != 0) return false;
     if (a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1 || a.nb01 != row_bytes(a.type, a.K)) return false;
     pl.wbytes = ((size_t)a.M * (size_t)a.K * 2 + 255) & ~(size_t)255;
     ggml_b200_mul_mat_args & b = pl.b;

@@ -20,8 +20,6 @@
 #include "b200_iq.cuh"
 #include "b200_ptx.cuh"
 
-#include <cstdlib>
-
 namespace b200 {
 
 // =============================================================================== activation quantizer
@@ -234,16 +232,12 @@ bool plan_tma(const ggml_b200_mul_mat_args & a, tma_plan & pl) {
     const int nc = a.N == 1 ? 1 : a.N == 2 ? 2 : a.N <= 4 ? 4 : 8;
     const int nunits = (int)(a.K / 64);
     int P = (nunits + 31) / 32; if (P > 8) P = 8;
-    // tunables (env, for sweeps): stage size target, ring depth, CTAs per SM
-    static const int env_stage_kb = getenv("GGML_B200_GEMV_STAGE_KB") ? atoi(getenv("GGML_B200_GEMV_STAGE_KB")) : 18;
-    static const int env_stages   = getenv("GGML_B200_GEMV_STAGES")   ? atoi(getenv("GGML_B200_GEMV_STAGES"))   : 3;
-    static const int env_per_sm   = getenv("GGML_B200_GEMV_CTAS")     ? atoi(getenv("GGML_B200_GEMV_CTAS"))     : 0;
-    static const int env_warps    = getenv("GGML_B200_GEMV_WARPS")    ? atoi(getenv("GGML_B200_GEMV_WARPS"))    : 4;
-    const size_t target = (size_t)env_stage_kb * 1024;
+    // stage size target 18 KB, a ring of 3 stages, at most 4 warps' worth of row-groups
+    const size_t target = 18 * 1024;
     int granule = 1; while ((granule * rb) % 16 != 0) granule *= 2;
     // rows per tile pass: G row-groups x R rows (register blocking); pick the largest G*R that fits the stage target
     const int rpref = nc == 1 ? 4 : nc == 2 ? 2 : 1;
-    int gmax = env_warps / P; if (gmax < 1) gmax = 1;
+    int gmax = 4 / P; if (gmax < 1) gmax = 1;
     int G = 1, r = 1;
     for (int rr = rpref; rr >= 1; rr >>= 1)
         for (int gg = gmax; gg >= 1; --gg)
@@ -251,21 +245,19 @@ bool plan_tma(const ggml_b200_mul_mat_args & a, tma_plan & pl) {
     int step = G * r; while (step % granule != 0) step += G * r;
     int RB = (int)(target / rb) / step * step; if (RB < step) RB = step;
     if ((size_t)RB * rb > 56 * 1024) return false;
-    int nstages = env_stages < 2 ? 2 : env_stages > TMA_MAX_STAGES ? TMA_MAX_STAGES : env_stages;
 
     tma_params & p = pl.p;
     p.w = (const uint8_t *)a.src0; p.x = a.src1; p.y = a.dst; p.nb11 = a.nb11; p.M = a.M; p.K = a.K; p.N = (int)a.N;
     p.row_bytes = (int)rb; p.RB = RB; p.P = P; p.G = G;
     p.nchunks = (int)((a.M + RB - 1) / RB);
     p.stage_bytes = (int)(((size_t)RB * rb + 127) & ~(size_t)127);
-    p.L = L; p.nstages = nstages;
+    p.L = L; p.nstages = 3;
     pl.nc = nc; pl.r = r;
     pl.block = 32 * P * G;
     pl.smem = p.nstages * p.stage_bytes + nc * L.bytes + 2 * RB * nc * P * 4 + TMA_MAX_STAGES * 8 + 16;
     while (pl.smem > 200 * 1024 && p.nstages > 2) { p.nstages--; pl.smem -= p.stage_bytes; }
     if (pl.smem > 200 * 1024) return false;
     int per_sm = (224 * 1024) / (pl.smem + 1024); if (per_sm < 1) per_sm = 1; if (per_sm > 8) per_sm = 8;
-    if (env_per_sm > 0 && env_per_sm < per_sm) per_sm = env_per_sm;
     if (per_sm * pl.block > 2048) per_sm = 2048 / pl.block;
     int grid = sm_count() * per_sm;
     if (grid > p.nchunks) grid = p.nchunks;

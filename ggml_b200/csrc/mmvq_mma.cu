@@ -1,11 +1,12 @@
 // mmvq_mma.cu — the bandwidth-path quantized mat-mul for small batches (2 <= n <= 8; n = 1 on request) on int8 mma.sync.
 //
 // Same streaming skeleton as mmvq_sb.cu (persistent CTAs, one TMA producer warp, a ring of bulk-copy stages with full / empty
-// mbarriers, chunks handed out by a self-resetting atomic slot, programmatic dependent launch, weights read once from HBM in the
-// reference's packed layout), different consume phase (b200_sb_mma.cuh):
-//   * a chunk is a TILE of 16 weight rows; the eight consumer warps of a group split the tile's K range by 256-weight task (task i of a
-//     slice goes to warp i mod 8), each multiplying its 16 x 256 weights with all (<= 8) activation columns on the tensor cores
-//     (m16n8k32, int8 x int8 -> int32, exactly the integer block dots of ggml-cpu) and keeping 4 f32 partial outputs per lane;
+// mbarriers, programmatic dependent launch, weights read once from HBM in the reference's packed layout), different consume phase
+// (b200_sb_mma.cuh):
+//   * a chunk is a TILE of 16 weight rows, dealt to the CTAs round-robin; the eight consumer warps split the tile's K range by
+//     256-weight task (task i of a slice goes to warp i mod 8), each multiplying its 16 x 256 weights with all (<= 8) activation
+//     columns on the tensor cores (m16n8k32, int8 x int8 -> int32, exactly the integer block dots of ggml-cpu) and keeping 4 f32
+//     partial outputs per lane;
 //   * rows too long for a ring of whole-row stages are streamed in K slices of KS tasks (consecutive stages of the same tile, the
 //     accumulators stay in registers across them);
 //   * every row of a stage is its own bulk copy into a padded pitch (= 32 mod 128 bytes), so that the 8-byte fragment loads of the
@@ -23,13 +24,12 @@
 #include "b200_sb_mma.cuh"
 
 #include <algorithm>
-#include <cstdlib>
 
 namespace b200 {
 
 constexpr int MMA_MAX_STAGES = 8;
 constexpr int MMA_TILE = 16;             // rows per tile (the m of m16n8k32)
-constexpr int MMA_GROUP_WARPS = 8;       // consumer warps per group
+constexpr int MMA_GROUP_WARPS = 8;       // consumer warps per CTA
 
 // one act-task (256 activations of one column) per half-warp.  Always waits for the preceding kernel: it may have produced x, and the
 // records live in the launch-shared workspace that the previous mat-mul's CTAs may still be reading.
@@ -43,46 +43,38 @@ __global__ void __launch_bounds__(256) mma_quantize_kernel(const float * __restr
     mma_quantize_task_h<KQ, S16, S81>(x + (size_t)c * x_stride, ok, rec + (size_t)c * A.col_bytes, A, t);
 }
 
-// NG consumer groups per CTA, each = 8 consumer warps + its own producer warp, stage ring, barriers and tile sequence (group v of the
-// NG * grid "virtual CTAs" takes tiles v, v + NG * grid, ...); the groups share the activation records.  Two groups drift out of phase, so one
-// group's fragment loads overlap the other's mma / scaling arithmetic, and a tile round costs a group-time instead of a CTA-time.
-template <int T, int NG>
-__global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_kernel(const mma_params p) {
+// 8 consumer warps and one producer warp with its stage ring.  Tiles are dealt round-robin (b, b + grid, ...): a dynamic hand-out (one
+// global atomic per tile) gained nothing, with a few tiles per CTA the atomic's round trip sits between consecutive stages of the ring.
+template <int T>
+__global__ void __launch_bounds__((MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_kernel(const mma_params p) {
     using F = mmafmt<T>;
     constexpr int GW = MMA_GROUP_WARPS;
     extern __shared__ __align__(128) uint8_t smem[];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int grp = warp / (GW + 1), wg = warp - grp * (GW + 1);                    // group, warp within the group (GW = the producer)
-    uint8_t * stages = smem + (size_t)grp * p.nstages * p.stage_bytes;              // this group's ring (p.nstages stages per group)
-    uint8_t * rec    = smem + (size_t)NG * p.nstages * p.stage_bytes;               // ncols planar records
-    float * partial  = (float *)(rec + (size_t)p.ncols * p.A.col_bytes) + grp * (2 * GW * 128);   // per group [2][GW][128]
-    uint64_t * bars  = (uint64_t *)((float *)(rec + (size_t)p.ncols * p.A.col_bytes) + NG * (2 * GW * 128));
-    uint64_t * full  = bars + grp * (2 * MMA_MAX_STAGES);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;                  // warp GW is the producer
+    uint8_t * stages = smem;                                                        // p.nstages stages
+    uint8_t * rec    = smem + (size_t)p.nstages * p.stage_bytes;                    // ncols planar records
+    float * partial  = (float *)(rec + (size_t)p.ncols * p.A.col_bytes);            // [2][GW][128]
+    uint64_t * full  = (uint64_t *)(partial + 2 * GW * 128);
     uint64_t * empty = full + MMA_MAX_STAGES;
-    uint64_t * rec_full = bars + NG * (2 * MMA_MAX_STAGES);                         // the activation records have landed
-    int2 * unit_of   = (int2 *)(rec_full + 2) + grp * MMA_MAX_STAGES;               // (tile, slice) held by each stage; tile < 0 = end
+    uint64_t * rec_full = full + 2 * MMA_MAX_STAGES;                                // the activation records have landed
+    int2 * unit_of   = (int2 *)(rec_full + 2);                                      // (tile, slice) held by each stage; tile < 0 = end
 
     pdl_launch_dependents();
-    if (wg == 0 && lane == 0) {
+    if (tid == 0) {
         for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], GW); }
-        if (grp == 0) mbar_init(rec_full, 1);
+        mbar_init(rec_full, 1);
         mbar_fence_init();
     }
     __syncthreads();
-    const int vcta = (int)blockIdx.x * NG + grp, vgrid = (int)gridDim.x * NG;
 
-    if (wg == GW) {
+    if (warp == GW) {
         // ===== producer warp: lane r copies row r of the tile (slice) — sixteen bulk copies per stage, one barrier
         if (!p.src0_static) pdl_wait();
         int s = 0; uint32_t par = 0; bool wrapped = false;        // ring position: stage, parity of the round, past the first round
-        int tile = vcta;
+        int tile = (int)blockIdx.x;
         bool first = true;
         while (true) {
             const bool valid = tile < p.ntiles;
-            // Tiles are dealt round-robin (v, v + vgrid, ...) unless p.counters is set.  Dynamic hand-out (one global atomic per tile) gained
-            // nothing here: with a few tiles per group the atomic's round trip sits between consecutive stages of the ring.
-            int next = tile + vgrid;
-            if (p.counters && valid && lane == 0) next = (int)atomicAdd(&p.counters[0], 1u) + vgrid;
             const int nsl = valid ? p.nslices : 1;
             for (int sl = 0; sl < nsl; ++sl) {
                 if (wrapped) mbar_wait(&empty[s], par ^ 1u);
@@ -104,20 +96,15 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
             }
             if (first && p.l2_prefetch_bytes > 0 && lane == 0) {
                 // a dependent launch cannot consume before its predecessor's output is visible, but HBM need not idle meanwhile:
-                // virtual CTA v pulls slice v of the matrix into L2, the rings then stream from L2
-                const int64_t per = ((p.l2_prefetch_bytes + vgrid - 1) / vgrid + 15) & ~(int64_t)15;
-                const int64_t lo = (int64_t)vcta * per;
+                // CTA b pulls slice b of the matrix into L2, the rings then stream from L2
+                const int64_t per = ((p.l2_prefetch_bytes + gridDim.x - 1) / gridDim.x + 15) & ~(int64_t)15;
+                const int64_t lo = (int64_t)blockIdx.x * per;
                 const int64_t hi = min(lo + per, p.l2_prefetch_bytes & ~(int64_t)15);
                 for (int64_t o = lo; o < hi; o += 32768) bulk_prefetch_l2(p.w + o, (uint32_t)min((int64_t)32768, hi - o));
             }
             first = false;
             if (!valid) break;
-            tile = p.counters ? __shfl_sync(0xffffffffu, next, 0) : next;
-        }
-        if (p.counters && lane == 0) {
-            // last producer to finish its scheduling resets the counters for the next launch
-            __threadfence();
-            if (atomicAdd(&p.counters[1], 1u) == (unsigned)vgrid - 1) { p.counters[0] = 0; p.counters[1] = 0; __threadfence(); }
+            tile += (int)gridDim.x;
         }
         return;
     }
@@ -132,7 +119,6 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
     mbar_wait(rec_full, 0u);
 
     const int g = lane >> 2, t = lane & 3;
-    const int gtid = wg * 32 + lane;                                                // thread index within the group's consumers
     mma_cols C;
     C.b  = rec + (size_t)min(g, p.ncols - 1) * p.A.col_bytes;                       // columns beyond n repeat the last one (results discarded)
     C.c0 = rec + (size_t)min(2 * t, p.ncols - 1) * p.A.col_bytes;
@@ -146,20 +132,20 @@ __global__ void __launch_bounds__(NG * (MMA_GROUP_WARPS + 1) * 32, 1) mmvq_mma_k
         if (unit.x < 0) break;
         const int nt = min(p.ks, p.ntask_row - unit.y * p.ks);
         const uint8_t * st = stages + (size_t)s * p.stage_bytes + (size_t)g * p.pitch;
-        for (int i = wg; i < nt; i += GW)
+        for (int i = warp; i < nt; i += GW)
             mma_task<T>(st + (size_t)i * F::TASK_B, st + (size_t)i * F::TASK_B + (size_t)8 * p.pitch, C, p.A, unit.y * p.ks + i, t, facc);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);
         if (++s == p.nstages) { s = 0; par ^= 1u; }
         if (unit.y == p.nslices - 1) {
-            // tile finished: the group's eight partial fragments meet in shared memory and are summed in warp order
+            // tile finished: the eight partial fragments meet in shared memory and are summed in warp order
             float * part = partial + buf * (GW * 128);
-            *(float4 *)(part + wg * 128 + lane * 4) = make_float4(facc[0], facc[1], facc[2], facc[3]);
+            *(float4 *)(part + warp * 128 + lane * 4) = make_float4(facc[0], facc[1], facc[2], facc[3]);
             facc[0] = facc[1] = facc[2] = facc[3] = 0.0f;
-            asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "n"(GW * 32) : "memory");   // this group's consumers only
-            if (gtid < 128) {
+            asm volatile("bar.sync 1, %0;" ::"n"(GW * 32) : "memory");                  // consumers only
+            if (tid < 128) {
                 // thread o writes (column o / 16, row o % 16): consecutive threads, consecutive rows of one column
-                const int col = gtid >> 4, row = gtid & 15;
+                const int col = tid >> 4, row = tid & 15;
                 const int src = ((row & 7) * 4 + (col >> 1)) * 4 + (row >> 3) * 2 + (col & 1);
                 float sum = part[src];
 #pragma unroll
@@ -186,53 +172,35 @@ template <int T> static bool make_mma_plan(const ggml_b200_mul_mat_args & a, mma
     p.ntask_row = (int)(a.K / 256);
     p.A = make_mma_act(a.K, F::KQ, F::S16, F::RESIDUE, mma_s81<T>::value);
     p.ncols = (int32_t)a.N; p.x_stride = a.N > 1 ? (int64_t)(a.nb11 / 4) : 0;
-    p.counters = nullptr; p.rec_global = nullptr;
+    p.rec_global = nullptr;
     p.src0_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
     p.src1_static = (a.flags & GGML_B200_MM_SRC1_STATIC) ? 1 : 0;
-    const int64_t l2_cap = l2_prefetch_cap();
-    p.l2_prefetch_bytes = (p.src0_static && l2_cap > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)l2_cap) : 0;
-    // slices of KS tasks (a multiple of the warp count): whole rows when at least three such stages fit next to the records
-    static const int e_ks = getenv("GGML_B200_MMA_KS") ? atoi(getenv("GGML_B200_MMA_KS")) : 0;
-    static const int e_stages = getenv("GGML_B200_MMA_STAGES") ? atoi(getenv("GGML_B200_MMA_STAGES")) : 0;
-    // consumer groups per CTA: 1 by default, GGML_B200_MMA_GROUPS = 2 for two independent groups (the consume phase is bound by a per-SM
-    // rate, not by latency, so more warps on one tile do not help).
-    static const int e_groups = getenv("GGML_B200_MMA_GROUPS") ? atoi(getenv("GGML_B200_MMA_GROUPS")) : 1;
+    p.l2_prefetch_bytes = p.src0_static ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)L2_PREFETCH_CAP) : 0;
+    // the records, the partial fragments [2][GW][128], the full / empty barriers, the records' barrier, the (tile, slice) of each stage
     const size_t budget = 226 * 1024;
-    for (int ng = e_groups == 2 ? 2 : 1; ng >= 1; --ng) {            // two groups when each gets a ring of >= 2 stages next to the records
-        pl.ng = ng;
-        const size_t fixed = (size_t)p.ncols * p.A.col_bytes + (size_t)ng * 2 * MMA_GROUP_WARPS * 128 * 4 + (size_t)ng * 2 * MMA_MAX_STAGES * 8 + 16
-                           + (size_t)ng * MMA_MAX_STAGES * 8 + 128;
-        if (fixed + (size_t)ng * 2 * 8 * F::TASK_B * MMA_TILE > budget) continue;
-        auto geometry = [&](int ks) {
-            p.ks = ks;
-            p.nslices = (p.ntask_row + ks - 1) / ks;
-            int pitch = std::min(ks, p.ntask_row) * F::TASK_B;
-            pitch = (pitch + 15) & ~15;
-            while ((pitch & 127) != F::RESIDUE) pitch += 16;
-            p.pitch = pitch;
-            p.stage_bytes = (pitch * MMA_TILE + 127) & ~127;
-            return (int)std::min<size_t>((budget - fixed) / p.stage_bytes / ng, MMA_MAX_STAGES);   // stages per group
-        };
-        int ks = e_ks > 0 ? e_ks : 16;                   // 16 tasks x 16 rows: 36 KB (Q4_K) .. 70 KB (Q8_0) per stage
-        if (ks > p.ntask_row) ks = p.ntask_row;
-        int nst = geometry(ks);
-        while (nst < (ng == 1 ? 3 : 2) && ks > 8) { ks = std::max(8, ks / 2); nst = geometry(ks); }
-        if (nst < 2) continue;
-        if (e_stages >= 2 && e_stages <= nst) nst = e_stages;
-        p.nstages = nst;
-        pl.smem = (int)(fixed + (size_t)ng * p.nstages * p.stage_bytes);
-        pl.grid = std::min(sm_count(), (p.ntiles + ng - 1) / ng);
-        pl.workspace = (size_t)p.ncols * p.A.col_bytes + 256;       // the activation records, 256-byte aligned
-        return true;
-    }
-    return false;
-}
-
-template <int T, int NG> static int launch_mma_ng(const mma_plan & pl, cudaStream_t st) {
-    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_mma_kernel<T, NG>>(227 * 1024));
-    B200_CUDA_TRY(launch_pdl(mmvq_mma_kernel<T, NG>, dim3(pl.grid), dim3(NG * (MMA_GROUP_WARPS + 1) * 32), pl.smem, st, pl.p));
-    B200_LAUNCH_CHECK();
-    return GGML_B200_OK;
+    const size_t fixed = (size_t)p.ncols * p.A.col_bytes + (size_t)2 * MMA_GROUP_WARPS * 128 * 4 + (size_t)2 * MMA_MAX_STAGES * 8 + 16
+                       + (size_t)MMA_MAX_STAGES * 8 + 128;
+    if (fixed + (size_t)2 * 8 * F::TASK_B * MMA_TILE > budget) return false;
+    // slices of KS tasks (a multiple of the warp count): whole rows when at least three such stages fit next to the records
+    auto geometry = [&](int ks) {
+        p.ks = ks;
+        p.nslices = (p.ntask_row + ks - 1) / ks;
+        int pitch = std::min(ks, p.ntask_row) * F::TASK_B;
+        pitch = (pitch + 15) & ~15;
+        while ((pitch & 127) != F::RESIDUE) pitch += 16;
+        p.pitch = pitch;
+        p.stage_bytes = (pitch * MMA_TILE + 127) & ~127;
+        return (int)std::min<size_t>((budget - fixed) / p.stage_bytes, MMA_MAX_STAGES);
+    };
+    int ks = std::min(16, p.ntask_row);                  // 16 tasks x 16 rows: 36 KB (Q4_K) .. 70 KB (Q8_0) per stage
+    int nst = geometry(ks);
+    while (nst < 3 && ks > 8) { ks = std::max(8, ks / 2); nst = geometry(ks); }
+    if (nst < 2) return false;
+    p.nstages = nst;
+    pl.smem = (int)(fixed + (size_t)p.nstages * p.stage_bytes);
+    pl.grid = std::min(sm_count(), p.ntiles);
+    pl.workspace = (size_t)p.ncols * p.A.col_bytes + 256;       // the activation records, 256-byte aligned
+    return true;
 }
 
 template <int T> static int launch_mma_t(const ggml_b200_mul_mat_args & a, mma_plan pl, cudaStream_t st) {
@@ -240,14 +208,13 @@ template <int T> static int launch_mma_t(const ggml_b200_mul_mat_args & a, mma_p
     if (!a.workspace || a.workspace_size < pl.workspace) { set_error("mul_mat: workspace %zu < %zu", a.workspace_size, pl.workspace); return GGML_B200_EWORKSPACE; }
     uint8_t * rec = (uint8_t *)(((uintptr_t)a.workspace + 255) & ~(uintptr_t)255);
     pl.p.rec_global = rec;
-    unsigned int * ctl = control_block();
-    if (!ctl) return GGML_B200_ECUDA;
-    static const bool e_dynamic = getenv("GGML_B200_MMA_DYNAMIC") && atoi(getenv("GGML_B200_MMA_DYNAMIC")) != 0;
-    pl.p.counters = e_dynamic ? sb_next_slot(ctl) : nullptr;
     B200_CUDA_TRY(launch_pdl(mma_quantize_kernel<F::KQ, F::S16, mma_s81<T>::value>, dim3((unsigned)((pl.p.ncols * pl.p.A.ntask + 15) / 16)), dim3(256), 0, st,
                              a.src1, pl.p.x_stride, (int)pl.p.ncols, pl.p.A, rec));
     B200_LAUNCH_CHECK();
-    return pl.ng == 1 ? launch_mma_ng<T, 1>(pl, st) : launch_mma_ng<T, 2>(pl, st);
+    B200_CUDA_TRY(set_max_dynamic_smem<mmvq_mma_kernel<T>>(227 * 1024));
+    B200_CUDA_TRY(launch_pdl(mmvq_mma_kernel<T>, dim3(pl.grid), dim3((MMA_GROUP_WARPS + 1) * 32), pl.smem, st, pl.p));
+    B200_LAUNCH_CHECK();
+    return GGML_B200_OK;
 }
 
 bool plan_mma(const ggml_b200_mul_mat_args & a, mma_plan & pl) {

@@ -59,13 +59,6 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     pdl_launch_dependents();
-    // trace slot of this launch (host-chosen): CTA 0 stamps [0..5]; every CTA folds its own times into [6] (latest exit) and
-    // [7] (latest consumer release from griddepcontrol.wait)
-    unsigned long long * dbg = nullptr, * dbg_all = p.dbg;
-    if (p.dbg && blockIdx.x == 0) {
-        dbg = p.dbg;
-        if (tid == 0) dbg[0] = gtime();                          // CTA 0 entry
-    }
 
     if (tid == 0) {
         for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], SB_CONSUMER_WARPS); }
@@ -99,9 +92,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
                 const int64_t hi = min(lo + per, p.l2_prefetch_bytes & ~(int64_t)15);
                 for (int64_t o = lo; o < hi; o += 32768) bulk_prefetch_l2(p.w + o, (uint32_t)min((int64_t)32768, hi - o));
             }
-            if (dbg) dbg[1] = gtime();                            // first TMA issued
             // (the scheduling counters are per launch slot, so the producer never has to wait for the previous grid on their account)
-            if (dbg) dbg[2] = gtime();                            // producer past griddepcontrol.wait                                           // the chunk counter belongs to the previous launch until it completes
             // the next chunk index is fetched (one global atomic round trip) BEFORE waiting for a free stage, so the atomic's
             // latency overlaps the consumers' work instead of delaying the refill
             int it = 1;
@@ -135,8 +126,6 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
 
     // ===== consumers: quantize the activation vector (needs the previous kernel's output)
     if (!p.src1_static) pdl_wait();
-    if (dbg && tid == 0) dbg[3] = gtime();                       // consumers past griddepcontrol.wait
-    if (dbg_all && tid == 0) atomicMax(dbg_all + 7, gtime());
     // one act-task per half-warp per round (this phase is on the critical path of a dependent launch: it can only start once
     // the previous kernel's output is visible)
     for (int i0 = 2 * warp; i0 < p.ncols * p.A.ntask; i0 += 2 * SB_CONSUMER_WARPS) {
@@ -156,9 +145,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, NC > 1 ? 1 : NW == 8 ? 2 : 4) m
     for (int it = 0;; ++it) {
         const int s = it % p.nstages;
         mbar_wait(&full[s], (uint32_t)(it / p.nstages) & 1u);
-        if (dbg && tid == 0 && it == 0) dbg[4] = gtime();        // first stage landed
         const int chunk = chunk_of[s];
-        if (chunk < 0) { if (dbg && tid == 0) dbg[5] = gtime(); if (dbg_all && tid == 0) atomicMax(dbg_all + 6, gtime()); break; }   // last stage done
+        if (chunk < 0) break;                                     // last stage done
         const int64_t row0 = (int64_t)chunk * p.rows_per_chunk;
         const int rows = (int)min((int64_t)p.rows_per_chunk, p.M - row0);
         const uint8_t * st = stages + (size_t)s * p.stage_bytes;
@@ -280,13 +268,6 @@ __global__ void gather_wait_kernel(const uint32_t * flags, int world, uint32_t e
 static std::atomic<unsigned> g_sb_slot_seq{0};
 unsigned int * sb_next_slot(unsigned int * ctl) { return ctl + 64 + (g_sb_slot_seq.fetch_add(1, std::memory_order_relaxed) % 64u) * 8; }
 
-// L2 prefetch cap of dependent launches (mmvq_sb and mmvq_mma), in MB below: 8 MB of the H100's 50 MB L2 (scripts/gemv_sweep.py on an H100,
-// sweeping this knob: q4_K n = 1 and n = 8 dependent launches 12-17 % faster than with 48 MB, within a few % of no prefetch)
-int64_t l2_prefetch_cap() {
-    static const int mb = getenv("GGML_B200_SB_L2_MB") ? atoi(getenv("GGML_B200_SB_L2_MB")) : 8;
-    return mb > 0 ? (int64_t)mb << 20 : 0;
-}
-
 template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_plan & pl) {
     using F = sbfmt<T>;
     if (a.N < 1 || a.N > 8 || a.ne02 != 1 || a.ne03 != 1 || a.ne12 != 1 || a.ne13 != 1) return false;
@@ -301,22 +282,14 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     // small CTAs (4 consumer warps, 18 KB stages) of which four launches share an SM, a deep pipeline ACROSS launches; a dependent
     // launch wants its prologue short and its prefetch deep: 8 consumer warps, 36 KB stages, two launches per SM, W pulled into L2.
     const bool ind = (a.flags & GGML_B200_MM_SRC1_STATIC) != 0 && a.N == 1;
-    static const int e_stage_kb = getenv("GGML_B200_SB_STAGE_KB") ? atoi(getenv("GGML_B200_SB_STAGE_KB")) : 0;
-    static const int env_stages = getenv("GGML_B200_SB_STAGES")   ? atoi(getenv("GGML_B200_SB_STAGES"))   : 0;
-    static const int env_ctas   = getenv("GGML_B200_SB_CTAS")     ? atoi(getenv("GGML_B200_SB_CTAS"))     : 1;
-    static const int e_warps    = getenv("GGML_B200_SB_WARPS")    ? atoi(getenv("GGML_B200_SB_WARPS"))    : 0;
-    static const int e_resident = getenv("GGML_B200_SB_RESIDENT") ? atoi(getenv("GGML_B200_SB_RESIDENT")) : 0;
-    const int env_warps    = e_warps    ? e_warps    : (ind ? 4 : 8);
-    const int env_resident = e_resident ? e_resident : (ind ? 4 : 2);
-    const int env_stage_kb = e_stage_kb ? e_stage_kb : (ind ? 18 : 36);
-    const int SB_CONSUMER_WARPS = (env_warps == 4 && nc == 1) ? 4 : 8;
+    const int stage_kb = ind ? 18 : 36;
+    const int SB_CONSUMER_WARPS = ind ? 4 : 8;
     pl.nw = SB_CONSUMER_WARPS;
     constexpr int RPW = 32 / F::LPR;
     // two rows per lane group sharing the activation loads (Q4_K / Q5_K, n = 1): faster on dependent launches (the consume phase is bounded by
-    // shared-memory traffic, most of it activation reads), slower for independent launches (fewer co-resident CTAs): default for DEPENDENT
-    // launches with enough tasks per row.  GGML_B200_SB_TWOROW = 0 off, 1 always
-    static const int e_two = getenv("GGML_B200_SB_TWOROW") ? atoi(getenv("GGML_B200_SB_TWOROW")) : 2;
-    pl.two = nc == 1 && (T == T_Q4_K || T == T_Q5_K) && (e_two == 1 || (e_two == 2 && !ind && a.K >= 2048 && a.M >= 2048 && (size_t)(SB_CONSUMER_WARPS * RPW * 2) * rb <= 100 * 1024));
+    // shared-memory traffic, most of it activation reads), slower for independent launches (fewer co-resident CTAs): used for DEPENDENT
+    // launches with enough tasks per row, which always run 8-warp CTAs
+    pl.two = nc == 1 && (T == T_Q4_K || T == T_Q5_K) && !ind && a.K >= 2048 && a.M >= 2048 && (size_t)(SB_CONSUMER_WARPS * RPW * 2) * rb <= 100 * 1024;
     // activations held in registers (Q4_K / Q5_K, n = 1, at most 16 tasks per row) in the 4-warp kernel of independent launches: each stage
     // byte is read from shared memory once instead of with a re-read activation record (faster on an H100 at 400 W; the 8-warp kernel of
     // dependent launches, where it measured slower than the two-row form, keeps the shared-memory paths).  The chunk geometry is unchanged.
@@ -325,7 +298,7 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     pl.act_regs = e_areg != 0 && nc == 1 && (T == T_Q4_K || T == T_Q5_K) && a.K <= 16 * 256 && SB_CONSUMER_WARPS == 4;
     int granule = 1; while ((granule * rb) % 16 != 0) granule *= 2;
     int step = SB_CONSUMER_WARPS * RPW * (pl.two ? 2 : 1); while (step % granule != 0) step *= 2;
-    int rpc = (int)(((size_t)env_stage_kb * 1024) / rb) / step * step; if (rpc < step) rpc = step;
+    int rpc = (int)(((size_t)stage_kb * 1024) / rb) / step * step; if (rpc < step) rpc = step;
     if ((size_t)rpc * rb > 100 * 1024) {                         // very long rows: fewer rows per chunk than one full pass
         rpc = granule; while ((size_t)(rpc + granule) * rb <= 48 * 1024) rpc += granule;
         if ((size_t)rpc * rb > 100 * 1024) return false;
@@ -334,58 +307,43 @@ template <int T> static bool make_sb_plan(const ggml_b200_mul_mat_args & a, sb_p
     p.M = a.M; p.K = a.K;
     p.row_bytes = (int)rb; p.rows_per_chunk = rpc; p.nchunks = (int)((a.M + rpc - 1) / rpc);
     p.stage_bytes = (int)(((size_t)rpc * rb + 127) & ~(size_t)127);
-    p.nstages = env_stages;       // 0 = automatic (below)
     p.ntasks_row = (int)(a.K / F::TASK_W);
     p.A = make_sb_act(a.K);
     p.w = nullptr; p.x = nullptr; p.y = nullptr;                 // bound at launch (launch_sb_t)
-    p.ctl = nullptr; p.counters = nullptr; p.dbg = nullptr;      // assigned at launch (assign_sb_slot): planning has no side effects
+    p.ctl = nullptr; p.counters = nullptr;                       // assigned at launch (assign_sb_slot): planning has no side effects
     p.src0_static = (a.flags & GGML_B200_MM_SRC0_STATIC) ? 1 : 0;
-    const int64_t l2_cap = l2_prefetch_cap();
-    p.l2_prefetch_bytes = (!ind && p.src0_static && l2_cap > 0) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)l2_cap) : 0;
+    p.l2_prefetch_bytes = (!ind && p.src0_static) ? (int64_t)std::min<size_t>((size_t)a.M * rb, (size_t)L2_PREFETCH_CAP) : 0;
     p.world = 0; p.rank = 0; p.row_offset = 0; p.epoch = 0;
     p.ep_bias = nullptr; p.ep_y2 = nullptr; p.ep_y3 = nullptr; p.ep_res = nullptr;
     p.src1_static = (a.flags & GGML_B200_MM_SRC1_STATIC) ? 1 : 0;
-    // GGML_B200_SB_STATIC: 0 = dynamic hand-out everywhere, 1 = round-robin everywhere, 2 = round-robin for dependent launches only;
-    // unset: round-robin for independent launches with few chunks per CTA (below)
-    static const int e_static = getenv("GGML_B200_SB_STATIC") ? atoi(getenv("GGML_B200_SB_STATIC")) : -1;
     p.ncols = (int32_t)a.N; p.x_stride = a.N > 1 ? (int64_t)(a.nb11 / 4) : 0;
     for (int q = 0; q < 8; ++q) { p.y_peers[q] = nullptr; p.flag_peers[q] = nullptr; }
     auto smem_of = [&]() { return p.nstages * p.stage_bytes + nc * p.A.bytes + 2 * SB_MAX_STAGES * 8 + SB_MAX_STAGES * 4 + 64; };
     const int max_res = nc > 1 ? 1 : SB_CONSUMER_WARPS == 8 ? 2 : 4;                       // register-limited residency (__launch_bounds__)
-    int ctas = env_ctas < 1 ? 1 : env_ctas > max_res ? max_res : env_ctas;
-    int resident = env_resident < ctas ? ctas : env_resident > max_res ? max_res : env_resident;
-    if (p.nstages <= 0) {
-        // deepest ring that still lets `resident` CTAs (of consecutive launches) share an SM, so that programmatic dependent
-        // launch can overlap the next mat-vec's prologue and first TMA round trip with this one's tail
-        p.nstages = 4;
-        while (p.nstages > 2 && smem_of() * resident > 226 * 1024) p.nstages--;
-    }
-    if (p.nstages < 2) p.nstages = 2;
-    if (p.nstages > SB_MAX_STAGES) p.nstages = SB_MAX_STAGES;
-    while (smem_of() * ctas > 222 * 1024 && p.nstages > 2) p.nstages--;
-    while (smem_of() * ctas > 222 * 1024 && ctas > 1) ctas--;
+    const int resident = std::min(ind ? 4 : 2, max_res);
+    // deepest ring that still lets `resident` CTAs (of consecutive launches) share an SM, so that programmatic dependent
+    // launch can overlap the next mat-vec's prologue and first TMA round trip with this one's tail
+    p.nstages = 4;
+    while (p.nstages > 2 && smem_of() * resident > 226 * 1024) p.nstages--;
+    while (smem_of() > 222 * 1024 && p.nstages > 2) p.nstages--;
     if (smem_of() > 222 * 1024) return false;
     pl.smem = smem_of();
-    pl.grid = sm_count() * ctas;
-    if (pl.grid > p.nchunks) pl.grid = p.nchunks;
+    pl.grid = std::min(sm_count(), p.nchunks);
     // Independent launches with at most 16 chunks per CTA take them round-robin: the producer's atomic round trip before each refill is
     // not hidden by two stages, and the co-resident launches absorb the imbalance of a few chunks.  With more chunks per CTA the SMs'
     // speed differences add up and the atomic counter balances better.  Measured on an H100 at 700 W: Q4_K 4096 -> 11008 (10 chunks per
     // CTA) 3164 instead of 3144 GB/s, Q4_0 4096 x 4096 (4) 2937 instead of 2792; Q4_K / Q8_0 4096 -> 32000 (30 / 61) 2.5 / 3.8 % slower
     // round-robin.  Dependent launches keep the atomic counter.
-    p.static_chunks = (e_static == 1 || (e_static == 2 && !ind) || (e_static < 0 && ind && p.nchunks <= 16 * pl.grid)) ? 1 : 0;
+    p.static_chunks = (ind && p.nchunks <= 16 * pl.grid) ? 1 : 0;
     return true;
 }
 
 // a launch takes the next of the 64 scheduling slots of this device's control block (self-resetting counters: a slot is free again
-// when its launch has finished scheduling, and 64 launches never overlap on one device) and, in trace mode, the next trace record
+// when its launch has finished scheduling, and 64 launches never overlap on one device)
 static int assign_sb_slot(sb_params & p) {
     p.ctl = control_block();
     if (!p.ctl) return GGML_B200_ECUDA;
     p.counters = sb_next_slot(p.ctl);
-    static const bool env_dbg = getenv("GGML_B200_SB_DEBUG") && atoi(getenv("GGML_B200_SB_DEBUG")) != 0;
-    static std::atomic<unsigned> dbg_seq{0};
-    p.dbg = env_dbg ? (unsigned long long *)(p.ctl + 1024) + (dbg_seq.fetch_add(1, std::memory_order_relaxed) % 32u) * 8 : nullptr;
     return GGML_B200_OK;
 }
 
@@ -412,7 +370,7 @@ template <int T> static int launch_sb_t(const ggml_b200_mul_mat_args & a, sb_pla
         case 1:
             if constexpr (T == T_Q4_K || T == T_Q5_K) {
                 if (pl.act_regs) return launch_sb_nw<T, 4, 1, SB_ACT_REGS>(pl, st);
-                if (pl.two) return pl.nw == 4 ? launch_sb_nw<T, 4, 1, SB_TWO_ROWS>(pl, st) : launch_sb_nw<T, 8, 1, SB_TWO_ROWS>(pl, st);
+                if (pl.two) return launch_sb_nw<T, 8, 1, SB_TWO_ROWS>(pl, st);
             }
             return pl.nw == 4 ? launch_sb_nw<T, 4, 1>(pl, st) : launch_sb_nw<T, 8, 1>(pl, st);
         case 2:  return launch_sb_nw<T, 8, 2>(pl, st);
@@ -431,14 +389,6 @@ int launch_sb(const ggml_b200_mul_mat_args & a, const sb_plan & pl, cudaStream_t
     int rc = GGML_B200_EUNSUPPORTED;                                 // plan_sb accepts TC_FORMATS only
     with_format(TC_FORMATS(), a.type, [&](auto t) { rc = launch_sb_t<t>(a, pl, ga, st, ep); });
     return rc;
-}
-
-int debug_read_trace(unsigned long long * out) {
-    unsigned int * c = control_block();
-    if (!c) return GGML_B200_ECUDA;
-    B200_CUDA_TRY(cudaDeviceSynchronize());
-    B200_CUDA_TRY(cudaMemcpy(out, c + 1024, 32 * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    return GGML_B200_OK;
 }
 
 int launch_gather_wait(const uint32_t * flags, int world, uint32_t epoch, cudaStream_t st) {

@@ -412,11 +412,7 @@ GGML_B200_API int          ggml_b200_sm_count(void);
 GGML_B200_API int          ggml_b200_prepare(void);
 /* number of kernels this library has launched since load (for bench.py's gpu_launches) */
 GGML_B200_API uint64_t     ggml_b200_launch_count(void);
-/* developer diagnostic kept for ABI stability: the GEMM kernel records no per-CTA stamps, so this copies nothing and returns 0 */
-GGML_B200_API int          ggml_b200_debug_gemm_trace(uint64_t * host_dst, int32_t max_ctas);
 GGML_B200_API const char * ggml_b200_version(void);
-/* developer aid (GGML_B200_SB_DEBUG=1): %globaltimer stamps of CTA 0 for the last 32 mat-vec launches, 8 per launch */
-GGML_B200_API int          ggml_b200_debug_trace(unsigned long long * out256);
 
 #ifdef __cplusplus
 }

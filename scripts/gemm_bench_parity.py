@@ -1,6 +1,6 @@
 """Developer aid: the bench's batched-GEMM leg (NBUF distinct matrices, CUDA-graph replays of PDL-overlapped launches flagged
 SRC0|SRC1_STATIC, weights streaming from HBM) with EVERY element of every output checked against the exact f64 product.
-usage: python scripts/gemm_bench_parity.py TYPE M N K [--plain] [--noflags]   (env GGML_B200_TC* select the kernel variant)
+usage: python scripts/gemm_bench_parity.py TYPE M N K [--plain] [--noflags]
   --plain    plain stream launches instead of a CUDA graph        --noflags  MM_AUTO instead of the static flags"""
 import os
 import sys

@@ -1,5 +1,5 @@
 """Developer aid: one batched mul_mat shape on the tensor-core path, timed with CUDA events over CUDA-graph replays (and a plain warm loop for ncu).
-usage: python scripts/gemm_prof.py TYPE M N K [--ncu]   (env GGML_B200_TC2_BN / TC_SPLITK / TC2_STAGES select the kernel variant)"""
+usage: python scripts/gemm_prof.py TYPE M N K [--ncu]"""
 import os
 import sys
 from pathlib import Path

@@ -1,5 +1,7 @@
-"""Developer sweep (not the bench contract): device-time of the mat-vec kernels over shapes / tunables.
-Usage: python scripts/gemv_sweep.py [--types q4_K,q8_0] [--n 1]   (env GGML_B200_GEMV_* select tunables)"""
+"""Developer sweep (not the bench contract): device-time of the mat-vec kernels over shapes.  A retuning edits a planner's constant
+and times the build with this script; each line records the GGML_B200_* variables set (GGML_B200_SB_ACT_REGS=0: the shared-memory
+consume path).
+Usage: python scripts/gemv_sweep.py [--types q4_K,q8_0] [--n 1]"""
 import argparse
 import json
 import os
@@ -78,7 +80,7 @@ def main():
 
 
 def run(a):
-    tun = {k: v for k, v in os.environ.items() if k.startswith("GGML_B200_")}
+    env = {k: v for k, v in os.environ.items() if k.startswith("GGML_B200_")}
     for tn in a.types.split(","):
         t = NAMES[tn]
         for sh in a.shapes.split(","):
@@ -92,7 +94,7 @@ def run(a):
                     us, wb = time_mm(t, M, n, K, flags)
                     kname = ("dp4a" if a.dp4a else "mma" if (a.mma or n > 1) else "gemv") + ("_ind" if IND else "")
                     print(json.dumps({"type": tn, "M": M, "K": K, "N": n, "kernel": {base: kname, g.MM_GEMV | g.MM_GEMV_V1: "gemv_v1"}.get(flags, "generic"),
-                                      "us": round(us, 2), "GBps": round(wb / us / 1e3, 1), "tun": tun}), flush=True)
+                                      "us": round(us, 2), "GBps": round(wb / us / 1e3, 1), "env": env}), flush=True)
 
 
 if __name__ == "__main__":

@@ -3,7 +3,8 @@
 * every function declared in include/ggml-b200.h is exported by libggml-b200-kernels.so, every entry point declared in
   include/ggml-b200-backend.h and the include/ggml-cuda.h facade by libggml-b200.so (symbols only: no compute without a GPU);
 * argument validation of the shim works without a device (error codes, never a CPU fallback);
-* the product (ggml_b200/, the two shared libraries) neither imports nor links anything under oracle/."""
+* the product (ggml_b200/, the two shared libraries) neither imports nor links anything under oracle/;
+* the product reads exactly the environment variables INTEGRATION.md lists."""
 import ctypes as C
 import re
 import subprocess
@@ -117,6 +118,23 @@ def test_product_does_not_touch_the_oracle():
         if so.exists():
             needed = subprocess.run(["readelf", "-d", str(so)], capture_output=True, text=True).stdout
             assert "oracle" not in needed and "probe" not in needed, needed
+
+
+# The plug-in's reference arms (no fusion, no CUDA graphs, the graph-update limit, the host-time profile), the generic-kernel arm, the
+# shared-memory consume arm of the n = 1 mat-vec and the opt-in grouped MUL_MAT_ID.  Everything else is planned from a call's arguments.
+PRODUCT_ENV = {"GGML_B200_DISABLE_FUSION", "GGML_B200_DISABLE_GRAPHS", "GGML_B200_GRAPH_MAX_UPDATES", "GGML_B200_PROFILE",
+               "GGML_B200_FORCE_GENERIC", "GGML_B200_SB_ACT_REGS", "GGML_B200_MMID_GROUPED"}
+
+
+def test_product_reads_only_the_documented_environment():
+    csrc = ROOT / "ggml_b200" / "csrc"
+    read = set()
+    for src in csrc.rglob("*"):
+        if src.suffix in (".cu", ".cuh", ".h", ".cpp"):
+            read |= set(re.findall(r'getenv\(\s*"(GGML_B200_[A-Z0-9_]+)"', src.read_text()))
+    assert read == PRODUCT_ENV, (sorted(read - PRODUCT_ENV), sorted(PRODUCT_ENV - read))
+    doc = next(par for par in (ROOT / "INTEGRATION.md").read_text().split("\n\n") if par.startswith("Environment variables"))
+    assert set(re.findall(r"`(GGML_B200_[A-Z0-9_]+)`", doc)) == PRODUCT_ENV
 
 
 def test_missing_library_fails_loudly(tmp_path, monkeypatch):

@@ -4,8 +4,8 @@ Route pin: ggml_b200_mul_mat_plan (the family code, and the error text on errors
 ggml_b200_mul_mat_gather_supported, ggml_b200_mul_mat_id_workspace_size and ggml_b200_mul_mat_f16_workspace_size over a fixed grid,
 compared with a fixture under tests/golden/.  Planning reads no memory (the pointers are aligned dummies), but it depends on the machine:
 without a CUDA driver no GEMM shape is eligible (no tensor-map encoder), and grid and split-K sizes follow the SM count.  So each
-fixture records the environment it was made in, and the test uses the one that matches, or skips.  Planning also reads GGML_B200_*
-variables, so the test skips when any is set.  Regenerate a fixture for the machine at hand with
+fixture records the environment it was made in, and the test uses the one that matches, or skips.  Planning also reads two
+environment variables (PLANNING_ENV), so the test skips when either is set.  Regenerate a fixture for the machine at hand with
 
     python tests/test_mul_mat_routes.py --regen [--lib path/to/libggml-b200-kernels.so]
 
@@ -45,6 +45,8 @@ MOE = [(g.Q4_K, 1408, 2048, 64, 6, 1, 1), (g.Q4_K, 1408, 2048, 64, 6, 6, 512), (
        (g.Q6_K, 4096, 14336, 8, 2, 2, 512), (g.IQ2_XXS, 2048, 4096, 32, 4, 1, 128), (g.Q4_0, 256, 320, 4, 2, 1, 7)]
 # dense fp16 weights: (M, N, K)
 F16 = [(4096, 512, 4096), (4096, 9, 4096), (4096, 8, 4096), (11008, 64, 4096), (100, 16, 320), (4096, 1, 4096)]
+# the variables a plan depends on besides the call's arguments
+PLANNING_ENV = ("GGML_B200_FORCE_GENERIC", "GGML_B200_MMID_GROUPED")
 
 
 def load(path: Path) -> C.CDLL:
@@ -154,8 +156,8 @@ def regen(lib: Path, out: Path) -> Path:
 @pytest.mark.parametrize("fixture", [pytest.param("mul_mat_routes_nodevice.json.gz", id="nodevice"),
                                      pytest.param("mul_mat_routes_h100.json.gz", id="h100", marks=pytest.mark.gpu)])
 def test_route_pin(fixture):
-    if any(k.startswith("GGML_B200_") for k in os.environ):
-        pytest.skip("a GGML_B200_* variable is set: planning reads them")
+    if any(k in os.environ for k in PLANNING_ENV):
+        pytest.skip(f"one of {PLANNING_ENV} is set: planning reads them")
     L = load(g.KERNELS_SO)
     env = environment(L)
     want = json.loads(gzip.decompress((GOLDEN / fixture).read_bytes()))
