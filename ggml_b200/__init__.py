@@ -121,8 +121,9 @@ class Workspace:
 _ws = Workspace()
 
 
-def mul_mat_args(t, W, X, Y, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, nb=None) -> MulMatArgs:
-    """W: cuda uint8 tensor of packed blocks; X: cuda float32; Y: cuda float32 [ne13, ne12, N, M]."""
+def mul_mat_args(t, W, X, Y, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, nb=None, workspace=None) -> MulMatArgs:
+    """W: cuda uint8 tensor of packed blocks; X: cuda float32; Y: cuda float32 [ne13, ne12, N, M].  workspace: a cuda uint8 tensor
+    handed over whole (its size is what the launch may use), None for the shared grow-only one."""
     ne02, ne03, ne12, ne13 = batch
     rb = row_size(t, K)
     a = MulMatArgs()
@@ -134,18 +135,17 @@ def mul_mat_args(t, W, X, Y, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, nb=None
     else:
         a.nb01, a.nb02, a.nb03, a.nb11, a.nb12, a.nb13 = nb
     a.src0, a.src1, a.dst = W.data_ptr(), X.data_ptr(), Y.data_ptr()
-    need = int(lib().ggml_b200_mul_mat_workspace_size(C.byref(a)))
-    ws = _ws.get(need)
+    ws = workspace if workspace is not None else _ws.get(int(lib().ggml_b200_mul_mat_workspace_size(C.byref(a))))
     a.workspace, a.workspace_size = ws.data_ptr(), ws.numel()
     return a
 
 
-def mul_mat(t, W, X, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, out=None, nb=None):
+def mul_mat(t, W, X, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, out=None, nb=None, workspace=None):
     """GGML_OP_MUL_MAT on the current CUDA stream.  Returns Y[ne13, ne12, N, M] (float32, cuda)."""
     import torch
     ne02, ne03, ne12, ne13 = batch
     Y = out if out is not None else torch.empty((ne13, ne12, N, M), dtype=torch.float32, device="cuda")
-    a = mul_mat_args(t, W, X, Y, M, N, K, batch, flags, nb)
+    a = mul_mat_args(t, W, X, Y, M, N, K, batch, flags, nb, workspace)
     check(lib().ggml_b200_mul_mat(C.byref(a), _stream()), "ggml_b200_mul_mat")
     return Y
 
@@ -161,10 +161,11 @@ def mul_mat_plan(t, M, N, K, flags=MM_AUTO) -> int:
     return int(lib().ggml_b200_mul_mat_plan(C.byref(a)))
 
 
-def mul_mat_id(t, W, X, ids, M, K, n_expert, n_used, nb1cols, n_tok):
-    """GGML_OP_MUL_MAT_ID.  W: packed [n_expert, M, row]; X: f32 [n_tok, nb1cols, K]; ids: int32 [n_tok, >= n_used]."""
+def mul_mat_id(t, W, X, ids, M, K, n_expert, n_used, nb1cols, n_tok, out=None, workspace=None):
+    """GGML_OP_MUL_MAT_ID.  W: packed [n_expert, M, row]; X: f32 [n_tok, nb1cols, K]; ids: int32 [n_tok, >= n_used] (any row stride).
+    out: None (a new tensor) or a contiguous f32 [n_tok, n_used, M]; workspace: as for mul_mat."""
     import torch
-    Y = torch.empty((n_tok, n_used, M), dtype=torch.float32, device="cuda")
+    Y = out if out is not None else torch.empty((n_tok, n_used, M), dtype=torch.float32, device="cuda")
     rb = row_size(t, K)
     a = MulMatIdArgs()
     a.type, a.flags, a.K, a.M = t, 0, K, M
@@ -172,8 +173,7 @@ def mul_mat_id(t, W, X, ids, M, K, n_expert, n_used, nb1cols, n_tok):
     a.nb01, a.nb02, a.nb11, a.nb12 = rb, rb * M, K * 4, K * 4 * nb1cols
     a.ids_nb1 = ids.stride(0) * 4
     a.src0, a.src1, a.ids, a.dst = W.data_ptr(), X.data_ptr(), ids.data_ptr(), Y.data_ptr()
-    need = int(lib().ggml_b200_mul_mat_id_workspace_size(C.byref(a)))
-    ws = _ws.get(need)
+    ws = workspace if workspace is not None else _ws.get(int(lib().ggml_b200_mul_mat_id_workspace_size(C.byref(a))))
     a.workspace, a.workspace_size = ws.data_ptr(), ws.numel()
     check(lib().ggml_b200_mul_mat_id(C.byref(a), _stream()), "ggml_b200_mul_mat_id")
     return Y
@@ -308,15 +308,19 @@ def tensor_desc(t) -> TensorDesc:
     return d
 
 
-def mul_mat_fused(t, W, X, M, K, bias, gelu: bool, residual=None):
-    """y = W.x ; y2 = y + bias ; y3 = gelu(y2) (or y2 + residual) in one launch (n = 1).  Returns (y, y2, y3 or None)."""
+def mul_mat_fused(t, W, X, M, K, bias, gelu: bool, residual=None, out=None, workspace=None):
+    """y = W.x ; y2 = y + bias ; y3 = gelu(y2) (or y2 + residual) in one launch (n = 1).  Returns (y, y2, y3 or None).
+    out: None (new tensors) or (y, y2, y3) f32 tensors of M elements (y3 None without gelu or residual); workspace: as for mul_mat."""
     import torch
     L = lib()
     L.ggml_b200_mul_mat_fused.argtypes = [C.POINTER(MulMatArgs), C.POINTER(Epilogue), C.c_void_p]
-    Y = torch.empty((1, 1, 1, M), dtype=torch.float32, device="cuda")
-    Y2 = torch.empty(M, dtype=torch.float32, device="cuda")
-    Y3 = torch.empty(M, dtype=torch.float32, device="cuda") if (gelu or residual is not None) else None
-    a = mul_mat_args(t, W, X, Y, M, 1, K)
+    if out is not None:
+        Y, Y2, Y3 = out[0].view(1, 1, 1, M), out[1], out[2]
+    else:
+        Y = torch.empty((1, 1, 1, M), dtype=torch.float32, device="cuda")
+        Y2 = torch.empty(M, dtype=torch.float32, device="cuda")
+        Y3 = torch.empty(M, dtype=torch.float32, device="cuda") if (gelu or residual is not None) else None
+    a = mul_mat_args(t, W, X, Y, M, 1, K, workspace=workspace)
     ep = Epilogue()
     ep.bias, ep.dst_bias, ep.unary, ep.dst_unary = bias.data_ptr(), Y2.data_ptr(), (2 if residual is not None else 1 if gelu else 0), (Y3.data_ptr() if Y3 is not None else None)
     ep.residual = residual.data_ptr() if residual is not None else None
@@ -337,12 +341,13 @@ def op_unary(uop: int, x):
     return y
 
 
-def op_norm(x, eps: float, rms: bool = False):
-    """GGML_OP_NORM / RMS_NORM along the last dim of an f32 x (any view with that dim contiguous) -> a new contiguous tensor"""
+def op_norm(x, eps: float, rms: bool = False, out=None):
+    """GGML_OP_NORM / RMS_NORM along the last dim of an f32 x (any view with that dim contiguous) -> a new contiguous tensor, or into
+    out (a contiguous tensor of x's shape)"""
     import torch
     L = lib()
     L.ggml_b200_op_norm.argtypes = [C.c_int32, C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_float, C.c_void_p]
-    y = torch.empty(x.shape, dtype=x.dtype, device=x.device)
+    y = out if out is not None else torch.empty(x.shape, dtype=x.dtype, device=x.device)
     s, d = strided_desc(x), tensor_desc(y)
     check(L.ggml_b200_op_norm(int(rms), C.byref(s), C.byref(d), eps, _stream()), "ggml_b200_op_norm")
     return y

@@ -544,8 +544,10 @@ constexpr int MMID_MAX_EXPERTS = 1024;
 __global__ void __launch_bounds__(1024) mmid_group_kernel(const uint8_t * ids, size_t ids_nb1, int n_tok, int n_used, int n_expert, int BN,
                                                           int32_t * off, int32_t * tile_base, int32_t * perm) {
     __shared__ int hist[MMID_MAX_EXPERTS], cursor[MMID_MAX_EXPERTS];
+    __shared__ int invalid_cursor;
     const int n_pairs = n_tok * n_used;
     for (int x = threadIdx.x; x < n_expert; x += blockDim.x) { hist[x] = 0; cursor[x] = 0; }
+    if (threadIdx.x == 0) invalid_cursor = 0;
     __syncthreads();
     for (int pr = threadIdx.x; pr < n_pairs; pr += blockDim.x) {
         const int x = *(const int32_t *)(ids + (size_t)(pr / n_used) * ids_nb1 + (size_t)(pr % n_used) * 4);
@@ -561,14 +563,22 @@ __global__ void __launch_bounds__(1024) mmid_group_kernel(const uint8_t * ids, s
     for (int pr = threadIdx.x; pr < n_pairs; pr += blockDim.x) {
         const int x = *(const int32_t *)(ids + (size_t)(pr / n_used) * ids_nb1 + (size_t)(pr % n_used) * 4);
         if (x >= 0 && x < n_expert) perm[off[x] + atomicAdd(&cursor[x], 1)] = pr;
+        else                        perm[off[n_expert] + atomicAdd(&invalid_cursor, 1)] = pr;      // after the valid pairs: zeroed, never multiplied
     }
 }
 
-// activation row of sorted position `pos` = b[t][e % nb1cols] of pair perm[pos] -> fp16 row pos with its exact power-of-two scale
+// activation row of sorted position `pos` = b[t][e % nb1cols] of pair perm[pos] -> fp16 row pos with its exact power-of-two scale.
+// A position past the valid pairs holds a pair with an invalid expert id: its dst row is zeroed here (the GEMM never stores it), as the
+// per-pair kernel writes 0 for it.
 __global__ void __launch_bounds__(256) mmid_x_to_f16_kernel(const uint8_t * __restrict__ b, size_t nb11, size_t nb12, int n_used, int nb1cols, const int32_t * __restrict__ off,
-                                                            const int32_t * __restrict__ perm, int n_expert, __half * __restrict__ xh, float * __restrict__ inv_scale, int64_t K) {
+                                                            const int32_t * __restrict__ perm, int n_expert, __half * __restrict__ xh, float * __restrict__ inv_scale, int64_t K,
+                                                            float * __restrict__ y, int64_t M) {
     const int pos = blockIdx.x;
-    if (pos >= off[n_expert]) return;                            // positions past the valid pairs (invalid expert ids) stay unused
+    if (pos >= off[n_expert]) {
+        float * yr = y + (size_t)perm[pos] * M;
+        for (int64_t m = threadIdx.x; m < M; m += blockDim.x) yr[m] = 0.0f;
+        return;
+    }
     const int pr = perm[pos], t = pr / n_used, e = pr % n_used;
     row_to_f16((const float *)(b + (size_t)t * nb12 + (size_t)(e % nb1cols) * nb11), xh + (size_t)pos * K, inv_scale + pos, K);
 }
@@ -609,7 +619,8 @@ template <int T> static int launch_mmid_g(const ggml_b200_mul_mat_id_args & a, c
     int32_t * perm = (int32_t *)(ws + pl.xb_bytes + pl.scale_bytes + pl.tab_bytes);
     mmid_group_kernel<<<1, 1024, 0, st>>>((const uint8_t *)a.ids, a.ids_nb1, (int)a.n_tok, (int)a.n_used, (int)a.n_expert, pl.BN, off, tile_base, perm);
     B200_LAUNCH_CHECK();
-    mmid_x_to_f16_kernel<<<(unsigned)pl.n_pairs, 256, 0, st>>>((const uint8_t *)a.src1, a.nb11, a.nb12, (int)a.n_used, (int)a.nb1cols, off, perm, (int)a.n_expert, xb, inv_scale, a.K);
+    mmid_x_to_f16_kernel<<<(unsigned)pl.n_pairs, 256, 0, st>>>((const uint8_t *)a.src1, a.nb11, a.nb12, (int)a.n_used, (int)a.nb1cols, off, perm, (int)a.n_expert, xb, inv_scale, a.K,
+                                                                      a.dst, a.M);
     B200_LAUNCH_CHECK();
     const size_t rb = row_bytes(a.type, a.K);
     alignas(64) CUtensorMap map_w, map_x;

@@ -172,7 +172,8 @@ GGML_B200_API int ggml_b200_ipc_close(void * dev_ptr);
  * MUL_MAT_ID (src/ggml.c:2735-2762): as[K, M, n_expert] quantized, b[K, nb1cols, n_tok] f32,
  * ids[n_used, n_tok] i32 (row stride ids_nb1 bytes) -> dst[M, n_used, n_tok] f32 contiguous:
  *   dst[t][e][:] = as[ids[t][e]] . b[t][e % nb1cols]
- * Expert routing is resolved on the device (no host synchronisation).
+ * Expert routing is resolved on the device (no host synchronisation).  An id outside [0, n_expert) (the CPU backend asserts on
+ * it) gives dst[t][e][:] = 0, on the per-pair and on the expert-grouped form alike; no weight row is read for it.
  * ------------------------------------------------------------------------------------------- */
 typedef struct ggml_b200_mul_mat_id_args {
     int32_t      type;
