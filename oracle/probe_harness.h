@@ -1,6 +1,6 @@
 // oracle/probe_harness.h — TEST INFRASTRUCTURE ONLY.
 //
-// What the one-node op probes (attn_probe.cpp, conv_probe.cpp, core_probe.cpp, moe_probe.cpp, pool_probe.cpp, rope_probe.cpp,
+// What the op probes (attn_probe.cpp, conv_probe.cpp, core_probe.cpp, grad_probe.cpp, moe_probe.cpp, pool_probe.cpp, rope_probe.cpp,
 // sam_probe.cpp, ssm_probe.cpp, train_probe.cpp, wkv_probe.cpp) share: the context their graph lives in, the view-of-a-parent source of
 // oracle/pool.py's Source, and the run of that graph on a named device.  A probe builds its tensors in probe_ctx(), then hands the context to probe_run, which frees it.
 #pragma once

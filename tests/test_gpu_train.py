@@ -84,18 +84,30 @@ def test_reference_gradients(plugin, op):
     print(f"test-backend-ops grad {op}: {m.group(0) if m else 'no summary'}")
 
 
+# test_reference_mul_mat_gradients: at most this many failing MUL_MAT lines per run, each an MAA failure of at most MAA_FLOOR_MAX
+MAA_FLOOR_LINES = 8
+MAA_FLOOR_MAX = 1e-2
+
+
 def test_reference_mul_mat_gradients(plugin):
-    """MUL_MAT's gradient (OUT_PROD for both sources, REPEAT_BACK over broadcast batches) on B2000.  An OPEN DEFECT is pinned here, not a
-    pass: test-backend-ops draws fresh inputs every run, and on B2000 a run has had up to three f32 x f32 cases (none in some runs) with m = 16, K = 256
-    (different ones from run to run, permuted or not) whose finite-difference check exceeds its MAA bound of 1e-4 (1.1e-4 to 6.8e-4 seen),
-    where ggml-cpu passed all 3504 cases.  The cause is not isolated.  What is held: every other case passes, and a failure is only that
-    MAA check on such a case."""
+    """MUL_MAT's gradient (OUT_PROD for both sources, REPEAT_BACK over broadcast batches) on B2000.  Every case passes but for the
+    finite-difference MAA check of f32 x f32 cases (all of them m = 16, K = 256), which fails on ggml-cpu at the same rate:
+    tests/test_oracle_mul_mat_grad.py replays it on fixed inputs, and ggml-cpu fails 40 of 760 (case, seed, parameter) checks (5.3%, about
+    two per test-backend-ops run); on the same inputs B2000's gradients are bit-identical to ggml-cpu's and its MAA failures are as few
+    (tests/test_gpu_mul_mat_grad.py: 1 against ggml-cpu's 2 of 152, on the same element where both fail).  Each failure is
+    an element whose exact gradient is at the numerical gradient's rounding floor (|gn - ga| <= 1.6e-4 everywhere): its term
+    |(gn - ga) / (gn + ga)| is of order 1 (exactly 1 where fu == fd) against a gate of 1e-4 on the mean, so the MAA comes out near
+    1 / (the parameter's element count), 3.9e-3 at most for test-backend-ops' cases (measured: 1.1e-4 to 6.9e-4).  Correctness is held
+    element by element, without this allowance, by those two files.  What this test allows: at most MAA_FLOOR_LINES failing lines (P < 3e-4
+    at two expected), each an MAA failure of at most MAA_FLOOR_MAX on such a case."""
     rc, out, failed = grad_run(plugin, "MUL_MAT", "B2000")
     lines = [l for l in out.splitlines() if "FAIL" in l and l.strip().startswith("MUL_MAT(")]
     print(f"MUL_MAT grad on B2000: {len(lines)} failing case(s)")
     print("\n".join(lines))
+    assert len(lines) <= MAA_FLOOR_LINES, len(lines)
     for l in lines:
-        assert "type_a=f32,type_b=f32,m=16," in l and ",k=256," in l and re.search(r"MAA = [0-9.e+-]+ > 0\.000100000 compare failed", l), l
+        m = re.search(r"MAA = ([0-9.e+-]+) > 0\.000100000 compare failed", l)
+        assert "type_a=f32,type_b=f32,m=16," in l and ",k=256," in l and m and float(m.group(1)) <= MAA_FLOOR_MAX, l
 
 
 # ------------------------------------------------------------------ (b) probe parity, device vs ggml-cpu

@@ -1,8 +1,8 @@
-"""CPU-only: the ctypes fronts of the one-node op probes (oracle/{attn,conv,core,moe,pool,rope,sam,ssm,train,wkv}.py) against their libraries
+"""CPU-only: the ctypes fronts of the one-node op probes (oracle/{attn,conv,core,grad,moe,pool,rope,sam,ssm,train,wkv}.py) against their libraries
 (oracle/_ref/libggml_<family>_probe.so, over oracle/probe_harness.h).
   - each module's SIGNATURES names exactly the probe_* symbols its library exports, so a signature table cannot drift from the library;
   - every public probe function reports -1 for a device that does not exist ("NOPE"): with raw=True as its code, otherwise as a
-    RuntimeError.  This is the harness's first exit path in all ten libraries; no device is needed for it."""
+    RuntimeError.  This is the harness's first exit path in all eleven libraries; no device is needed for it."""
 import shutil
 import subprocess
 
@@ -12,6 +12,7 @@ import pytest
 from oracle import attn as A
 from oracle import conv as V
 from oracle import core as K
+from oracle import grad as G
 from oracle import moe as M
 from oracle import oracle as O
 from oracle import pool as P
@@ -21,7 +22,7 @@ from oracle import ssm as SS
 from oracle import train as TR
 from oracle import wkv as W
 
-MODULES = {"attn": A, "conv": V, "core": K, "moe": M, "pool": P, "rope": R, "sam": S, "ssm": SS, "train": TR, "wkv": W}
+MODULES = {"attn": A, "conv": V, "core": K, "grad": G, "moe": M, "pool": P, "rope": R, "sam": S, "ssm": SS, "train": TR, "wkv": W}
 
 
 def need(family):
@@ -92,6 +93,7 @@ CALLS = [
     ("train", "probe_sum", lambda: TR.sum_("NOPE", _train_source(), _f32(1, 1, 2, 3), raw=True)),
     ("train", "probe_repeat_back", lambda: TR.repeat_back("NOPE", _train_source(), (3, 1), _f32(1, 1, 2, 3), raw=True)),
     ("train", "probe_step", lambda: TR.step("NOPE", _f32(4), raw=True)),
+    ("grad", "probe_mul_mat_grad", lambda: G.mul_mat_grad("NOPE", G.GradCase(2, 1, 3), *G.GradCase(2, 1, 3).inputs(0), [0], [0], raw=True)),
     ("wkv", "probe_rwkv_wkv6", lambda: W.wkv("NOPE", W.grid(False)[0], raw=True)),
     ("wkv", "probe_gated_linear_attn", lambda: W.wkv("NOPE", W.grid(True)[0], raw=True)),
     ("wkv", "probe_sqr_sqrt", lambda: W.sqr_sqrt("NOPE", 0, _f32(4), raw=True)),
