@@ -459,14 +459,16 @@ def rope_params(n_dims: int, mode: int = ROPE_NORM, sections=(0, 0, 0, 0), n_ctx
     return p
 
 
-def op_rope(x, pos, params: RopeParams, freq_factors=None, inplace: bool = False):
-    """GGML_OP_ROPE on a contiguous f32 / f16 torch tensor [ne3, n_pos, n_head, ne0] (ggml order reversed) with i32 positions `pos`
-    ([n_pos], or [4 * n_pos] for MROPE / VISION) and optional f32 freq_factors; params from rope_params().  inplace: dst is x."""
+def op_rope(x, pos, params: RopeParams, freq_factors=None, inplace: bool = False, out=None):
+    """GGML_OP_ROPE on an f32 / f16 torch tensor [ne3, n_pos, n_head, ne0] (ggml order reversed; any view with the last dim contiguous, e.g.
+    the heads of a KV cache) with i32 positions `pos` ([n_pos], or [4 * n_pos] for MROPE / VISION) and optional f32 freq_factors; params
+    from rope_params().  inplace: dst is x (the K-shift of a cache view); out: None (a new contiguous tensor) or a tensor of x's shape and
+    type with the last dim contiguous."""
     import torch
     L = lib()
     L.ggml_b200_op_rope.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.POINTER(RopeParams), C.c_void_p]
-    y = x if inplace else torch.empty_like(x)
-    s, p, d = tensor_desc(x), tensor_desc(pos), tensor_desc(y)
+    y = x if inplace else out if out is not None else torch.empty(x.shape, dtype=x.dtype, device=x.device)
+    s, p, d = strided_desc(x), tensor_desc(pos), strided_desc(y)
     f = C.byref(tensor_desc(freq_factors)) if freq_factors is not None else None
     check(L.ggml_b200_op_rope(C.byref(s), C.byref(p), f, C.byref(d), C.byref(params), _stream()), "ggml_b200_op_rope")
     return y
@@ -546,74 +548,79 @@ def op_mul_mat_f(a, b, out=None):
     return y
 
 
-def op_concat(a, b, dim: int):
+def op_concat(a, b, dim: int, out=None):
     """GGML_OP_CONCAT of two f32 (or two i32) torch tensors of equal rank <= 4 along ggml's dim (0 = the last torch dim): a, then b.
-    a must be contiguous along its last dim; b may be any view (a transposed one, as in the Mamba layer).  A new contiguous tensor."""
+    a must be contiguous along its last dim; b may be any view (a transposed one, as in the Mamba layer).  A new contiguous tensor, or
+    written into out (a contiguous tensor of the result's shape)."""
     import torch
     L = lib()
     L.ggml_b200_op_concat.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_int32, C.c_void_p]
     shape = list(a.shape)
     if 0 <= dim < a.dim():
         shape[a.dim() - 1 - dim] += b.shape[a.dim() - 1 - dim]
-    y = torch.empty(shape, dtype=a.dtype, device=a.device)
+    y = out.view(shape) if out is not None else torch.empty(shape, dtype=a.dtype, device=a.device)
     s0, s1, d = strided_desc(a), strided_desc(b), tensor_desc(y)
     check(L.ggml_b200_op_concat(C.byref(s0), C.byref(s1), C.byref(d), int(dim), _stream()), "ggml_b200_op_concat")
     return y
 
 
-def op_ssm_conv(sx, c):
+def op_ssm_conv(sx, c, out=None):
     """GGML_OP_SSM_CONV: sx f32 [n_s, d_inner, d_conv - 1 + n_t] (rows packed), c f32 [d_inner, d_conv] -> f32 [n_s, n_t, d_inner],
-    out[s, t, i] = sum_k sx[s, i, t + k] * c[i, k], bit-identical to ggml-cpu"""
+    y[s, t, i] = sum_k sx[s, i, t + k] * c[i, k], bit-identical to ggml-cpu; a new tensor, or written into out (contiguous, that size)"""
     import torch
     L = lib()
     L.ggml_b200_op_ssm_conv.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_void_p]
     n_s, d_inner, ncs = sx.shape
-    y = torch.empty((n_s, ncs - c.shape[-1] + 1, d_inner), dtype=torch.float32, device=sx.device)
+    shape = (n_s, ncs - c.shape[-1] + 1, d_inner)
+    y = out.view(shape) if out is not None else torch.empty(shape, dtype=torch.float32, device=sx.device)
     x, w, d = strided_desc(sx), strided_desc(c), tensor_desc(y)
     check(L.ggml_b200_op_ssm_conv(C.byref(x), C.byref(w), C.byref(d), _stream()), "ggml_b200_op_ssm_conv")
     return y
 
 
-def op_ssm_scan(s, x, dt, A, B, C_):
+def op_ssm_scan(s, x, dt, A, B, C_, out=None):
     """GGML_OP_SSM_SCAN (Mamba-1): s f32 [n_s, d_inner, d_state], x and dt f32 [n_s, n_t, d_inner], A f32 [d_inner, d_state] (all four
     contiguous), B and C f32 [n_s, n_t, d_state] (last dim contiguous, any other strides).  Returns (y [n_s, n_t, d_inner], s_new
-    [n_s, d_inner, d_state]): views of the one flat result in ggml's layout (y, then the final states)."""
+    [n_s, d_inner, d_state]): views of the one flat result in ggml's layout (y, then the final states).  out: None (a new tensor) or a
+    contiguous f32 tensor of x.numel() + s.numel() elements to hold that result."""
     import torch
     L = lib()
     L.ggml_b200_op_ssm_scan.argtypes = [C.POINTER(TensorDesc)] * 7 + [C.c_void_p]
-    out = torch.empty(x.numel() + s.numel(), dtype=torch.float32, device=x.device)
+    out = out.view(-1) if out is not None else torch.empty(x.numel() + s.numel(), dtype=torch.float32, device=x.device)
     t = [strided_desc(v) for v in (s, x, dt, A, B, C_)]
     d = tensor_desc(out)
     check(L.ggml_b200_op_ssm_scan(*[C.byref(v) for v in t], C.byref(d), _stream()), "ggml_b200_op_ssm_scan")
     return out[: x.numel()].view(x.shape), out[x.numel():].view(s.shape)
 
 
-def _wkv(fn, name, k, s, srcs, extra):
-    """the flat ggml result of RWKV_WKV6 / GATED_LINEAR_ATTN as (y [T, H, S], s_new [n_seqs, H, S, S]) views; s is read as [n_seqs, S S H]"""
+def _wkv(fn, name, k, s, srcs, extra, out=None):
+    """the flat ggml result of RWKV_WKV6 / GATED_LINEAR_ATTN as (y [T, H, S], s_new [n_seqs, H, S, S]) views; s is read as [n_seqs, S S H].
+    out: None (a new tensor) or a contiguous f32 tensor of (T + S n_seqs) H S elements to hold that result."""
     import torch
     T, H, S = k.shape
     n_seqs = s.shape[0]
-    out = torch.empty((T + S * n_seqs, H * S), dtype=torch.float32, device=k.device)
+    shape = (T + S * n_seqs, H * S)
+    out = out.view(shape) if out is not None else torch.empty(shape, dtype=torch.float32, device=k.device)
     t = [strided_desc(v) for v in srcs] + [strided_desc(s.reshape(n_seqs, -1))]
     check(fn(*[C.byref(v) for v in t], C.byref(tensor_desc(out)), *extra, _stream()), name)
     return out[:T].view(T, H, S), out[T:].view(n_seqs, H, S, S)
 
 
-def op_rwkv_wkv6(k, v, r, tf, td, s):
+def op_rwkv_wkv6(k, v, r, tf, td, s, out=None):
     """GGML_OP_RWKV_WKV6: k, v, r, td f32 [T, H, S], tf f32 [H, S], s f32 [n_seqs, H, S, S] (state[i][j] at [q, h, i, j]), all contiguous;
     sequence q owns tokens [q T / n_seqs, (q + 1) T / n_seqs).  Returns (y [T, H, S], s_new [n_seqs, H, S, S]): views of the one flat
-    result in ggml's layout (y, then the final states)."""
+    result in ggml's layout (y, then the final states).  out: as for _wkv."""
     L = lib()
     L.ggml_b200_op_rwkv_wkv6.argtypes = [C.POINTER(TensorDesc)] * 7 + [C.c_void_p]
-    return _wkv(L.ggml_b200_op_rwkv_wkv6, "ggml_b200_op_rwkv_wkv6", k, s, (k, v, r, tf, td), ())
+    return _wkv(L.ggml_b200_op_rwkv_wkv6, "ggml_b200_op_rwkv_wkv6", k, s, (k, v, r, tf, td), (), out)
 
 
-def op_gated_linear_attn(k, v, q, g, s, scale: float):
+def op_gated_linear_attn(k, v, q, g, s, scale: float, out=None):
     """GGML_OP_GATED_LINEAR_ATTN: k, v, q, g f32 [T, H, S], s f32 [n_seqs, H, S, S], all contiguous; as op_rwkv_wkv6 with the gate g in
-    place of the decay and q * scale in place of r (no bonus term).  Returns (y [T, H, S], s_new [n_seqs, H, S, S])."""
+    place of the decay and q * scale in place of r (no bonus term).  Returns (y [T, H, S], s_new [n_seqs, H, S, S]); out: as for _wkv."""
     L = lib()
     L.ggml_b200_op_gated_linear_attn.argtypes = [C.POINTER(TensorDesc)] * 6 + [C.c_float, C.c_void_p]
-    return _wkv(L.ggml_b200_op_gated_linear_attn, "ggml_b200_op_gated_linear_attn", k, s, (k, v, q, g), (float(scale),))
+    return _wkv(L.ggml_b200_op_gated_linear_attn, "ggml_b200_op_gated_linear_attn", k, s, (k, v, q, g), (float(scale),), out)
 
 
 class Im2colParams(C.Structure):

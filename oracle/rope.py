@@ -35,6 +35,8 @@ class Case:
     beta_fast: float = 32.0
     beta_slow: float = 1.0
     seed: int = 0
+    positions: tuple | None = None  # the positions, cycled over n_pos (every stream in MROPE); None: random in [0, 4096) with 4095 first
+    llama3_ff: bool = False         # with ff: llama-3's factors (llama3_freq_factors) instead of uniform(1, 4) noise
 
     @property
     def multi(self) -> bool:
@@ -54,15 +56,40 @@ class Case:
             x = x.astype(np.float16)
         pos = rng.integers(0, 4096, self.ne[2] * (4 if self.multi else 1)).astype(np.int32)
         pos[0] = 4095
+        if self.positions is not None:
+            pos = np.resize(np.array(self.positions, dtype=np.int32), pos.size)
         ff = None
         if self.ff:
             nff = self.n_dims if self.mode == ROPE_VISION else self.n_dims // 2
-            ff = rng.uniform(1.0, 4.0, max(nff, 1)).astype(np.float32)
+            if self.llama3_ff:
+                ff = llama3_freq_factors(self.n_dims, self.freq_base)
+            else:
+                ff = rng.uniform(1.0, 4.0, max(nff, 1)).astype(np.float32)
         return x, pos, ff
 
     def __str__(self):
-        return (f"{O.TYPE_NAMES[self.type]} {MODE_NAMES[self.mode]} ne={self.ne} n_dims={self.n_dims} sec={self.sections} ff={int(self.ff)} "
-                f"ef={self.ext_factor} fs={self.freq_scale} af={self.attn_factor} view={int(self.view)} inplace={int(self.inplace)}")
+        ff = "llama3" if self.ff and self.llama3_ff else int(self.ff)
+        pos = "" if self.positions is None else f" pos={min(self.positions)}..{max(self.positions)} ({len(self.positions)} cycled)"
+        return (f"{O.TYPE_NAMES[self.type]} {MODE_NAMES[self.mode]} ne={self.ne} n_dims={self.n_dims} sec={self.sections} ff={ff} "
+                f"ef={self.ext_factor} fs={self.freq_scale} af={self.attn_factor} base={self.freq_base:g} view={int(self.view)} "
+                f"inplace={int(self.inplace)}{pos}")
+
+
+def llama3_freq_factors(n_dims: int, freq_base: float, factor: float = 8.0, low_freq_factor: float = 1.0, high_freq_factor: float = 4.0,
+                        n_ctx_orig: int = 8192) -> np.ndarray:
+    """the rope_freqs of a llama-3.1 model (its published rope-scaling rule): 1 for pairs whose wavelength is under
+    n_ctx_orig / high_freq_factor, `factor` above n_ctx_orig / low_freq_factor, and a smooth ramp between"""
+    out = []
+    for j in range(n_dims // 2):
+        wavelen = 2 * np.pi / freq_base ** (-2.0 * j / n_dims)
+        if wavelen < n_ctx_orig / high_freq_factor:
+            out.append(1.0)
+        elif wavelen > n_ctx_orig / low_freq_factor:
+            out.append(factor)
+        else:
+            smooth = (n_ctx_orig / wavelen - low_freq_factor) / (high_freq_factor - low_freq_factor)
+            out.append(1.0 / ((1.0 - smooth) / factor + smooth))
+    return np.array(out, dtype=np.float32)
 
 
 def grid(inplace: bool = False) -> list:

@@ -27,6 +27,7 @@ class WkvCase:
     gla: bool = False
     scale: float = 1.0          # GLA only
     seed: int = 0
+    w_range: tuple = (-8.0, 2.0)  # decay / gate exp(-exp(w)), w uniform in this range
 
     @property
     def T(self):
@@ -41,7 +42,7 @@ class WkvCase:
         v = f(rng.standard_normal((T, H, S)))
         r = f(rng.standard_normal((T, H, S)))
         # decay / gate exp(-exp(w)), w over the range trained RWKV-6 layers reach: from ~1 (forgets at once) to ~0.9997 (keeps)
-        w = f(np.exp(-np.exp(rng.uniform(-8.0, 2.0, (T, H, S)))))
+        w = f(np.exp(-np.exp(rng.uniform(*self.w_range, (T, H, S)))))
         state = f(rng.standard_normal((self.n_seqs, H, S, S)))
         if self.gla:
             return [k, v, r, w, state]

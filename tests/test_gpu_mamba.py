@@ -3,11 +3,12 @@ ggml_b200_op_concat / _ssm_conv / _ssm_scan and the plug-in), and Mamba decoder 
 
   (a) the reference's own test-backend-ops runs every CONCAT, SSM_CONV and SSM_SCAN case on B2000 against ggml-cpu: all executed, none declined;
   (b) one-node graphs (oracle/ssm_probe.cpp) on B2000 and on ggml-cpu over the host test's grid: CONCAT and SSM_CONV bit-identical, SSM_SCAN
-      y and states within NMSE 1e-10 (the device expf / log1pf against glibc's); what the C ABI declines the plug-in declines;
+      y and states within NMSE 1e-10; what the C ABI declines the plug-in declines;
   (c) the C ABI: invalid arguments give error codes; a captured CUDA graph of the three ops, replayed on new inputs, matches eager launches;
   (d) the `mamba` (Mamba-130m widths, two sequences) and `falcon` (FalconMamba form) presets: every node matches ggml-cpu on identical inputs,
       free-running logits stay close, the whole graph is one split with no CPU node, teacher-forced logits track ggml-cpu, and fusions /
-      CUDA-graph replay change no logit bit (a replayed decode graph reads the states the previous replay wrote)."""
+      CUDA-graph replay change no logit bit (a replayed decode graph reads the states the previous replay wrote).
+Every output element against an f64 reference and its bound, at model widths, long prompts and chunked, is tests/test_gpu_seq_elements.py's."""
 import numpy as np
 import pytest
 

@@ -3,10 +3,10 @@
   * the reference's own test-backend-ops runs every ROPE case (f32 / f16; llama, neox, stablelm, phi-2, qwen2vl m-rope and ViT shapes;
     strided views, freq factors, YaRN) on B2000 against ggml-cpu: all executed, none declined, none failing;
   * one-node ROPE graphs through the reference's graph API (oracle/rope_probe.cpp) on B2000 and on ggml-cpu agree over the grid of
-    tests/test_hostemu_rope.py plus in-place cases: f32 to NMSE <= 1e-12, f16 to one f16 ulp per element (only the device sinf / cosf
-    differ from glibc's);
+    tests/test_hostemu_rope.py plus in-place cases: f32 to NMSE <= 1e-12, f16 to one f16 ulp per element;
   * the C ABI directly: positions are read on the device (a captured CUDA graph rotates by the positions set before each replay), and
-    what the CPU backend asserts comes back as an error code."""
+    what the CPU backend asserts comes back as an error code.
+Every output element against an f64 reference and its bound, at model sizes and positions, is tests/test_gpu_seq_elements.py's."""
 import re
 import subprocess
 

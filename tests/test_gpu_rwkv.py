@@ -10,7 +10,9 @@ _gated_linear_attn and the plug-in), GGML_OP_SQR / GGML_OP_SQRT through the unar
   (c) the C ABI: invalid arguments give error codes; a captured CUDA graph of both ops, replayed on new inputs, matches eager launches;
   (d) the `rwkv6` (RWKV-6 1.6B widths, two sequences) and `qrwkv` (RWKV6-Qwen2 form) presets: every node matches ggml-cpu on identical
       inputs, free-running logits stay close, the whole graph is one split with no CPU node, teacher-forced logits track ggml-cpu, and
-      fusions / CUDA-graph replay change no logit bit (a replayed decode graph reads the states the previous replay wrote)."""
+      fusions / CUDA-graph replay change no logit bit (a replayed decode graph reads the states the previous replay wrote).
+Every output element against an f64 reference and its bound, at head sizes up to 256, long prompts and chunked, is
+tests/test_gpu_seq_elements.py's."""
 import numpy as np
 import pytest
 
