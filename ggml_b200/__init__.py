@@ -335,9 +335,10 @@ UNARY_STEP = 13                                # GGML_B200_UNARY_STEP (GGML_UNAR
 def op_unary(uop: int, x):
     import torch
     L = lib()
-    L.ggml_b200_op_unary.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+    L.ggml_b200_op_unary.argtypes = [C.c_int32, C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p]
     y = torch.empty_like(x)
-    check(L.ggml_b200_op_unary(uop, x.data_ptr(), y.data_ptr(), x.numel(), _stream()), "ggml_b200_op_unary")
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_unary(uop, C.byref(s), C.byref(d), _stream()), "ggml_b200_op_unary")
     return y
 
 
@@ -356,11 +357,10 @@ def op_norm(x, eps: float, rms: bool = False, out=None):
 def op_norm_affine(x, gain, bias, eps: float, rms: bool = False):
     import torch
     L = lib()
-    L.ggml_b200_op_norm_affine.argtypes = [C.c_int32, C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p, C.POINTER(TensorDesc),
-                                           C.c_void_p, C.POINTER(TensorDesc), C.c_float, C.c_void_p]
+    L.ggml_b200_op_norm_affine.argtypes = [C.c_int32] + [C.POINTER(TensorDesc)] * 6 + [C.c_float, C.c_void_p]
     y1, y2, y3 = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
-    s, d1, d2, d3 = tensor_desc(x), tensor_desc(y1), tensor_desc(y2), tensor_desc(y3)
-    check(L.ggml_b200_op_norm_affine(int(rms), C.byref(s), C.byref(d1), gain.data_ptr(), C.byref(d2), bias.data_ptr(), C.byref(d3), eps, _stream()),
+    s, d1, gd, d2, bd, d3 = (strided_desc(t) for t in (x, y1, gain, y2, bias, y3))
+    check(L.ggml_b200_op_norm_affine(int(rms), C.byref(s), C.byref(d1), C.byref(gd), C.byref(d2), C.byref(bd), C.byref(d3), eps, _stream()),
           "ggml_b200_op_norm_affine")
     return y1, y2, y3
 
@@ -368,9 +368,10 @@ def op_norm_affine(x, gain, bias, eps: float, rms: bool = False):
 def op_scale(x, s: float):
     import torch
     L = lib()
-    L.ggml_b200_op_scale.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_int64, C.c_void_p]
+    L.ggml_b200_op_scale.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_float, C.c_void_p]
     y = torch.empty_like(x)
-    check(L.ggml_b200_op_scale(x.data_ptr(), y.data_ptr(), s, x.numel(), _stream()), "ggml_b200_op_scale")
+    sd, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_scale(C.byref(sd), C.byref(d), s, _stream()), "ggml_b200_op_scale")
     return y
 
 
@@ -378,9 +379,10 @@ def op_diag_mask_inf(x, n_past: int):
     """x: [..., ne1, ne0] contiguous f32"""
     import torch
     L = lib()
-    L.ggml_b200_op_diag_mask_inf.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]
+    L.ggml_b200_op_diag_mask_inf.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_int32, C.c_void_p]
     y = torch.empty_like(x)
-    check(L.ggml_b200_op_diag_mask_inf(x.data_ptr(), y.data_ptr(), x.shape[-1], x.shape[-2], x.numel(), n_past, _stream()), "ggml_b200_op_diag_mask_inf")
+    s, d = strided_desc(x), tensor_desc(y)
+    check(L.ggml_b200_op_diag_mask_inf(C.byref(s), C.byref(d), n_past, _stream()), "ggml_b200_op_diag_mask_inf")
     return y
 
 
@@ -390,12 +392,11 @@ def op_soft_max(x, scale: float = 1.0, diag_n_past: int = -1, mask=None, max_bia
     as ggml_soft_max_ext broadcasts it.  inplace: the result is written into x."""
     import torch
     L = lib()
-    L.ggml_b200_op_soft_max_diag.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int64] * 4 + [C.c_float, C.c_float, C.c_int32, C.c_void_p]
-    sh = [1] * (4 - x.dim()) + list(x.shape)
+    L.ggml_b200_op_soft_max.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_float, C.c_float, C.c_int32, C.c_void_p]
     y = x if inplace else torch.empty_like(x)
-    mp, mt = (None, 0) if mask is None else (mask.data_ptr(), {torch.float32: F32, torch.float16: F16}[mask.dtype])
-    check(L.ggml_b200_op_soft_max_diag(x.data_ptr(), mp, mt, y.data_ptr(), sh[3], sh[2], sh[1], sh[0], scale, max_bias, diag_n_past, _stream()),
-          "ggml_b200_op_soft_max_diag")
+    s, d = strided_desc(x), tensor_desc(y)
+    m = None if mask is None else C.byref(strided_desc(mask))
+    check(L.ggml_b200_op_soft_max(C.byref(s), m, C.byref(d), scale, max_bias, diag_n_past, _stream()), "ggml_b200_op_soft_max")
     return y
 
 

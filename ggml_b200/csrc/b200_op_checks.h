@@ -1,4 +1,4 @@
-// b200_op_checks.h — what each descriptor-taking op launcher of ops.cu accepts, decided in one place.  Every ggml_b200_op_* below returns
+// b200_op_checks.h — what each op launcher of ops.cu accepts, decided in one place.  Every ggml_b200_op_* below returns
 // the verdict of its check before it launches anything, and the backend's supports_op asks the same check for each such node, on descriptors
 // built by the same code that builds the launch's (bound_op in backend/ggml-b200.cpp), so that a node the plug-in accepts is one its
 // launcher runs.  The checks read only the descriptors and the op's scalars: what the launcher cannot see (graph structure, ggml-cpu's
@@ -94,15 +94,66 @@ inline op_check check_bin_bcast(int32_t op, const ggml_b200_tensor * src0, const
     return accepted;
 }
 
+// NORM / RMS_NORM: the kernel writes dst's rows with src's extents
 inline op_check check_norm(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
     B200_REQUIRE(src->type == F32 && dst->type == F32 && src->nb[0] == 4 && dst->nb[0] == 4, "f32 rows contiguous along dim 0");
+    B200_VALID(same_shape(*src, *dst), "src and dst shapes differ");
     return accepted;
 }
 
+// NORM / RMS_NORM -> MUL(gain) -> ADD(bias): the kernel writes the three dsts' rows with src's extents and reads gain[i] and bias[i] for
+// every i < ne0 through these two pointers
 inline op_check check_norm_affine(const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const float * gain, const ggml_b200_tensor * dst_mul,
                                   const float * bias, const ggml_b200_tensor * dst_add) {
     B200_REQUIRE(src->type == F32 && dst_norm->type == F32 && dst_mul->type == F32 && dst_add->type == F32, "f32 only");
     B200_REQUIRE(src->nb[0] == 4 && dst_norm->nb[0] == 4 && dst_mul->nb[0] == 4 && dst_add->nb[0] == 4 && gain && bias, "rows contiguous along dim 0");
+    B200_VALID(same_shape(*src, *dst_norm) && same_shape(*src, *dst_mul) && same_shape(*src, *dst_add), "the dsts must have src's shape");
+    return accepted;
+}
+
+// ... with gain and bias described, as the launcher takes them: packed f32 [ne0] (nb0 == 4, every other extent 1)
+inline op_check check_norm_affine(const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const ggml_b200_tensor * gain,
+                                  const ggml_b200_tensor * dst_mul, const ggml_b200_tensor * bias, const ggml_b200_tensor * dst_add) {
+    B200_REQUIRE(gain && bias, "gain and bias are required");
+    B200_REQUIRE(gain->type == F32 && bias->type == F32 && gain->nb[0] == 4 && bias->nb[0] == 4, "gain and bias must be f32, contiguous");
+    const op_check rows = check_norm_affine(src, dst_norm, (const float *) gain->data, dst_mul, (const float *) bias->data, dst_add);
+    if (!rows.ok()) return rows;
+    const int64_t n = src->ne[0];
+    B200_VALID(gain->ne[0] == n && nelem(*gain) == n && bias->ne[0] == n && nelem(*bias) == n, "gain and bias must be [ne0]");
+    return accepted;
+}
+
+// SCALE, and with it DIAG_MASK_INF and the unary functions: one thread per element of packed f32 tensors
+inline op_check check_scale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    B200_REQUIRE(src->type == F32 && dst->type == F32, "src and dst must be f32");
+    B200_REQUIRE(is_packed4(*src) && is_packed4(*dst), "src and dst must be packed");
+    B200_VALID(same_shape(*src, *dst), "src and dst shapes differ");
+    if (nelem(*dst) == 0) return accepted;
+    B200_REQUIRE((nelem(*dst) + 255) / 256 <= 0x7fffffff, "too many elements for one grid");
+    return accepted;
+}
+
+inline op_check check_diag_mask_inf(const ggml_b200_tensor * src, const ggml_b200_tensor * dst) { return check_scale(src, dst); }
+
+inline op_check check_unary(int32_t uop, const ggml_b200_tensor * src, const ggml_b200_tensor * dst) {
+    B200_VALID(uop >= 0 && uop <= GGML_B200_UNARY_STEP, "bad unary op (0 .. 13, enum ggml_b200_unary)");
+    return check_scale(src, dst);
+}
+
+// SOFT_MAX: src and dst packed f32 of one shape, one CTA per row; the kernel reads mask row i1 at i1 ne0 elements, so the mask is what
+// ggml_soft_max_impl asserts: a packed f32 or f16 matrix [ne0, >= ne1]
+inline op_check check_soft_max(const ggml_b200_tensor * src, const ggml_b200_tensor * mask, const ggml_b200_tensor * dst) {
+    B200_REQUIRE(src && dst, "src and dst are required");
+    B200_REQUIRE(src->type == F32 && dst->type == F32, "src and dst must be f32");
+    B200_REQUIRE(is_packed4(*src) && is_packed4(*dst), "src and dst must be packed");
+    B200_VALID(same_shape(*src, *dst), "src and dst shapes differ");
+    if (mask) {
+        B200_REQUIRE(is_float(mask->type) && is_packed(*mask, mask->type == F32 ? 4 : 2), "mask must be packed f32 or f16");
+        B200_VALID(mask->ne[2] == 1 && mask->ne[3] == 1 && mask->ne[0] == src->ne[0] && mask->ne[1] >= src->ne[1], "mask must be [ne0, >= ne1]");
+    }
+    if (nelem(*src) == 0) return accepted;
+    B200_REQUIRE(nrows(*src) <= 0x7fffffff, "too many rows for one grid");
     return accepted;
 }
 

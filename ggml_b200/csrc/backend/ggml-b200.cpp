@@ -15,8 +15,9 @@
 // (unsupported nodes reaching graph_compute abort, as in the reference, ggml-cuda.cu:2655-2659).  Each op has one binding (bound_op) that
 // builds its launcher's arguments from the node; supports_op and graph_compute both go through it, the first to ask the launcher's own
 // check (ggml_b200/csrc/b200_op_checks.h) plus what the launcher cannot see, the second to launch, so the check sees the descriptors the
-// launch passes.  The quantized MUL_MAT / MUL_MAT_ID decide in supports_mul_mat*; mul_mat_route picks a MUL_MAT node's kernel family and
-// scratch, for the pre-capture sizing and the launch alike.
+// launch passes.  Every ggml_b200_op_* launcher takes descriptors and applies its check, and the graph-level fusions (try_fuse_*) ask the
+// check of the fused launcher on the descriptors they pass it.  The quantized MUL_MAT / MUL_MAT_ID decide in supports_mul_mat*;
+// mul_mat_route picks a MUL_MAT node's kernel family and scratch, for the pre-capture sizing and the launch alike.
 
 #include "ggml.h"
 #include "ggml-backend.h"
@@ -477,8 +478,6 @@ bool supports_mul_mat_id(const ggml_tensor * op) {
     return true;
 }
 
-bool is_f32_contig(const ggml_tensor * t) { return t->type == GGML_TYPE_F32 && ggml_is_contiguous(t); }
-
 ggml_b200_tensor desc(const ggml_tensor * t) {
     ggml_b200_tensor d;
     d.data = t->data; d.type = (int32_t) t->type;
@@ -534,11 +533,10 @@ int unary_code(const ggml_tensor * node) {
 
 // How each node becomes its launcher's arguments (every op but the quantized MUL_MAT / MUL_MAT_ID and the tensor-core f16 MUL_MAT, whose
 // arguments are mul_mat_args / mul_mat_id_args / mul_mat_route below).  launch == false: only ask, for supports_op: the launcher's own check
-// on these descriptors, plus what the launcher cannot see (ggml-cpu's own layout rules, and the layout of the bare pointers some launchers
-// take); launch == true: launch on `stream`.  Returns the check's / the launcher's status code.
+// on these descriptors, plus what the launcher cannot see (ggml-cpu's own layout rules); launch == true: launch on `stream`.  Returns the
+// check's / the launcher's status code.
 int bound_op(const ggml_tensor * node, bool launch, void * stream) {
     const ggml_tensor * a = node->src[0], * b = node->src[1];
-    const auto verdict = [](bool ok) { return ok ? GGML_B200_OK : GGML_B200_EUNSUPPORTED; };
     if (!launch && !a) return GGML_B200_EUNSUPPORTED;      // every op below has a src0 (ARANGE and the like have none)
     switch (node->op) {
         case GGML_OP_GET_ROWS: {
@@ -732,24 +730,26 @@ int bound_op(const ggml_tensor * node, bool launch, void * stream) {
             if (!launch) return b200::check_gated_linear_attn(&t[0], &t[1], &t[2], &t[3], &t[4], &d).code;
             return ggml_b200_op_gated_linear_attn(&t[0], &t[1], &t[2], &t[3], &t[4], &d, ggml_get_op_params_f32(node, 0), stream);
         }
-        // the launchers that take bare pointers: their layout conditions are the caller's
-        case GGML_OP_SCALE:
-            if (!launch) return verdict(is_f32_contig(a) && is_f32_contig(node));
-            return ggml_b200_op_scale((const float *) a->data, (float *) node->data, ggml_get_op_params_f32(node, 0), ggml_nelements(node), stream);
-        case GGML_OP_DIAG_MASK_INF:
-            if (!launch) return verdict(is_f32_contig(a) && is_f32_contig(node));
-            return ggml_b200_op_diag_mask_inf((const float *) a->data, (float *) node->data, node->ne[0], node->ne[1], ggml_nelements(node), ggml_get_op_params_i32(node, 0), stream);
-        case GGML_OP_SOFT_MAX:
-            if (!launch) return verdict(is_f32_contig(a) && is_f32_contig(node) && (!b || ((b->type == GGML_TYPE_F32 || b->type == GGML_TYPE_F16) && ggml_is_contiguous(b))));
-            return ggml_b200_op_soft_max((const float *) a->data, b ? b->data : nullptr, b ? (int32_t) b->type : 0, (float *) node->data,
-                                         node->ne[0], node->ne[1], node->ne[2], node->ne[3], ggml_get_op_params_f32(node, 0), ggml_get_op_params_f32(node, 1), stream);
+        case GGML_OP_SCALE: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_scale(&x, &d, ggml_get_op_params_f32(node, 0), stream) : b200::check_scale(&x, &d).code;
+        }
+        case GGML_OP_DIAG_MASK_INF: {
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_diag_mask_inf(&x, &d, ggml_get_op_params_i32(node, 0), stream) : b200::check_diag_mask_inf(&x, &d).code;
+        }
+        case GGML_OP_SOFT_MAX: {                           // src1: the optional mask
+            const auto x = desc(a), d = desc(node), m = b ? desc(b) : ggml_b200_tensor{};
+            if (!launch) return b200::check_soft_max(&x, b ? &m : nullptr, &d).code;
+            return ggml_b200_op_soft_max(&x, b ? &m : nullptr, &d, ggml_get_op_params_f32(node, 0), ggml_get_op_params_f32(node, 1), -1, stream);
+        }
         // SQR and SQRT: x * x and sqrtf, correctly rounded on both backends: bit-identical to ggml-cpu.  SIN and COS: the device's sinf / cosf
         // (within 2 ulp), not bit-identical to glibc's
         case GGML_OP_UNARY: case GGML_OP_SQR: case GGML_OP_SQRT: case GGML_OP_SIN: case GGML_OP_COS: {
-            const int u = node->op == GGML_OP_SQR ? GGML_B200_UNARY_SQR : node->op == GGML_OP_SQRT ? GGML_B200_UNARY_SQRT
-                        : node->op == GGML_OP_SIN ? GGML_B200_UNARY_SIN : node->op == GGML_OP_COS ? GGML_B200_UNARY_COS : unary_code(node);
-            if (!launch) return verdict(u >= 0 && is_f32_contig(a) && is_f32_contig(node));
-            return ggml_b200_op_unary(u, (const float *) a->data, (float *) node->data, ggml_nelements(node), stream);
+            const int32_t u = node->op == GGML_OP_SQR ? GGML_B200_UNARY_SQR : node->op == GGML_OP_SQRT ? GGML_B200_UNARY_SQRT
+                            : node->op == GGML_OP_SIN ? GGML_B200_UNARY_SIN : node->op == GGML_OP_COS ? GGML_B200_UNARY_COS : unary_code(node);
+            const auto x = desc(a), d = desc(node);
+            return launch ? ggml_b200_op_unary(u, &x, &d, stream) : b200::check_unary(u, &x, &d).code;
         }
         default:
             if (!launch) return GGML_B200_EUNSUPPORTED;
@@ -1092,6 +1092,8 @@ size_t node_scratch_need(const ggml_tensor * node) {
     return 0;
 }
 
+bool is_f32_contig(const ggml_tensor * t) { return t->type == GGML_TYPE_F32 && ggml_is_contiguous(t); }
+
 bool is_row_vector_f32(const ggml_tensor * t, int64_t n) {      // a contiguous f32 [n] (bias / gain) tensor
     return t && t->type == GGML_TYPE_F32 && t->ne[0] == n && ggml_nelements(t) == n && t->nb[0] == sizeof(float);
 }
@@ -1137,13 +1139,10 @@ int try_fuse_norm(backend_ctx * ctx, ggml_cgraph * cgraph, int i) {
     ggml_tensor * nm = cgraph->nodes[i];
     if (i + 2 >= cgraph->n_nodes) return 0;
     ggml_tensor * mul = cgraph->nodes[i + 1], * add = cgraph->nodes[i + 2];
-    const int64_t n = nm->ne[0];
-    if (mul->op != GGML_OP_MUL || mul->src[0] != nm || !is_row_vector_f32(mul->src[1], n) || !ggml_are_same_shape(mul, nm)) return 0;
-    if (add->op != GGML_OP_ADD || add->src[0] != mul || !is_row_vector_f32(add->src[1], n) || !ggml_are_same_shape(add, nm)) return 0;
-    auto s = desc(nm->src[0]), d1 = desc(nm), d2 = desc(mul), d3 = desc(add);
-    const float * gain = (const float *) mul->src[1]->data, * bias = (const float *) add->src[1]->data;
-    if (!b200::check_norm_affine(&s, &d1, gain, &d2, bias, &d3).ok()) return 0;
-    SHIM_OK(ggml_b200_op_norm_affine(nm->op == GGML_OP_RMS_NORM, &s, &d1, gain, &d2, bias, &d3, ggml_get_op_params_f32(nm, 0), ctx->stream));
+    if (mul->op != GGML_OP_MUL || mul->src[0] != nm || add->op != GGML_OP_ADD || add->src[0] != mul) return 0;
+    const auto s = desc(nm->src[0]), d1 = desc(nm), g = desc(mul->src[1]), d2 = desc(mul), bs = desc(add->src[1]), d3 = desc(add);
+    if (!b200::check_norm_affine(&s, &d1, &g, &d2, &bs, &d3).ok()) return 0;
+    SHIM_OK(ggml_b200_op_norm_affine(nm->op == GGML_OP_RMS_NORM, &s, &d1, &g, &d2, &bs, &d3, ggml_get_op_params_f32(nm, 0), ctx->stream));
     return 2;
 }
 
@@ -1165,13 +1164,14 @@ int try_fuse_soft_max(backend_ctx * ctx, ggml_cgraph * cgraph, int i) {
     if (i + 2 >= cgraph->n_nodes) return 0;
     ggml_tensor * sc = cgraph->nodes[i], * dm = cgraph->nodes[i + 1], * sm = cgraph->nodes[i + 2];
     if (dm->op != GGML_OP_DIAG_MASK_INF || dm->src[0] != sc || sm->op != GGML_OP_SOFT_MAX || sm->src[0] != dm || sm->src[1] != nullptr) return 0;
-    if (!is_f32_contig(sc->src[0]) || !is_f32_contig(sc) || !is_f32_contig(dm) || !is_f32_contig(sm)) return 0;
+    if (!is_f32_contig(sc) || !is_f32_contig(dm)) return 0;
     if (ggml_get_op_params_f32(sm, 0) != 1.0f || ggml_get_op_params_f32(sm, 1) != 0.0f) return 0;
     const int n_past = ggml_get_op_params_i32(dm, 0);
     if (n_past < 0) return 0;
     if (has_other_consumer(cgraph, sc, dm) || has_other_consumer(cgraph, dm, sm)) return 0;
-    SHIM_OK(ggml_b200_op_soft_max_diag((const float *) sc->src[0]->data, nullptr, 0, (float *) sm->data, sm->ne[0], sm->ne[1], sm->ne[2], sm->ne[3],
-                                       ggml_get_op_params_f32(sc, 0), 0.0f, n_past, ctx->stream));
+    const auto x = desc(sc->src[0]), d = desc(sm);
+    if (!b200::check_soft_max(&x, nullptr, &d).ok()) return 0;
+    SHIM_OK(ggml_b200_op_soft_max(&x, nullptr, &d, ggml_get_op_params_f32(sc, 0), 0.0f, n_past, ctx->stream));
     return 2;
 }
 

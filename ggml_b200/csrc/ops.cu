@@ -1082,7 +1082,7 @@ static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + p
 
 using namespace b200;
 
-// every launcher below that takes tensor descriptors first applies its acceptance rule from b200_op_checks.h (the one supports_op asks)
+// every launcher below first applies its acceptance rule from b200_op_checks.h (the one supports_op asks)
 #define CHECK_ARGS(check) do { const op_check r_ = (check); if (!r_.ok()) { set_error("%s: %s", __func__, r_.reason); return r_.code; } } while (0)
 
 extern "C" {
@@ -1120,10 +1120,11 @@ int ggml_b200_op_norm(int32_t rms, const ggml_b200_tensor * src, const ggml_b200
     return GGML_B200_OK;
 }
 
-int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const float * gain, const ggml_b200_tensor * dst_mul,
-                             const float * bias, const ggml_b200_tensor * dst_add, float eps, void * stream) {
-    CHECK_ARGS(check_norm_affine(src, dst_norm, gain, dst_mul, bias, dst_add));
+int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const ggml_b200_tensor * gain_t,
+                             const ggml_b200_tensor * dst_mul, const ggml_b200_tensor * bias_t, const ggml_b200_tensor * dst_add, float eps, void * stream) {
+    CHECK_ARGS(check_norm_affine(src, dst_norm, gain_t, dst_mul, bias_t, dst_add));
     const tdesc s = T(src), d1 = T(dst_norm), d2 = T(dst_mul), d3 = T(dst_add);
+    const float * gain = (const float *) gain_t->data, * bias = (const float *) bias_t->data;
     const int64_t rows = nrows(s);
     if (rows == 0 || s.ne[0] == 0) return GGML_B200_OK;
     const int threads = s.ne[0] >= 1024 ? 256 : s.ne[0] >= 256 ? 128 : 32;
@@ -1133,42 +1134,47 @@ int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const gg
     return GGML_B200_OK;
 }
 
-int ggml_b200_op_scale(const float * src, float * dst, float s, int64_t n, void * stream) {
-    if (n <= 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(scale_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, src, dst, s, n));
+int ggml_b200_op_scale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, float s, void * stream) {
+    CHECK_ARGS(check_scale(src, dst));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(scale_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (const float *)src->data, (float *)dst->data, s, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
-int ggml_b200_op_diag_mask_inf(const float * src, float * dst, int64_t ne0, int64_t ne1, int64_t n, int32_t n_past, void * stream) {
-    if (n <= 0) return GGML_B200_OK;
-    B200_CUDA_TRY(launch_pdl(diag_mask_inf_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, src, dst, ne0, ne1, n_past, n));
+int ggml_b200_op_diag_mask_inf(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t n_past, void * stream) {
+    CHECK_ARGS(check_diag_mask_inf(src, dst));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(diag_mask_inf_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (const float *)src->data, (float *)dst->data,
+                             dst->ne[0], dst->ne[1], n_past, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
-int ggml_b200_op_unary(int32_t uop, const float * src, float * dst, int64_t n, void * stream) {
-    if (n <= 0) return GGML_B200_OK;
-    if (uop < 0 || uop > U_STEP) { set_error("unary: bad op %d", uop); return GGML_B200_EINVAL; }
-    B200_CUDA_TRY(launch_pdl(unary_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, uop, src, dst, n));
+int ggml_b200_op_unary(int32_t uop, const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream) {
+    CHECK_ARGS(check_unary(uop, src, dst));
+    const int64_t n = nelem(*dst);
+    if (n == 0) return GGML_B200_OK;
+    B200_CUDA_TRY(launch_pdl(unary_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, uop, (const float *)src->data, (float *)dst->data, n));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }
 
-int ggml_b200_op_soft_max(const float * src, const void * mask, int32_t mask_type, float * dst, int64_t ne0, int64_t ne1, int64_t ne2, int64_t ne3,
-                          float scale, float max_bias, void * stream) {
-    return ggml_b200_op_soft_max_diag(src, mask, mask_type, dst, ne0, ne1, ne2, ne3, scale, max_bias, -1, stream);
-}
-
-int ggml_b200_op_soft_max_diag(const float * src, const void * mask, int32_t mask_type, float * dst, int64_t ne0, int64_t ne1, int64_t ne2, int64_t ne3,
-                               float scale, float max_bias, int32_t diag_n_past, void * stream) {
-    const int64_t rows = ne1 * ne2 * ne3;
+int ggml_b200_op_soft_max(const ggml_b200_tensor * src, const ggml_b200_tensor * mask, const ggml_b200_tensor * dst, float scale, float max_bias,
+                          int32_t diag_n_past, void * stream) {
+    CHECK_ARGS(check_soft_max(src, mask, dst));
+    const int64_t ne0 = src->ne[0], ne1 = src->ne[1], ne2 = src->ne[2], rows = nrows(*src);
     if (rows == 0 || ne0 == 0) return GGML_B200_OK;
     const uint32_t n_head = (uint32_t)ne2;
     uint32_t n_head_log2 = 1; while (n_head_log2 * 2 <= n_head) n_head_log2 *= 2;
     const float m0 = powf(2.0f, -(max_bias) / n_head_log2), m1 = powf(2.0f, -(max_bias / 2.0f) / n_head_log2);
     const int threads = ne0 >= 1024 ? 256 : ne0 >= 128 ? 128 : 32;
-    B200_CUDA_TRY(launch_pdl(soft_max_kernel, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, src, (const uint8_t *)mask, mask_type, dst, ne0, ne1, ne2, scale, max_bias, m0, m1, n_head_log2, (int)diag_n_past));
+    const uint8_t * mp = mask ? (const uint8_t *)mask->data : nullptr;
+    const int mask_type = mask ? mask->type : 0;
+    B200_CUDA_TRY(launch_pdl(soft_max_kernel, dim3((unsigned)rows), dim3(threads), 0, (cudaStream_t)stream, (const float *)src->data, mp, mask_type,
+                             (float *)dst->data, ne0, ne1, ne2, scale, max_bias, m0, m1, n_head_log2, (int)diag_n_past));
     B200_LAUNCH_CHECK();
     return GGML_B200_OK;
 }

@@ -233,18 +233,20 @@ GGML_B200_API int ggml_b200_op_get_rows(const ggml_b200_tensor * src0, const ggm
 /* op: 0 add, 1 mul, 2 sub, 3 div; src1 broadcasts into dst's shape; dst may alias src0 */
 GGML_B200_API int ggml_b200_op_bin_bcast(int32_t op, const ggml_b200_tensor * src0, const ggml_b200_tensor * src1, const ggml_b200_tensor * dst, void * stream);
 GGML_B200_API int ggml_b200_op_norm(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst, float eps, void * stream);
-/* NORM / RMS_NORM followed by MUL(gain[ne0]) and ADD(bias[ne0]) in one pass; the three ggml nodes' outputs are all written */
-GGML_B200_API int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const float * gain, const ggml_b200_tensor * dst_mul,
-                                           const float * bias, const ggml_b200_tensor * dst_add, float eps, void * stream);
-GGML_B200_API int ggml_b200_op_scale(const float * src, float * dst, float s, int64_t n, void * stream);
-GGML_B200_API int ggml_b200_op_diag_mask_inf(const float * src, float * dst, int64_t ne0, int64_t ne1, int64_t n, int32_t n_past, void * stream);
-GGML_B200_API int ggml_b200_op_unary(int32_t uop, const float * src, float * dst, int64_t n, void * stream);
-GGML_B200_API int ggml_b200_op_soft_max(const float * src, const void * mask, int32_t mask_type, float * dst, int64_t ne0, int64_t ne1, int64_t ne2, int64_t ne3,
-                                        float scale, float max_bias, void * stream);
-/* SCALE -> DIAG_MASK_INF(n_past) -> SOFT_MAX in one row pass: softmax over x * scale with element i0 of row i1 masked where i0 > diag_n_past + i1
- * (diag_n_past < 0: no mask; then identical to ggml_b200_op_soft_max) */
-GGML_B200_API int ggml_b200_op_soft_max_diag(const float * src, const void * mask, int32_t mask_type, float * dst, int64_t ne0, int64_t ne1, int64_t ne2, int64_t ne3,
-                                             float scale, float max_bias, int32_t diag_n_past, void * stream);
+/* NORM / RMS_NORM followed by MUL(gain) and ADD(bias) in one pass, gain and bias packed f32 [ne0]; the three ggml nodes' outputs are all
+ * written */
+GGML_B200_API int ggml_b200_op_norm_affine(int32_t rms, const ggml_b200_tensor * src, const ggml_b200_tensor * dst_norm, const ggml_b200_tensor * gain,
+                                           const ggml_b200_tensor * dst_mul, const ggml_b200_tensor * bias, const ggml_b200_tensor * dst_add, float eps,
+                                           void * stream);
+/* SCALE, DIAG_MASK_INF and the unary functions (uop: enum ggml_b200_unary): src and dst packed f32 of one shape */
+GGML_B200_API int ggml_b200_op_scale(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, float s, void * stream);
+GGML_B200_API int ggml_b200_op_diag_mask_inf(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, int32_t n_past, void * stream);
+GGML_B200_API int ggml_b200_op_unary(int32_t uop, const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
+/* SOFT_MAX of packed f32 rows: softmax(x * scale + slope * mask row i1), mask NULL or a packed f32 / f16 [ne0, >= ne1] as ggml_soft_max_ext
+ * takes it.  diag_n_past >= 0 also folds a preceding DIAG_MASK_INF(n_past) (and, through scale, a preceding SCALE) into the same row pass:
+ * element i0 of row i1 is masked where i0 > diag_n_past + i1 (diag_n_past < 0: no such mask) */
+GGML_B200_API int ggml_b200_op_soft_max(const ggml_b200_tensor * src, const ggml_b200_tensor * mask, const ggml_b200_tensor * dst, float scale, float max_bias,
+                                        int32_t diag_n_past, void * stream);
 GGML_B200_API int ggml_b200_op_cpy(const ggml_b200_tensor * src, const ggml_b200_tensor * dst, void * stream);
 /* two independent float copies of the same element count in one launch (the K and V cache updates of a layer) */
 GGML_B200_API int ggml_b200_op_cpy2(const ggml_b200_tensor * src_a, const ggml_b200_tensor * dst_a, const ggml_b200_tensor * src_b, const ggml_b200_tensor * dst_b, void * stream);

@@ -11,9 +11,13 @@ extern "C" {
 int emu_check_get_rows(const T * a, const T * ids, const T * d) { return code(check_get_rows(a, ids, d)); }
 int emu_check_bin_bcast(int32_t op, const T * a, const T * b, const T * d) { return code(check_bin_bcast(op, a, b, d)); }
 int emu_check_norm(const T * s, const T * d) { return code(check_norm(s, d)); }
-int emu_check_norm_affine(const T * s, const T * d1, const float * gain, const T * d2, const float * bias, const T * d3) {
+int emu_check_norm_affine(const T * s, const T * d1, const T * gain, const T * d2, const T * bias, const T * d3) {
     return code(check_norm_affine(s, d1, gain, d2, bias, d3));
 }
+int emu_check_scale(const T * s, const T * d) { return code(check_scale(s, d)); }
+int emu_check_diag_mask_inf(const T * s, const T * d) { return code(check_diag_mask_inf(s, d)); }
+int emu_check_unary(int32_t uop, const T * s, const T * d) { return code(check_unary(uop, s, d)); }
+int emu_check_soft_max(const T * s, const T * mask, const T * d) { return code(check_soft_max(s, mask, d)); }
 int emu_check_cpy(const T * s, const T * d) { return code(check_cpy(s, d)); }
 int emu_check_cpy2(const T * s, const T * d, const T * s2, const T * d2) { return code(check_cpy2(s, d, s2, d2)); }
 int emu_check_flash_attn_ext(const T * q, const T * k, const T * v, const T * mask, const T * d) { return code(check_flash_attn_ext(q, k, v, mask, d)); }

@@ -8,9 +8,9 @@ on an H100 (DESIGN.md §5).
       divisors; NORM / RMS_NORM at row lengths either side of the launcher's 32 / 128 / 256-thread steps, no further from f64 than ggml-cpu
       on the same row; every unary function over finite values, +-0, +-inf, NaN and subnormals (bit-exact where it is one IEEE operation or
       ggml-cpu's f16 table, within the CUDA math library's ulp bound otherwise); SCALE and DIAG_MASK_INF bit-exact; float CPY / CONT / DUP
-      bit-exact through permuted, transposed and padded views;
+      bit-exact through permuted, transposed and padded views; a descriptor their checks refuse raises the check's code and launches nothing;
   (b) the same ops as graphs (oracle/core_probe.cpp) on B2000 against ggml-cpu, and the two chains the plug-in fuses (NORM -> MUL -> ADD,
-      SCALE -> DIAG_MASK_INF -> SOFT_MAX), whose bits do not depend on the fusion."""
+      SCALE -> DIAG_MASK_INF -> SOFT_MAX), whose bits do not depend on the fusion and which run as one launch each."""
 import os
 import subprocess
 import sys
@@ -179,6 +179,25 @@ def test_scale_and_diag_mask_inf_c_abi_are_exact():
         assert K.same_bits(m, np.where(i0 > n_past + i1, -np.inf, want_s)).all()
 
 
+def test_descriptor_launchers_refuse_what_their_checks_refuse():
+    """SCALE, DIAG_MASK_INF, the unary ops, SOFT_MAX and the fused norm: one bad descriptor each gives its check's code and launches nothing"""
+    import torch
+    import ggml_b200 as g
+    x = torch.randn(3, 9, 37, device="cuda")
+    v = torch.randn(37, device="cuda")
+    bad = [(lambda: g.op_scale(x.half(), 0.5), -1),                                 # f16 src
+           (lambda: g.op_diag_mask_inf(x.transpose(1, 2), 0), -1),                  # transposed src
+           (lambda: g.op_unary(14, x), -2),                                         # no such function
+           (lambda: g.op_soft_max(x, mask=torch.zeros(9, 36, device="cuda")), -2),  # mask narrower than ne0
+           (lambda: g.op_norm_affine(x, v[:36], v, 1e-5), -2)]                      # gain of ne0 - 1
+    for i, (launch, code) in enumerate(bad):
+        n0 = g.launch_count()
+        with pytest.raises(g.B200Error, match=rf"failed \({code}\)"):
+            launch()
+        assert g.launch_count() == n0, i
+    torch.cuda.synchronize()
+
+
 # ------------------------------------------------------------------ (a) float CPY / CONT / DUP
 @pytest.mark.parametrize("case", K.cpy_grid(), ids=lambda c: f"{('cpy', 'cont', 'dup')[c[0]]}-{c[1].type}-{c[1].ne}{'T' * c[1].transpose}")
 def test_float_cpy_c_abi_is_bit_exact(case):
@@ -267,18 +286,36 @@ def softmax_chain_cases():
             for s, scale, n_past in (((1, 12, 7, 7), 0.125, 0), ((2, 4, 5, 69), 0.0883883, 64), ((1, 2, 3, 1500), 1.0, 1497))]
 
 
+def plugin_launch_count() -> int:
+    """the kernels the plug-in loaded into the reference has launched so far (its ggml_backend_b200_launch_count, found through the registry)"""
+    import ctypes as C
+    ggml = C.CDLL(str(O.REF_DIR / "libggml.so"))
+    ggml.ggml_backend_reg_by_name.restype, ggml.ggml_backend_reg_by_name.argtypes = C.c_void_p, [C.c_char_p]
+    ggml.ggml_backend_reg_get_proc_address.restype, ggml.ggml_backend_reg_get_proc_address.argtypes = C.c_void_p, [C.c_void_p, C.c_char_p]
+    fn = ggml.ggml_backend_reg_get_proc_address(ggml.ggml_backend_reg_by_name(b"B200"), b"ggml_backend_b200_launch_count")
+    assert fn
+    return int(C.CFUNCTYPE(C.c_uint64)(fn)())
+
+
 def run_fused_chains(dev_name):
-    """every output of the two chains on `dev_name`, in one list"""
-    out = []
+    """every output of the two chains on `dev_name`, in one list, and the plug-in's kernel launches for each chain (the probe graphs have
+    fewer than 8 nodes, so they run eagerly and every launch is counted)"""
+    out, launches = [], []
+
+    def counted(probe, *args):
+        n0 = plugin_launch_count()
+        r = probe(dev_name, *args)
+        launches.append(plugin_launch_count() - n0)
+        return r
     for rms, eps, x, gain, bias in fused_chain_cases():
-        out += list(K.norm_affine(dev_name, rms, eps, x, gain, bias))
+        out += list(counted(K.norm_affine, rms, eps, x, gain, bias))
     for x, scale, n_past in softmax_chain_cases():
-        out.append(K.scale_mask_softmax(dev_name, x, scale, n_past))
-    return out
+        out.append(counted(K.scale_mask_softmax, x, scale, n_past))
+    return out, launches
 
 
 def test_fused_chains_match_ggml_cpu_and_the_unfused_nodes(plugin, tmp_path):
-    got, cpu = run_fused_chains("B2000"), run_fused_chains("CPU")
+    (got, launches), (cpu, _) = run_fused_chains("B2000"), run_fused_chains("CPU")
     n_norm = 3 * len(fused_chain_cases())
     worst_n = max(K.nmse64(a, b) for a, b in zip(got[:n_norm], cpu[:n_norm]))
     worst_s = max(K.nmse64(a, b) for a, b in zip(got[n_norm:], cpu[n_norm:]))
@@ -287,7 +324,7 @@ def test_fused_chains_match_ggml_cpu_and_the_unfused_nodes(plugin, tmp_path):
     # the same graphs with fusion disabled (read once per process: a fresh interpreter)
     script = ("import sys, numpy as np; sys.path[:0] = [sys.argv[1], sys.argv[1] + '/tests']; from oracle import decoder; "
               "from test_gpu_core_ops import run_fused_chains; decoder.plugin('libggml_core_probe.so'); "
-              "np.savez(sys.argv[2], *run_fused_chains('B2000'))")
+              "out, launches = run_fused_chains('B2000'); np.savez(sys.argv[2], *out, launches=launches)")
     env = dict(os.environ, GGML_B200_DISABLE_FUSION="1")
     p = subprocess.run([sys.executable, "-c", script, str(ROOT), str(tmp_path / "unfused.npz")], env=env, capture_output=True, text=True,
                        timeout=600)
@@ -295,3 +332,5 @@ def test_fused_chains_match_ggml_cpu_and_the_unfused_nodes(plugin, tmp_path):
     unfused = np.load(tmp_path / "unfused.npz")
     for i, a in enumerate(got):
         assert K.same_bits(a, unfused[f"arr_{i}"]).all(), i
+    # each chain ran as one launch instead of three: a chain the plug-in stopped fusing would still pass on bits
+    assert [u - 2 for u in unfused["launches"]] == launches, (launches, list(unfused["launches"]))

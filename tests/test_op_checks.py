@@ -1,7 +1,9 @@
 """CPU-only: the acceptance rules of ggml_b200/csrc/b200_op_checks.h compiled for the HOST (tests/hostemu/op_checks_emu.cpp).  The
 ggml_b200_op_* launchers return what these checks return, and the plug-in's supports_op asks the same checks, so this pins both without a
 device:
-  * every case the GPU suites assert through the C ABI (test_gpu_rope.py, test_gpu_moe.py, test_gpu_mamba.py) gives the same status code;
+  * every case the GPU suites assert through the C ABI (test_gpu_rope.py, test_gpu_moe.py, test_gpu_mamba.py, and the SCALE,
+    DIAG_MASK_INF, unary, SOFT_MAX and fused norm cases of test_gpu_core_ops.py, test_gpu_attention.py and test_gpu_parity.py) gives the
+    same status code;
   * the sources the plug-in declines in those suites are refused by the check (rows longer than 1024, unpacked SSM_CONV rows, ...);
   * the nodes of the llama (norm, neox), MoE (moe, moe60) and Mamba (mamba, falcon) decoder presets of oracle/*_graph.cpp are accepted,
     for a prompt and for a decode step;
@@ -137,6 +139,76 @@ def test_sum_rows_beyond_one_grid(checks):
     assert call(checks.emu_check_sum_rows, T(F32, (1, rows - 1)), T(F32, (1, rows - 1))) == OK
 
 
+# ------------------------------------------------------------------ SCALE, DIAG_MASK_INF, the unary ops, SOFT_MAX and the fused norm
+def test_elementwise_cases_of_the_gpu_suite(checks):
+    x = z(2, 4, 9, 37)                                                              # test_gpu_core_ops (a): SCALE, DIAG_MASK_INF
+    for fn in (checks.emu_check_scale, checks.emu_check_diag_mask_inf):
+        assert call(fn, D(x), D(x)) == OK
+        assert call(fn, T(F32, (37, 0)), T(F32, (37, 0))) == OK                                                   # empty
+        assert call(fn, D(x.half()), D(x)) == EUNSUPPORTED and call(fn, D(x), D(x.half())) == EUNSUPPORTED         # f16
+        assert call(fn, D(z(37, 9).t()), D(z(9, 37))) == EUNSUPPORTED                                               # transposed src
+        assert call(fn, D(z(9, 40)[:, :37]), D(z(9, 37))) == EUNSUPPORTED                                           # padded src rows
+        assert call(fn, D(z(9, 37)), D(z(9, 40)[:, :37])) == EUNSUPPORTED                                           # padded dst rows
+        assert call(fn, D(x), D(z(2, 4, 9, 36))) == EINVAL and call(fn, D(x), D(z(4, 2, 9, 37))) == EINVAL         # dst of another shape
+        assert call(fn, T(F32, (256 * 0x7fffffff + 1,)), T(F32, (256 * 0x7fffffff + 1,))) == EUNSUPPORTED           # beyond one grid
+        assert call(fn, T(F32, (256 * 0x7fffffff,)), T(F32, (256 * 0x7fffffff,))) == OK
+    for n in (1 << 16, 1 << 14, 10, 768, 3072):                                     # every unary op's inputs; y + bias of the mat-mul suites
+        u = D(z(n))
+        for op in range(14):
+            assert call(checks.emu_check_unary, op, u, u) == OK
+    u = D(z(16))
+    for op in (-1, 14):                                                             # no such function (the plug-in's code for one it lacks is -1)
+        assert call(checks.emu_check_unary, op, u, u) == EINVAL
+    assert call(checks.emu_check_unary, 0, D(z(16).half()), u) == EUNSUPPORTED
+    assert call(checks.emu_check_unary, 0, D(z(4, 8).t()), D(z(8, 4))) == EUNSUPPORTED
+    assert call(checks.emu_check_unary, 0, u, D(z(15))) == EINVAL
+
+
+def test_soft_max_cases_of_the_gpu_suite(checks):
+    from test_gpu_attention import soft_max_grid
+    for case in soft_max_grid():                                                    # test_gpu_attention (c): masks of ne1 or more rows
+        x = T(F32, case.ne)
+        mask = None if case.mask_type is None else T(case.mask_type, (case.ne[0], case.mask_rows or case.ne[1]))
+        assert call(checks.emu_check_soft_max, x, mask, x) == OK, str(case)
+    for heads, n1, n0 in ((12, 1, 37), (12, 5, 9), (3, 64, 200), (1, 1, 1), (12, 1, 1030), (12, 7, 7), (4, 5, 69), (2, 3, 1500)):
+        x = D(z(heads, n1, n0))                                                     # the fused SCALE -> DIAG_MASK_INF -> SOFT_MAX
+        assert call(checks.emu_check_soft_max, x, None, x) == OK
+    x, m = D(z(2, 3, 7, 64)), D(z(9, 64, dt=torch.float16))
+    assert call(checks.emu_check_soft_max, x, m, x) == OK
+    assert call(checks.emu_check_soft_max, T(F32, (64, 0, 3, 2)), m, T(F32, (64, 0, 3, 2))) == OK                  # empty
+    assert call(checks.emu_check_soft_max, D(z(2, 3, 7, 64).half()), m, x) == EUNSUPPORTED                         # f16 src
+    assert call(checks.emu_check_soft_max, D(z(2, 3, 64, 7).transpose(2, 3)), m, x) == EUNSUPPORTED                # transposed src
+    assert call(checks.emu_check_soft_max, D(z(2, 3, 7, 72)[..., :64]), m, x) == EUNSUPPORTED                      # padded src rows
+    assert call(checks.emu_check_soft_max, x, m, D(z(2, 3, 7, 72)[..., :64])) == EUNSUPPORTED                      # padded dst rows
+    assert call(checks.emu_check_soft_max, x, D(z(9, 72, dt=torch.float16)[:, :64]), x) == EUNSUPPORTED           # mask rows not packed
+    assert call(checks.emu_check_soft_max, x, D(z(9, 64, dt=torch.int32)), x) == EUNSUPPORTED                      # i32 mask
+    assert call(checks.emu_check_soft_max, x, D(z(9, 63, dt=torch.float16)), x) == EINVAL                          # mask narrower than ne0
+    assert call(checks.emu_check_soft_max, x, D(z(6, 64, dt=torch.float16)), x) == EINVAL                          # fewer mask rows than ne1
+    assert call(checks.emu_check_soft_max, x, D(z(2, 9, 64, dt=torch.float16)), x) == EINVAL                       # not a matrix
+    assert call(checks.emu_check_soft_max, x, m, D(z(2, 3, 6, 64))) == EINVAL                                      # dst of another shape
+    big = T(F32, (1, 0x7fffffff + 1))
+    assert call(checks.emu_check_soft_max, big, None, big) == EUNSUPPORTED                                         # rows beyond one grid
+
+
+def test_norm_affine_cases_of_the_gpu_suite(checks):
+    # test_gpu_parity's fused norm, and the chains test_gpu_core_ops runs through the plug-in
+    for shape in ((7, 768), (1, 2, 7, 768), (1, 2, 3, 4096), (1, 2, 5, 33), (1, 2, 2, 14336)):
+        x, v = D(z(*shape)), D(z(shape[-1]))
+        assert call(checks.emu_check_norm, x, x) == OK
+        assert call(checks.emu_check_norm_affine, x, x, v, x, v, x) == OK
+    x, v = D(z(7, 768)), D(z(768))
+    assert call(checks.emu_check_norm_affine, x, x, D(z(767)), x, v, x) == EINVAL                                  # gain of ne0 - 1
+    assert call(checks.emu_check_norm_affine, x, x, v, x, D(z(769)), x) == EINVAL                                  # bias of ne0 + 1
+    assert call(checks.emu_check_norm_affine, x, x, D(z(2, 768)), x, v, x) == EINVAL                               # a matrix gain
+    assert call(checks.emu_check_norm_affine, x, x, D(z(768, 2)[:, 0]), x, v, x) == EUNSUPPORTED                    # strided gain
+    assert call(checks.emu_check_norm_affine, x, x, D(z(768).half()), x, v, x) == EUNSUPPORTED                     # f16 gain
+    for k in range(3):                                                              # a dst of another shape
+        d = [x, x, x]
+        d[k] = D(z(6, 768))
+        assert call(checks.emu_check_norm_affine, x, d[0], v, d[1], v, d[2]) == EINVAL
+    assert call(checks.emu_check_norm, x, D(z(6, 768))) == EINVAL
+
+
 # ------------------------------------------------------------------ the decoder presets' nodes
 @pytest.mark.parametrize("preset", ["norm", "neox"])
 @pytest.mark.parametrize("N,n_past", [(7, 0), (1, 7)], ids=["prompt", "decode"])
@@ -147,7 +219,7 @@ def test_llama_preset_nodes_are_accepted(checks, preset, N, n_past):
     x = T(F32, (n_embd, N))
     assert call(checks.emu_check_get_rows, T(Q4_K, (n_embd, n_vocab)), T(I32, (N,)), x) == OK
     assert call(checks.emu_check_norm, x, x) == OK
-    assert call(checks.emu_check_norm_affine, x, x, C.c_void_p(64), x, C.c_void_p(64), x) == OK
+    assert call(checks.emu_check_norm_affine, x, x, T(F32, (n_embd,)), x, T(F32, (n_embd,)), x) == OK
     assert call(checks.emu_check_bin_bcast, 1, x, T(F32, (n_embd,)), x) == OK
     assert call(checks.emu_check_bin_bcast, 0, x, x, x) == OK
     p = g.rope_params(32 if neox else 64, g.ROPE_NEOX if neox else g.ROPE_NORM, n_ctx_orig=512, freq_scale=0.25 if neox else 1.0,
@@ -169,6 +241,7 @@ def test_llama_preset_nodes_are_accepted(checks, preset, N, n_past):
         assert call(checks.emu_check_cpy, T(F32, (N, ngqa), (4 * ngqa, 4, 4 * ngqa * N, 4 * ngqa * N)), vt) == OK   # CPY(transpose(v), view of the V cache)
         kq = T(F32, (n_kv, N, n_head))
         assert call(checks.emu_check_mul_mat_f, K, Q, kq) == OK
+        assert call(checks.emu_check_soft_max, kq, T(F32, (n_kv, N)), kq) == OK                                      # SOFT_MAX_EXT(kq, kq_mask)
         V = T(F16, (n_kv, hd, n_head_kv), (2, 2 * n_ctx, 2 * n_ctx * hd, 2 * n_ctx * hd * n_head_kv))
         kqv = T(F32, (hd, N, n_head))
         assert call(checks.emu_check_mul_mat_f, V, kq, kqv) == OK
