@@ -20,6 +20,7 @@ F32, F16, Q4_0, Q8_0, Q4_K, Q5_K, Q6_K = 0, 1, 2, 8, 12, 13, 14
 Q4_1, Q5_0, Q5_1, Q2_K, Q3_K, IQ4_NL, IQ4_XS = 3, 6, 7, 10, 11, 20, 23      # SURVEY §8f-2 formats
 IQ2_XXS, IQ3_XXS, IQ1_S = 16, 18, 19                                       # grid-codebook i-quants (generic kernels)
 IQ2_XS, IQ3_S, IQ2_S, IQ1_M, TQ1_0, TQ2_0 = 17, 21, 22, 29, 34, 35
+I16, I32, I64, BF16 = 25, 26, 27, 30                                       # the small ops' indices, counts and raw 2-byte words
 QUANT_TYPES = (Q4_0, Q8_0, Q4_K, Q5_K, Q6_K)
 NEXT_TYPES = (Q4_1, Q5_0, Q5_1, Q2_K, Q3_K, IQ4_NL, IQ4_XS)
 TYPE_NAMES = {F32: "f32", F16: "f16", Q4_0: "q4_0", Q8_0: "q8_0", Q4_K: "q4_K", Q5_K: "q5_K", Q6_K: "q6_K",
@@ -55,41 +56,143 @@ class MulMatIdArgs(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_size", C.c_size_t)]
 
 
+class Gather(C.Structure):
+    _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("row_offset", C.c_int64), ("epoch", C.c_uint32),
+                ("y_peers", C.c_void_p * 8), ("flag_peers", C.c_void_p * 8)]
+
+
+class Epilogue(C.Structure):
+    _fields_ = [("bias", C.c_void_p), ("dst_bias", C.c_void_p), ("unary", C.c_int32), ("dst_unary", C.c_void_p), ("residual", C.c_void_p)]
+
+
+class TensorDesc(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("type", C.c_int32), ("ne", C.c_int64 * 4), ("nb", C.c_size_t * 4)]
+
+
+class RopeParams(C.Structure):
+    """ggml_b200_rope_params (include/ggml-b200.h)"""
+    _fields_ = [("n_dims", C.c_int32), ("mode", C.c_int32), ("sections", C.c_int32 * 4), ("freq_scale", C.c_float), ("ext_factor", C.c_float),
+                ("mscale", C.c_float), ("theta_scale", C.c_float), ("corr_dims", C.c_float * 2)]
+
+
+class Im2colParams(C.Structure):
+    """ggml_b200_im2col_params (include/ggml-b200.h)"""
+    _fields_ = [("s0", C.c_int32), ("s1", C.c_int32), ("p0", C.c_int32), ("p1", C.c_int32), ("d0", C.c_int32), ("d1", C.c_int32), ("is_2D", C.c_int32)]
+
+
+class PoolParams(C.Structure):
+    """ggml_b200_pool_params (include/ggml-b200.h)"""
+    _fields_ = [("op", C.c_int32), ("k0", C.c_int32), ("k1", C.c_int32), ("s0", C.c_int32), ("s1", C.c_int32), ("p0", C.c_int32), ("p1", C.c_int32)]
+
+
+# restype and argtypes of every function include/ggml-b200.h declares; tests/test_abi_mirror.py checks them against the header.  An
+# undeclared argument goes to C as an int, which cuts a device pointer or an int64 extent to 32 bits.
+_INT, _I32, _I64, _U32, _SZ, _F32, _PTR = C.c_int, C.c_int32, C.c_int64, C.c_uint32, C.c_size_t, C.c_float, C.c_void_p
+_MM, _MMID, _T = C.POINTER(MulMatArgs), C.POINTER(MulMatIdArgs), C.POINTER(TensorDesc)
+_F16_GEMM = [_PTR, _SZ, _PTR, _SZ, _PTR, _I64, _I64, _I64, _PTR, _SZ, _U32, _PTR]
+SIGNATURES = {
+    "ggml_b200_mul_mat_workspace_size": (_SZ, [_MM]),
+    "ggml_b200_mul_mat": (_INT, [_MM, _PTR]),
+    "ggml_b200_mul_mat_plan": (_INT, [_MM]),
+    "ggml_b200_mul_mat_f16_workspace_size": (_SZ, [_I64] * 3),
+    "ggml_b200_mul_mat_f16": (_INT, _F16_GEMM),
+    "ggml_b200_mul_mat_f16_f16_workspace_size": (_SZ, [_I64] * 3),
+    "ggml_b200_mul_mat_f16_f16": (_INT, _F16_GEMM),
+    "ggml_b200_mul_mat_fused": (_INT, [_MM, C.POINTER(Epilogue), _PTR]),
+    "ggml_b200_mul_mat_host": (_INT, [_MM, _PTR, _PTR, _PTR]),
+    "ggml_b200_mul_mat_host_batch": (_INT, [_MM, _I32, _PTR, C.POINTER(_PTR), _PTR]),
+    "ggml_b200_mul_mat_gather": (_INT, [_MM, C.POINTER(Gather), _PTR]),
+    "ggml_b200_mul_mat_gather_supported": (_INT, [_MM]),
+    "ggml_b200_gather_wait": (_INT, [_PTR, _I32, _U32, _PTR]),
+    "ggml_b200_ipc_alloc": (_INT, [_SZ, C.POINTER(_PTR), _PTR]),
+    "ggml_b200_ipc_free": (_INT, [_PTR]),
+    "ggml_b200_ipc_open": (_INT, [_PTR, C.POINTER(_PTR)]),
+    "ggml_b200_ipc_close": (_INT, [_PTR]),
+    "ggml_b200_mul_mat_id_workspace_size": (_SZ, [_MMID]),
+    "ggml_b200_mul_mat_id": (_INT, [_MMID, _PTR]),
+    "ggml_b200_row_size": (_SZ, [_I32, _I64]),
+    "ggml_b200_dequantize": (_INT, [_I32, _PTR, _PTR, _I32, _I64, _PTR]),
+    "ggml_b200_quantize": (_INT, [_I32, _PTR, _PTR, _I64, _PTR]),
+    "ggml_b200_act_record_size": (_SZ, [_I32, _I64]),
+    "ggml_b200_quantize_activations": (_INT, [_I32, _PTR, _SZ, _I64, _I64, _PTR, _PTR]),
+    "ggml_b200_op_get_rows": (_INT, [_T] * 3 + [_PTR]),
+    "ggml_b200_op_bin_bcast": (_INT, [_I32] + [_T] * 3 + [_PTR]),
+    "ggml_b200_op_norm": (_INT, [_I32, _T, _T, _F32, _PTR]),
+    "ggml_b200_op_norm_affine": (_INT, [_I32] + [_T] * 6 + [_F32, _PTR]),
+    "ggml_b200_op_scale": (_INT, [_T, _T, _F32, _PTR]),
+    "ggml_b200_op_diag_mask_inf": (_INT, [_T, _T, _I32, _PTR]),
+    "ggml_b200_op_unary": (_INT, [_I32, _T, _T, _PTR]),
+    "ggml_b200_op_soft_max": (_INT, [_T] * 3 + [_F32, _F32, _I32, _PTR]),
+    "ggml_b200_op_cpy": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_cpy2": (_INT, [_T] * 4 + [_PTR]),
+    "ggml_b200_op_flash_attn_ext": (_INT, [_T] * 5 + [_F32] * 3 + [_PTR]),
+    "ggml_b200_op_mul_mat_f": (_INT, [_T] * 3 + [_PTR]),
+    "ggml_b200_op_rope": (_INT, [_T] * 4 + [C.POINTER(RopeParams), _PTR]),
+    "ggml_b200_op_argsort": (_INT, [_T, _T, _I32, _PTR]),
+    "ggml_b200_op_sum_rows": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_concat": (_INT, [_T] * 3 + [_I32, _PTR]),
+    "ggml_b200_op_ssm_conv": (_INT, [_T] * 3 + [_PTR]),
+    "ggml_b200_op_ssm_scan": (_INT, [_T] * 7 + [_PTR]),
+    "ggml_b200_op_rwkv_wkv6": (_INT, [_T] * 7 + [_PTR]),
+    "ggml_b200_op_gated_linear_attn": (_INT, [_T] * 6 + [_F32, _PTR]),
+    "ggml_b200_op_im2col": (_INT, [_T] * 3 + [C.POINTER(Im2colParams), _PTR]),
+    "ggml_b200_op_pool_2d": (_INT, [_T] * 2 + [C.POINTER(PoolParams), _PTR]),
+    "ggml_b200_op_upscale": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_leaky_relu": (_INT, [_T] * 2 + [_F32, _PTR]),
+    "ggml_b200_op_repeat": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_win_part": (_INT, [_T] * 2 + [_I32] * 3 + [_PTR]),
+    "ggml_b200_op_win_unpart": (_INT, [_T] * 2 + [_I32, _PTR]),
+    "ggml_b200_op_get_rel_pos": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_add_rel_pos": (_INT, [_T] * 4 + [_PTR]),
+    "ggml_b200_op_conv_transpose_2d": (_INT, [_T] * 3 + [_I32, _PTR]),
+    "ggml_b200_op_out_prod": (_INT, [_T] * 3 + [_PTR]),
+    "ggml_b200_op_cross_entropy_loss": (_INT, [_T] * 3 + [_PTR]),
+    "ggml_b200_op_cross_entropy_loss_back": (_INT, [_T] * 4 + [_PTR]),
+    "ggml_b200_op_opt_step_adamw": (_INT, [_T] * 5 + [_PTR]),
+    "ggml_b200_op_argmax": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_count_equal": (_INT, [_T] * 3 + [_PTR]),
+    "ggml_b200_op_sum": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_op_repeat_back": (_INT, [_T] * 2 + [_PTR]),
+    "ggml_b200_last_error": (C.c_char_p, []),
+    "ggml_b200_device_count": (_INT, []),
+    "ggml_b200_sm_count": (_INT, []),
+    "ggml_b200_prepare": (_INT, []),
+    "ggml_b200_launch_count": (C.c_uint64, []),
+    "ggml_b200_version": (C.c_char_p, []),
+}
+
+
+def load(path) -> C.CDLL:
+    """Opens a build of the kernel library with every function of SIGNATURES declared on it."""
+    L = C.CDLL(str(path))
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return L
+
+
 _lib = None
 
 
 def lib() -> C.CDLL:
-    """The kernel-launch shim.  Fails loudly when it has not been built (no fallback)."""
+    """The kernel-launch shim, loaded once.  Fails loudly when it has not been built (no fallback)."""
     global _lib
     if _lib is None:
         if not KERNELS_SO.exists():
             raise B200Error(f"{KERNELS_SO} is not built: run `python -c 'import __graft_entry__ as g; g.build()'`")
-        L = C.CDLL(str(KERNELS_SO))
-        L.ggml_b200_last_error.restype = C.c_char_p
-        L.ggml_b200_version.restype = C.c_char_p
-        L.ggml_b200_launch_count.restype = C.c_uint64
-        L.ggml_b200_row_size.restype = C.c_size_t
-        L.ggml_b200_row_size.argtypes = [C.c_int32, C.c_int64]
-        L.ggml_b200_act_record_size.restype = C.c_size_t
-        L.ggml_b200_act_record_size.argtypes = [C.c_int32, C.c_int64]
-        L.ggml_b200_quantize_activations.argtypes = [C.c_int32, C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
-        L.ggml_b200_mul_mat_workspace_size.restype = C.c_size_t
-        L.ggml_b200_mul_mat_workspace_size.argtypes = [C.POINTER(MulMatArgs)]
-        L.ggml_b200_mul_mat_plan.argtypes = [C.POINTER(MulMatArgs)]
-        L.ggml_b200_mul_mat.argtypes = [C.POINTER(MulMatArgs), C.c_void_p]
-        L.ggml_b200_mul_mat_host.argtypes = [C.POINTER(MulMatArgs), C.c_void_p, C.c_void_p, C.c_void_p]
-        L.ggml_b200_mul_mat_id_workspace_size.restype = C.c_size_t
-        L.ggml_b200_mul_mat_id_workspace_size.argtypes = [C.POINTER(MulMatIdArgs)]
-        L.ggml_b200_mul_mat_id.argtypes = [C.POINTER(MulMatIdArgs), C.c_void_p]
-        L.ggml_b200_dequantize.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p]
-        L.ggml_b200_quantize.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
-        _lib = L
+        _lib = load(KERNELS_SO)
     return _lib
 
 
 def check(rc: int, what: str) -> None:
     if rc != 0:
         raise B200Error(f"{what} failed ({rc}): {lib().ggml_b200_last_error().decode()}")
+
+
+def _launch(name: str, *args) -> None:
+    """Calls `name` with args and the current CUDA stream; a nonzero status raises B200Error.  A structure argument is passed as
+    itself: its declared POINTER argtype passes it by reference."""
+    check(getattr(lib(), name)(*args, _stream()), name)
 
 
 def row_size(t: int, k: int) -> int:
@@ -135,7 +238,7 @@ def mul_mat_args(t, W, X, Y, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, nb=None
     else:
         a.nb01, a.nb02, a.nb03, a.nb11, a.nb12, a.nb13 = nb
     a.src0, a.src1, a.dst = W.data_ptr(), X.data_ptr(), Y.data_ptr()
-    ws = workspace if workspace is not None else _ws.get(int(lib().ggml_b200_mul_mat_workspace_size(C.byref(a))))
+    ws = workspace if workspace is not None else _ws.get(int(lib().ggml_b200_mul_mat_workspace_size(a)))
     a.workspace, a.workspace_size = ws.data_ptr(), ws.numel()
     return a
 
@@ -145,8 +248,7 @@ def mul_mat(t, W, X, M, N, K, batch=(1, 1, 1, 1), flags=MM_AUTO, out=None, nb=No
     import torch
     ne02, ne03, ne12, ne13 = batch
     Y = out if out is not None else torch.empty((ne13, ne12, N, M), dtype=torch.float32, device="cuda")
-    a = mul_mat_args(t, W, X, Y, M, N, K, batch, flags, nb, workspace)
-    check(lib().ggml_b200_mul_mat(C.byref(a), _stream()), "ggml_b200_mul_mat")
+    _launch("ggml_b200_mul_mat", mul_mat_args(t, W, X, Y, M, N, K, batch, flags, nb, workspace))
     return Y
 
 
@@ -158,7 +260,7 @@ def mul_mat_plan(t, M, N, K, flags=MM_AUTO) -> int:
     rb = row_size(t, K)
     a.nb01, a.nb02, a.nb03, a.nb11, a.nb12, a.nb13 = rb, rb * M, rb * M, K * 4, K * 4 * N, K * 4 * N
     a.src0 = a.src1 = a.dst = 256      # aligned dummies: plan() never dereferences
-    return int(lib().ggml_b200_mul_mat_plan(C.byref(a)))
+    return int(lib().ggml_b200_mul_mat_plan(a))
 
 
 def mul_mat_id(t, W, X, ids, M, K, n_expert, n_used, nb1cols, n_tok, out=None, workspace=None):
@@ -173,9 +275,9 @@ def mul_mat_id(t, W, X, ids, M, K, n_expert, n_used, nb1cols, n_tok, out=None, w
     a.nb01, a.nb02, a.nb11, a.nb12 = rb, rb * M, K * 4, K * 4 * nb1cols
     a.ids_nb1 = ids.stride(0) * 4
     a.src0, a.src1, a.ids, a.dst = W.data_ptr(), X.data_ptr(), ids.data_ptr(), Y.data_ptr()
-    ws = workspace if workspace is not None else _ws.get(int(lib().ggml_b200_mul_mat_id_workspace_size(C.byref(a))))
+    ws = workspace if workspace is not None else _ws.get(int(lib().ggml_b200_mul_mat_id_workspace_size(a)))
     a.workspace, a.workspace_size = ws.data_ptr(), ws.numel()
-    check(lib().ggml_b200_mul_mat_id(C.byref(a), _stream()), "ggml_b200_mul_mat_id")
+    _launch("ggml_b200_mul_mat_id", a)
     return Y
 
 
@@ -183,8 +285,7 @@ def dequantize(t, blocks, n, dtype=None):
     import torch
     dtype = dtype or torch.float32
     out = torch.empty(n, dtype=dtype, device="cuda")
-    check(lib().ggml_b200_dequantize(t, blocks.data_ptr(), out.data_ptr(), F32 if dtype == torch.float32 else F16, n, _stream()),
-          "ggml_b200_dequantize")
+    _launch("ggml_b200_dequantize", t, blocks.data_ptr(), out.data_ptr(), F32 if dtype == torch.float32 else F16, n)
     return out
 
 
@@ -192,7 +293,7 @@ def quantize(t, x):
     import torch
     x = x.contiguous()
     out = torch.empty(row_size(t, x.numel()), dtype=torch.uint8, device="cuda")
-    check(lib().ggml_b200_quantize(t, x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "ggml_b200_quantize")
+    _launch("ggml_b200_quantize", t, x.data_ptr(), out.data_ptr(), x.numel())
     return out
 
 
@@ -202,30 +303,18 @@ def quantize_activations(weight_type, x):
     rows, K = x.shape
     rs = int(lib().ggml_b200_act_record_size(weight_type, K))
     out = torch.zeros((rows, rs), dtype=torch.uint8, device="cuda")
-    check(lib().ggml_b200_quantize_activations(weight_type, x.data_ptr(), x.stride(0) * 4, rows, K, out.data_ptr(), _stream()),
-          "ggml_b200_quantize_activations")
+    _launch("ggml_b200_quantize_activations", weight_type, x.data_ptr(), x.stride(0) * 4, rows, K, out.data_ptr())
     return out
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # Row-sharded multi-GPU mat-vec with the exchange fused into the kernel (peer stores over NVLink, CUDA IPC buffers)
-class Gather(C.Structure):
-    _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("row_offset", C.c_int64), ("epoch", C.c_uint32),
-                ("y_peers", C.c_void_p * 8), ("flag_peers", C.c_void_p * 8)]
-
-
 class PeerExchange:
     """Per-rank gathered-y buffers (`slots` full-length vectors) + flag array, visible to every peer through CUDA IPC."""
 
     def __init__(self, m_total: int, rank: int, world: int, row_offset: int, slots: int = 1):
         import torch.distributed as dist
         L = lib()
-        L.ggml_b200_ipc_alloc.argtypes = [C.c_size_t, C.POINTER(C.c_void_p), C.c_void_p]
-        L.ggml_b200_ipc_open.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        L.ggml_b200_ipc_close.argtypes = [C.c_void_p]
-        L.ggml_b200_ipc_free.argtypes = [C.c_void_p]
-        L.ggml_b200_mul_mat_gather.argtypes = [C.POINTER(MulMatArgs), C.POINTER(Gather), C.c_void_p]
-        L.ggml_b200_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_uint32, C.c_void_p]
         assert 1 <= world <= 8
         self.rank, self.world, self.m_total, self.slots = rank, world, m_total, slots
         self.y_ptr, self.f_ptr = C.c_void_p(), C.c_void_p()
@@ -256,11 +345,11 @@ class PeerExchange:
 
     def mul_mat_gather(self, args: MulMatArgs, slot: int = 0):
         """compute this rank's rows and store them into every peer's gathered y (slot); publishes one exchange epoch"""
-        check(lib().ggml_b200_mul_mat_gather(C.byref(args), C.byref(self.ga[slot]), _stream()), "ggml_b200_mul_mat_gather")
+        _launch("ggml_b200_mul_mat_gather", args, self.ga[slot])
 
     def wait(self):
         """stream-wait until every rank has published as many exchanges as this rank has"""
-        check(lib().ggml_b200_gather_wait(self.f_ptr, self.world, 0, _stream()), "ggml_b200_gather_wait")
+        _launch("ggml_b200_gather_wait", self.f_ptr, self.world, 0)
 
     def y_full(self, slot: int = 0):
         """zero-copy torch view of this rank's gathered y (slot)"""
@@ -284,20 +373,20 @@ class PeerExchange:
 
 # ---------------------------------------------------------------------------------------------------------------
 # fused epilogue / small ops used by the backend's graph-level fusion (thin ctypes mirrors, for the tests)
-class Epilogue(C.Structure):
-    _fields_ = [("bias", C.c_void_p), ("dst_bias", C.c_void_p), ("unary", C.c_int32), ("dst_unary", C.c_void_p), ("residual", C.c_void_p)]
-
-
-class TensorDesc(C.Structure):
-    _fields_ = [("data", C.c_void_p), ("type", C.c_int32), ("ne", C.c_int64 * 4), ("nb", C.c_size_t * 4)]
+def _desc_type(t) -> int:
+    """the ggml type id of a torch tensor's dtype"""
+    import torch
+    return {torch.float32: F32, torch.float16: F16, torch.int32: I32, torch.int16: I16, torch.bfloat16: BF16, torch.int64: I64}[t.dtype]
 
 
 def tensor_desc(t) -> TensorDesc:
-    """descriptor of a contiguous torch tensor in ggml order (ne[0] = last torch dim)"""
-    import torch
+    """descriptor of a contiguous torch tensor in ggml order (ne[0] = last torch dim), with packed strides; strided_desc describes
+    any other"""
+    if not t.is_contiguous():
+        raise B200Error(f"tensor_desc: a tensor of shape {tuple(t.shape)} and strides {t.stride()} is not contiguous")
     d = TensorDesc()
     d.data = t.data_ptr()
-    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30, torch.int64: 27}[t.dtype]
+    d.type = _desc_type(t)
     shape = list(t.shape)[::-1] + [1] * (4 - t.dim())
     es = t.element_size()
     nb = es
@@ -312,8 +401,6 @@ def mul_mat_fused(t, W, X, M, K, bias, gelu: bool, residual=None, out=None, work
     """y = W.x ; y2 = y + bias ; y3 = gelu(y2) (or y2 + residual) in one launch (n = 1).  Returns (y, y2, y3 or None).
     out: None (new tensors) or (y, y2, y3) f32 tensors of M elements (y3 None without gelu or residual); workspace: as for mul_mat."""
     import torch
-    L = lib()
-    L.ggml_b200_mul_mat_fused.argtypes = [C.POINTER(MulMatArgs), C.POINTER(Epilogue), C.c_void_p]
     if out is not None:
         Y, Y2, Y3 = out[0].view(1, 1, 1, M), out[1], out[2]
     else:
@@ -324,7 +411,7 @@ def mul_mat_fused(t, W, X, M, K, bias, gelu: bool, residual=None, out=None, work
     ep = Epilogue()
     ep.bias, ep.dst_bias, ep.unary, ep.dst_unary = bias.data_ptr(), Y2.data_ptr(), (2 if residual is not None else 1 if gelu else 0), (Y3.data_ptr() if Y3 is not None else None)
     ep.residual = residual.data_ptr() if residual is not None else None
-    check(L.ggml_b200_mul_mat_fused(C.byref(a), C.byref(ep), _stream()), "ggml_b200_mul_mat_fused")
+    _launch("ggml_b200_mul_mat_fused", a, ep)
     return Y.view(-1), Y2, Y3
 
 
@@ -334,11 +421,8 @@ UNARY_STEP = 13                                # GGML_B200_UNARY_STEP (GGML_UNAR
 
 def op_unary(uop: int, x):
     import torch
-    L = lib()
-    L.ggml_b200_op_unary.argtypes = [C.c_int32, C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p]
     y = torch.empty_like(x)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_unary(uop, C.byref(s), C.byref(d), _stream()), "ggml_b200_op_unary")
+    _launch("ggml_b200_op_unary", uop, strided_desc(x), strided_desc(y))
     return y
 
 
@@ -346,43 +430,30 @@ def op_norm(x, eps: float, rms: bool = False, out=None):
     """GGML_OP_NORM / RMS_NORM along the last dim of an f32 x (any view with that dim contiguous) -> a new contiguous tensor, or into
     out (a contiguous tensor of x's shape)"""
     import torch
-    L = lib()
-    L.ggml_b200_op_norm.argtypes = [C.c_int32, C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_float, C.c_void_p]
     y = out if out is not None else torch.empty(x.shape, dtype=x.dtype, device=x.device)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_norm(int(rms), C.byref(s), C.byref(d), eps, _stream()), "ggml_b200_op_norm")
+    _launch("ggml_b200_op_norm", int(rms), strided_desc(x), tensor_desc(y), eps)
     return y
 
 
 def op_norm_affine(x, gain, bias, eps: float, rms: bool = False):
     import torch
-    L = lib()
-    L.ggml_b200_op_norm_affine.argtypes = [C.c_int32] + [C.POINTER(TensorDesc)] * 6 + [C.c_float, C.c_void_p]
     y1, y2, y3 = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
-    s, d1, gd, d2, bd, d3 = (strided_desc(t) for t in (x, y1, gain, y2, bias, y3))
-    check(L.ggml_b200_op_norm_affine(int(rms), C.byref(s), C.byref(d1), C.byref(gd), C.byref(d2), C.byref(bd), C.byref(d3), eps, _stream()),
-          "ggml_b200_op_norm_affine")
+    _launch("ggml_b200_op_norm_affine", int(rms), *(strided_desc(t) for t in (x, y1, gain, y2, bias, y3)), eps)
     return y1, y2, y3
 
 
 def op_scale(x, s: float):
     import torch
-    L = lib()
-    L.ggml_b200_op_scale.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_float, C.c_void_p]
     y = torch.empty_like(x)
-    sd, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_scale(C.byref(sd), C.byref(d), s, _stream()), "ggml_b200_op_scale")
+    _launch("ggml_b200_op_scale", strided_desc(x), strided_desc(y), s)
     return y
 
 
 def op_diag_mask_inf(x, n_past: int):
     """x: [..., ne1, ne0] contiguous f32"""
     import torch
-    L = lib()
-    L.ggml_b200_op_diag_mask_inf.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_int32, C.c_void_p]
     y = torch.empty_like(x)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_diag_mask_inf(C.byref(s), C.byref(d), n_past, _stream()), "ggml_b200_op_diag_mask_inf")
+    _launch("ggml_b200_op_diag_mask_inf", strided_desc(x), strided_desc(y), n_past)
     return y
 
 
@@ -391,34 +462,19 @@ def op_soft_max(x, scale: float = 1.0, diag_n_past: int = -1, mask=None, max_bia
     mask: a contiguous f16 or f32 [ne01 >= ne1, ne0] added (times the ALiBi slope of head i2 when max_bias > 0) to row i1 of every matrix,
     as ggml_soft_max_ext broadcasts it.  inplace: the result is written into x."""
     import torch
-    L = lib()
-    L.ggml_b200_op_soft_max.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_float, C.c_float, C.c_int32, C.c_void_p]
     y = x if inplace else torch.empty_like(x)
-    s, d = strided_desc(x), tensor_desc(y)
-    m = None if mask is None else C.byref(strided_desc(mask))
-    check(L.ggml_b200_op_soft_max(C.byref(s), m, C.byref(d), scale, max_bias, diag_n_past, _stream()), "ggml_b200_op_soft_max")
+    m = None if mask is None else strided_desc(mask)
+    _launch("ggml_b200_op_soft_max", strided_desc(x), m, strided_desc(y), scale, max_bias, diag_n_past)
     return y
 
 
 def op_cpy(src, dst):
     """GGML_OP_CPY: src and dst torch tensors (any views) or TensorDescs (bytes_desc: a view into a quantized cache)"""
-    L = lib()
-    L.ggml_b200_op_cpy.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p]
-    s, d = (t if isinstance(t, TensorDesc) else strided_desc(t) for t in (src, dst))
-    check(L.ggml_b200_op_cpy(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_cpy")
+    _launch("ggml_b200_op_cpy", *(t if isinstance(t, TensorDesc) else strided_desc(t) for t in (src, dst)))
 
 
 def op_cpy2(src_a, dst_a, src_b, dst_b):
-    L = lib()
-    L.ggml_b200_op_cpy2.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.c_void_p]
-    a, b, c, d = tensor_desc(src_a), tensor_desc(dst_a), tensor_desc(src_b), tensor_desc(dst_b)
-    check(L.ggml_b200_op_cpy2(C.byref(a), C.byref(b), C.byref(c), C.byref(d), _stream()), "ggml_b200_op_cpy2")
-
-
-class RopeParams(C.Structure):
-    """ggml_b200_rope_params (include/ggml-b200.h)"""
-    _fields_ = [("n_dims", C.c_int32), ("mode", C.c_int32), ("sections", C.c_int32 * 4), ("freq_scale", C.c_float), ("ext_factor", C.c_float),
-                ("mscale", C.c_float), ("theta_scale", C.c_float), ("corr_dims", C.c_float * 2)]
+    _launch("ggml_b200_op_cpy2", *(tensor_desc(t) for t in (src_a, dst_a, src_b, dst_b)))
 
 
 ROPE_NORM, ROPE_NEOX, ROPE_MROPE, ROPE_VISION = 0, 2, 8, 24
@@ -466,12 +522,9 @@ def op_rope(x, pos, params: RopeParams, freq_factors=None, inplace: bool = False
     from rope_params().  inplace: dst is x (the K-shift of a cache view); out: None (a new contiguous tensor) or a tensor of x's shape and
     type with the last dim contiguous."""
     import torch
-    L = lib()
-    L.ggml_b200_op_rope.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.POINTER(RopeParams), C.c_void_p]
     y = x if inplace else out if out is not None else torch.empty(x.shape, dtype=x.dtype, device=x.device)
-    s, p, d = strided_desc(x), tensor_desc(pos), strided_desc(y)
-    f = C.byref(tensor_desc(freq_factors)) if freq_factors is not None else None
-    check(L.ggml_b200_op_rope(C.byref(s), C.byref(p), f, C.byref(d), C.byref(params), _stream()), "ggml_b200_op_rope")
+    f = tensor_desc(freq_factors) if freq_factors is not None else None
+    _launch("ggml_b200_op_rope", strided_desc(x), tensor_desc(pos), f, strided_desc(y), params)
     return y
 
 
@@ -479,31 +532,24 @@ def op_argsort(x, descending: bool = False):
     """GGML_OP_ARGSORT of a contiguous f32 torch tensor along its last dim (ggml's ne0, <= 1024): int32 indices of the same shape.
     Ties come out in ascending index and NaNs last, so every row is a permutation."""
     import torch
-    L = lib()
-    L.ggml_b200_op_argsort.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_int32, C.c_void_p]
     y = torch.empty(x.shape, dtype=torch.int32, device=x.device)
-    s, d = tensor_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_argsort(C.byref(s), C.byref(d), int(descending), _stream()), "ggml_b200_op_argsort")
+    _launch("ggml_b200_op_argsort", tensor_desc(x), tensor_desc(y), int(descending))
     return y
 
 
 def op_sum_rows(x):
     """GGML_OP_SUM_ROWS of a contiguous f32 torch tensor: the sums over its last dim (accumulated in double), shape [..., 1]"""
     import torch
-    L = lib()
-    L.ggml_b200_op_sum_rows.argtypes = [C.POINTER(TensorDesc), C.POINTER(TensorDesc), C.c_void_p]
     y = torch.empty(tuple(x.shape[:-1]) + (1,), dtype=torch.float32, device=x.device)
-    s, d = tensor_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_sum_rows(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_sum_rows")
+    _launch("ggml_b200_op_sum_rows", tensor_desc(x), tensor_desc(y))
     return y
 
 
 def strided_desc(t) -> TensorDesc:
     """descriptor of a torch tensor with any strides (a view) in ggml order: ne[i] / nb[i] from the torch dim ndim - 1 - i"""
-    import torch
     d = TensorDesc()
     d.data = t.data_ptr()
-    d.type = {torch.float32: F32, torch.float16: F16, torch.int32: 26, torch.int16: 25, torch.bfloat16: 30, torch.int64: 27}[t.dtype]
+    d.type = _desc_type(t)
     es = t.element_size()
     shape, strides = list(t.shape)[::-1], list(t.stride())[::-1]
     for i in range(4):
@@ -531,11 +577,8 @@ def op_flash_attn_ext(q, k, v, mask, scale: float, max_bias: float = 0.0, softca
     ne3, n_head, n_q, D = q.shape
     y = torch.empty((ne3, n_q, n_head, D), dtype=torch.float32, device=q.device)
     descs = [strided_desc(q)] + [t if isinstance(t, TensorDesc) else strided_desc(t) for t in (k, v)]
-    L = lib()
-    L.ggml_b200_op_flash_attn_ext.argtypes = [C.POINTER(TensorDesc)] * 5 + [C.c_float] * 3 + [C.c_void_p]
-    m = C.byref(strided_desc(mask)) if mask is not None else None
-    check(L.ggml_b200_op_flash_attn_ext(*(C.byref(d) for d in descs), m, C.byref(tensor_desc(y)), scale, max_bias, softcap, _stream()),
-          "ggml_b200_op_flash_attn_ext")
+    m = strided_desc(mask) if mask is not None else None
+    _launch("ggml_b200_op_flash_attn_ext", *descs, m, tensor_desc(y), scale, max_bias, softcap)
     return y
 
 
@@ -554,14 +597,11 @@ def op_concat(a, b, dim: int, out=None):
     a must be contiguous along its last dim; b may be any view (a transposed one, as in the Mamba layer).  A new contiguous tensor, or
     written into out (a contiguous tensor of the result's shape)."""
     import torch
-    L = lib()
-    L.ggml_b200_op_concat.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_int32, C.c_void_p]
     shape = list(a.shape)
     if 0 <= dim < a.dim():
         shape[a.dim() - 1 - dim] += b.shape[a.dim() - 1 - dim]
     y = out.view(shape) if out is not None else torch.empty(shape, dtype=a.dtype, device=a.device)
-    s0, s1, d = strided_desc(a), strided_desc(b), tensor_desc(y)
-    check(L.ggml_b200_op_concat(C.byref(s0), C.byref(s1), C.byref(d), int(dim), _stream()), "ggml_b200_op_concat")
+    _launch("ggml_b200_op_concat", strided_desc(a), strided_desc(b), tensor_desc(y), int(dim))
     return y
 
 
@@ -569,13 +609,10 @@ def op_ssm_conv(sx, c, out=None):
     """GGML_OP_SSM_CONV: sx f32 [n_s, d_inner, d_conv - 1 + n_t] (rows packed), c f32 [d_inner, d_conv] -> f32 [n_s, n_t, d_inner],
     y[s, t, i] = sum_k sx[s, i, t + k] * c[i, k], bit-identical to ggml-cpu; a new tensor, or written into out (contiguous, that size)"""
     import torch
-    L = lib()
-    L.ggml_b200_op_ssm_conv.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_void_p]
     n_s, d_inner, ncs = sx.shape
     shape = (n_s, ncs - c.shape[-1] + 1, d_inner)
     y = out.view(shape) if out is not None else torch.empty(shape, dtype=torch.float32, device=sx.device)
-    x, w, d = strided_desc(sx), strided_desc(c), tensor_desc(y)
-    check(L.ggml_b200_op_ssm_conv(C.byref(x), C.byref(w), C.byref(d), _stream()), "ggml_b200_op_ssm_conv")
+    _launch("ggml_b200_op_ssm_conv", strided_desc(sx), strided_desc(c), tensor_desc(y))
     return y
 
 
@@ -585,16 +622,12 @@ def op_ssm_scan(s, x, dt, A, B, C_, out=None):
     [n_s, d_inner, d_state]): views of the one flat result in ggml's layout (y, then the final states).  out: None (a new tensor) or a
     contiguous f32 tensor of x.numel() + s.numel() elements to hold that result."""
     import torch
-    L = lib()
-    L.ggml_b200_op_ssm_scan.argtypes = [C.POINTER(TensorDesc)] * 7 + [C.c_void_p]
     out = out.view(-1) if out is not None else torch.empty(x.numel() + s.numel(), dtype=torch.float32, device=x.device)
-    t = [strided_desc(v) for v in (s, x, dt, A, B, C_)]
-    d = tensor_desc(out)
-    check(L.ggml_b200_op_ssm_scan(*[C.byref(v) for v in t], C.byref(d), _stream()), "ggml_b200_op_ssm_scan")
+    _launch("ggml_b200_op_ssm_scan", *(strided_desc(v) for v in (s, x, dt, A, B, C_)), tensor_desc(out))
     return out[: x.numel()].view(x.shape), out[x.numel():].view(s.shape)
 
 
-def _wkv(fn, name, k, s, srcs, extra, out=None):
+def _wkv(name, k, s, srcs, extra, out=None):
     """the flat ggml result of RWKV_WKV6 / GATED_LINEAR_ATTN as (y [T, H, S], s_new [n_seqs, H, S, S]) views; s is read as [n_seqs, S S H].
     out: None (a new tensor) or a contiguous f32 tensor of (T + S n_seqs) H S elements to hold that result."""
     import torch
@@ -602,8 +635,7 @@ def _wkv(fn, name, k, s, srcs, extra, out=None):
     n_seqs = s.shape[0]
     shape = (T + S * n_seqs, H * S)
     out = out.view(shape) if out is not None else torch.empty(shape, dtype=torch.float32, device=k.device)
-    t = [strided_desc(v) for v in srcs] + [strided_desc(s.reshape(n_seqs, -1))]
-    check(fn(*[C.byref(v) for v in t], C.byref(tensor_desc(out)), *extra, _stream()), name)
+    _launch(name, *(strided_desc(v) for v in srcs), strided_desc(s.reshape(n_seqs, -1)), tensor_desc(out), *extra)
     return out[:T].view(T, H, S), out[T:].view(n_seqs, H, S, S)
 
 
@@ -611,22 +643,13 @@ def op_rwkv_wkv6(k, v, r, tf, td, s, out=None):
     """GGML_OP_RWKV_WKV6: k, v, r, td f32 [T, H, S], tf f32 [H, S], s f32 [n_seqs, H, S, S] (state[i][j] at [q, h, i, j]), all contiguous;
     sequence q owns tokens [q T / n_seqs, (q + 1) T / n_seqs).  Returns (y [T, H, S], s_new [n_seqs, H, S, S]): views of the one flat
     result in ggml's layout (y, then the final states).  out: as for _wkv."""
-    L = lib()
-    L.ggml_b200_op_rwkv_wkv6.argtypes = [C.POINTER(TensorDesc)] * 7 + [C.c_void_p]
-    return _wkv(L.ggml_b200_op_rwkv_wkv6, "ggml_b200_op_rwkv_wkv6", k, s, (k, v, r, tf, td), (), out)
+    return _wkv("ggml_b200_op_rwkv_wkv6", k, s, (k, v, r, tf, td), (), out)
 
 
 def op_gated_linear_attn(k, v, q, g, s, scale: float, out=None):
     """GGML_OP_GATED_LINEAR_ATTN: k, v, q, g f32 [T, H, S], s f32 [n_seqs, H, S, S], all contiguous; as op_rwkv_wkv6 with the gate g in
     place of the decay and q * scale in place of r (no bonus term).  Returns (y [T, H, S], s_new [n_seqs, H, S, S]); out: as for _wkv."""
-    L = lib()
-    L.ggml_b200_op_gated_linear_attn.argtypes = [C.POINTER(TensorDesc)] * 6 + [C.c_float, C.c_void_p]
-    return _wkv(L.ggml_b200_op_gated_linear_attn, "ggml_b200_op_gated_linear_attn", k, s, (k, v, q, g), (float(scale),), out)
-
-
-class Im2colParams(C.Structure):
-    """ggml_b200_im2col_params (include/ggml-b200.h)"""
-    _fields_ = [("s0", C.c_int32), ("s1", C.c_int32), ("p0", C.c_int32), ("p1", C.c_int32), ("d0", C.c_int32), ("d1", C.c_int32), ("is_2D", C.c_int32)]
+    return _wkv("ggml_b200_op_gated_linear_attn", k, s, (k, v, q, g), (float(scale),), out)
 
 
 def conv_out_size(ins: int, ks: int, s: int, p: int, d: int) -> int:
@@ -640,8 +663,6 @@ def op_im2col(kernel, x, s0: int, p0: int, d0: int, s1: int = 1, p1: int = 0, d1
     -> a new contiguous tensor [N, OW, IC KW] (2-D: [N, OH, OW, IC KH KW]) of `dtype` (default float16, as ggml_conv_1d builds it),
     bit-identical to ggml-cpu"""
     import torch
-    L = lib()
-    L.ggml_b200_op_im2col.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.POINTER(Im2colParams), C.c_void_p]
     dtype = torch.float16 if dtype is None else dtype
     kw, ic = kernel.shape[-1], x.shape[1]
     ow = conv_out_size(x.shape[-1], kw, s0, p0, d0)
@@ -652,26 +673,19 @@ def op_im2col(kernel, x, s0: int, p0: int, d0: int, s1: int = 1, p1: int = 0, d1
         shape = (x.shape[0], ow, ic * kw)
     y = torch.empty(shape, dtype=dtype, device=x.device)
     p = Im2colParams(s0, s1, p0, p1, d0, d1, 1 if is_2d else 0)
-    k, s, d = strided_desc(kernel), strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_im2col(C.byref(k), C.byref(s), C.byref(d), C.byref(p), _stream()), "ggml_b200_op_im2col")
+    _launch("ggml_b200_op_im2col", strided_desc(kernel), strided_desc(x), tensor_desc(y), p)
     return y
 
 
 def mul_mat_f16_f16_workspace_size(M: int, N: int, K: int) -> int:
     """bytes the tensor-core f16 x f16 GEMM needs for [M, K] x [N, K]; 0 when the shape is not eligible for it"""
-    L = lib()
-    L.ggml_b200_mul_mat_f16_f16_workspace_size.restype = C.c_size_t
-    L.ggml_b200_mul_mat_f16_f16_workspace_size.argtypes = [C.c_int64] * 3
-    return int(L.ggml_b200_mul_mat_f16_f16_workspace_size(M, N, K))
+    return int(lib().ggml_b200_mul_mat_f16_f16_workspace_size(M, N, K))
 
 
 def mul_mat_f16_f16(w, x, flags: int = 0, out=None):
     """f16 w [M, K] x f16 x [N, K] (rows contiguous, any row stride that is a multiple of 16 bytes) -> f32 [N, M] on the tensor cores
     (ggml_b200_mul_mat_f16_f16); raises when the shape is not eligible (N >= 9, K % 64 == 0)"""
     import torch
-    L = lib()
-    L.ggml_b200_mul_mat_f16_f16.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
-                                            C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
     M, K = w.shape
     N = x.shape[0]
     need = mul_mat_f16_f16_workspace_size(M, N, K)
@@ -679,14 +693,9 @@ def mul_mat_f16_f16(w, x, flags: int = 0, out=None):
         raise B200Error(f"mul_mat_f16_f16: ({M}, {N}, {K}) is not eligible for the tensor-core path")
     y = out if out is not None else torch.empty((N, M), dtype=torch.float32, device=w.device)
     ws = _ws.get(need)
-    check(L.ggml_b200_mul_mat_f16_f16(w.data_ptr(), w.stride(0) * 2, x.data_ptr(), x.stride(0) * 2, y.data_ptr(), M, N, K, ws.data_ptr(), ws.numel(),
-                                      flags, _stream()), "ggml_b200_mul_mat_f16_f16")
+    _launch("ggml_b200_mul_mat_f16_f16", w.data_ptr(), w.stride(0) * 2, x.data_ptr(), x.stride(0) * 2, y.data_ptr(), M, N, K, ws.data_ptr(), ws.numel(),
+            flags)
     return y
-
-
-class PoolParams(C.Structure):
-    """ggml_b200_pool_params (include/ggml-b200.h)"""
-    _fields_ = [("op", C.c_int32), ("k0", C.c_int32), ("k1", C.c_int32), ("s0", C.c_int32), ("s1", C.c_int32), ("p0", C.c_int32), ("p1", C.c_int32)]
 
 
 POOL_MAX, POOL_AVG = 0, 1
@@ -704,13 +713,10 @@ def op_pool_2d(x, op: int, k0: int, k1: int, s0: int, s1: int, p0: float = 0.0, 
     (width x height), stride s0 / s1, paddings p0 / p1 as ggml_pool_2d takes them (float: they size the output, and the kernel uses them
     truncated, as ggml-cpu does) -> a new contiguous f32 tensor [N, C, OH, OW], bit-identical to ggml-cpu"""
     import torch
-    L = lib()
-    L.ggml_b200_op_pool_2d.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.POINTER(PoolParams), C.c_void_p]
     oh, ow = pool_out_size(x.shape[-2], k1, s1, p1), pool_out_size(x.shape[-1], k0, s0, p0)
     y = torch.empty(tuple(x.shape[:-2]) + (oh, ow), dtype=torch.float32, device=x.device)
     p = PoolParams(int(op), k0, k1, s0, s1, int(p0), int(p1))
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_pool_2d(C.byref(s), C.byref(d), C.byref(p), _stream()), "ggml_b200_op_pool_2d")
+    _launch("ggml_b200_op_pool_2d", strided_desc(x), tensor_desc(y), p)
     return y
 
 
@@ -719,11 +725,8 @@ def op_upscale(x, shape):
     every extent >= x's; torch order), element i = x[i * x.shape / shape] per dim with ggml-cpu's float factors, bit-identical.
     ggml_upscale(x, f) is shape = x.shape with the last two dims times f."""
     import torch
-    L = lib()
-    L.ggml_b200_op_upscale.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_void_p]
     y = torch.empty(tuple(shape), dtype=torch.float32, device=x.device)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_upscale(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_upscale")
+    _launch("ggml_b200_op_upscale", strided_desc(x), tensor_desc(y))
     return y
 
 
@@ -731,11 +734,8 @@ def op_leaky_relu(x, slope: float, inplace: bool = False):
     """GGML_OP_LEAKY_RELU of an f32 torch tensor (last dim contiguous, any other strides): ((x > 0) ? x : 0) + slope ((x < 0) ? x : 0),
     bit-identical to ggml-cpu (NaN and -0 give +0).  inplace: the result is written into x."""
     import torch
-    L = lib()
-    L.ggml_b200_op_leaky_relu.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_float, C.c_void_p]
     y = x if inplace else torch.empty(x.shape, dtype=torch.float32, device=x.device)
-    s, d = strided_desc(x), strided_desc(y)
-    check(L.ggml_b200_op_leaky_relu(C.byref(s), C.byref(d), float(slope), _stream()), "ggml_b200_op_leaky_relu")
+    _launch("ggml_b200_op_leaky_relu", strided_desc(x), strided_desc(y), float(slope))
     return y
 
 
@@ -743,11 +743,8 @@ def op_repeat(x, shape):
     """GGML_OP_REPEAT: x (float32, int32, float16, bfloat16 or int16; last dim contiguous, any other strides) tiled into a new contiguous
     tensor of `shape` (torch order, each extent a whole multiple of x's), copied as raw words: every bit pattern is kept"""
     import torch
-    L = lib()
-    L.ggml_b200_op_repeat.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_void_p]
     y = torch.empty(tuple(shape), dtype=x.dtype, device=x.device)
-    s, d = strided_desc(x), strided_desc(y)
-    check(L.ggml_b200_op_repeat(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_repeat")
+    _launch("ggml_b200_op_repeat", strided_desc(x), strided_desc(y))
     return y
 
 
@@ -755,13 +752,10 @@ def op_win_part(x, w: int):
     """GGML_OP_WIN_PART (ggml_win_part): x f32 [H0, W0, C] (packed; torch order of ggml's [C, W0, H0]) -> a new f32 tensor
     [npx npy, w, w, C], window py npx + px holding pixels (px w + i1, py w + i2), zeros past the image; raw words, bit-identical to ggml-cpu"""
     import torch
-    L = lib()
-    L.ggml_b200_op_win_part.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_int32] * 3 + [C.c_void_p]
     h0, w0, c = x.shape[-3:]
     npx, npy = -(-w0 // w), -(-h0 // w)
     y = torch.empty((npx * npy, w, w, c), dtype=torch.float32, device=x.device)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_win_part(C.byref(s), C.byref(d), npx, npy, w, _stream()), "ggml_b200_op_win_part")
+    _launch("ggml_b200_op_win_part", strided_desc(x), tensor_desc(y), npx, npy, w)
     return y
 
 
@@ -769,11 +763,8 @@ def op_win_unpart(x, w0: int, h0: int, w: int):
     """GGML_OP_WIN_UNPART (ggml_win_unpart): x f32 [np, w, w, C] (packed, np >= ceil(w0 / w) ceil(h0 / w)) -> a new f32 tensor [h0, w0, C],
     the inverse of op_win_part without its padding; raw words, bit-identical to ggml-cpu"""
     import torch
-    L = lib()
-    L.ggml_b200_op_win_unpart.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_int32, C.c_void_p]
     y = torch.empty((h0, w0, x.shape[-1]), dtype=torch.float32, device=x.device)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_win_unpart(C.byref(s), C.byref(d), w, _stream()), "ggml_b200_op_win_unpart")
+    _launch("ggml_b200_op_win_unpart", strided_desc(x), tensor_desc(y), w)
     return y
 
 
@@ -781,12 +772,9 @@ def op_get_rel_pos(x):
     """GGML_OP_GET_REL_POS (ggml_get_rel_pos): x f16 [2w - 1, C] (packed) -> a new f16 tensor [w, w, C], y[i2, i1] = x[(w - 1 - i1) + i2];
     raw 2-byte words, bit-identical to ggml-cpu"""
     import torch
-    L = lib()
-    L.ggml_b200_op_get_rel_pos.argtypes = [C.POINTER(TensorDesc)] * 2 + [C.c_void_p]
     w = (x.shape[-2] + 1) // 2
     y = torch.empty((w, w, x.shape[-1]), dtype=x.dtype, device=x.device)
-    s, d = strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_get_rel_pos(C.byref(s), C.byref(d), _stream()), "ggml_b200_op_get_rel_pos")
+    _launch("ggml_b200_op_get_rel_pos", strided_desc(x), tensor_desc(y))
     return y
 
 
@@ -795,11 +783,8 @@ def op_add_rel_pos(a, pw, ph, inplace: bool = False):
     a[p, q, kh L + kw] + ph[p, q, kh] + pw[p, q, kw] with ggml-cpu's order of the two adds (ph first when kh <= kw): bit-identical.
     inplace: the result is written into a."""
     import torch
-    L = lib()
-    L.ggml_b200_op_add_rel_pos.argtypes = [C.POINTER(TensorDesc)] * 4 + [C.c_void_p]
     y = a if inplace else torch.empty(a.shape, dtype=torch.float32, device=a.device)
-    s, w, h, d = strided_desc(a), strided_desc(pw), strided_desc(ph), strided_desc(y)
-    check(L.ggml_b200_op_add_rel_pos(C.byref(s), C.byref(w), C.byref(h), C.byref(d), _stream()), "ggml_b200_op_add_rel_pos")
+    _launch("ggml_b200_op_add_rel_pos", strided_desc(a), strided_desc(pw), strided_desc(ph), strided_desc(y))
     return y
 
 
@@ -808,13 +793,10 @@ def op_conv_transpose_2d(kernel, x, stride: int):
     [1, Cin, H, W] (last dim contiguous) -> a new f32 tensor [(1,) Cout, (H-1) s + Kh, (W-1) s + Kw], padding 0.  x is rounded to fp16 as
     ggml-cpu rounds it; each tap's dot over Cin is summed in f32 and the taps are added in ggml-cpu's order."""
     import torch
-    L = lib()
-    L.ggml_b200_op_conv_transpose_2d.argtypes = [C.POINTER(TensorDesc)] * 3 + [C.c_int32, C.c_void_p]
     cout, kh, kw = kernel.shape[1:]
     h, w = x.shape[-2:]
     y = torch.empty(tuple(x.shape[:-3]) + (cout, (h - 1) * stride + kh, (w - 1) * stride + kw), dtype=torch.float32, device=x.device)
-    k, s, d = strided_desc(kernel), strided_desc(x), tensor_desc(y)
-    check(L.ggml_b200_op_conv_transpose_2d(C.byref(k), C.byref(s), C.byref(d), stride, _stream()), "ggml_b200_op_conv_transpose_2d")
+    _launch("ggml_b200_op_conv_transpose_2d", strided_desc(kernel), strided_desc(x), tensor_desc(y), stride)
     return y
 
 
@@ -831,18 +813,8 @@ def op_bin_bcast(op: int, a, b, out=None):
     any views (out = a: in place).  out None: a new contiguous tensor"""
     import torch
     y = out if out is not None else torch.empty(a.shape, dtype=torch.float32, device=a.device)
-    L = lib()
-    L.ggml_b200_op_bin_bcast.argtypes = [C.c_int32] + [C.POINTER(TensorDesc)] * 3 + [C.c_void_p]
-    s0, s1, d = strided_desc(a), strided_desc(b), strided_desc(y)
-    check(L.ggml_b200_op_bin_bcast(op, C.byref(s0), C.byref(s1), C.byref(d), _stream()), "ggml_b200_op_bin_bcast")
+    _launch("ggml_b200_op_bin_bcast", op, strided_desc(a), strided_desc(b), strided_desc(y))
     return y
-
-
-def _launch(name: str, *descs):
-    L = lib()
-    fn = getattr(L, name)
-    fn.argtypes = [C.POINTER(TensorDesc)] * len(descs) + [C.c_void_p]
-    check(fn(*(C.byref(d) for d in descs), _stream()), name)
 
 
 def op_out_prod(a, b):

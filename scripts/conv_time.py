@@ -60,7 +60,6 @@ def time_op(fn, iters):
 def plain_mul_mat(cols, w, y):
     """ggml_b200_op_mul_mat_f on f16 cols [M, K] x f16 w [N, K] -> y f32 [N, M]"""
     L = g.lib()
-    L.ggml_b200_op_mul_mat_f.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.c_void_p]
     a, b, d = g.strided_desc(cols), g.strided_desc(w), g.tensor_desc(y)
     g.check(L.ggml_b200_op_mul_mat_f(C.byref(a), C.byref(b), C.byref(d), g._stream()), "ggml_b200_op_mul_mat_f")
 

@@ -128,7 +128,6 @@ VIT_B_MATMULS = [
 
 def plain_kernel(iters):
     L = g.lib()
-    L.ggml_b200_op_mul_mat_f.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.c_void_p]
     gen = torch.Generator(device="cuda").manual_seed(1)
     total_us, total_flop = 0.0, 0.0
     for name, ne_a, ta, ne_b, count in VIT_B_MATMULS:

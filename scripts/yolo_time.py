@@ -83,7 +83,6 @@ def kernels(iters):
 def plain_kernel(iters):
     """us of the three plain-kernel conv mat-muls: ggml_b200_op_mul_mat_f, src0 the f16 columns [K, M], src1 the f16 kernel [K, N]"""
     L = g.lib()
-    L.ggml_b200_op_mul_mat_f.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.c_void_p]
     gen = torch.Generator(device="cuda").manual_seed(1)
     total = 0.0
     for name, M, N, K in PLAIN:

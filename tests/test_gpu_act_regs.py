@@ -58,7 +58,6 @@ def _child(out_path):
         else:
             # ggml_b200.mul_mat_fused with the independent-launch flags
             L = g.lib()
-            L.ggml_b200_mul_mat_fused.argtypes = [C.POINTER(g.MulMatArgs), C.POINTER(g.Epilogue), C.c_void_p]
             Y, Y2, Y3 = (torch.empty(M, dtype=torch.float32, device="cuda") for _ in range(3))
             a = g.mul_mat_args(t, W, X, Y, M, 1, K, flags=g.MM_SRC0_STATIC | g.MM_SRC1_STATIC)
             ep = g.Epilogue()

@@ -83,9 +83,6 @@ def test_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    L.ggml_b200_op_concat.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.c_int32, C.c_void_p]
-    L.ggml_b200_op_ssm_conv.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.c_void_p]
-    L.ggml_b200_op_ssm_scan.argtypes = [C.POINTER(g.TensorDesc)] * 7 + [C.c_void_p]
     D = g.strided_desc
     z = lambda *shape, dt=torch.float32: torch.zeros(shape, dtype=dt, device="cuda")
 

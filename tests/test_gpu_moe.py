@@ -107,8 +107,6 @@ def test_argsort_and_sum_rows_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    L.ggml_b200_op_argsort.argtypes = [C.POINTER(g.TensorDesc), C.POINTER(g.TensorDesc), C.c_int32, C.c_void_p]
-    L.ggml_b200_op_sum_rows.argtypes = [C.POINTER(g.TensorDesc), C.POINTER(g.TensorDesc), C.c_void_p]
     x = torch.zeros((3, 16), dtype=torch.float32, device="cuda")
     ids = torch.zeros((3, 16), dtype=torch.int32, device="cuda")
 

@@ -51,10 +51,7 @@ def env():
     import torch
     import ggml_b200 as g
     assert torch.cuda.is_available(), "these tests need an H100"
-    L = R.load(g.KERNELS_SO)
-    L.ggml_b200_mul_mat_f16_f16_workspace_size.restype = C.c_size_t
-    L.ggml_b200_mul_mat_f16_f16_workspace_size.argtypes = [C.c_int64] * 3
-    L.ggml_b200_mul_mat_f16_f16.argtypes = L.ggml_b200_mul_mat_f16.argtypes
+    L = g.lib()
     return g, L, O.Oracle()
 
 

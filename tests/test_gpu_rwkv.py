@@ -89,8 +89,6 @@ def test_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    L.ggml_b200_op_rwkv_wkv6.argtypes = [C.POINTER(g.TensorDesc)] * 7 + [C.c_void_p]
-    L.ggml_b200_op_gated_linear_attn.argtypes = [C.POINTER(g.TensorDesc)] * 6 + [C.c_float, C.c_void_p]
     D = g.strided_desc
     z = lambda *shape, dt=torch.float32: torch.zeros(shape, dtype=dt, device="cuda")
     S, H, T, ns = 16, 2, 6, 2

@@ -128,12 +128,6 @@ def test_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    TD = C.POINTER(g.TensorDesc)
-    L.ggml_b200_op_win_part.argtypes = [TD, TD, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-    L.ggml_b200_op_win_unpart.argtypes = [TD, TD, C.c_int32, C.c_void_p]
-    L.ggml_b200_op_get_rel_pos.argtypes = [TD, TD, C.c_void_p]
-    L.ggml_b200_op_add_rel_pos.argtypes = [TD] * 4 + [C.c_void_p]
-    L.ggml_b200_op_conv_transpose_2d.argtypes = [TD] * 3 + [C.c_int32, C.c_void_p]
     D = g.strided_desc
     z = lambda *shape, dt=torch.float32: torch.zeros(shape, dtype=dt, device="cuda")
     wp = lambda s, d, npx, npy, w: L.ggml_b200_op_win_part(C.byref(D(s)), C.byref(D(d)), npx, npy, w, None)

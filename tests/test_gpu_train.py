@@ -252,24 +252,18 @@ def test_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    TD = C.POINTER(g.TensorDesc)
     D = g.strided_desc
     z = lambda *shape, dt=torch.float32: torch.zeros(shape, dtype=dt, device="cuda")
-    L.ggml_b200_op_out_prod.argtypes = [TD] * 3 + [C.c_void_p]
     op = lambda a, b, d: L.ggml_b200_op_out_prod(C.byref(D(a)), C.byref(D(b)), C.byref(D(d)), None)
     assert op(z(7, 16), z(7, 5), z(5, 16)) == 0 and op(z(7, 16), z(6, 5), z(5, 16)) == -2 and op(z(7, 16).half(), z(7, 5), z(5, 16)) == -1
     assert op(z(16, 7).t(), z(7, 5), z(5, 16)) == -1 and op(z(7, 16), z(5, 7).t(), z(5, 16)) == 0
-    L.ggml_b200_op_opt_step_adamw.argtypes = [TD] * 5 + [C.c_void_p]
     ad = lambda w, p: L.ggml_b200_op_opt_step_adamw(*(C.byref(D(t)) for t in (w, w, w, w, p)), None)
     assert ad(z(10, 5), z(7)) == 0 and ad(z(10, 5), z(6)) == -2 and ad(z(10, 6)[:, :5], z(7)) == -1
-    L.ggml_b200_op_count_equal.argtypes = [TD] * 3 + [C.c_void_p]
     ce = lambda a, d: L.ggml_b200_op_count_equal(C.byref(D(a)), C.byref(D(a)), C.byref(D(d)), None)
     i32 = torch.int32
     assert ce(z(5, 4, dt=i32), z(1, dt=torch.int64)) == 0 and ce(z(5, 4, dt=i32), z(1, dt=i32)) == -1 and ce(z(3, 5, 4, dt=i32), z(1, dt=torch.int64)) == -1
-    L.ggml_b200_op_argmax.argtypes = [TD] * 2 + [C.c_void_p]
     am = lambda x, d: L.ggml_b200_op_argmax(C.byref(D(x)), C.byref(D(d)), None)
     assert am(z(5, 100), z(5, dt=i32)) == 0 and am(z(5, 100), z(4, dt=i32)) == -2 and am(z(5, 100), z(5)) == -1
-    L.ggml_b200_op_repeat_back.argtypes = [TD] * 2 + [C.c_void_p]
     rb = lambda x, d: L.ggml_b200_op_repeat_back(C.byref(D(x)), C.byref(D(d)), None)
     assert rb(z(4, 6), z(2, 3)) == 0 and rb(z(4, 6), z(3, 3)) == -2 and rb(z(4, 6, dt=i32), z(2, 3, dt=i32)) == -1
     torch.cuda.synchronize()

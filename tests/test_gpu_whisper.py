@@ -114,7 +114,6 @@ def test_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    L.ggml_b200_op_im2col.argtypes = [C.POINTER(g.TensorDesc)] * 3 + [C.POINTER(g.Im2colParams), C.c_void_p]
     D = g.strided_desc
     z = lambda *shape, dt=torch.float32: torch.zeros(shape, dtype=dt, device="cuda")
 
@@ -134,8 +133,6 @@ def test_c_abi_error_codes():
     w, xx = z(1500, 1152, dt=torch.float16), z(384, 1152, dt=torch.float16)
     need = g.mul_mat_f16_f16_workspace_size(1500, 384, 1152)
     assert need > 0 and g.mul_mat_f16_f16_workspace_size(1500, 8, 1152) == 0 and g.mul_mat_f16_f16_workspace_size(1500, 384, 1000) == 0
-    L.ggml_b200_mul_mat_f16_f16.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
-                                            C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
     out, ws = z(384, 1500), torch.empty(need, dtype=torch.uint8, device="cuda")
 
     def mm(M, N, K, nb01=2 * 1152, nb11=2 * 1152, wsz=need):

@@ -110,11 +110,6 @@ def test_c_abi_error_codes():
     import torch
     import ggml_b200 as g
     L = g.lib()
-    TD = C.POINTER(g.TensorDesc)
-    L.ggml_b200_op_pool_2d.argtypes = [TD, TD, C.POINTER(g.PoolParams), C.c_void_p]
-    L.ggml_b200_op_upscale.argtypes = [TD, TD, C.c_void_p]
-    L.ggml_b200_op_leaky_relu.argtypes = [TD, TD, C.c_float, C.c_void_p]
-    L.ggml_b200_op_repeat.argtypes = [TD, TD, C.c_void_p]
     D = g.strided_desc
     z = lambda *shape, dt=torch.float32: torch.zeros(shape, dtype=dt, device="cuda")
     x, y = z(1, 16, 13, 13), z(1, 16, 6, 6)

@@ -49,27 +49,6 @@ F16 = [(4096, 512, 4096), (4096, 9, 4096), (4096, 8, 4096), (11008, 64, 4096), (
 PLANNING_ENV = ("GGML_B200_FORCE_GENERIC", "GGML_B200_MMID_GROUPED")
 
 
-def load(path: Path) -> C.CDLL:
-    L = C.CDLL(str(path))
-    L.ggml_b200_last_error.restype = C.c_char_p
-    L.ggml_b200_mul_mat_plan.argtypes = [C.POINTER(g.MulMatArgs)]
-    L.ggml_b200_mul_mat.argtypes = [C.POINTER(g.MulMatArgs), C.c_void_p]
-    L.ggml_b200_mul_mat_id.argtypes = [C.POINTER(g.MulMatIdArgs), C.c_void_p]
-    L.ggml_b200_mul_mat_workspace_size.restype = C.c_size_t
-    L.ggml_b200_mul_mat_workspace_size.argtypes = [C.POINTER(g.MulMatArgs)]
-    L.ggml_b200_mul_mat_gather_supported.argtypes = [C.POINTER(g.MulMatArgs)]
-    L.ggml_b200_mul_mat_id_workspace_size.restype = C.c_size_t
-    L.ggml_b200_mul_mat_id_workspace_size.argtypes = [C.POINTER(g.MulMatIdArgs)]
-    L.ggml_b200_mul_mat_f16_workspace_size.restype = C.c_size_t
-    L.ggml_b200_mul_mat_f16_workspace_size.argtypes = [C.c_int64, C.c_int64, C.c_int64]
-    L.ggml_b200_mul_mat_f16.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
-                                        C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
-    L.ggml_b200_launch_count.restype = C.c_uint64
-    L.ggml_b200_row_size.restype = C.c_size_t
-    L.ggml_b200_row_size.argtypes = [C.c_int32, C.c_int64]
-    return L
-
-
 def environment(L: C.CDLL) -> dict:
     try:
         C.CDLL("libcuda.so.1")
@@ -145,7 +124,7 @@ def fixture_name(env: dict) -> str:
 
 
 def regen(lib: Path, out: Path) -> Path:
-    L = load(lib)
+    L = g.load(lib)
     env = environment(L)
     path = out / fixture_name(env)
     data = {"environment": env, **record(L)}
@@ -158,7 +137,7 @@ def regen(lib: Path, out: Path) -> Path:
 def test_route_pin(fixture):
     if any(k in os.environ for k in PLANNING_ENV):
         pytest.skip(f"one of {PLANNING_ENV} is set: planning reads them")
-    L = load(g.KERNELS_SO)
+    L = g.lib()
     env = environment(L)
     want = json.loads(gzip.decompress((GOLDEN / fixture).read_bytes()))
     if want["environment"] != env:
@@ -205,7 +184,7 @@ def agreement() -> list[str]:
     import numpy as np
     import torch
     from oracle import oracle as O
-    L = load(g.KERNELS_SO)
+    L = g.lib()
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     rng = np.random.default_rng(0)
     fails = []
